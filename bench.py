@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- fused KNN + gather throughput of the FFB6D fusion hot path on B200.
+"""bench.py -- fused KNN + gather throughput of the FFB6D fusion hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W          (N>1: launched by torchrun)
     python bench.py --impl reference ...                    (the reference's CPU ops, host cores)
@@ -30,7 +30,7 @@ if ROOT not in sys.path:
 
 METRIC = "fused KNN+gather points/sec at 12288 pts"
 UNIT = "points/s"
-FALLBACK_HBM_GBS = 6650.0      # /opt/skills/guides/B200_PROFILING.md fallback
+FALLBACK_HBM_GBS = 3350.0      # H100 SXM data sheet (HBM3), used when MEASURED_PEAKS.json is absent
 
 
 def env_int(name, default):
@@ -248,16 +248,7 @@ def load_peaks():
             d = json.load(fh)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
-
-
-def load_ncu_traffic():
-    """{kernel family: dram bytes per launch} from the committed ncu summary, if any."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as fh:
-            return json.load(fh)
-    except Exception:
-        return {}
+        return FALLBACK_HBM_GBS, "H100 SXM data sheet (no MEASURED_PEAKS.json)"
 
 
 K1_FAMILY = "K=1 searches (grid_search_k1_tile_kernel for image queries, grid_search_kernel<1>, knn_brute for S<512)"
@@ -281,6 +272,34 @@ def kernel_family(op_name):
     return SELF_FAMILY if key.startswith("cld_nei") else NONSELF_FAMILY
 
 
+DUMP_CAP = 1 << 17      # elements per dumped array: the 54 arrays stay under 64 MB
+
+
+def dump_outputs(dirname, gathers, res):
+    """Write what one step of the timed path returned -- the 22 KNN index tensors (+ the derived ones
+    and `choose`) and the 23 gather outputs -- as DIR/<name>.npy: float32 features, float64 indices.
+    An array above DUMP_CAP elements is replaced by the same seeded sample of DUMP_CAP positions in
+    every run (one position drawn from each of DUMP_CAP equal strides), so that two builds can be
+    compared output for output."""
+    import numpy as np
+    import torch
+    inputs, outs = res
+    arrays = {k: v for k, v in inputs.items() if torch.is_tensor(v)}
+    for i, ((op, key, C, S, Q, K), o) in enumerate(zip(gathers, outs)):
+        arrays["gather%02d_%s_%s" % (i, op, key)] = o
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in sorted(arrays.items()):
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_CAP:
+            stride = flat.numel() // DUMP_CAP
+            rs = np.random.RandomState(flat.numel() % (1 << 31))
+            pos = np.arange(DUMP_CAP, dtype=np.int64) * stride + rs.randint(0, stride, size=DUMP_CAP)
+            flat = flat[torch.from_numpy(pos).to(flat.device)]
+        a = flat.cpu().numpy()
+        a = a.astype(np.float32) if t.is_floating_point() else a.astype(np.float64)
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -299,7 +318,11 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="time eager launches instead of CUDA graph replays")
     ap.add_argument("--per-op", action="store_true", help="also print the per-op table to stderr")
     ap.add_argument("--l2-fetch", type=int, default=0, help="experiment: cudaLimitMaxL2FetchGranularity (32/64/128 bytes)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the arrays the last timed step computed to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
     rank, local_rank, world = env_int("RANK", 0), env_int("LOCAL_RANK", 0), env_int("WORLD_SIZE", 1)
@@ -389,12 +412,14 @@ def main():
     torch.cuda.synchronize()
     e0.record()
     for _ in range(args.steps):
-        run_resident()
+        last_res = run_resident()
     e1.record()
     torch.cuda.synchronize()
     barrier()
     launches = launches_per_step * args.steps
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, p.gathers, last_res)
     resident_res = run_resident()          # untimed: the results the end-to-end path must reproduce
     torch.cuda.synchronize()
 
@@ -524,18 +549,15 @@ def main():
     tot_ms = sum(f["ms"] for f in fam.values())
     # `roofline` = the dominant HBM-BOUND kernel family, chosen deterministically: the gather family that
     # moves the most algorithmic bytes (a function of the configuration, not of a timing that flips
-    # between runs).  The KNN searches are instruction-issue bound (DRAM < 2 % busy in ncu): they are
-    # reported in `compute` with instructions per query instead of a meaningless HBM fraction.
+    # between runs).  The KNN searches move a few bytes per query and are bound by instruction issue: they
+    # are reported in `compute` with time per query instead of a meaningless HBM fraction.
     gfam = [k for k in fam if k.startswith("gather")]
     dom = max(gfam, key=lambda k: (fam[k]["bytes"], k))
     dd = fam[dom]
     achieved = dd["bytes"] / (dd["ms"] / 1e3) / 1e9
-    ncu = load_ncu_traffic()
-    cap = ncu.get(dom, {}) if isinstance(ncu.get(dom), dict) else {}
-    traffic = cap.get("traffic_bytes")
     roofline = {
         "bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-        "frac": achieved / peak, "traffic": traffic, "traffic_capture": cap or None, "peak_source": peak_src,
+        "frac": achieved / peak, "peak_source": peak_src,
         "selection": "gather family with the most algorithmic bytes per step (deterministic)",
         "share_of_step": dd["ms"] / tot_ms, "ops_per_step": dd["n"] // steps,
         "alg_bytes_per_launch": dd["bytes"] / dd["n"], "avg_launch_ms": dd["ms"] / dd["n"],
@@ -548,8 +570,7 @@ def main():
     for key_, s_, q_, kk_ in knn_schedule(N0, k=args.k):
         q_n = set_size(q_, N0)
         n_q["k1" if kk_ == 1 else ("k16_self" if s_ == q_ else "k16")] += q_n * B
-    compute = {"note": "KNN index build: integer/fp32 issue bound, HBM traffic ~ algorithmic (12S + 12Q + 4QK per call); "
-                       "instructions per query from the committed ncu captures (profiles/ncu_traffic.json)",
+    compute = {"note": "KNN index build: integer/fp32 issue bound, HBM traffic ~ algorithmic (12S + 12Q + 4QK per call)",
                "families": {}}
     for k, v in sorted(fam.items()):
         if k.startswith("gather"):
@@ -566,9 +587,6 @@ def main():
             entry["note"] = "4 of the 7 searches are row slices of the other 3 (cloud levels are prefixes): not run"
         if "queries_per_step" in entry and v["ms"] > 0:
             entry["ns_per_query"] = v["ms"] / steps * 1e6 / entry["queries_per_step"]
-        cap_k = ncu.get(k)
-        if isinstance(cap_k, dict) and "warp_instructions_per_query" in cap_k:
-            entry["warp_instructions_per_query"] = cap_k["warp_instructions_per_query"]
         compute["families"][k] = entry
     knn_ms = sum(v["ms"] for k, v in fam.items() if not k.startswith("gather")) / steps
     compute["knn_ms_per_step"] = knn_ms
@@ -602,13 +620,13 @@ def main():
             with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
                 bf16_peak = float(json.load(fh)["bf16_tflops"])
         except Exception:
-            bf16_peak = 1590.0
+            bf16_peak = 989.0          # H100 SXM data sheet, dense BF16
         tf32_tflops = 3.0 * mlps.flops / (mlp_ms / 1e3) / 1e12          # three TF32 MMAs per fp32 product
         mlp_line = {"layers": len(mlps.layers), "ms_per_step": mlp_ms, "fp32_equiv_tflops": tf32_tflops / 3.0,
                     "tf32_tflops_issued": tf32_tflops,
                     "roofline": {"bound": "tensor", "achieved": tf32_tflops, "peak": bf16_peak / 2.0,
                                  "unit": "TFLOP/s", "frac": tf32_tflops / (bf16_peak / 2.0),
-                                 "note": "kind::tf32 peak taken as half the measured bf16 peak; 3xTF32 split for "
+                                 "note": "TF32 peak taken as half the bf16 peak; 3xTF32 split for "
                                          "fp32 fidelity (1e-5 contract)"},
                     "note": "28 fused cat+conv1x1+BN(eval)+ReLU layers of the fusion stack (models/ffb6d.py:55-80,"
                             "104-129), frames_per_gpu x 34.1 GFLOP; not part of `value`; weights split into TF32 hi/lo "
@@ -846,7 +864,7 @@ def main():
                         % (B, N0, args.k),
             "frames_per_gpu": B, "n_points": N0, "k": args.k, "feature_layout": args.layout,
             "parallelism": "frames sharded over %d GPU(s), no data-path collective" % world,
-            "l2": "per-step inputs (%.1f GB of features + xyz) exceed the 126 MB L2; no flush needed"
+            "l2": "per-step inputs (%.1f GB of features + xyz) exceed the 50 MB L2; no flush needed"
                   % ((feat_bytes + xyz_h.numel() * 4) / 1e9),
         },
         "e2e": {"value": e2e_value, "unit": UNIT, "ms_per_step": e2e_ms / steps,

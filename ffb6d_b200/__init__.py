@@ -1,4 +1,4 @@
-"""ffb6d_b200 -- B200 (sm_100a) implementation of FFB6D's bidirectional-fusion hot path.
+"""ffb6d_b200 -- H100 (sm_90a) implementation of FFB6D's bidirectional-fusion hot path.
 
 Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
 

@@ -41,7 +41,7 @@ const DeviceInfo &device_info()
         DeviceInfo d;
         if (cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.num_sms < 1) {
             cudaGetLastError();
-            d.num_sms = 148;   // B200
+            d.num_sms = 132;   // H100 SXM
         }
         if (cudaDeviceGetAttribute(&d.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) {
             cudaGetLastError();
@@ -59,8 +59,6 @@ const Env &env()
         Env v;
         auto on = [](const char *n) { const char *x = getenv(n); return x && *x && strcmp(x, "0") != 0; };
         v.gather_direct = on("FFB6D_GATHER_DIRECT");
-        v.mlp_no_direct = on("FFB6D_MLP_NO_DIRECT");
-        v.mlp_no_pair_tiles = on("FFB6D_MLP_NO_MT2");
         v.check_indices = on("FFB6D_CHECK_INDICES");
         v.grid_thread_search = on("FFB6D_GRID_THREAD_SEARCH");
         v.subset_nn = on("FFB6D_SUBSET_NN");

@@ -1,4 +1,4 @@
-// backproject.cu -- depth map -> the point sets the fusion schedule searches (sm_100a).
+// backproject.cu -- depth map -> the point sets the fusion schedule searches (sm_90a).
 //
 // The reference back-projects the depth image on the CPU (dpt_2_pcld, datasets/ycb/ycb_dataset.py:
 // 165-176), keeps the organised cloud [H,W,3], samples N pixels from it (`choose`, :218-237) and

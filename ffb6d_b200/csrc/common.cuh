@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libffb6d_b200.so (sm_100a only).
+// common.cuh -- shared helpers for libffb6d_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -51,7 +51,7 @@ static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; 
 // and SM counts belong to the CURRENT device, never to the process).
 constexpr int kMaxDevices = 64;
 struct DeviceInfo {
-    int num_sms;          // 148 on B200
+    int num_sms;          // 132 on H100 SXM
     int max_smem_optin;   // bytes of dynamic shared memory a kernel may opt into
 };
 int current_device();                 // cudaGetDevice, 0 on error
@@ -78,8 +78,6 @@ int wgrad_small_launch(const float *grad_z, const float *x1, int64_t C1, const f
 // Experiment switches, read ONCE per process (never in a launch path; results never depend on them).
 struct Env {
     bool gather_direct;     // FFB6D_GATHER_DIRECT=1: K-lane gathers through the older direct kernel
-    bool mlp_no_direct;     // FFB6D_MLP_NO_DIRECT=1
-    bool mlp_no_pair_tiles; // FFB6D_MLP_NO_MT2=1: one 128-row weight tile per CTA for every layer (A/B timing)
     bool check_indices;     // FFB6D_CHECK_INDICES=1: validate gather indices (synchronises; debugging aid)
     bool grid_thread_search;
     bool subset_nn;         // FFB6D_SUBSET_NN=1: ffb6d_build_indices reads cld_interp_idx{0,1} off the self searches (ffb6d_knn_subset_nn)

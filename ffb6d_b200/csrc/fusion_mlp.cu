@@ -1,4 +1,4 @@
-// fusion_mlp.cu -- the 1x1 fusion MLP of FFB6D on 5th-generation tensor cores (sm_100a).
+// fusion_mlp.cu -- the 1x1 fusion MLP of FFB6D on Hopper tensor cores (sm_90a, wgmma).
 //
 // Reference: pt_utils.Conv2d(in, out, kernel_size=(1,1), bn=True) = conv(bias=False) ->
 // BatchNorm2d -> ReLU (models/pytorch_utils.py:75-129, 168-201), 28 instances built at
@@ -9,32 +9,32 @@
 //
 // Kernels in this file (DESIGN.md 4.4):
 //   fusion_mlp_packed_kernel  the product path: weights pre-split once (ffb6d_fusion_mlp_pack) and
-//                             fetched by bulk-async copies, warp-specialised mbarrier pipeline,
-//                             16 staging warps (K > 128) or the 3-CTA/SM DIRECT variant (K <= 128)
+//                             fetched by bulk-async copies (TMA engine, mbarrier completion), the
+//                             activations staged by the CTA's threads
+//   fusion_wgrad_kernel       the weight gradient of training, same tile machinery
 //
 // All of them fuse the concat (two K ranges read from two tensors), the GEMM, BN and ReLU:
-//   * tcgen05.mma kind::tf32, M = N = 128 per CTA, accumulators in TMEM (128 lanes x 128 columns)
+//   * wgmma.mma_async m64n128k8 .tf32, two warpgroups per CTA (rows 0-63 and 64-127 of a 128 x 128
+//     tile), accumulators in registers
 //   * fp32 fidelity through 3xTF32: every fp32 operand is split into hi = tf32(x) and
 //     lo = tf32(x - hi) while it is staged, and D += Ahi*Bhi + Alo*Bhi + Ahi*Blo (the dropped lo*lo
 //     term is 2^-22 relative): results agree with the fp32 cuDNN path to ~1e-6 relative, inside the
 //     1e-5 contract of BASELINE.json
-//   * operands are staged by the CTA's threads (the split needs a register pass anyway) into the
-//     canonical K-major no-swizzle UMMA layout: 8-row x 16-byte core matrices, 128 B between 8-row
-//     groups (SBO), 2048 B between 16-byte K chunks (LBO); X is transposed on the fly (it is
-//     point-major in memory)
-//   * two stages: the MMAs of stage s run asynchronously (completion -> mbarrier via
-//     tcgen05.commit) while the threads stage s+1
-//   * the tensor core adds into its fp32 accumulator with truncation, which drifts by ~2^-24 per
-//     MMA (measured 1.2e-5 relative at K = 2048); K is therefore accumulated in chunks of 128 into
-//     two alternating TMEM accumulators that the warps drain into round-to-nearest fp32 register
-//     sums while the next chunk is being multiplied
-//   * epilogue: tcgen05.ld 32x32b -> scale/shift/ReLU in registers -> 128-bit stores along the
-//     point axis (NCHW output, no transposition needed because M = output channel = TMEM lane).
+//   * operands are staged into the canonical K-major no-swizzle layout: 8-row x 16-byte core
+//     matrices, 128 B between 8-row groups (SBO), 2048 B between 16-byte K chunks (LBO); X is
+//     transposed on the fly (it is point-major in memory)
+//   * three stages and one CTA barrier per k-tile: the MMAs of k-tile kt run asynchronously while
+//     the threads load k-tile kt + 1 from global memory; a stage is rewritten only after every
+//     warpgroup has waited for the MMAs that read it (wgmma.wait_group 1 before the barrier)
+//   * the tensor core's fp32 accumulation truncates, a bias that grows with every MMA into the same
+//     accumulator (chunks of 128 = 48 MMAs: ~4e-6 relative, enough to show in whole-network training
+//     gradients); K is therefore accumulated one k-tile (12 MMAs) at a time and every chunk is added
+//     into round-to-nearest fp32 register sums
+//   * epilogue: scale/shift/activation in registers, stores along the point axis (NCHW output)
 #include "common.cuh"
 
 #include <algorithm>
 #include <stdlib.h>
-#include <type_traits>
 
 namespace ffb6d {
 
@@ -42,48 +42,100 @@ constexpr int TM = 128, TN = 128, TK = 32;            // CTA tile
 constexpr int CHUNK_BYTES = TM * 16;                  // one 16-byte K chunk of all 128 rows
 constexpr int TILE_BYTES = (TK / 4) * CHUNK_BYTES;    // 16 KB
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;           // A_hi, A_lo, B_hi, B_lo
-constexpr int CH = 4;                                 // k-tiles per accumulation chunk (K = 128)
+constexpr int NST = 3;                                // stages
+constexpr int CH = 1;                                 // k-tiles per accumulation chunk (K = 32, 12 MMAs)
+constexpr int MLP_THREADS = 256;                      // two warpgroups
+constexpr int MLP_SMEM = NST * STAGE_BYTES + 64;      // stages + mbarriers: 192 KB, one CTA per SM
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // round-to-nearest (ties away) to TF32's 10-bit mantissa with two full-rate integer ops; identical to
-// cvt.rna.tf32.f32 for finite inputs (that conversion runs on the quarter-rate conversion pipe and was
-// the staging bottleneck)
+// cvt.rna.tf32.f32 for finite inputs (that conversion runs on the quarter-rate conversion pipe)
 __device__ __forceinline__ float to_tf32(float x)
 {
     return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
 
-#ifndef FFB6D_MLP_ROUND_LO
-#define FFB6D_MLP_ROUND_LO 1   // 0: leave the low part unrounded (the tensor core truncates it): 2 ops fewer per element
-#endif
-__device__ __forceinline__ float lo_part(float d) { return FFB6D_MLP_ROUND_LO ? to_tf32(d) : d; }
-
 __device__ __forceinline__ void split4(const float4 v, float4 &hi, float4 &lo)
 {
-    hi.x = to_tf32(v.x); lo.x = lo_part(v.x - hi.x);
-    hi.y = to_tf32(v.y); lo.y = lo_part(v.y - hi.y);
-    hi.z = to_tf32(v.z); lo.z = lo_part(v.z - hi.z);
-    hi.w = to_tf32(v.w); lo.w = lo_part(v.w - hi.w);
+    hi.x = to_tf32(v.x); lo.x = to_tf32(v.x - hi.x);
+    hi.y = to_tf32(v.y); lo.y = to_tf32(v.y - hi.y);
+    hi.z = to_tf32(v.z); lo.z = to_tf32(v.z - hi.z);
+    hi.w = to_tf32(v.w); lo.w = to_tf32(v.w - hi.w);
 }
 
-// K-major, SWIZZLE_NONE shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp: SmemDescriptor)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr)
+// K-major, no-swizzle (layout type 0) wgmma shared-memory matrix descriptor: start address, LBO = next
+// 16-byte K chunk, SBO = next 8-row group, all in 16-byte units
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr)
 {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(CHUNK_BYTES >> 4) << 16)   // LBO: next K chunk
-           | ((uint64_t)(128 >> 4) << 32)                                              // SBO: next 8 rows
-           | (1ull << 46);                                                             // version 1 (sm100)
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(CHUNK_BYTES >> 4) << 16) | ((uint64_t)(128 >> 4) << 32);
 }
 
-// kind::tf32, fp32 accumulate, A and B K-major, M = 128, N = 128 (InstrDescriptor bit layout)
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t accumulate)
+// D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, fp32 accumulate, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t a, uint64_t b, int accumulate)
 {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-        :: "r"(tmem_d), "l"(a), "l"(b), "r"(kIdesc), "r"(accumulate) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
+        "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, "
+        "%43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(accumulate));
+}
+
+// keeps the compiler from moving reads or writes of the accumulators across the asynchronous MMAs
+__device__ __forceinline__ void acc_fence(float (&d)[64])
+{
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+template <int N>
+__device__ __forceinline__ void wgmma_wait()
+{
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+
+// the 12 MMAs of one k-tile (4 k-steps x 3 split products) for warpgroup `wg` (rows 64 wg .. 64 wg + 63),
+// committed as one group; `first`: the k-tile opens an accumulation chunk.  The small lo products go first,
+// while the accumulator is small too, so that only the 4 hi * hi MMAs truncate at the full magnitude.
+__device__ __forceinline__ void mma_ktile(float (&d)[64], uint32_t s0, int wg, bool first)
+{
+    const uint64_t a_hi = gmma_desc(s0 + wg * 8 * 128), a_lo = gmma_desc(s0 + TILE_BYTES + wg * 8 * 128);
+    const uint64_t b_hi = gmma_desc(s0 + 2 * TILE_BYTES), b_lo = gmma_desc(s0 + 3 * TILE_BYTES);
+    acc_fence(d);
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+    for (int j = 0; j < TK / 8; ++j) {
+        const uint64_t off = (uint64_t)(j * ((2 * CHUNK_BYTES) >> 4));
+        wgmma_tf32(d, a_lo + off, b_hi + off, (first && j == 0) ? 0 : 1);
+        wgmma_tf32(d, a_hi + off, b_lo + off, 1);
+    }
+#pragma unroll
+    for (int j = 0; j < TK / 8; ++j) {
+        const uint64_t off = (uint64_t)(j * ((2 * CHUNK_BYTES) >> 4));
+        wgmma_tf32(d, a_hi + off, b_hi + off, 1);
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    acc_fence(d);
+}
+
+// waits for every MMA of this warpgroup and adds the finished chunk into the round-to-nearest sums
+__device__ __forceinline__ void drain(float (&d)[64], float (&sum)[64])
+{
+    wgmma_wait<0>();
+    acc_fence(d);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) sum[i] = __fadd_rn(sum[i], d[i]);
 }
 
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
@@ -102,18 +154,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
 // The weights are constants at inference: their hi/lo split is computed once
 // (fusion_mlp_pack_kernel) and written in exactly the shared-memory image the A operand needs, one
 // contiguous 32 KB block per (128-row tile, 32-column k-tile): [A_hi | A_lo], each 8 chunks x 128
-// rows x 16 B.  The main kernel is warp-specialised:
-//   warps 0-7  stage the activations (global -> registers -> split -> UMMA layout), drain the
-//              accumulator chunks into round-to-nearest register sums, run the epilogue
-//   warp  8    producer: one cp.async.bulk (TMA, no tensor map needed for a flat block) per k-tile
-//              brings the packed A block straight into shared memory
-//   warp  9    issues the tcgen05.mma's as soon as both halves of a stage have landed
-// Three stages, mbarriers only (no CTA-wide barrier in the main loop): full_a (TMA transaction
-// bytes), full_b (one arrival per staging warp), empty (tcgen05.commit), chunk (as above).
-// Layers with K <= 128 (one accumulation chunk; the P = 76800 / 19200 image-map layers, which are
-// bound by their activation traffic, not by the MMAs) use the DIRECT variant: a single stage and no
-// register sums, so that two CTAs fit on an SM and one's prologue / epilogue overlaps the other's
-// main loop.
+// rows x 16 B.  Thread 0 brings the block of k-tile kt + 1 with one cp.async.bulk while the MMAs of
+// k-tile kt run; its mbarrier counts the transaction bytes.
 constexpr int PACK_BLOCK_BYTES = 2 * TILE_BYTES;                 // A_hi + A_lo of one k-tile
 
 // Optional extras of the epilogue (all null / 0 for the plain layer):
@@ -126,9 +168,6 @@ struct MlpEpilogue {
     int idx_is_i64;
     int out_nsc;
 };
-constexpr int mlp2_threads(int nsw) { return (nsw + 2) * 32; }   // staging warps + producer + issuer
-constexpr int mlp2_stage(int mt) { return (2 * mt + 2) * TILE_BYTES; }           // MT x [A_hi | A_lo], B_hi, B_lo
-constexpr int mlp2_smem(int nst, int mt = 1) { return nst * mlp2_stage(mt) + 128; }
 
 __global__ void __launch_bounds__(256)
 fusion_mlp_pack_kernel(const float *__restrict__ w, int Co, int Ci, int nk, int nblocks, float4 *__restrict__ packed)
@@ -152,318 +191,156 @@ fusion_mlp_pack_kernel(const float *__restrict__ w, int Co, int Ci, int nk, int 
     dst[TILE_BYTES / 16 + r] = lo;
 }
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory");
-}
-
-// MT = 128-row tiles of W per CTA (1 or 2).  With MT = 2 a CTA multiplies ONE staged activation tile with two weight
-// tiles (256 output channels): the activation split + staging -- the instruction-bound part of this kernel, repeated
-// by every row tile of a layer -- halves per FLOP; all 512 TMEM columns are in use (2 row tiles x 2 chunk buffers).
-template <int NST, bool DIRECT, int NSW, int PD, int MT = 1>
-__global__ void __launch_bounds__(mlp2_threads(NSW), DIRECT ? 3 : 1)
+__global__ void __launch_bounds__(MLP_THREADS, 1)
 fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
                          const unsigned char *__restrict__ wpack, const float *__restrict__ scale,
                          const float *__restrict__ shift, float *__restrict__ out, int Co, int P, int act,
                          float slope, MlpEpilogue ep)
 {
-    static_assert(MT == 1 || !DIRECT, "the single-chunk variant keeps one row tile");
-    constexpr int STAGE = mlp2_stage(MT);
-    constexpr int TMEM_COLS = DIRECT ? TN : 2 * TN * MT;
     extern __shared__ __align__(1024) unsigned char smem[];
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + NST * STAGE);
-    uint64_t *full_a = bars, *full_b = bars + NST, *empty = bars + 2 * NST, *chunk = bars + 3 * NST;   // 11 barriers
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + NST * STAGE + 96);
-    const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31;
-    const int b = blockIdx.z, m0 = blockIdx.y * TM * MT, n0 = blockIdx.x * TN;
-    const int mt_valid = min(MT, (Co - m0 + TM - 1) / TM);   // row tiles of this CTA that exist
+    uint64_t *full_a = reinterpret_cast<uint64_t *>(smem + NST * STAGE_BYTES);
+    const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const int b = blockIdx.z, m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
     const int Ci = C1 + C2;
     const int nk = (Ci + TK - 1) / TK;
-
-    if (wid == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    if (tid == 32) {
-        for (int i = 0; i < NST; ++i) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(full_a + i)));
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(full_b + i)), "r"(NSW));
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(empty + i)));
-        }
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(chunk + 0)));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(chunk + 1)));
+    const unsigned char *wsrc = wpack + (size_t)blockIdx.y * nk * PACK_BLOCK_BYTES;
+    auto fetch_a = [&](int kt) {
+        const int st = kt % NST;
+        const uint32_t bar = smem_u32(full_a + st);
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(PACK_BLOCK_BYTES) : "memory");
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                     :: "r"(smem_u32(smem + st * STAGE_BYTES)), "l"(wsrc + (size_t)kt * PACK_BLOCK_BYTES),
+                        "r"(PACK_BLOCK_BYTES), "r"(bar) : "memory");
+    };
+    if (tid == 0) {
+        for (int i = 0; i < NST; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(full_a + i)));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = *tmem_slot;
+    if (tid == 0) fetch_a(0);
 
-    if (wid == NSW) {
-        // ---------------- A producer
-        if (lane == 0) {
-            const unsigned char *src = wpack + (size_t)blockIdx.y * MT * nk * PACK_BLOCK_BYTES;
-            for (int kt = 0; kt < nk; ++kt) {
-                const int st = kt % NST, n = kt / NST;
-                if (n >= 1) mbar_wait(smem_u32(empty + st), (uint32_t)((n - 1) & 1));
-                const uint32_t bar = smem_u32(full_a + st);
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(mt_valid * PACK_BLOCK_BYTES) : "memory");
-                for (int mt = 0; mt < mt_valid; ++mt)
-                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 :: "r"(smem_u32(smem + st * STAGE + mt * PACK_BLOCK_BYTES)),
-                                    "l"(src + ((size_t)mt * nk + kt) * PACK_BLOCK_BYTES), "r"(PACK_BLOCK_BYTES), "r"(bar) : "memory");
-            }
-        }
-        __syncwarp();
-    } else if (wid == NSW + 1) {
-        // ---------------- MMA issuer
-        if (lane == 0) {
-            for (int kt = 0; kt < nk; ++kt) {
-                const int st = kt % NST, n = kt / NST;
-                mbar_wait(smem_u32(full_a + st), (uint32_t)(n & 1));
-                mbar_wait(smem_u32(full_b + st), (uint32_t)(n & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                // this lane shares its scheduler with four staging warps: keep its per-tile instruction
-                // count small (one descriptor per operand tile, the k-steps are +256 in the address field)
-                const uint32_t s0 = smem_u32(smem + st * STAGE);
-                const uint64_t db_hi = umma_desc(s0 + 2 * MT * TILE_BYTES), db_lo = umma_desc(s0 + (2 * MT + 1) * TILE_BYTES);
+    const float *xb1 = x1 + (size_t)b * C1 * P;
+    const float *xb2 = x2 ? x2 + (size_t)b * C2 * P : nullptr;
+    const bool vec = ((P & 3) == 0) && ((reinterpret_cast<uintptr_t>(xb1) & 15) == 0) &&
+                     (!xb2 || (reinterpret_cast<uintptr_t>(xb2) & 15) == 0) &&
+                     ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+    // X tile (32 k x 128 n): warp -> K chunk kg (4 k rows), lane -> 4 n (128-bit loads); a thread ends up
+    // with whole 16-byte (n; k..k+3) slots of the K-major layout
+    const int kg = wid, nl = 4 * lane;
+    // fast path: whole tile inside the tensors, vector loads, and a 4-row K chunk never straddles the
+    // concat boundary -> one base pointer per tile, four loads at a row stride
+    const bool fast = vec && ((C1 & 3) == 0) && (n0 + TN <= P);
+    auto load_b = [&](int kt, float4 (&rb)[4]) {
+        const int gk0 = kt * TK + 4 * kg;
+        if (fast && gk0 + 3 < Ci) {
+            const float *p0 = ((gk0 < C1) ? xb1 + (size_t)gk0 * P : xb2 + (size_t)(gk0 - C1) * P) + (n0 + nl);
 #pragma unroll
-                for (int mt = 0; mt < MT; ++mt) {
-                    if (mt < mt_valid) {
-                        const uint64_t da_hi = umma_desc(s0 + mt * PACK_BLOCK_BYTES), da_lo = umma_desc(s0 + mt * PACK_BLOCK_BYTES + TILE_BYTES);
-                        const uint32_t d_buf = tmem_d + (uint32_t)((mt * 2 + ((kt / CH) & 1)) * TN);
-#pragma unroll
-                        for (int j = 0; j < TK / 8; ++j) {
-                            const uint64_t off = (uint64_t)(j * ((2 * CHUNK_BYTES) >> 4));
-                            umma_tf32(d_buf, da_hi + off, db_hi + off, (kt % CH != 0 || j > 0) ? 1u : 0u);
-                            umma_tf32(d_buf, da_lo + off, db_hi + off, 1u);
-                            umma_tf32(d_buf, da_hi + off, db_lo + off, 1u);
-                        }
-                    }
-                }
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                             :: "r"(smem_u32(empty + st)) : "memory");
-                if (kt % CH == CH - 1 || kt == nk - 1)
-                    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                                 :: "r"(smem_u32(chunk + ((kt / CH) & 1))) : "memory");
-            }
-        }
-        __syncwarp();
-    } else {
-        // ---------------- activation staging, accumulator drain, epilogue
-        const float *xb1 = x1 + (size_t)b * C1 * P;
-        const float *xb2 = x2 ? x2 + (size_t)b * C2 * P : nullptr;
-        const bool vec = ((P & 3) == 0) && ((reinterpret_cast<uintptr_t>(xb1) & 15) == 0) &&
-                         (!xb2 || (reinterpret_cast<uintptr_t>(xb2) & 15) == 0) &&
-                         ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
-        constexpr int COLS = 4 * TN / NSW, NI = COLS / 32;   // accumulator columns per thread: 64 or 32
-        const int q = wid & 3, cs = wid >> 2;                 // TMEM lane quarter (fixed by the warp id), column slice
-        float acc[MT][DIRECT ? 1 : COLS];
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-            for (int i = 0; i < (DIRECT ? 1 : COLS); ++i) acc[mt][i] = 0.f;
-        // columns COLS*cs + 32*i .. +31 of accumulator `buf`, this thread's row
-        auto tmem_load32 = [&](int buf, int i, uint32_t (&v)[32]) {
-            const uint32_t taddr = tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)(buf * TN + COLS * cs + 32 * i);
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-                : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                  "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                  "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                  "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        };
-        auto drain = [&](int c) {
-            if constexpr (!DIRECT) {
-                const int buf = c & 1;
-                mbar_wait(smem_u32(chunk + buf), (uint32_t)((c >> 1) & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-                for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-                for (int i = 0; i < COLS / 16; ++i) {   // 16 columns at a time keeps the temporaries small
-                    uint32_t v[16];
-                    const uint32_t taddr = tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)((mt * 2 + buf) * TN + COLS * cs + 16 * i);
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-                        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                        : "r"(taddr));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) acc[mt][16 * i + j] = __fadd_rn(acc[mt][16 * i + j], __uint_as_float(v[j]));
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            }
-        };
-        // X tile (32 k x 128 n): warp -> K chunk kg (4 k rows); with 8 staging warps a lane takes 4 n
-        // (128-bit loads), with 16 the two warps of a chunk take 64 n each and a lane 2 n (64-bit loads).
-        // Either way a thread ends up with whole 16-byte (n; k..k+3) slots of the K-major UMMA layout.
-        constexpr int NPL = (NSW == 8) ? 4 : 2;                 // n per lane
-        typedef typename std::conditional<NSW == 8, float4, float2>::type ldt;
-        const int kg = wid & 7, nl = (NSW == 8) ? 4 * lane : 64 * (wid >> 3) + 2 * lane;
-        // fast path: whole tile inside the tensors, vector loads, and a 4-row K chunk never straddles the
-        // concat boundary -> one base pointer per tile, four loads at a row stride
-        const bool fast = vec && ((C1 & 3) == 0) && (n0 + TN <= P);
-        auto load_b = [&](int kt, ldt (&rb)[4]) {
-            const int gk0 = kt * TK + 4 * kg;
-            if (fast && gk0 + 3 < Ci) {
-                const float *p0 = ((gk0 < C1) ? xb1 + (size_t)gk0 * P : xb2 + (size_t)(gk0 - C1) * P) + (n0 + nl);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) rb[j] = __ldg(reinterpret_cast<const ldt *>(p0 + (size_t)j * P));
-                return;
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int gk = kt * TK + 4 * kg + j, gn = n0 + nl;
-                float e[4] = {0.f, 0.f, 0.f, 0.f};
-                if (gk < Ci) {
-                    const float *row = (gk < C1) ? xb1 + (size_t)gk * P : xb2 + (size_t)(gk - C1) * P;
-                    if (vec && gn + NPL - 1 < P) {
-                        const ldt v = __ldg(reinterpret_cast<const ldt *>(row + gn));
-                        e[0] = v.x;
-                        e[1] = v.y;
-                        if constexpr (NSW == 8) {
-                            e[2] = v.z;
-                            e[3] = v.w;
-                        }
-                    } else {
-#pragma unroll
-                        for (int u = 0; u < NPL; ++u)
-                            if (gn + u < P) e[u] = __ldg(row + gn + u);
-                    }
-                }
-                if constexpr (NSW == 8) rb[j] = make_float4(e[0], e[1], e[2], e[3]);
-                else rb[j] = make_float2(e[0], e[1]);
-            }
-        };
-        auto store_b = [&](int st, const ldt (&rb)[4]) {
-            unsigned char *sB_hi = smem + st * STAGE + 2 * MT * TILE_BYTES, *sB_lo = sB_hi + TILE_BYTES;
-            unsigned char *bh = sB_hi + kg * CHUNK_BYTES + nl * 16, *bl = sB_lo + kg * CHUNK_BYTES + nl * 16;
-            float4 hi, lo;
-            if constexpr (NSW == 8) {
-                const float4 t0 = make_float4(rb[0].x, rb[1].x, rb[2].x, rb[3].x);   // n = nl + 0, k = 4kg .. 4kg+3
-                const float4 t1 = make_float4(rb[0].y, rb[1].y, rb[2].y, rb[3].y);
-                const float4 t2 = make_float4(rb[0].z, rb[1].z, rb[2].z, rb[3].z);
-                const float4 t3 = make_float4(rb[0].w, rb[1].w, rb[2].w, rb[3].w);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {   // rotated slots: every quarter-warp covers all 32 banks
-                    const int x = (i + (lane >> 1)) & 3;
-                    const float4 tx = (x == 0) ? t0 : (x == 1) ? t1 : (x == 2) ? t2 : t3;
-                    split4(tx, hi, lo);
-                    *reinterpret_cast<float4 *>(bh + 16 * x) = hi;
-                    *reinterpret_cast<float4 *>(bl + 16 * x) = lo;
-                }
-            } else {
-                const float4 t0 = make_float4(rb[0].x, rb[1].x, rb[2].x, rb[3].x);
-                const float4 t1 = make_float4(rb[0].y, rb[1].y, rb[2].y, rb[3].y);
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {   // 32-byte lane stride: lanes l and l+4 swap slots
-                    const int x = (i + (lane >> 2)) & 1;
-                    split4(x == 0 ? t0 : t1, hi, lo);
-                    *reinterpret_cast<float4 *>(bh + 16 * x) = hi;
-                    *reinterpret_cast<float4 *>(bl + 16 * x) = lo;
-                }
-            }
-        };
-        // register ring of PD tiles: tile kt lives in ring[kt % PD]; as soon as it has been written to
-        // shared memory the slot is refilled with tile kt + PD, so PD - 1 .. PD tiles of global-memory
-        // latency are in flight per thread (one tile was not enough: the staging warps sat on the
-        // scoreboard of their own loads)
-        ldt ring[PD][4];
-#pragma unroll
-        for (int d = 0; d < PD; ++d)
-            if (d < nk) load_b(d, ring[d]);
-        for (int kt0 = 0; kt0 < nk; kt0 += PD) {
-#pragma unroll
-            for (int d = 0; d < PD; ++d) {
-                const int kt = kt0 + d;
-                if (kt < nk) {
-                    const int st = kt % NST, n = kt / NST;
-                    if (n >= 1) mbar_wait(smem_u32(empty + st), (uint32_t)((n - 1) & 1));   // MMAs that read this stage are done
-                    store_b(st, ring[d]);
-                    if (kt + PD < nk) load_b(kt + PD, ring[d]);
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the MMA
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(smem_u32(full_b + st));
-                    // the previous chunk is drained while the tensor core works on this one
-                    if (kt % CH == 0 && kt > 0) drain(kt / CH - 1);
-                }
-            }
-        }
-        if constexpr (DIRECT) {   // single chunk: the epilogue reads the accumulator itself
-            mbar_wait(smem_u32(chunk), 0u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        } else {
-            drain((nk - 1) / CH);
+            for (int j = 0; j < 4; ++j) rb[j] = __ldg(reinterpret_cast<const float4 *>(p0 + (size_t)j * P));
+            return;
         }
 #pragma unroll
-        for (int mt = 0; mt < MT; ++mt) {
-        const int gm = m0 + mt * TM + 32 * q + lane;
-        const bool row_ok = gm < Co;
-        const float sc = row_ok ? __ldg(scale + gm) : 0.f, sh = row_ok ? __ldg(shift + gm) : 0.f;
-        float *orow = out + ((size_t)b * Co + (row_ok ? gm : 0)) * P;
+        for (int j = 0; j < 4; ++j) {
+            const int gk = gk0 + j, gn = n0 + nl;
+            float e[4] = {0.f, 0.f, 0.f, 0.f};
+            if (gk < Ci) {
+                const float *row = (gk < C1) ? xb1 + (size_t)gk * P : xb2 + (size_t)(gk - C1) * P;
+                if (vec && gn + 3 < P) {
+                    const float4 v = __ldg(reinterpret_cast<const float4 *>(row + gn));
+                    e[0] = v.x;
+                    e[1] = v.y;
+                    e[2] = v.z;
+                    e[3] = v.w;
+                } else {
+#pragma unroll
+                    for (int u = 0; u < 4; ++u)
+                        if (gn + u < P) e[u] = __ldg(row + gn + u);
+                }
+            }
+            rb[j] = make_float4(e[0], e[1], e[2], e[3]);
+        }
+    };
+    auto store_b = [&](int st, const float4 (&rb)[4]) {
+        unsigned char *sB_hi = smem + st * STAGE_BYTES + 2 * TILE_BYTES, *sB_lo = sB_hi + TILE_BYTES;
+        unsigned char *bh = sB_hi + kg * CHUNK_BYTES + nl * 16, *bl = sB_lo + kg * CHUNK_BYTES + nl * 16;
+        const float4 t0 = make_float4(rb[0].x, rb[1].x, rb[2].x, rb[3].x);   // n = nl + 0, k = 4kg .. 4kg+3
+        const float4 t1 = make_float4(rb[0].y, rb[1].y, rb[2].y, rb[3].y);
+        const float4 t2 = make_float4(rb[0].z, rb[1].z, rb[2].z, rb[3].z);
+        const float4 t3 = make_float4(rb[0].w, rb[1].w, rb[2].w, rb[3].w);
+        float4 hi, lo;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {   // rotated slots: every quarter-warp covers all 32 banks
+            const int x = (i + (lane >> 1)) & 3;
+            const float4 tx = (x == 0) ? t0 : (x == 1) ? t1 : (x == 2) ? t2 : t3;
+            split4(tx, hi, lo);
+            *reinterpret_cast<float4 *>(bh + 16 * x) = hi;
+            *reinterpret_cast<float4 *>(bl + 16 * x) = lo;
+        }
+    };
+
+    float acc[64], sum[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = sum[i] = 0.f;
+    float4 rb[4];
+    load_b(0, rb);
+    for (int kt = 0; kt < nk; ++kt) {
+        const int st = kt % NST;
+        store_b(st, rb);   // stage st was last read by the MMAs of k-tile kt - 3: complete (see the loop end)
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the MMA
+        __syncthreads();   // every warpgroup has passed its wait for the MMAs of k-tile kt - 2
+        if (tid == 0 && kt + 1 < nk) fetch_a(kt + 1);   // into the stage of k-tile kt - 2
+        if (kt + 1 < nk) load_b(kt + 1, rb);            // in flight during this k-tile's MMAs
+        mbar_wait(smem_u32(full_a + st), (uint32_t)((kt / NST) & 1));
+        if (kt % CH == 0 && kt > 0) drain(acc, sum);
+        mma_ktile(acc, smem_u32(smem + st * STAGE_BYTES), wg, kt % CH == 0);
+        wgmma_wait<1>();   // the MMAs of k-tile kt - 1 are done
+    }
+    drain(acc, sum);
+
+    // accumulator fragment of m64n128: register 4i + 2h + c holds row 16 w + lane / 4 + 8 h,
+    // column 8 i + 2 (lane % 4) + c of the warpgroup's 64 x 128 tile
+    const int row0 = m0 + 64 * wg + 16 * (wid & 3) + (lane >> 2), col0 = n0 + 2 * (lane & 3);
+    const int *idx32 = (ep.addend && !ep.idx_is_i64) ? reinterpret_cast<const int *>(ep.idx) + (size_t)b * P : nullptr;
+    const long long *idx64 = (ep.addend && ep.idx_is_i64) ? reinterpret_cast<const long long *>(ep.idx) + (size_t)b * P : nullptr;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int gm = row0 + 8 * h;
+        if (gm >= Co) continue;
+        const float sc = __ldg(scale + gm), sh = __ldg(shift + gm);
+        float *orow = out + ((size_t)b * Co + gm) * P;
         // optional epilogue extras (MlpEpilogue): a gathered addend in front of the affine -- the second half
         // of a concat-GEMM restructured as W1*x + (W2*p)[idx] -- and a channels-last store
-        const float *add_row = ep.addend ? ep.addend + (size_t)b * ep.NA * Co + (row_ok ? gm : 0) : nullptr;
-        const int *idx32 = (ep.addend && !ep.idx_is_i64) ? reinterpret_cast<const int *>(ep.idx) + (size_t)b * P : nullptr;
-        const long long *idx64 = (ep.addend && ep.idx_is_i64) ? reinterpret_cast<const long long *>(ep.idx) + (size_t)b * P : nullptr;
-        float *ocol = ep.out_nsc ? out + (size_t)b * P * Co + (row_ok ? gm : 0) : nullptr;
+        const float *add_row = ep.addend ? ep.addend + (size_t)b * ep.NA * Co + gm : nullptr;
+        float *ocol = ep.out_nsc ? out + (size_t)b * P * Co + gm : nullptr;
 #pragma unroll
-        for (int i = 0; i < NI; ++i) {
-            uint32_t v[32];
-            if constexpr (DIRECT) {
-                tmem_load32(0, i, v);   // warp-collective: rows beyond Co take part, they just do not store
-            } else {
+        for (int i = 0; i < TN / 8; ++i) {
+            const int gn = col0 + 8 * i;
+            float y[2] = {sum[4 * i + 2 * h], sum[4 * i + 2 * h + 1]};
+            if (add_row) {   // the addend row is channels-last: the 8 rows of a warp read 32 contiguous bytes
 #pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(acc[mt][32 * i + j]);
-            }
-            if (row_ok) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const int gn = n0 + COLS * cs + 32 * i + j;
-                    float y[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) y[u] = __uint_as_float(v[j + u]);
-                    if (add_row) {   // the column's index is the same for the whole warp (one broadcast load),
-                                     // the addend row is channels-last: 32 lanes read 128 contiguous bytes
-                        int a[4];
-#pragma unroll
-                        for (int u = 0; u < 4; ++u)
-                            a[u] = (gn + u < P) ? (idx32 ? __ldg(idx32 + gn + u) : (int)__ldg(idx64 + gn + u)) : 0;
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) y[u] = __fadd_rn(y[u], __ldg(add_row + (size_t)a[u] * Co));
-                    }
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        y[u] = __fadd_rn(__fmul_rn(y[u], sc), sh);
-                        if (act == 1) y[u] = fmaxf(y[u], 0.f);
-                        else if (act == 2) y[u] = (y[u] > 0.f) ? y[u] : __fmul_rn(y[u], slope);
-                    }
-                    if (ocol) {
-#pragma unroll
-                        for (int u = 0; u < 4; ++u)
-                            if (gn + u < P) ocol[(size_t)(gn + u) * Co] = y[u];
-                    } else if (vec && gn + 3 < P) {
-                        *reinterpret_cast<float4 *>(orow + gn) = make_float4(y[0], y[1], y[2], y[3]);
-                    } else {
-#pragma unroll
-                        for (int u = 0; u < 4; ++u)
-                            if (gn + u < P) orow[gn + u] = y[u];
-                    }
+                for (int u = 0; u < 2; ++u) {
+                    const int a = (gn + u < P) ? (idx32 ? __ldg(idx32 + gn + u) : (int)__ldg(idx64 + gn + u)) : 0;
+                    y[u] = __fadd_rn(y[u], __ldg(add_row + (size_t)a * Co));
                 }
             }
-        }
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                y[u] = __fadd_rn(__fmul_rn(y[u], sc), sh);
+                if (act == 1) y[u] = fmaxf(y[u], 0.f);
+                else if (act == 2) y[u] = (y[u] > 0.f) ? y[u] : __fmul_rn(y[u], slope);
+            }
+            if (ocol) {
+#pragma unroll
+                for (int u = 0; u < 2; ++u)
+                    if (gn + u < P) ocol[(size_t)(gn + u) * Co] = y[u];
+            } else if (vec && gn + 1 < P) {
+                *reinterpret_cast<float2 *>(orow + gn) = make_float2(y[0], y[1]);
+            } else {
+#pragma unroll
+                for (int u = 0; u < 2; ++u)
+                    if (gn + u < P) orow[gn + u] = y[u];
+            }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (wid == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_d), "r"(DIRECT ? TN : 2 * TN * MT));
 }
 
 
@@ -471,109 +348,48 @@ fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__re
 // dW[co, ci] = sum_b sum_p dZ[b, co, p] * X[b, ci, p],  X = [X1; X2]  (backward of the 1x1 conv w.r.t. its
 // weight: a GEMM with M = Co, N = Ci and the long axis K = B * P).  Both operands are K-contiguous in memory
 // (dZ and X are NCHW: the point axis is the fast one), so every thread loads 16 bytes along K and writes one
-// whole (row; k..k+3) slot of the K-major UMMA layout -- no transposition.  Same numerics as the forward
-// layer: 3xTF32 split of both operands while they are staged, K accumulated in chunks of 128 into two
-// alternating TMEM accumulators that are drained into round-to-nearest fp32 register sums.  Split-K over
-// the grid's z axis: every CTA owns a run of (frame, 32-point) k-tiles and adds its 128x128 partial to dW
-// with fp32 atomics (dW is zero-filled by the entry point), like cuDNN's own wgrad: summation order is not
-// deterministic, values agree to fp32 round-off.
-constexpr int WG_SMEM = 2 * STAGE_BYTES + 64;
-
-__global__ void __launch_bounds__(256, 1)
+// whole (row; k..k+3) slot of the K-major layout -- no transposition.  Same numerics and pipeline as the
+// forward layer: 3xTF32 split of both operands while they are staged, K accumulated in chunks of one k-tile that are
+// added into round-to-nearest fp32 register sums.  Split-K over the grid's z axis: every CTA owns a run of
+// (frame, 32-point) k-tiles and adds its 128x128 partial to dW with fp32 atomics (dW is zero-filled by the
+// entry point), like cuDNN's own wgrad: summation order is not deterministic, values agree to fp32 round-off.
+__global__ void __launch_bounds__(MLP_THREADS, 1)
 fusion_wgrad_kernel(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
                     float *__restrict__ dw, int Co, int P, int tiles_per_frame, int total_tiles, int tiles_per_split)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 2 * STAGE_BYTES);   // [0],[1]: stage free; [2],[3]: chunk done
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + 2 * STAGE_BYTES + 48);
-    const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31, wg = tid >> 7;
     const int m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
     const int Ci = C1 + C2;
     const int kt_begin = blockIdx.z * tiles_per_split, kt_end = min(total_tiles, kt_begin + tiles_per_split);
     const int nk = kt_end - kt_begin;
     if (nk <= 0) return;   // CTA-uniform
 
-    if (wid == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "r"(2 * TN));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    if (tid == 32) {
-        for (int i = 0; i < 4; ++i)
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(bars + i)));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = *tmem_slot;
-
     const bool vec = ((P & 3) == 0) && ((reinterpret_cast<uintptr_t>(dz) & 15) == 0) &&
                      ((reinterpret_cast<uintptr_t>(x1) & 15) == 0) && (!x2 || (reinterpret_cast<uintptr_t>(x2) & 15) == 0);
-    const int q = wid & 3, half = wid >> 2;   // this thread's accumulator row = 32q + lane, columns 64*half ..
-    float acc[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    auto drain = [&](int c) {
-        const int buf = c & 1;
-        mbar_wait(smem_u32(bars + 2 + buf), (uint32_t)((c >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            uint32_t v[16];
-            const uint32_t taddr = tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)(buf * TN + 64 * half + 16 * i);
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-                : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                  "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int j = 0; j < 16; ++j) acc[16 * i + j] = __fadd_rn(acc[16 * i + j], __uint_as_float(v[j]));
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    };
     // global -> registers: warp w stages K chunk w (4 points) of both operands; lanes take rows lane + 32*i
-    auto load_rows = [&](const float *base, int rows, int row0, int p0, float4 (&r)[4]) {
-        // base: [rows_total, P] of this frame; element (row, p0 + 4*wid .. +3)
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int gr = row0 + lane + 32 * i, gp = p0 + 4 * wid;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (gr < rows && gp < P) {
-                const float *src = base + (size_t)gr * P + gp;
-                if (vec && gp + 3 < P) {
-                    v = __ldg(reinterpret_cast<const float4 *>(src));
-                } else {
-                    v.x = __ldg(src);
-                    if (gp + 1 < P) v.y = __ldg(src + 1);
-                    if (gp + 2 < P) v.z = __ldg(src + 2);
-                    if (gp + 3 < P) v.w = __ldg(src + 3);
-                }
-            }
-            r[i] = v;
+    auto load4 = [&](const float *src, int gp) {
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (vec && gp + 3 < P) {
+            v = __ldg(reinterpret_cast<const float4 *>(src));
+        } else {
+            v.x = __ldg(src);
+            if (gp + 1 < P) v.y = __ldg(src + 1);
+            if (gp + 2 < P) v.z = __ldg(src + 2);
+            if (gp + 3 < P) v.w = __ldg(src + 3);
         }
+        return v;
     };
     auto load_tile = [&](int kt, float4 (&ra)[4], float4 (&rb)[4]) {
-        const int b = kt / tiles_per_frame, p0 = (kt % tiles_per_frame) * TK;
-        load_rows(dz + (size_t)b * Co * P, Co, m0, p0, ra);
-        // B rows = input channels n0 .. n0+127 of cat(x1, x2); a 128-row tile may straddle the concat
+        const int b = kt / tiles_per_frame, gp = (kt % tiles_per_frame) * TK + 4 * wid;
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            const int gn = n0 + lane + 32 * i, gp = p0 + 4 * wid;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (gn < Ci && gp < P) {
-                const float *src = (gn < C1) ? x1 + ((size_t)b * C1 + gn) * P + gp : x2 + ((size_t)b * C2 + (gn - C1)) * P + gp;
-                if (vec && gp + 3 < P) {
-                    v = __ldg(reinterpret_cast<const float4 *>(src));
-                } else {
-                    v.x = __ldg(src);
-                    if (gp + 1 < P) v.y = __ldg(src + 1);
-                    if (gp + 2 < P) v.z = __ldg(src + 2);
-                    if (gp + 3 < P) v.w = __ldg(src + 3);
-                }
-            }
-            rb[i] = v;
+            const int gm = m0 + lane + 32 * i, gn = n0 + lane + 32 * i;
+            ra[i] = (gm < Co && gp < P) ? load4(dz + ((size_t)b * Co + gm) * P + gp, gp) : make_float4(0.f, 0.f, 0.f, 0.f);
+            // B rows = input channels n0 .. n0+127 of cat(x1, x2); a 128-row tile may straddle the concat
+            rb[i] = (gn < Ci && gp < P)
+                        ? load4((gn < C1) ? x1 + ((size_t)b * C1 + gn) * P + gp : x2 + ((size_t)b * C2 + (gn - C1)) * P + gp, gp)
+                        : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     };
     auto store_tile = [&](int st, const float4 (&ra)[4], const float4 (&rb)[4]) {
@@ -592,57 +408,36 @@ fusion_wgrad_kernel(const float *__restrict__ dz, const float *__restrict__ x1, 
         }
     };
 
-    float4 ra[4], rb[4], na[4], nb[4];
+    float acc[64], sum[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = sum[i] = 0.f;
+    float4 ra[4], rb[4];
     load_tile(kt_begin, ra, rb);
     for (int kt = 0; kt < nk; ++kt) {
-        const int st = kt & 1;
-        if (kt + 1 < nk) load_tile(kt_begin + kt + 1, na, nb);
-        if (kt >= 2) mbar_wait(smem_u32(bars + st), ((kt >> 1) - 1) & 1);   // MMAs that read this stage are done
-        store_tile(st, ra, rb);
+        const int st = kt % NST;
+        store_tile(st, ra, rb);   // stage st was last read by the MMAs of k-tile kt - 3: complete
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t a_hi = smem_u32(smem + st * STAGE_BYTES);
-            const uint64_t da_hi = umma_desc(a_hi), da_lo = umma_desc(a_hi + TILE_BYTES);
-            const uint64_t db_hi = umma_desc(a_hi + 2 * TILE_BYTES), db_lo = umma_desc(a_hi + 3 * TILE_BYTES);
-            const uint32_t d_buf = tmem_d + (uint32_t)(((kt / CH) & 1) * TN);
-#pragma unroll
-            for (int j = 0; j < TK / 8; ++j) {
-                const uint64_t off = (uint64_t)(j * ((2 * CHUNK_BYTES) >> 4));
-                umma_tf32(d_buf, da_hi + off, db_hi + off, (kt % CH != 0 || j > 0) ? 1u : 0u);
-                umma_tf32(d_buf, da_lo + off, db_hi + off, 1u);
-                umma_tf32(d_buf, da_hi + off, db_lo + off, 1u);
-            }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                         :: "r"(smem_u32(bars + st)) : "memory");
-            if (kt % CH == CH - 1 || kt == nk - 1)
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                             :: "r"(smem_u32(bars + 2 + ((kt / CH) & 1))) : "memory");
-        }
-        if (kt % CH == 0 && kt > 0) drain(kt / CH - 1);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            ra[i] = na[i];
-            rb[i] = nb[i];
-        }
+        if (kt + 1 < nk) load_tile(kt_begin + kt + 1, ra, rb);
+        if (kt % CH == 0 && kt > 0) drain(acc, sum);
+        mma_ktile(acc, smem_u32(smem + st * STAGE_BYTES), wg, kt % CH == 0);
+        wgmma_wait<1>();
     }
-    drain((nk - 1) / CH);
-    {
-        const int gm = m0 + 32 * q + lane;
-        if (gm < Co) {
-            float *row = dw + (size_t)gm * Ci;
+    drain(acc, sum);
+    const int row0 = m0 + 64 * wg + 16 * (wid & 3) + (lane >> 2), col0 = n0 + 2 * (lane & 3);
 #pragma unroll
-            for (int j = 0; j < 64; ++j) {
-                const int gn = n0 + 64 * half + j;
-                if (gn < Ci) atomicAdd(row + gn, acc[j]);
+    for (int h = 0; h < 2; ++h) {
+        const int gm = row0 + 8 * h;
+        if (gm >= Co) continue;
+        float *row = dw + (size_t)gm * Ci;
+#pragma unroll
+        for (int i = 0; i < TN / 8; ++i)
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                const int gn = col0 + 8 * i + u;
+                if (gn < Ci) atomicAdd(row + gn, sum[4 * i + 2 * h + u]);
             }
-        }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (wid == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_d), "r"(2 * TN));
 }
 
 }  // namespace ffb6d
@@ -696,14 +491,7 @@ extern "C" int ffb6d_fusion_mlp_fwd_ex(const float *x1, int64_t C1, const float 
                     out_layout);
     FFB6D_CHECK_ARG((addend == nullptr) == (add_idx == nullptr), "fusion_mlp_fwd: addend and add_idx come together");
     FFB6D_CHECK_ARG(!addend || (NA >= 1 && NA < (1ll << 31)), "fusion_mlp_fwd: bad addend length");
-    {
-        auto k_big = fusion_mlp_packed_kernel<3, false, 16, 3>;
-        auto k_big2 = fusion_mlp_packed_kernel<2, false, 16, 2, 2>;
-        auto k_direct = fusion_mlp_packed_kernel<1, true, 8, 2>;
-        FFB6D_OPTIN_SMEM(k_big, mlp2_smem(3));
-        FFB6D_OPTIN_SMEM(k_big2, mlp2_smem(2, 2));
-        FFB6D_OPTIN_SMEM(k_direct, mlp2_smem(1));
-    }
+    FFB6D_OPTIN_SMEM(fusion_mlp_packed_kernel, MLP_SMEM);
     MlpEpilogue ep;
     ep.addend = addend;
     ep.idx = add_idx;
@@ -711,19 +499,9 @@ extern "C" int ffb6d_fusion_mlp_fwd_ex(const float *x1, int64_t C1, const float 
     ep.idx_is_i64 = add_idx_is_i64;
     ep.out_nsc = out_layout == FFB6D_LAYOUT_NSC;
     dim3 grid((unsigned)ceil_div(P, TN), (unsigned)ceil_div(Co, TM), (unsigned)B);
-    if (ceil_div(C1 + C2, TK) <= CH && !env().mlp_no_direct)
-        fusion_mlp_packed_kernel<1, true, 8, 2><<<grid, mlp2_threads(8), mlp2_smem(1), (cudaStream_t)stream>>>(
-            x1, (int)C1, C2 ? x2 : nullptr, (int)C2, (const unsigned char *)packed, scale, shift, out, (int)Co, (int)P,
-            act, negative_slope, ep);
-    else if (Co > TM && !env().mlp_no_pair_tiles) {   // two row tiles per CTA: one staged activation tile feeds 256 output channels
-        dim3 grid2(grid.x, (unsigned)ceil_div(ceil_div(Co, TM), 2), grid.z);
-        fusion_mlp_packed_kernel<2, false, 16, 2, 2><<<grid2, mlp2_threads(16), mlp2_smem(2, 2), (cudaStream_t)stream>>>(
-            x1, (int)C1, C2 ? x2 : nullptr, (int)C2, (const unsigned char *)packed, scale, shift, out, (int)Co, (int)P,
-            act, negative_slope, ep);
-    } else
-        fusion_mlp_packed_kernel<3, false, 16, 3><<<grid, mlp2_threads(16), mlp2_smem(3), (cudaStream_t)stream>>>(
-            x1, (int)C1, C2 ? x2 : nullptr, (int)C2, (const unsigned char *)packed, scale, shift, out, (int)Co, (int)P,
-            act, negative_slope, ep);
+    fusion_mlp_packed_kernel<<<grid, MLP_THREADS, MLP_SMEM, (cudaStream_t)stream>>>(
+        x1, (int)C1, C2 ? x2 : nullptr, (int)C2, (const unsigned char *)packed, scale, shift, out, (int)Co, (int)P,
+        act, negative_slope, ep);
     FFB6D_LAUNCH_OK("fusion_mlp_packed_kernel");
     return FFB6D_OK;
 }
@@ -778,7 +556,7 @@ extern "C" int ffb6d_fusion_mlp_wgrad(const float *grad_z, const float *x1, int6
     FFB6D_CHECK_ARG(grad_z && x1 && (C2 == 0 || x2), "fusion_mlp_wgrad: null pointer");
     if (Co <= 64 && Ci <= 64)   // narrow layer: a 128x128 tensor-core tile would be mostly padding (train.cu)
         return wgrad_small_launch(grad_z, x1, C1, x2, C2, B, Co, P, grad_w, st);
-    FFB6D_OPTIN_SMEM(fusion_wgrad_kernel, WG_SMEM);
+    FFB6D_OPTIN_SMEM(fusion_wgrad_kernel, MLP_SMEM);
     const int64_t tpf = ceil_div(P, TK), total = B * tpf;
     FFB6D_CHECK_ARG(total < (1ll << 31), "fusion_mlp_wgrad: B * P too large");
     const int64_t tiles = ceil_div(Ci, TN) * ceil_div(Co, TM);
@@ -788,7 +566,7 @@ extern "C" int ffb6d_fusion_mlp_wgrad(const float *grad_z, const float *x1, int6
     const int64_t per = ceil_div(total, splits);
     splits = ceil_div(total, per);
     dim3 grid((unsigned)ceil_div(Ci, TN), (unsigned)ceil_div(Co, TM), (unsigned)splits);
-    fusion_wgrad_kernel<<<grid, 256, WG_SMEM, st>>>(grad_z, x1, (int)C1, C2 ? x2 : nullptr, (int)C2, grad_w, (int)Co, (int)P,
+    fusion_wgrad_kernel<<<grid, MLP_THREADS, MLP_SMEM, st>>>(grad_z, x1, (int)C1, C2 ? x2 : nullptr, (int)C2, grad_w, (int)Co, (int)P,
                                                     (int)tpf, (int)total, (int)per);
     FFB6D_LAUNCH_OK("fusion_wgrad_kernel");
     return FFB6D_OK;

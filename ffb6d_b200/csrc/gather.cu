@@ -1,5 +1,5 @@
 // gather.cu -- gather + max-pool over neighbours, nearest-feature gather, neighbour
-// gather and relative position encoding (sm_100a).
+// gather and relative position encoding (sm_90a).
 //
 // Reference ops (ffb6d/models/ffb6d.py:159-194, 309-312; models/RandLA/RandLANet.py:
 // 87-117, 216-234) are chains of reshape / repeat / torch.gather / max that
@@ -269,7 +269,7 @@ gather_max_ncs_klane_kernel(const float *__restrict__ feat, const IdxT *__restri
     constexpr int QPW = 32 / KT;      // queries per warp at a time
     constexpr int CCH = 8;            // channels per CTA: many CTAs per frame keep ONE frame's rows in L2
                                       // (ncu: with 64 channels per CTA twelve frames were in flight,
-                                      // 235 MB of rows thrashed the 126 MB L2 and DRAM read them twice)
+                                      // 235 MB of rows thrashed the L2 and DRAM read them twice)
     __shared__ float tile[CCH][TQ + 1];
     const int b = blockIdx.z;
     const int q_tile = blockIdx.x * TQ;
@@ -475,10 +475,13 @@ gather_neighbour_kernel(const float *__restrict__ pc, const IdxT *__restrict__ i
     }
 }
 
+// The scatter-add runs in float64: every source element receives up to N * K terms in whatever order the
+// atomics land, and in fp32 a sum that nearly cancels would depend on that order.  The float64 sum carries
+// 29 more bits than the fp32 result, so its order-dependent round-off stays far below the final rounding.
 template <typename IdxT>
 __global__ void __launch_bounds__(256)
 gather_neighbour_bwd_kernel(const float *__restrict__ gout, const IdxT *__restrict__ idx,
-                            float *__restrict__ gpc, int S, int D, long long rows_per_b,
+                            double *__restrict__ acc, int S, int D, long long rows_per_b,
                             long long total)
 {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -487,7 +490,14 @@ gather_neighbour_bwd_kernel(const float *__restrict__ gout, const IdxT *__restri
     const int j = (int)(t % D);
     const int b = (int)(row / rows_per_b);
     const int s = (int)__ldg(idx + row);
-    if ((unsigned)s < (unsigned)S) atomicAdd(gpc + ((size_t)b * S + s) * D + j, gout[t]);
+    if ((unsigned)s < (unsigned)S) atomicAdd(acc + ((size_t)b * S + s) * D + j, (double)gout[t]);
+}
+
+__global__ void __launch_bounds__(256)
+round_to_f32_kernel(const double *__restrict__ acc, float *__restrict__ out, long long n)
+{
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n) out[t] = __double2float_rn(acc[t]);
 }
 
 // ------------------------------------------------------------------ relative position encoding
@@ -894,14 +904,30 @@ int ffb6d_gather_neighbour_bwd(const float *grad_out, const void *idx, int idx_i
     FFB6D_CHECK_ARG(grad_out && idx, "gather_neighbour_bwd: null pointer");
     const long long rows_per_b = (long long)N * K;
     const long long total = (long long)B * rows_per_b * D;
-    const unsigned blocks = (unsigned)ceil_div(total, 256);
-    if (idx_is_i64)
-        gather_neighbour_bwd_kernel<long long><<<blocks, 256, 0, st>>>(
-            grad_out, (const long long *)idx, grad_pc, (int)S, (int)D, rows_per_b, total);
-    else
-        gather_neighbour_bwd_kernel<int><<<blocks, 256, 0, st>>>(grad_out, (const int *)idx, grad_pc,
-                                                                (int)S, (int)D, rows_per_b, total);
-    FFB6D_LAUNCH_OK("gather_neighbour_bwd_kernel");
+    const long long n_out = (long long)B * S * D;
+    double *acc = nullptr;
+    FFB6D_CUDA(cudaMallocAsync((void **)&acc, (size_t)n_out * sizeof(double), st));
+    cudaError_t e = cudaMemsetAsync(acc, 0, (size_t)n_out * sizeof(double), st);
+    if (e == cudaSuccess) {
+        const unsigned blocks = (unsigned)ceil_div(total, 256);
+        if (idx_is_i64)
+            gather_neighbour_bwd_kernel<long long><<<blocks, 256, 0, st>>>(
+                grad_out, (const long long *)idx, acc, (int)S, (int)D, rows_per_b, total);
+        else
+            gather_neighbour_bwd_kernel<int><<<blocks, 256, 0, st>>>(grad_out, (const int *)idx, acc,
+                                                                    (int)S, (int)D, rows_per_b, total);
+        e = cudaGetLastError();
+        if (e == cudaSuccess) {
+            count_launch();
+            round_to_f32_kernel<<<(unsigned)ceil_div(n_out, 256), 256, 0, st>>>(acc, grad_pc, n_out);
+        }
+    }
+    cudaFreeAsync(acc, st);
+    if (e != cudaSuccess) {
+        set_error("gather_neighbour_bwd: %s", cudaGetErrorString(e));
+        return FFB6D_ERR_CUDA;
+    }
+    FFB6D_LAUNCH_OK("round_to_f32_kernel");
     return FFB6D_OK;
 }
 

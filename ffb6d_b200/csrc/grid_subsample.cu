@@ -1,4 +1,4 @@
-// grid_subsample.cu -- voxel-grid barycentre subsampling on the GPU (sm_100a).
+// grid_subsample.cu -- voxel-grid barycentre subsampling on the GPU (sm_90a).
 //
 // Replaces grid_subsampling() (GS/cpp_subsampling/grid_subsampling/grid_subsampling.cpp:5-106),
 // which walks the cloud once and accumulates per-voxel sums in an unordered_map.  The GPU

@@ -1,4 +1,4 @@
-// knn_brute.cu -- tiled all-pairs exact KNN (sm_100a).
+// knn_brute.cu -- tiled all-pairs exact KNN (sm_90a).
 //
 // One thread owns one query and keeps its K best (distance, index) pairs sorted
 // in registers; the support cloud streams through shared memory in float4

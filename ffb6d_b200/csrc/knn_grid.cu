@@ -1,4 +1,4 @@
-// knn_grid.cu -- exact KNN through a uniform grid over the support cloud (sm_100a).
+// knn_grid.cu -- exact KNN through a uniform grid over the support cloud (sm_90a).
 //
 // The reference answers every query with a KD-tree descent (NN/nanoflann.hpp:1350-1408).
 // On the GPU the same *result* -- the K support points with the smallest reference-arithmetic

@@ -1,4 +1,4 @@
-// lfa_fused.cu -- RandLA local feature aggregation, one fused kernel per attentive pooling (sm_100a).
+// lfa_fused.cu -- RandLA local feature aggregation, one fused kernel per attentive pooling (sm_90a).
 //
 // Reference (models/RandLA/RandLANet.py:196-250), per point n with its K neighbours idx[n, :]:
 //     f_xyz  = mlp1(relative_pos_encoding(xyz, idx))                 [B, d/2, N, K]     (:197-199, 216-223)

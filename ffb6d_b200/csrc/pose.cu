@@ -1,4 +1,4 @@
-// pose.cu -- keypoint voting (mean shift) and least-squares pose fitting on the device (sm_100a).
+// pose.cu -- keypoint voting (mean shift) and least-squares pose fitting on the device (sm_90a).
 //
 // The step right after the network (SURVEY.md §8 f-4): every point of an object votes for the
 // object's keypoints and centre, the votes are clustered with a Gaussian mean shift

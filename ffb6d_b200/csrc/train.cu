@@ -1,11 +1,11 @@
-// train.cu -- training-mode pieces of the fusion / RandLA 1x1 layers (sm_100a): batch-statistics
+// train.cu -- training-mode pieces of the fusion / RandLA 1x1 layers (sm_90a): batch-statistics
 // BatchNorm around the tensor-core GEMMs of fusion_mlp.cu, and the backward of attentive pooling.
 //
 // Reference layer: pt_utils.Conv2d = conv1x1(bias=False) -> BatchNorm2d -> ReLU / LeakyReLU / none
 // (models/pytorch_utils.py:75-129 for the fusion layers, models/RandLA/pytorch_utils.py:35-111 for
 // RandLA: eps 1e-6, momentum 0.99).  In training mode BatchNorm normalises with the statistics of the
 // batch, which sit between the GEMM and the activation, so the layer runs as
-//     z = W * cat(x1, x2)                      ffb6d_fusion_mlp_fwd_ex (tcgen05), z kept for the backward
+//     z = W * cat(x1, x2)                      ffb6d_fusion_mlp_fwd_ex (wgmma), z kept for the backward
 //     (mean, var) per channel over B x P       bn_stats_kernel + bn_finalize_kernel (also the running stats)
 //     y = act((z - mean) * gamma / sqrt(var + eps) + beta)      bn_apply_kernel
 // and backwards

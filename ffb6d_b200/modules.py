@@ -11,9 +11,9 @@ Both modes run on the CUDA library:
 
 * ``eval()``: one fused tensor-core kernel per layer (``ffb6d_fusion_mlp_fwd_ex``: concat + conv + folded
   BatchNorm + activation).
-* ``train()``: batch-statistics BatchNorm and autograd -- forward = GEMM (tcgen05) + ``ffb6d_bn_train_fwd``
+* ``train()``: batch-statistics BatchNorm and autograd -- forward = GEMM (wgmma) + ``ffb6d_bn_train_fwd``
   (running statistics updated like ``nn.BatchNorm2d``); backward = ``ffb6d_bn_train_bwd``, weight gradient
-  ``ffb6d_fusion_mlp_wgrad`` (tcgen05, split-K), input gradient = the forward GEMM with the transposed
+  ``ffb6d_fusion_mlp_wgrad`` (wgmma, split-K), input gradient = the forward GEMM with the transposed
   weight; neighbour gathers and attentive pooling have their own backward kernels.
 
 A layer accepts its input as one tensor or as the two halves of a concat (``layer(x1, x2)`` ==
@@ -50,7 +50,7 @@ def _ones_zeros(n, device):
 
 
 def _gemm(x1, x2, w2d):
-    """z = W . cat(x1, x2), no affine, no activation (tcgen05 kernel)."""
+    """z = W . cat(x1, x2), no affine, no activation (wgmma kernel)."""
     one, zero = _ones_zeros(w2d.shape[0], x1.device)
     return ops.fusion_mlp(x1, x2, w2d, one, zero, relu=False)
 

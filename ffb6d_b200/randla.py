@@ -5,7 +5,7 @@ Functional mirrors of ``Att_pooling``, ``Building_block`` and ``Dilated_res_bloc
 are the reference's (``mlp1.conv.weight``, ``mlp1.bn.bn.running_mean``, ``lfa.att_pooling_1.fc.weight``
 ...), so published checkpoints work unchanged.  Every step is one of this package's CUDA kernels:
 
-* 1x1 convs (+ BN(eps 1e-6) + LeakyReLU(0.2), RandLA's ``pt_utils.Conv2d``) -> ``fusion_mlp`` (tcgen05),
+* 1x1 convs (+ BN(eps 1e-6) + LeakyReLU(0.2), RandLA's ``pt_utils.Conv2d``) -> ``fusion_mlp`` (wgmma),
   with the ``torch.cat`` in front of every attentive pooling fused as its two K ranges
 * neighbour gathers (``gather_neighbour`` + ``permute(0,3,1,2).contiguous()``) -> the K = 1 gather
   kernel writing channel-major ``[B,C,N,K]`` directly

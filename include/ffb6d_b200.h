@@ -1,5 +1,5 @@
 /*
- * ffb6d_b200.h -- C ABI of libffb6d_b200.so: the B200 (sm_100a) implementation of
+ * ffb6d_b200.h -- C ABI of libffb6d_b200.so: the H100 (sm_90a) implementation of
  * FFB6D's bidirectional-fusion hot path (KNN index build, gather + max-pool /
  * nearest-feature gather, RandLA set-abstraction ops).
  *
@@ -236,7 +236,7 @@ int ffb6d_relative_pos_encoding_cm_fwd(const float *xyz, const void *idx, int id
  * Replaces torch.cat + pt_utils.Conv2d(kernel_size=(1,1), bn=True) with frozen (eval)
  * BatchNorm statistics (models/pytorch_utils.py:75-129,168-201; built models/ffb6d.py:55-80,
  * 104-129; applied :246-262, 282-298): scale = gamma/sqrt(var+eps), shift = beta - mean*scale.
- * tcgen05 TF32 tensor cores with 3xTF32 operand splitting: agrees with the fp32 path to ~1e-6
+ * Hopper wgmma TF32 tensor cores with 3xTF32 operand splitting: agrees with the fp32 path to ~1e-6
  * relative (the 1e-5 contract).  x1 [B,C1,P], x2 [B,C2,P] or NULL (C2 = 0), weight [Co,C1+C2]
  * row-major, out [B,Co,P]; all f32, NCHW (point axis contiguous).
  * act: 0 none, 1 ReLU (the fusion layers), 2 LeakyReLU(negative_slope) (RandLA's pt_utils.Conv2d,
@@ -288,7 +288,7 @@ int ffb6d_fusion_mlp_fwd_ex(const float *x1, int64_t C1, const float *x2, int64_
  *   y = act(BN_batch(z))                ffb6d_bn_train_fwd   (also updates the running statistics)
  * and backwards
  *   dz, dgamma, dbeta from dy           ffb6d_bn_train_bwd
- *   dW = sum_b dz_b * X_b^T             ffb6d_fusion_mlp_wgrad (tcgen05, split-K, fp32 atomics into dW)
+ *   dW = sum_b dz_b * X_b^T             ffb6d_fusion_mlp_wgrad (wgmma, split-K, fp32 atomics into dW)
  *   dX = W^T * dz                       ffb6d_fusion_mlp_fwd_ex with the packed transposed weight
  * stats [C][4] f32 = (mean, 1/sqrt(var+eps), gamma/sqrt(var+eps), beta) per channel, written by the forward
  * and read by the backward; workspace: ffb6d_bn_workspace_bytes(C, P) bytes of device memory.

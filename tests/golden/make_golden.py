@@ -426,6 +426,74 @@ def pose_cases():
     return out
 
 
+STRESS_SIZES = (4096, 40960, 131072)
+STRESS_ROWS = 1024          # seeded sample of query rows kept per stress-sweep search
+
+
+def stress_searches(n_points):
+    """(name, support, query, K) of tests/test_oracle_vs_ref.py::test_knn_stress_sweep_sizes."""
+    fr = make_frame(21, n_points=n_points)
+    lvl1 = fr["cld"][None, : n_points // 4]
+    lvl2 = fr["cld"][None, : n_points // 16]
+    img = np.ascontiguousarray(fr["dpt_xyz"][::4, ::4].reshape(1, -1, 3))
+    return [("self", lvl1, lvl1, 16), ("img2cld", lvl2, img, 1), ("cld2img", img, lvl2, 32)]
+
+
+def stress_rows(n_queries, n_points):
+    rs = np.random.RandomState(n_points)
+    return np.sort(rs.choice(n_queries, min(n_queries, STRESS_ROWS), replace=False))
+
+
+def wrap_padded_frame(n=3072):
+    """A frame padded with repeated pixels (np.pad 'wrap', ycb_dataset.py:230): cloud + point sets."""
+    fr = make_frame(11, n_points=n)
+    rs = np.random.RandomState(5)
+    keep = fr["choose"][0][: n * 5 // 8]
+    choose = np.pad(keep, (0, n - len(keep)), "wrap")[rs.permutation(n)]
+    fr = dict(fr, cld=fr["dpt_xyz"].reshape(-1, 3)[choose])
+    return fr, point_sets(fr, n), rs
+
+
+def refcheck_cases():
+    """Outputs of the reference's compiled KNN / grid subsampling and of its torch gathers on the seeded
+    inputs of tests/test_oracle_vs_ref.py (the inputs are regenerated there from the same seeds)."""
+    f = R.torch_functions()
+    out = {}
+    for seed, S, Q, K in KNN_RANDOM:
+        rs = np.random.RandomState(seed)
+        sup = rs.randn(2, S, 3).astype(np.float32)
+        qry = rs.randn(2, Q, 3).astype(np.float32)
+        out["knn_random/%d" % seed] = R.knn_batch(sup, qry, K, omp=True).astype(np.int32)
+    cld = make_frame(9, n_points=3072)["cld"][None]
+    out["surface_frame/idx"] = R.knn_batch(cld, cld, 16).astype(np.int32)
+    for n in STRESS_SIZES:
+        for name, sup, qry, k in stress_searches(n):
+            rows = stress_rows(qry.shape[1], n)
+            out["stress/%d_%s" % (n, name)] = R.knn_batch(sup, qry[:, rows], k).astype(np.int32)
+    g = torch.Generator().manual_seed(7)
+    feat = torch.randn(3, 17, 211, 1, generator=g)
+    idx = torch.randint(0, 211, (3, 50, 16), generator=g)
+    out["torch/random_sample"] = f["random_sample"](feat, idx).numpy()
+    idx1 = torch.randint(0, 211, (3, 400, 1), generator=g)
+    out["torch/nearest_interpolation"] = f["nearest_interpolation"](feat, idx1).numpy()
+    pc = torch.randn(2, 90, 6, generator=g)
+    nidx = torch.randint(0, 90, (2, 90, 16), generator=g)
+    out["torch/gather_neighbour"] = f["gather_neighbour"](pc, nidx).numpy()
+    rs = np.random.RandomState(5)
+    pts = (rs.randn(4000, 3) * 0.5).astype(np.float32)
+    feats = rs.rand(4000, 3).astype(np.float32)
+    rp, rf = R.grid_subsampling(pts, feats, None, 0.07)
+    o = np.lexsort((rp[:, 2], rp[:, 1], rp[:, 0]))
+    out["grid/points"], out["grid/features"] = rp[o], rf[o]
+    _, sets, _ = wrap_padded_frame()
+    for key, s, q, kk in knn_schedule(3072):
+        out["wrap_padded/" + key] = R.knn_search(sets[s][None], sets[q][None], kk)
+    return out
+
+
+KNN_RANDOM = [(0, 500, 300, 16), (1, 2000, 100, 1), (2, 64, 64, 32), (3, 5, 9, 8), (4, 3000, 700, 4)]
+
+
 def main():
     if not R.reference_sources_present():
         raise SystemExit("needs /root/reference")
@@ -433,7 +501,7 @@ def main():
     if len(sys.argv) > 2 and sys.argv[1] == "--only":      # regenerate one fixture file
         which = sys.argv[2]
         fn = {"lfa": lfa_cases, "knn": knn_cases, "gather": gather_cases, "grid": grid_cases, "train": train_cases,
-              "fusion": fusion_cases, "pose": pose_cases}[which]
+              "fusion": fusion_cases, "pose": pose_cases, "refcheck": refcheck_cases}[which]
         np.savez_compressed(os.path.join(OUT, which + "_cases.npz"), **fn())
         print("rewrote", which + "_cases.npz")
         return
@@ -444,6 +512,7 @@ def main():
     np.savez_compressed(os.path.join(OUT, "fusion_cases.npz"), **fusion_cases())
     np.savez_compressed(os.path.join(OUT, "train_cases.npz"), **train_cases())
     np.savez_compressed(os.path.join(OUT, "pose_cases.npz"), **pose_cases())
+    np.savez_compressed(os.path.join(OUT, "refcheck_cases.npz"), **refcheck_cases())
     dig = {"generator": "ffb6d_b200.synthetic.make_frame", "frames": {}}
     for seed, n in ((0, 12288), (1, 12288), (2, 3072)):
         dig["frames"]["seed%d_n%d" % (seed, n)] = {"seed": seed, "n_points": n,

@@ -1,103 +1,96 @@
-"""CPU, only where /root/reference exists (this container): the oracle against the
-reference's own code executed live on fresh random inputs."""
+"""CPU: the oracle against outputs of the reference's own code (its compiled KNN and grid
+subsampling, its torch gathers) on seeded inputs, stored in tests/golden/refcheck_cases.npz by
+tests/golden/make_golden.py; the inputs are regenerated here from the same seeds."""
+import os
+import sys
+
 import numpy as np
 import pytest
 
 from oracle import cpu_oracle as O
-from oracle import ref_loader as R
 
-pytestmark = pytest.mark.skipif(not (R.reference_sources_present() and R.knn_available()),
-                                reason="reference sources / oracle/_ref not present on this box")
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+import make_golden as G  # noqa: E402
 
 
-@pytest.mark.parametrize("seed,S,Q,K", [(0, 500, 300, 16), (1, 2000, 100, 1), (2, 64, 64, 32),
-                                        (3, 5, 9, 8), (4, 3000, 700, 4)])
-def test_knn_random(seed, S, Q, K):
+@pytest.fixture(scope="module")
+def ref():
+    from conftest import GOLDEN
+    z = np.load(os.path.join(GOLDEN, "refcheck_cases.npz"))
+    return {k: z[k] for k in z.files}
+
+
+@pytest.mark.parametrize("seed,S,Q,K", G.KNN_RANDOM)
+def test_knn_random(ref, seed, S, Q, K):
     rs = np.random.RandomState(seed)
     sup = rs.randn(2, S, 3).astype(np.float32)
     qry = rs.randn(2, Q, 3).astype(np.float32)
-    want = R.knn_batch(sup, qry, K, omp=True)
+    want = ref["knn_random/%d" % seed].astype(np.int64)
     got = O.knn_batch(sup, qry, K)
     ok, ndiff, _, msg = O.knn_matches(sup, qry, got, want)
     assert ok and ndiff == 0, msg
 
 
-def test_knn_surface_frame():
+def test_knn_surface_frame(ref):
     from ffb6d_b200.synthetic import make_frame
     fr = make_frame(9, n_points=3072)
     cld = fr["cld"][None]
-    assert np.array_equal(O.knn_batch(cld, cld, 16), R.knn_batch(cld, cld, 16))
+    assert np.array_equal(O.knn_batch(cld, cld, 16), ref["surface_frame/idx"].astype(np.int64))
 
 
-@pytest.mark.parametrize("n_points", [4096, 40960, 131072])
-def test_knn_stress_sweep_sizes(n_points):
+@pytest.mark.parametrize("n_points", G.STRESS_SIZES)
+def test_knn_stress_sweep_sizes(ref, n_points):
     """BASELINE configs[4] sizes: the port still equals the reference's KD-tree on the big clouds
-    (self search K = 16 on level 1, image -> cloud K = 1 and cloud -> image K = 32 on level 2)."""
-    from ffb6d_b200.synthetic import make_frame
-    fr = make_frame(21, n_points=n_points)
-    lvl1 = fr["cld"][None, : n_points // 4]
-    lvl2 = fr["cld"][None, : n_points // 16]
-    img = np.ascontiguousarray(fr["dpt_xyz"][::4, ::4].reshape(1, -1, 3))
+    (self search K = 16 on level 1, image -> cloud K = 1 and cloud -> image K = 32 on level 2), on a
+    seeded sample of query rows."""
     # dense clouds do produce the odd exact fp32 distance tie (seen: one row of 10240 at N0 = 40960), and
     # the hole pixels of the image level are exact duplicates: rows may then differ in ORDER only
-    for sup, qry, k in ((lvl1, lvl1, 16), (lvl2, img, 1), (img, lvl2, 32)):
-        got, want = O.knn_batch(sup, qry, k), R.knn_batch(sup, qry, k)
-        ok, ndiff, nties, msg = O.knn_matches(sup, qry, got, want)
+    for name, sup, qry, k in G.stress_searches(n_points):
+        q = qry[:, G.stress_rows(qry.shape[1], n_points)]
+        got, want = O.knn_batch(sup, q, k), ref["stress/%d_%s" % (n_points, name)].astype(np.int64)
+        ok, ndiff, nties, msg = O.knn_matches(sup, q, got, want)
         assert ok and ndiff == nties, msg
-        assert ndiff <= max(4, got.shape[1] // 1000) or sup is img, msg
+        assert ndiff <= max(4, q.shape[1] // 1000) or name == "cld2img", msg
 
 
-def test_torch_ops_random():
+def test_torch_ops_random(ref):
     import torch
-    f = R.torch_functions()
     g = torch.Generator().manual_seed(7)
     feat = torch.randn(3, 17, 211, 1, generator=g)
     idx = torch.randint(0, 211, (3, 50, 16), generator=g)
-    assert np.array_equal(f["random_sample"](feat, idx).numpy(), O.random_sample(feat.numpy(), idx.numpy()))
+    assert np.array_equal(ref["torch/random_sample"], O.random_sample(feat.numpy(), idx.numpy()))
     idx1 = torch.randint(0, 211, (3, 400, 1), generator=g)
-    assert np.array_equal(f["nearest_interpolation"](feat, idx1).numpy(),
-                          O.nearest_interpolation(feat.numpy(), idx1.numpy()))
+    assert np.array_equal(ref["torch/nearest_interpolation"], O.nearest_interpolation(feat.numpy(), idx1.numpy()))
     pc = torch.randn(2, 90, 6, generator=g)
     nidx = torch.randint(0, 90, (2, 90, 16), generator=g)
-    assert np.array_equal(f["gather_neighbour"](pc, nidx).numpy(),
-                          O.gather_neighbour(pc.numpy(), nidx.numpy()))
+    assert np.array_equal(ref["torch/gather_neighbour"], O.gather_neighbour(pc.numpy(), nidx.numpy()))
 
 
-@pytest.mark.skipif(not R.grid_available(), reason="oracle/_ref/libgrid_ref.so missing")
-def test_grid_random():
+def test_grid_random(ref):
     rs = np.random.RandomState(5)
     pts = (rs.randn(4000, 3) * 0.5).astype(np.float32)
     feats = rs.rand(4000, 3).astype(np.float32)
-    rp, rf = R.grid_subsampling(pts, feats, None, 0.07)
     op, of, _ = O.grid_sub_sampling(pts, feats, None, 0.07)
-    o1 = np.lexsort((rp[:, 2], rp[:, 1], rp[:, 0]))
     o2 = np.lexsort((op[:, 2], op[:, 1], op[:, 0]))
-    assert np.array_equal(rp[o1], op[o2]) and np.array_equal(rf[o1], of[o2])
+    assert np.array_equal(ref["grid/points"], op[o2]) and np.array_equal(ref["grid/features"], of[o2])
 
 
-def test_wrap_padded_frame_tie_order_differs_but_gathers_agree():
+def test_wrap_padded_frame_tie_order_differs_but_gathers_agree(ref):
     """A frame padded with repeated pixels (np.pad 'wrap', ycb_dataset.py:230): thousands of index rows differ
     between the reference's KD-tree order and the (distance, index) order -- within the tie contract -- yet every
     gather of the forward pass returns the same values, because tied points are duplicates with identical features."""
-    from conftest import frame_point_sets
-    from ffb6d_b200.synthetic import make_frame
     from ffb6d_b200.tables import gather_schedule, knn_schedule
     n = 3072
-    fr = make_frame(11, n_points=n)
-    rs = np.random.RandomState(5)
-    keep = fr["choose"][0][: n * 5 // 8]
-    choose = np.pad(keep, (0, n - len(keep)), "wrap")[rs.permutation(n)]
-    fr = dict(fr, cld=fr["dpt_xyz"].reshape(-1, 3)[choose])
-    sets = frame_point_sets(fr, n)
-    ref, ours, differing = {}, {}, 0
+    _, sets, rs = G.wrap_padded_frame(n)
+    refi, ours, differing = {}, {}, 0
     for key, s, q, kk in knn_schedule(n):
-        ref[key] = R.knn_search(sets[s][None], sets[q][None], kk)
+        refi[key] = ref["wrap_padded/" + key]
         ours[key] = O.knn_search(sets[s][None], sets[q][None], kk)
-        ok, _, _, msg = O.knn_matches(sets[s][None], sets[q][None], ours[key], ref[key])
+        ok, _, _, msg = O.knn_matches(sets[s][None], sets[q][None], ours[key], refi[key])
         assert ok, (key, msg)
-        differing += int((ref[key] != ours[key]).any(axis=2).sum())
+        differing += int((refi[key] != ours[key]).any(axis=2).sum())
     assert differing > 1000
-    for d in (ref, ours):
+    for d in (refi, ours):
         d.update({"cld_sub_idx%d" % i: d["cld_nei_idx%d" % i][:, : n // 4 ** (i + 1)] for i in range(4)})
     support_of = {key: s for key, s, q, kk in knn_schedule(n)}
     for op, key, C, S, Q, K in gather_schedule(n):
@@ -107,4 +100,4 @@ def test_wrap_padded_frame_tie_order_differs_but_gathers_agree():
         w = rs.normal(size=(min(C, 16), 3)).astype(np.float32)
         feat = np.sin(pts @ w.T * 7.0).T[None, :, :, None].astype(np.float32).copy()     # features = f(xyz)
         f = O.random_sample if op == "random_sample" else O.nearest_interpolation
-        assert np.array_equal(f(feat, ref[key].astype(np.int64)), f(feat, ours[key].astype(np.int64))), key
+        assert np.array_equal(f(feat, refi[key].astype(np.int64)), f(feat, ours[key].astype(np.int64))), key

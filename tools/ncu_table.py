@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """One markdown row per kernel launch of an .ncu-rep captured with `ncu --set full`: duration, DRAM bytes, and the
-utilisation figures the rooflines quote.  usage: ncu_table.py report.ncu-rep > profiles/rNN_ncu_<what>.md"""
+utilisation figures the rooflines quote.  usage: ncu_table.py report.ncu-rep > ncu_<what>.md"""
 import csv
 import io
 import re

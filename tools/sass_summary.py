@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Per-kernel SASS evidence of libffb6d_b200.so: counts of the Blackwell-specific opcodes (tcgen05 -> UTC*MMA,
-tcgen05.ld -> LDTM, bulk / tensor TMA -> UBLKCP / UTMALDG, mbarrier -> SYNCS, tcgen05.commit -> UTCBAR, cluster
-barriers -> UCGABAR, distributed shared memory -> *.CLUSTER / MAPA), plus LDGSTS / HMMA (legacy paths, expected 0)
-and the total instruction count.  usage: sass_summary.py [lib.so] > profiles/rNN_sass.md   (no GPU needed)"""
+"""Per-kernel SASS evidence of libffb6d_b200.so: counts of the Hopper-specific opcodes (wgmma -> HGMMA, wgmma
+fence / wait -> WARPGROUP, bulk / tensor TMA -> UBLKCP / UTMALDG, mbarrier -> SYNCS, cluster barriers -> UCGABAR,
+distributed shared memory -> *.CLUSTER / MAPA), plus LDGSTS / HMMA (legacy paths, expected 0) and the total
+instruction count.  usage: sass_summary.py [lib.so] > sass.md   (no GPU needed)"""
 import collections
 import os
 import re
@@ -12,7 +12,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "ffb6d_b200", "libffb6d_b200.so")
 out = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
-OPS = ["UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTCBAR", "UBLKCP", "UTMALDG", "UTMASTG", "SYNCS", "UCGABAR", "MAPA",
+OPS = ["HGMMA", "WARPGROUP", "UBLKCP", "UTMALDG", "UTMASTG", "SYNCS", "UCGABAR", "MAPA",
        "REDUX", "ATOM", "RED", "LDGSTS", "HMMA", "SHFL", "LDS", "STS"]
 counts, order, cur = {}, [], None
 for line in out.splitlines():
@@ -35,7 +35,7 @@ for line in out.splitlines():
                 counts[cur][o] += 1
         if ".CLUSTER" in op or "SHARED::CLUSTER" in op:
             counts[cur]["cluster-scope"] += 1
-print("# SASS opcode counts per kernel (`cuobjdump -sass ffb6d_b200/libffb6d_b200.so`, sm_100a)\n")
+print("# SASS opcode counts per kernel (`cuobjdump -sass ffb6d_b200/libffb6d_b200.so`, sm_90a)\n")
 cols = ["total"] + OPS + ["cluster-scope"]
 print("| kernel | " + " | ".join(cols) + " |")
 print("|---|" + "---:|" * len(cols))
