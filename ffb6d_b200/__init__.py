@@ -11,6 +11,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
 * :func:`grid_sub_sampling` -- ``DataProcessing.grid_sub_sampling`` (helper_tool.py:199-219)
 * :func:`build_ffb6d_indices` -- the 22-call KNN schedule of the datasets
   (datasets/ycb/ycb_dataset.py:269-309) run on the GPU in one go.
+* :func:`fill_missing` -- ``Basic_Utils.fill_missing`` (utils/basic_utils.py:467-487) as the YCB dataset calls it
+  (datasets/ycb/ycb_dataset.py:204); :func:`build_ffb6d_indices_from_raw_depth` -- the depth half of its
+  ``get_item`` from the raw depth PNG to the 22 index tensors.
 * :mod:`ffb6d_b200.pose` -- ``MeanShiftTorch``, ``best_fit_transform``, ``cal_frame_poses(_lm)``
   (utils/meanshift_pytorch.py:27-57, utils/pvn3d_eval_utils_kpls.py:28-160, 220-284): keypoint voting on the GPU.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
@@ -26,8 +29,10 @@ import importlib
 
 _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbour", "relative_pos_encoding",
         "choose_gather", "grid_sub_sampling", "KnnGrid", "backproject", "fusion_mlp", "fusion_mlp_pack",
-        "PackedWeight", "fold_batchnorm", "att_pool", "sample_valid_pixels", "check_indices", "mean_shift_fit", "best_fit_transform")
-_SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native")
+        "PackedWeight", "fold_batchnorm", "att_pool", "sample_valid_pixels", "check_indices", "mean_shift_fit", "best_fit_transform",
+        "fill_missing")
+_SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
+             "build_ffb6d_indices_from_raw_depth")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
                "helper_tool", "model", "pose", "_lib")

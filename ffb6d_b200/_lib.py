@@ -80,6 +80,8 @@ def _load():
         "ffb6d_backproject": (ci, [vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp, vp, vp]),
         "ffb6d_sample_pixels_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_sample_pixels": (ci, [vp, i64, i64, i64, fp, i64, C.c_uint64, vp, vp, vp, sz, vp]),
+        "ffb6d_fill_depth_workspace_bytes": (sz, [i64, i64, i64]),
+        "ffb6d_fill_depth": (ci, [vp, i64, i64, i64, fp, vp, vp, vp, sz, vp]),
         "ffb6d_mean_shift_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_mean_shift_fit": (ci, [vp, vp, i64, i64, i64, fp, ci, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_best_fit_transform": (ci, [vp, vp, i64, i64, vp, vp]),

@@ -262,3 +262,30 @@ def build_ffb6d_indices_from_depth(depth, K, choose, k=K_NEIGH, index_dtype=torc
     cld, pyr = backproject(depth, K, choose)
     return build_ffb6d_indices(cld, None, k=k, index_dtype=index_dtype, streams=streams, pyramid=pyr,
                                image_hw=(depth.shape[1], depth.shape[2]))
+
+
+# float32(1e-6): the dataset's `msk_dp = dpt_um > 1e-6` on the completed raw depth (ycb_dataset.py:205)
+MSK_DP_THRESHOLD = 1e-6
+
+
+def build_ffb6d_indices_from_raw_depth(dpt_raw, cam_scale, K, n_points, seed=0, k=K_NEIGH, index_dtype=torch.int32,
+                                       streams=None):
+    """The depth half of ``YCB_Dataset.get_item`` on the GPU (datasets/ycb/ycb_dataset.py:204-309 without
+    normals): depth completion (:func:`ffb6d_b200.ops.fill_missing`, :204), ``msk_dp`` and the sampling of
+    ``n_points`` valid pixels (:205, 218-235, :func:`ffb6d_b200.ops.sample_valid_pixels` with ``seed``),
+    ``dpt_m`` (:215), back-projection and the 22 searches (:func:`build_ffb6d_indices_from_depth`).
+
+    :param dpt_raw: ``[B,H,W]`` ``torch.uint16`` CUDA, the depth PNGs' raw values
+    :param cam_scale: raw units per metre (``meta['factor_depth']``); :param K: camera matrix as for
+      :func:`ffb6d_b200.ops.backproject`
+    :return: the dict of :func:`build_ffb6d_indices`, plus ``choose [B,1,n_points]`` int32 and
+      ``dpt_map_m [B,H,W]`` float32 (the reference's ``item_dict`` key)"""
+    from .ops import _fill_depth, sample_valid_pixels
+    if not isinstance(dpt_raw, torch.Tensor) or dpt_raw.dim() != 3:
+        raise ValueError("dpt_raw must be a [B,H,W] torch.uint16 CUDA tensor")
+    filled, depth_m = _fill_depth(dpt_raw, cam_scale)
+    choose = sample_valid_pixels(filled, n_points, seed=seed, min_depth=MSK_DP_THRESHOLD)
+    inputs = build_ffb6d_indices_from_depth(depth_m, K, choose, k=k, index_dtype=index_dtype, streams=streams)
+    inputs["choose"] = choose
+    inputs["dpt_map_m"] = depth_m
+    return inputs

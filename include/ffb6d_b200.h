@@ -369,6 +369,26 @@ int ffb6d_sample_pixels(const float *depth, int64_t B, int64_t H, int64_t W, flo
                         uint64_t seed, int *choose, int *valid_count, void *workspace, size_t workspace_bytes,
                         ffb6d_stream_t stream);
 
+/*
+ * Depth completion of the raw sensor depth, replacing the CPU call
+ * `dpt_um = bs_utils.fill_missing(dpt_um, cam_scale, 1)` of datasets/ycb/ycb_dataset.py:204
+ * (utils/basic_utils.py:467-487 -> ip_basic's fill_in_multiscale,
+ * utils/ip_basic/ip_basic/depth_map_utils_ycb.py:290-443, with max_depth 3.0, no extrapolation and the
+ * bilateral blur -- the only configuration the datasets use).
+ *   depth_raw [B,H,W] uint16 (the depth PNG's values), cam_scale > 0 raw units per metre
+ *   -> filled_raw [B,H,W] f32 (fill_missing's return, raw units; may be NULL)
+ *   -> depth_m    [B,H,W] f32 (the dataset's dpt_m = filled_raw / cam_scale, metres; may be NULL)
+ * Every pixel the final bilateral blur does not write is bit-identical to the reference; the blurred ones
+ * use exact float64 weights where OpenCV interpolates a table, and differ from it by at most 2e-6 m.
+ * Any H, W >= 1.  No allocation, no host synchronisation (capturable in a CUDA graph); deterministic.
+ * workspace: ffb6d_fill_depth_workspace_bytes(B,H,W) bytes.  FFB6D_ERR_INVALID on bad sizes, cam_scale <= 0
+ * or both outputs NULL; FFB6D_ERR_WORKSPACE on a missing or small workspace.
+ */
+size_t ffb6d_fill_depth_workspace_bytes(int64_t B, int64_t H, int64_t W);
+int ffb6d_fill_depth(const uint16_t *depth_raw, int64_t B, int64_t H, int64_t W, float cam_scale,
+                     float *filled_raw, float *depth_m, void *workspace, size_t workspace_bytes,
+                     ffb6d_stream_t stream);
+
 /* ---- keypoint voting and pose fitting (the step after the network) -------- */
 /*
  * Gaussian mean shift of G independent vote sets, replacing MeanShiftTorch.fit
