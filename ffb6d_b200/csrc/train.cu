@@ -14,7 +14,7 @@
 //     dW = dz * X^T (ffb6d_fusion_mlp_wgrad),  dX = W^T * dz (the forward GEMM with the transposed weight).
 // These kernels are HBM bound: every element of z / g is read once per pass with 128-bit loads; the
 // per-channel sums are accumulated in fp32 per thread (<= a few hundred terms) and in fp64 across
-// threads, CTAs and frames.
+// threads, CTAs and frames; the forward's (sum, sum of squares) are taken about a per-channel pivot.
 #include "common.cuh"
 
 #include <algorithm>
@@ -36,26 +36,30 @@ __device__ __forceinline__ double block_sum(double v, double *red)
     return t;
 }
 
-// partial[c][s] = (sum, sum of squares) of z[:, c, chunk s] over all frames
+// partial[c][s] = (sum, sum of squares) of z[:, c, chunk s] - k over all frames, k = z[0, c, 0].
+// The shift keeps the one-pass variance Q/n - (A/n)^2 free of cancellation when a channel's |mean| is
+// large next to its spread: the terms are O(std), not O(|mean|), and a constant channel sums to exactly 0.
 __global__ void __launch_bounds__(BN_THREADS)
 bn_stats_kernel(const float *__restrict__ z, int B, int C, int P, int chunk, int nsplit, double *__restrict__ partial)
 {
     __shared__ double red[BN_THREADS / 32];
     const int c = blockIdx.y, s = blockIdx.x;
     const int p0 = s * chunk, p1 = min(P, p0 + chunk);
+    const float k = __ldg(z + (size_t)c * P);
     float a = 0.f, q = 0.f;
     const bool vec = ((P & 3) == 0) && ((chunk & 3) == 0) && ((reinterpret_cast<uintptr_t>(z) & 15) == 0);
     for (int b = 0; b < B; ++b) {
         const float *row = z + ((size_t)b * C + c) * P;
         if (vec) {
             for (int p = p0 + 4 * threadIdx.x; p < p1; p += 4 * BN_THREADS) {
-                const float4 v = __ldg(reinterpret_cast<const float4 *>(row + p));
+                float4 v = __ldg(reinterpret_cast<const float4 *>(row + p));
+                v.x -= k; v.y -= k; v.z -= k; v.w -= k;
                 a += (v.x + v.y) + (v.z + v.w);
                 q += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
             }
         } else {
             for (int p = p0 + threadIdx.x; p < p1; p += BN_THREADS) {
-                const float v = __ldg(row + p);
+                const float v = __ldg(row + p) - k;
                 a += v;
                 q += v * v;
             }
@@ -70,9 +74,9 @@ bn_stats_kernel(const float *__restrict__ z, int B, int C, int P, int chunk, int
 
 // stats[c] = (mean, invstd, gamma * invstd, beta); running statistics updated like torch.nn.BatchNorm2d
 __global__ void __launch_bounds__(BN_THREADS)
-bn_finalize_kernel(const double *__restrict__ partial, int C, int nsplit, double n, float eps, float momentum,
-                   const float *__restrict__ gamma, const float *__restrict__ beta, float *__restrict__ running_mean,
-                   float *__restrict__ running_var, float4 *__restrict__ stats)
+bn_finalize_kernel(const double *__restrict__ partial, const float *__restrict__ z, int C, int P, int nsplit, double n,
+                   float eps, float momentum, const float *__restrict__ gamma, const float *__restrict__ beta,
+                   float *__restrict__ running_mean, float *__restrict__ running_var, float4 *__restrict__ stats)
 {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
@@ -81,8 +85,9 @@ bn_finalize_kernel(const double *__restrict__ partial, int C, int nsplit, double
         A += partial[((size_t)c * nsplit + s) * 2];
         Q += partial[((size_t)c * nsplit + s) * 2 + 1];
     }
-    const double mean = A / n;
-    double var = Q / n - mean * mean;   // biased, as BatchNorm normalises with
+    const double d = A / n;                              // mean - k, with bn_stats_kernel's pivot k
+    const double mean = (double)z[(size_t)c * P] + d;
+    double var = Q / n - d * d;         // biased, as BatchNorm normalises with
     if (var < 0.0) var = 0.0;
     const float invstd = (float)(1.0 / sqrt(var + (double)eps));
     const float g = gamma ? gamma[c] : 1.f;
@@ -385,8 +390,8 @@ int ffb6d_bn_train_fwd(const float *z, int64_t B, int64_t C, int64_t P, const fl
                     "bn_train_fwd: bad size");
     FFB6D_CHECK_ARG(z && stats && y && workspace, "bn_train_fwd: null pointer");
     FFB6D_CHECK_ARG(act >= 0 && act <= 2, "bn_train_fwd: act=%d", act);
-    FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_train_fwd: workspace too small");
     FFB6D_CHECK_ARG((reinterpret_cast<uintptr_t>(stats) & 15) == 0, "bn_train_fwd: stats must be 16-byte aligned");
+    FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_train_fwd: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     int chunk, nsplit;
     split_plan(C, P, chunk, nsplit);
@@ -394,7 +399,8 @@ int ffb6d_bn_train_fwd(const float *z, int64_t B, int64_t C, int64_t P, const fl
     bn_stats_kernel<<<dim3((unsigned)nsplit, (unsigned)C), BN_THREADS, 0, st>>>(z, (int)B, (int)C, (int)P, chunk, nsplit, partial);
     FFB6D_LAUNCH_OK("bn_stats_kernel");
     bn_finalize_kernel<<<(unsigned)ceil_div(C, BN_THREADS), BN_THREADS, 0, st>>>(
-        partial, (int)C, nsplit, (double)B * (double)P, eps, momentum, gamma, beta, running_mean, running_var, (float4 *)stats);
+        partial, z, (int)C, (int)P, nsplit, (double)B * (double)P, eps, momentum, gamma, beta, running_mean, running_var,
+        (float4 *)stats);
     FFB6D_LAUNCH_OK("bn_finalize_kernel");
     const unsigned gx = (unsigned)std::min<int64_t>(ceil_div(P, 4 * BN_THREADS), 64);
     bn_apply_kernel<<<dim3((unsigned)(B * C), gx), BN_THREADS, 0, st>>>(z, (const float4 *)stats, (int)C, (int)P, act,
@@ -410,6 +416,8 @@ int ffb6d_bn_train_bwd(const float *z, const float *grad_y, const float *stats, 
     FFB6D_CHECK_ARG(B >= 1 && C >= 1 && P >= 1 && B < 65536 && C <= 65535 && P < (1ll << 31) && B * C < (1ll << 31),
                     "bn_train_bwd: bad size");
     FFB6D_CHECK_ARG(z && grad_y && stats && grad_z && workspace, "bn_train_bwd: null pointer");
+    FFB6D_CHECK_ARG(act >= 0 && act <= 2, "bn_train_bwd: act=%d", act);
+    FFB6D_CHECK_ARG((reinterpret_cast<uintptr_t>(stats) & 15) == 0, "bn_train_bwd: stats must be 16-byte aligned");
     FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_train_bwd: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     int chunk, nsplit;

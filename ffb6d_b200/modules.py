@@ -19,6 +19,8 @@ Both modes run on the CUDA library:
 A layer accepts its input as one tensor or as the two halves of a concat (``layer(x1, x2)`` ==
 ``layer(torch.cat((x1, x2), 1))`` without materialising the concat, models/ffb6d.py:251-262).
 """
+import math
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F_
@@ -208,10 +210,16 @@ class _ConvBase(nn.Module):
         need_grad = torch.is_grad_enabled() and (x.requires_grad or conv.weight.requires_grad or
                                                  (x2 is not None and x2.requires_grad))
         if self.training and bn is not None:
+            if x.shape[0] * math.prod(x.shape[2:]) == 1:     # as torch's BatchNorm in training
+                raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                                 % (torch.Size((x.shape[0], bn.num_features) + tuple(x.shape[2:])),))
             if bn.track_running_stats and bn.num_batches_tracked is not None:
                 bn.num_batches_tracked += 1
+            momentum = bn.momentum
+            if momentum is None:     # cumulative moving average, as nn.BatchNorm2d(momentum=None)
+                momentum = 1.0 / float(bn.num_batches_tracked) if bn.num_batches_tracked is not None else 0.0
             return _ConvBnActTrain.apply(x, x2, conv.weight, None, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                                         bn.eps, bn.momentum if bn.momentum is not None else 0.1, self.act, self.slope, True)
+                                         bn.eps, momentum, self.act, self.slope, True)
         if need_grad and bn is None:
             return _ConvBnActTrain.apply(x, x2, conv.weight, conv.bias, None, None, None, None, 0.0, 0.0, self.act,
                                          self.slope, False)

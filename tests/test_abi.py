@@ -58,6 +58,57 @@ def test_argument_validation_needs_no_gpu():
     assert lib.ffb6d_knn_workspace_bytes(1, 0, 1, 1) == 0
 
 
+def test_train_argument_validation_needs_no_gpu():
+    """The training entry points reject bad sizes, activations, null and misaligned pointers before any launch."""
+    lib = _lib.lib
+    buf = (C.c_float * 64)()
+    p = (C.addressof(buf) + 15) & ~15           # 16-byte aligned
+    BIG = 1 << 40                               # a workspace size that passes its check
+
+    def fwd(z=p, B=2, Cc=3, P=5, act=1, stats=p, y=p, ws=p, nbytes=BIG):
+        return lib.ffb6d_bn_train_fwd(z, B, Cc, P, p, p, 1e-5, 0.1, p, p, act, 0.0, stats, y, ws, nbytes, None)
+
+    def bwd(z=p, gy=p, stats=p, B=2, Cc=3, P=5, act=1, gz=p, ws=p, nbytes=BIG):
+        return lib.ffb6d_bn_train_bwd(z, gy, stats, B, Cc, P, act, 0.0, p, p, gz, ws, nbytes, None)
+
+    for call, name in ((fwd, "bn_train_fwd"), (bwd, "bn_train_bwd")):
+        for size in (dict(B=0), dict(Cc=0), dict(P=0), dict(B=-1), dict(B=65536), dict(Cc=65536), dict(P=1 << 31),
+                     dict(B=40000, Cc=60000)):
+            assert call(**size) == _lib.ERR_INVALID, (name, size)
+            assert name + ": bad size" in _lib.last_error()
+        for act in (-1, 3):
+            assert call(act=act) == _lib.ERR_INVALID, (name, act)
+            assert "act=%d" % act in _lib.last_error()
+        assert call(stats=p + 4) == _lib.ERR_INVALID, name
+        assert "16-byte aligned" in _lib.last_error()
+        assert call(nbytes=0) == _lib.ERR_INVALID, name
+        assert "workspace too small" in _lib.last_error()
+    for ptr in ("z", "stats", "y", "ws"):
+        assert fwd(**{ptr: None}) == _lib.ERR_INVALID, ptr
+        assert "null pointer" in _lib.last_error()
+    for ptr in ("z", "gy", "stats", "gz", "ws"):
+        assert bwd(**{ptr: None}) == _lib.ERR_INVALID, ptr
+        assert "null pointer" in _lib.last_error()
+    assert lib.ffb6d_bn_workspace_bytes(0, 5) == 0 and lib.ffb6d_bn_workspace_bytes(3, 0) == 0
+
+    assert lib.ffb6d_act_bwd(p, p, -1, 1, 0.0, p, None) == _lib.ERR_INVALID
+    assert lib.ffb6d_act_bwd(p, p, 8, 3, 0.0, p, None) == _lib.ERR_INVALID
+    assert lib.ffb6d_act_bwd(p, p, 8, -1, 0.0, p, None) == _lib.ERR_INVALID
+    for i in range(3):
+        ptrs = [p, p, p]
+        ptrs[i] = None
+        assert lib.ffb6d_act_bwd(ptrs[0], ptrs[1], 8, 1, 0.0, ptrs[2], None) == _lib.ERR_INVALID
+        assert "null pointer" in _lib.last_error()
+    assert lib.ffb6d_act_bwd(None, None, 0, 1, 0.0, None, None) == _lib.OK      # nothing to do
+
+    assert lib.ffb6d_att_pool_bwd(p, 0, None, 0, p, p, 1, 4, 16, p, None, p, None) == _lib.ERR_INVALID   # C1 = 0
+    assert lib.ffb6d_att_pool_bwd(p, 2, None, 0, p, p, 1, 4, 0, p, None, p, None) == _lib.ERR_INVALID    # K = 0
+    assert lib.ffb6d_att_pool_bwd(p, 2, None, 0, p, p, 1, 4, 65, p, None, p, None) == _lib.ERR_INVALID   # K > 64
+    assert lib.ffb6d_att_pool_bwd(p, 2, None, 3, p, p, 1, 4, 16, p, None, p, None) == _lib.ERR_INVALID   # f2 missing
+    assert "null pointer" in _lib.last_error()
+    assert lib.ffb6d_att_pool_bwd(p, 2, None, 0, p, p, 0, 4, 16, p, None, p, None) == _lib.OK            # B == 0
+
+
 @pytest.mark.skipif(HAS_GPU, reason="only meaningful on a box without a GPU")
 def test_no_cpu_fallback():
     """Without a device the product must fail loudly, never compute on the CPU."""
