@@ -30,7 +30,7 @@ import importlib
 _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbour", "relative_pos_encoding",
         "choose_gather", "grid_sub_sampling", "KnnGrid", "backproject", "fusion_mlp", "fusion_mlp_pack",
         "PackedWeight", "fold_batchnorm", "att_pool", "sample_valid_pixels", "check_indices", "mean_shift_fit", "best_fit_transform",
-        "fill_missing")
+        "fill_missing", "segment_plan", "segment_sum")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")

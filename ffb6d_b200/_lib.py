@@ -73,6 +73,9 @@ def _load():
         "ffb6d_bn_train_bwd": (ci, [vp, vp, vp, i64, i64, i64, ci, fp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_act_bwd": (ci, [vp, vp, i64, ci, fp, vp, vp]),
         "ffb6d_fusion_mlp_wgrad": (ci, [vp, vp, i64, vp, i64, i64, i64, i64, vp, vp]),
+        "ffb6d_segment_plan_bytes": (sz, [i64, i64, i64]),
+        "ffb6d_segment_plan": (ci, [vp, ci, i64, i64, i64, vp, sz, vp]),
+        "ffb6d_segment_sum": (ci, [vp, vp, sz, i64, i64, i64, i64, vp, vp]),
         "ffb6d_att_pool_bwd": (ci, [vp, i64, vp, i64, vp, vp, i64, i64, ci, vp, vp, vp, vp]),
         "ffb6d_lfa_att_pool_fused": (ci, [vp, vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i64, ci, i64, i64, fp, vp, vp]),
         "ffb6d_att_pool_fwd": (ci, [vp, i64, vp, i64, vp, i64, i64, ci, vp, vp]),

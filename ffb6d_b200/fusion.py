@@ -1,4 +1,5 @@
-"""The bidirectional fusion stage of FFB6D on this package's kernels (inference, frozen BatchNorm).
+"""The bidirectional fusion stage of FFB6D on this package's kernels (inference, frozen BatchNorm; the training
+form of the restructured pixel branch is :meth:`ffb6d_b200.modules.Conv2d.forward_interp`).
 
 One stage of ``FFB6D.forward`` (models/ffb6d.py:231-263 encoder, :267-298 decoder) after the CNN /
 RandLA layers of the stage have produced ``rgb_emb0 [B, C_r, h, w]`` and the point features::
@@ -49,16 +50,27 @@ class FusedConv:
 
 class SplitFuse:
     """``p2r_fuse`` split at the concat boundary: ``W1 = W[:, :C_r]`` (image half, keeps the BatchNorm and
-    the ReLU) and ``W2 = W[:, C_r:]`` (point half, applied on the N' points, no affine, channels-last out)."""
+    the activation) and ``W2 = W[:, C_r:]`` (point half, applied on the N' points, no affine, channels-last out).
+    ``relu`` / ``negative_slope``: the activation, as :func:`ffb6d_b200.ops.fusion_mlp` takes it."""
 
-    def __init__(self, fused, c_rgb):
-        w = fused.weight
+    def __init__(self, fused, c_rgb, relu=True, negative_slope=None):
+        self._setup(fused.weight, fused.scale, fused.shift, c_rgb, relu, negative_slope)
+
+    @classmethod
+    def from_weight(cls, weight, scale, shift, c_rgb, relu=True, negative_slope=None):
+        """From a layer's ``conv.weight`` and its folded BatchNorm (``scale``, ``shift``)."""
+        self = cls.__new__(cls)
+        self._setup(weight.detach().reshape(weight.shape[0], -1).float(), scale, shift, c_rgb, relu, negative_slope)
+        return self
+
+    def _setup(self, w, scale, shift, c_rgb, relu, negative_slope):
         self.c_rgb = int(c_rgb)
         self.w1 = ops.fusion_mlp_pack(w[:, :c_rgb].contiguous())
         self.w2 = ops.fusion_mlp_pack(w[:, c_rgb:].contiguous())
-        self.scale, self.shift = fused.scale, fused.shift
-        self.ones = torch.ones_like(fused.scale)
-        self.zeros = torch.zeros_like(fused.scale)
+        self.scale, self.shift = scale, shift
+        self.ones = torch.ones_like(scale)
+        self.zeros = torch.zeros_like(scale)
+        self.relu, self.negative_slope = relu, negative_slope
 
 
 def p2r_fuse(rgb_emb0, p2r, p2r_idx, split):
@@ -69,7 +81,8 @@ def p2r_fuse(rgb_emb0, p2r, p2r_idx, split):
     :param p2r_idx: ``[B, h*w, 1]`` nearest cloud point of every pixel; :param split: :class:`SplitFuse`
     :return: ``[B, C_r, h, w]``"""
     z = ops.fusion_mlp(p2r, None, split.w2, split.ones, split.zeros, relu=False, out_channels_last=True)   # [B, N', C_r]
-    return ops.fusion_mlp(rgb_emb0, None, split.w1, split.scale, split.shift, add=z, add_idx=p2r_idx)
+    return ops.fusion_mlp(rgb_emb0, None, split.w1, split.scale, split.shift, relu=split.relu,
+                          negative_slope=split.negative_slope, add=z, add_idx=p2r_idx)
 
 
 class FusionStage:

@@ -34,9 +34,14 @@ def _head(in_c, out_c):
 
 
 class FFB6DFusionNet(nn.Module):
-    def __init__(self, n_classes=2, n_pts=12288, n_kps=8, in_c=9, d_out=(32, 64, 128, 256)):
+    def __init__(self, n_classes=2, n_pts=12288, n_kps=8, in_c=9, d_out=(32, 64, 128, 256), restructured=False):
+        """``restructured``: run the pixel branch of every fusion as ``W1 . rgb + (W2 . p2r)[idx]``
+        (:meth:`ffb6d_b200.modules.Conv2d.forward_interp`) instead of the reference's order of operations; the
+        interpolated maps are never built.  A plain attribute: it can be switched on a built or loaded model, and
+        the state dict is the same either way."""
         super().__init__()
         self.n_cls, self.n_pts, self.n_kps = n_classes, n_pts, n_kps
+        self.restructured = bool(restructured)
         # RandLA branch (models/RandLA/RandLANet.py:12-38)
         self.rndla_pre_stages = RandLAConv1d(in_c, 8, kernel_size=1, bn=True)
         self.rndla_ds_stages = nn.ModuleList()
@@ -75,11 +80,15 @@ class FFB6DFusionNet(nn.Module):
         self.kp_ofst_layer = _head(c, n_kps * 3)
 
     def _fuse(self, tag, i, rgb_emb0, p_emb0, p2r_idx, r2p_idx):
-        """One bidirectional fusion (models/ffb6d.py:245-263 / 281-298), reference order of operations."""
+        """One bidirectional fusion (models/ffb6d.py:245-263 / 281-298): the reference's order of operations, or
+        with ``restructured`` the pixel branch without the interpolated map."""
         bs, c, hr, wr = rgb_emb0.shape
         p2r = getattr(self, tag + "_fuse_p2r_pre_layers")[i](p_emb0)
-        p2r = ops.nearest_interpolation(p2r, p2r_idx).view(bs, -1, hr, wr)
-        rgb_emb = getattr(self, tag + "_fuse_p2r_fuse_layers")[i](rgb_emb0, p2r)          # concat fused in the layer
+        if self.restructured:
+            rgb_emb = getattr(self, tag + "_fuse_p2r_fuse_layers")[i].forward_interp(rgb_emb0, p2r, p2r_idx)
+        else:
+            p2r = ops.nearest_interpolation(p2r, p2r_idx).view(bs, -1, hr, wr)
+            rgb_emb = getattr(self, tag + "_fuse_p2r_fuse_layers")[i](rgb_emb0, p2r)      # concat fused in the layer
         r2p = ops.random_sample(rgb_emb0.reshape(bs, c, hr * wr, 1), r2p_idx)
         r2p = getattr(self, tag + "_fuse_r2p_pre_layers")[i](r2p)
         p_emb = getattr(self, tag + "_fuse_r2p_fuse_layers")[i](p_emb0, r2p)

@@ -18,6 +18,8 @@ Both modes run on the CUDA library:
 
 A layer accepts its input as one tensor or as the two halves of a concat (``layer(x1, x2)`` ==
 ``layer(torch.cat((x1, x2), 1))`` without materialising the concat, models/ffb6d.py:251-262).
+:meth:`Conv2d.forward_interp` takes the second half as point features and the pixel -> point index of the
+fusion's nearest interpolation, and never builds the interpolated map.
 """
 import math
 
@@ -25,7 +27,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F_
 
-from . import ops
+from . import fusion, ops
 from ._lib import lib, check
 
 _ACT_NONE, _ACT_RELU, _ACT_LEAKY = 0, 1, 2
@@ -57,6 +59,58 @@ def _gemm(x1, x2, w2d):
     return ops.fusion_mlp(x1, x2, w2d, one, zero, relu=False)
 
 
+def _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn):
+    """y = act(BatchNorm with batch statistics(z)) (``ffb6d_bn_train_fwd``, also updates the running statistics) or,
+    without BatchNorm, y = act(z).  Returns ``(y, stats)``; ``stats`` [Co, 4] is what :func:`_bn_act_bwd` reads."""
+    if not has_bn:
+        if act == _ACT_RELU:
+            return torch.relu(z), None
+        return (F_.leaky_relu(z, slope) if act == _ACT_LEAKY else z), None
+    stats = torch.empty((Co, 4), dtype=torch.float32, device=z.device)
+    y = torch.empty_like(z)
+    nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=z.device)
+    with torch.cuda.device(z.device):
+        check(lib.ffb6d_bn_train_fwd(
+            z.data_ptr(), B, Co, P, gamma.data_ptr() if gamma is not None else None,
+            beta.data_ptr() if beta is not None else None, float(eps), float(momentum),
+            running_mean.data_ptr() if running_mean is not None else None,
+            running_var.data_ptr() if running_var is not None else None, int(act), float(slope),
+            stats.data_ptr(), y.data_ptr(), ws.data_ptr(), nbytes, ops._stream(z.device)))
+    return y, stats
+
+
+def _bn_act_bwd(z, gy, stats, B, Co, P, act, slope, has_bn):
+    """Backward of :func:`_bn_act_fwd`: ``(dz, dgamma, dbeta)``; dgamma / dbeta are None without BatchNorm."""
+    dev = z.device
+    with torch.cuda.device(dev):
+        if has_bn:
+            dz = torch.empty_like(z)
+            ggamma = torch.empty(Co, dtype=torch.float32, device=dev)
+            gbeta = torch.empty(Co, dtype=torch.float32, device=dev)
+            nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            check(lib.ffb6d_bn_train_bwd(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
+                                         ggamma.data_ptr(), gbeta.data_ptr(), dz.data_ptr(), ws.data_ptr(), nbytes,
+                                         ops._stream(dev)))
+            return dz, ggamma, gbeta
+        if act != _ACT_NONE:
+            dz = torch.empty_like(z)
+            check(lib.ffb6d_act_bwd(z.data_ptr(), gy.data_ptr(), z.numel(), act, slope, dz.data_ptr(), ops._stream(dev)))
+            return dz, None, None
+    return gy, None, None
+
+
+def _wgrad(dz, x1, x2, B, Co, P):
+    """dW [Co, C1+C2] = sum over frames of dz [B, Co, P] . cat(x1, x2)^T (``ffb6d_fusion_mlp_wgrad``)."""
+    C1, C2 = x1.shape[1], (x2.shape[1] if x2 is not None else 0)
+    gw = torch.empty((Co, C1 + C2), dtype=torch.float32, device=dz.device)
+    with torch.cuda.device(dz.device):
+        check(lib.ffb6d_fusion_mlp_wgrad(dz.data_ptr(), x1.data_ptr(), C1, x2.data_ptr() if x2 is not None else None,
+                                         C2, B, Co, P, gw.data_ptr(), ops._stream(dz.device)))
+    return gw
+
+
 class _ConvBnActTrain(torch.autograd.Function):
     """conv1x1(cat(x1, x2)) -> [BatchNorm with batch statistics] -> activation, with its backward."""
 
@@ -74,25 +128,7 @@ class _ConvBnActTrain(torch.autograd.Function):
         else:
             z = _gemm(x1, x2, w2d)
         P = z.numel() // (B * Co)
-        stats = None
-        if has_bn:
-            stats = torch.empty((Co, 4), dtype=torch.float32, device=z.device)
-            y = torch.empty_like(z)
-            nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=z.device)
-            with torch.cuda.device(z.device):
-                check(lib.ffb6d_bn_train_fwd(
-                    z.data_ptr(), B, Co, P, gamma.data_ptr() if gamma is not None else None,
-                    beta.data_ptr() if beta is not None else None, float(eps), float(momentum),
-                    running_mean.data_ptr() if running_mean is not None else None,
-                    running_var.data_ptr() if running_var is not None else None, int(act), float(slope),
-                    stats.data_ptr(), y.data_ptr(), ws.data_ptr(), nbytes, ops._stream(z.device)))
-        elif act == _ACT_RELU:
-            y = torch.relu(z)
-        elif act == _ACT_LEAKY:
-            y = F_.leaky_relu(z, slope)
-        else:
-            y = z
+        y, stats = _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn)
         ctx.save_for_backward(x1, x2, w2d, z, stats, gamma)
         ctx.meta = (B, C1, C2, Co, P, int(act), float(slope), bool(has_bn), bias is not None, tuple(weight.shape))
         return y
@@ -102,30 +138,10 @@ class _ConvBnActTrain(torch.autograd.Function):
     def backward(ctx, gy):
         x1, x2, w2d, z, stats, gamma = ctx.saved_tensors
         B, C1, C2, Co, P, act, slope, has_bn, has_bias, wshape = ctx.meta
-        gy = gy.contiguous()
-        dev = z.device
-        ggamma = gbeta = gbias = None
-        with torch.cuda.device(dev):
-            if has_bn:
-                dz = torch.empty_like(z)
-                ggamma = torch.empty(Co, dtype=torch.float32, device=dev)
-                gbeta = torch.empty(Co, dtype=torch.float32, device=dev)
-                nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
-                ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-                check(lib.ffb6d_bn_train_bwd(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
-                                             ggamma.data_ptr(), gbeta.data_ptr(), dz.data_ptr(), ws.data_ptr(), nbytes,
-                                             ops._stream(dev)))
-            elif act != _ACT_NONE:
-                dz = torch.empty_like(z)
-                check(lib.ffb6d_act_bwd(z.data_ptr(), gy.data_ptr(), z.numel(), act, slope, dz.data_ptr(), ops._stream(dev)))
-            else:
-                dz = gy
-            gw = None
-            if ctx.needs_input_grad[2]:
-                gw = torch.empty((Co, C1 + C2), dtype=torch.float32, device=dev)
-                check(lib.ffb6d_fusion_mlp_wgrad(dz.data_ptr(), x1.data_ptr(), C1, x2.data_ptr() if x2 is not None else None,
-                                                 C2, B, Co, P, gw.data_ptr(), ops._stream(dev)))
-                gw = gw.reshape(wshape)
+        dz, ggamma, gbeta = _bn_act_bwd(z, gy.contiguous(), stats, B, Co, P, act, slope, has_bn)
+        gw = gbias = None
+        if ctx.needs_input_grad[2]:
+            gw = _wgrad(dz, x1, x2, B, Co, P).reshape(wshape)
         if has_bias:
             gbias = dz.reshape(B, Co, -1).sum(dim=(0, 2))
         # input gradients: dX = W^T . dz, one GEMM per half of the concat
@@ -137,6 +153,58 @@ class _ConvBnActTrain(torch.autograd.Function):
         if gamma is None:
             ggamma = None
         return gx1, gx2, gw, gbias, ggamma, gbeta, None, None, None, None, None, None, None
+
+
+class _InterpConvBnActTrain(torch.autograd.Function):
+    """conv1x1(cat(x1, nearest_interpolation(p, idx))) -> [BatchNorm with batch statistics] -> activation without
+    the interpolated map (SURVEY.md §8f-3): with W = [W1 | W2] split at C1,
+
+        forward   Z = W2 . p (on the N' points, channels-last)      z = W1 . x1 + Z[idx]      y = act(BN(z))
+        backward  dW1 = dz . x1^T    dx1 = W1^T . dz    dZ = segment_sum(dz, idx)    dW2 = dZ . p^T    dp = W2^T . dZ
+
+    dZ is the transpose of the gather: for every point, the sum of dz over the pixels that map to it, in fp64 in
+    ascending pixel order (``ffb6d_segment_sum``), so the gradients are bit-identical from run to run."""
+
+    @staticmethod
+    def forward(ctx, x1, p, idx, weight, bias, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn):
+        x1, p = x1.contiguous(), p.contiguous()
+        B, C1 = x1.shape[0], x1.shape[1]
+        C2, NA = p.shape[1], p.shape[2]
+        w2d = weight.reshape(weight.shape[0], -1)
+        Co = w2d.shape[0]
+        w1, w2 = w2d[:, :C1].contiguous(), w2d[:, C1:].contiguous()
+        one, zero = _ones_zeros(Co, x1.device)
+        zp = ops.fusion_mlp(p, None, w2, one, zero, relu=False, out_channels_last=True)          # [B, N', Co]
+        z = ops.fusion_mlp(x1, None, w1, one, bias if bias is not None else zero, relu=False, add=zp, add_idx=idx)
+        P = z.numel() // (B * Co)
+        y, stats = _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn)
+        # dZ feeds dW2 and dp only: without either, the backward needs no plan
+        ctx.plan = ops.segment_plan(idx, NA) if (ctx.needs_input_grad[1] or ctx.needs_input_grad[3]) else None
+        ctx.save_for_backward(x1, p, w1, w2, z, stats, gamma)
+        ctx.meta = (B, C1, C2, Co, P, NA, int(act), float(slope), bool(has_bn), bias is not None, tuple(weight.shape))
+        return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gy):
+        x1, p, w1, w2, z, stats, gamma = ctx.saved_tensors
+        B, C1, C2, Co, P, NA, act, slope, has_bn, has_bias, wshape = ctx.meta
+        dz, ggamma, gbeta = _bn_act_bwd(z, gy.contiguous(), stats, B, Co, P, act, slope, has_bn)
+        dz = dz.reshape(B, Co, P)
+        dzp = ops.segment_sum(dz, None, NA, plan=ctx.plan) if ctx.plan is not None else None     # [B, Co, N']
+        gx1 = gp = gw = gbias = None
+        if ctx.needs_input_grad[3]:
+            gw = torch.cat((_wgrad(dz, x1.reshape(B, C1, P), None, B, Co, P),
+                            _wgrad(dzp, p.reshape(B, C2, NA), None, B, Co, NA)), 1).reshape(wshape)
+        if has_bias:
+            gbias = dz.sum(dim=(0, 2))
+        if ctx.needs_input_grad[0]:
+            gx1 = _gemm(dz, None, w1.t().contiguous()).reshape(x1.shape)
+        if ctx.needs_input_grad[1]:
+            gp = _gemm(dzp, None, w2.t().contiguous()).reshape(p.shape)
+        if gamma is None:
+            ggamma = None
+        return gx1, gp, None, gw, gbias, ggamma, gbeta, None, None, None, None, None, None, None
 
 
 class _BNWrap(nn.Sequential):
@@ -177,6 +245,7 @@ class _ConvBase(nn.Module):
             self.add_module(name + "activation", activation)
         self.act, self.slope = _act_code(activation)
         self._packed = None      # (weight version, PackedWeight, scale, shift) of the eval path
+        self._split = None       # ((weight version, C1), fusion.SplitFuse) of forward_interp's eval path
 
     @property
     def _conv(self):
@@ -186,19 +255,47 @@ class _ConvBase(nn.Module):
     def _bn(self):
         return getattr(self, self._names[1]).bn if self.has_bn else None
 
-    def _eval_pack(self):
+    def _eval_version(self):
         conv, bn = self._conv, self._bn
-        ver = (conv.weight._version, conv.weight.data_ptr(), bn.weight._version if bn is not None else 0,
-               bn.running_mean._version if bn is not None else 0)
+        return (conv.weight._version, conv.weight.data_ptr(), bn.weight._version if bn is not None else 0,
+                bn.running_mean._version if bn is not None else 0)
+
+    def _eval_affine(self):
+        """The folded BatchNorm (or the conv bias) as the GEMM epilogue's per-channel (scale, shift)."""
+        conv, bn = self._conv, self._bn
+        if bn is not None:
+            return ops.fold_batchnorm(bn)
+        scale = torch.ones(conv.weight.shape[0], device=conv.weight.device)
+        return scale, (conv.bias.detach().float() if conv.bias is not None else torch.zeros_like(scale))
+
+    def _eval_pack(self):
+        ver = self._eval_version()
         if self._packed is None or self._packed[0] != ver:
-            w = conv.weight.detach()
-            if bn is not None:
-                scale, shift = ops.fold_batchnorm(bn)
-            else:
-                scale = torch.ones(w.shape[0], device=w.device)
-                shift = conv.bias.detach().float() if conv.bias is not None else torch.zeros_like(scale)
-            self._packed = (ver, ops.fusion_mlp_pack(w), scale, shift)
+            scale, shift = self._eval_affine()
+            self._packed = (ver, ops.fusion_mlp_pack(self._conv.weight.detach()), scale, shift)
         return self._packed[1:]
+
+    def _train_momentum(self, x):
+        """Training-mode BatchNorm bookkeeping before a forward, as nn.BatchNorm2d does it: rejects one value per
+        channel, counts the batch, returns the momentum to update the running statistics with."""
+        bn = self._bn
+        if x.shape[0] * math.prod(x.shape[2:]) == 1:     # as torch's BatchNorm in training
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (torch.Size((x.shape[0], bn.num_features) + tuple(x.shape[2:])),))
+        if bn.track_running_stats and bn.num_batches_tracked is not None:
+            bn.num_batches_tracked += 1
+        momentum = bn.momentum
+        if momentum is None:     # cumulative moving average, as nn.BatchNorm2d(momentum=None)
+            momentum = 1.0 / float(bn.num_batches_tracked) if bn.num_batches_tracked is not None else 0.0
+        return momentum
+
+    def _frozen_bn_act(self, z):
+        """Eval-mode BatchNorm and the activation as differentiable elementwise torch ops."""
+        bn = self._bn
+        y = F_.batch_norm(z, bn.running_mean, bn.running_var, bn.weight, bn.bias, False, 0.0, bn.eps)
+        if self.act == _ACT_RELU:
+            return torch.relu(y)
+        return F_.leaky_relu(y, self.slope) if self.act == _ACT_LEAKY else y
 
     def forward(self, x, x2=None):
         if self._dims == 1:     # [B, C, N] layers run as [B, C, N, 1]
@@ -210,14 +307,7 @@ class _ConvBase(nn.Module):
         need_grad = torch.is_grad_enabled() and (x.requires_grad or conv.weight.requires_grad or
                                                  (x2 is not None and x2.requires_grad))
         if self.training and bn is not None:
-            if x.shape[0] * math.prod(x.shape[2:]) == 1:     # as torch's BatchNorm in training
-                raise ValueError("Expected more than 1 value per channel when training, got input size %s"
-                                 % (torch.Size((x.shape[0], bn.num_features) + tuple(x.shape[2:])),))
-            if bn.track_running_stats and bn.num_batches_tracked is not None:
-                bn.num_batches_tracked += 1
-            momentum = bn.momentum
-            if momentum is None:     # cumulative moving average, as nn.BatchNorm2d(momentum=None)
-                momentum = 1.0 / float(bn.num_batches_tracked) if bn.num_batches_tracked is not None else 0.0
+            momentum = self._train_momentum(x)
             return _ConvBnActTrain.apply(x, x2, conv.weight, None, bn.weight, bn.bias, bn.running_mean, bn.running_var,
                                          bn.eps, momentum, self.act, self.slope, True)
         if need_grad and bn is None:
@@ -227,10 +317,7 @@ class _ConvBase(nn.Module):
             # eval-mode BatchNorm under autograd (fine-tuning with frozen statistics): GEMM with its backward,
             # then the per-channel affine and the activation as differentiable elementwise torch ops
             z = _ConvBnActTrain.apply(x, x2, conv.weight, None, None, None, None, None, 0.0, 0.0, _ACT_NONE, 0.0, False)
-            y = F_.batch_norm(z, bn.running_mean, bn.running_var, bn.weight, bn.bias, False, 0.0, bn.eps)
-            if self.act == _ACT_RELU:
-                return torch.relu(y)
-            return F_.leaky_relu(y, self.slope) if self.act == _ACT_LEAKY else y
+            return self._frozen_bn_act(z)
         packed, scale, shift = self._eval_pack()
         return ops.fusion_mlp(x, x2, packed, scale, shift, relu=(self.act == _ACT_RELU),
                               negative_slope=self.slope if self.act == _ACT_LEAKY else None)
@@ -245,6 +332,54 @@ class Conv2d(_ConvBase):
         if preact or tuple(stride) != (1, 1) or tuple(padding) != (0, 0) or tuple(dilation) != (1, 1):
             raise ValueError("only plain 1x1 layers (no preact / stride / padding / dilation) are implemented here")
         super().__init__(in_size, out_size, kernel_size, activation, bn, init, bias, name)
+
+    def forward_interp(self, x1, p, interp_idx):
+        """``self(x1, nearest_interpolation(p, interp_idx).view(B, -1, h, w))`` without building the interpolated
+        map (the pixel branch of FFB6D's fusion, models/ffb6d.py:246-253, 282-289, restructured as in SURVEY.md
+        §8f-3): ``W . cat(x1, p[idx]) = W1 . x1 + (W2 . p)[idx]``.  The same three modes as ``forward``:
+
+        * eval without autograd: :func:`ffb6d_b200.fusion.p2r_fuse` with the halves packed once per weight version;
+        * training: batch-statistics BatchNorm (running statistics and ``num_batches_tracked`` updated as
+          ``forward`` does), backward through the deterministic segment sum (``ffb6d_segment_sum``);
+        * eval under autograd: the restructured GEMM with its backward, then the frozen BatchNorm and the
+          activation as torch ops.
+
+        :param x1: ``[B, C1, h, w]``; :param p: ``[B, C2, N', 1]`` with C1 + C2 the layer's input width
+        :param interp_idx: ``[B, h*w, 1]`` (or ``[B, h*w]``) int32 / int64, values in ``[0, N')``
+        :return: ``[B, Co, h, w]``"""
+        conv, bn = self._conv, self._bn
+        ops._need_cuda(x1, "x1")
+        ops._need_cuda(p, "p")
+        ops._need_cuda(interp_idx, "interp_idx")
+        if x1.dim() != 4 or p.dim() != 4 or p.shape[3] != 1 or p.shape[0] != x1.shape[0]:
+            raise ValueError("forward_interp expects x1 [B,C1,h,w] and p [B,C2,N',1], got %s and %s"
+                             % (tuple(x1.shape), tuple(p.shape)))
+        B, C1, h, w = x1.shape
+        if C1 + p.shape[1] != conv.weight.shape[1]:
+            raise ValueError("the layer takes %d input channels, x1 and p have %d + %d"
+                             % (conv.weight.shape[1], C1, p.shape[1]))
+        if interp_idx.shape[0] != B or interp_idx.numel() != B * h * w:
+            raise ValueError("interp_idx must be [B, h*w, 1] = [%d, %d, 1], got %s" % (B, h * w, tuple(interp_idx.shape)))
+        idx = interp_idx.reshape(B, h * w)
+        need_grad = torch.is_grad_enabled() and (x1.requires_grad or p.requires_grad or conv.weight.requires_grad)
+        if self.training and bn is not None:
+            momentum = self._train_momentum(x1)
+            return _InterpConvBnActTrain.apply(x1, p, idx, conv.weight, None, bn.weight, bn.bias, bn.running_mean,
+                                               bn.running_var, bn.eps, momentum, self.act, self.slope, True)
+        if need_grad and bn is None:
+            return _InterpConvBnActTrain.apply(x1, p, idx, conv.weight, conv.bias, None, None, None, None, 0.0, 0.0,
+                                               self.act, self.slope, False)
+        if need_grad:
+            z = _InterpConvBnActTrain.apply(x1, p, idx, conv.weight, None, None, None, None, None, 0.0, 0.0, _ACT_NONE,
+                                            0.0, False)
+            return self._frozen_bn_act(z)
+        key = (self._eval_version(), C1)
+        if self._split is None or self._split[0] != key:
+            scale, shift = self._eval_affine()
+            self._split = (key, fusion.SplitFuse.from_weight(
+                conv.weight, scale, shift, C1, relu=(self.act == _ACT_RELU),
+                negative_slope=self.slope if self.act == _ACT_LEAKY else None))
+        return fusion.p2r_fuse(x1, p, idx, self._split[1])
 
 
 class RandLAConv2d(_ConvBase):

@@ -486,6 +486,72 @@ def fusion_mlp(x1, x2, weight, scale, shift, relu=True, negative_slope=None, add
     return out
 
 
+class SegmentPlan:
+    """The pixels of every segment of a ``[B, P]`` index map, grouped per segment in ascending order
+    (``ffb6d_segment_plan``): what :func:`segment_sum` reads.  Build it once per index map."""
+
+    def __init__(self, idx, n_segments):
+        if not isinstance(idx, torch.Tensor):
+            raise TypeError("idx must be a torch.Tensor, got %r" % type(idx))
+        if idx.dtype not in _IDX:
+            raise TypeError("idx must be int32 or int64, got %s" % idx.dtype)
+        if idx.dim() not in (2, 3) or (idx.dim() == 3 and idx.shape[2] != 1) or idx.numel() == 0:
+            raise ValueError("idx must be a non-empty [B, P] or [B, P, 1], got %s" % (tuple(idx.shape),))
+        if int(n_segments) < 1:
+            raise ValueError("n_segments must be >= 1, got %d" % int(n_segments))
+        _need_cuda(idx, "idx")
+        idx_c, i64 = _idx_arg(idx.reshape(idx.shape[0], -1), "idx")
+        self.B, self.P, self.NA = int(idx_c.shape[0]), int(idx_c.shape[1]), int(n_segments)
+        self.device = idx_c.device
+        self.nbytes = int(lib.ffb6d_segment_plan_bytes(self.B, self.P, self.NA))
+        if self.nbytes == 0:
+            raise ValueError("no segment plan for B=%d, P=%d, n_segments=%d" % (self.B, self.P, self.NA))
+        self.data = torch.empty(self.nbytes, dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            check(lib.ffb6d_segment_plan(idx_c.data_ptr(), i64, self.B, self.P, self.NA, self.data.data_ptr(),
+                                         self.nbytes, _stream(self.device)))
+
+
+def segment_plan(idx, n_segments):
+    """Plan the segment sum of the index map ``idx [B, P]`` / ``[B, P, 1]`` (int32 or int64 CUDA, values in
+    ``[0, n_segments)``; others belong to no segment).  Returns a :class:`SegmentPlan`."""
+    return SegmentPlan(idx, n_segments)
+
+
+def segment_sum(grad, idx, n_segments, plan=None):
+    """``out[b, c, s] = sum of grad[b, c, p] over the pixels p with idx[b, p] = s`` (``ffb6d_segment_sum``): the
+    backward of :func:`nearest_interpolation` with the same index, as a deterministic sum without atomics (fp64
+    in ascending pixel order, one rounding to fp32; a segment no pixel maps to gets 0).
+
+    :param grad: ``[B, C, P]`` or ``[B, C, h, w]`` (h * w = P) float32 CUDA
+    :param idx: ``[B, P]`` or ``[B, P, 1]`` int32 / int64; ignored when ``plan`` is given
+    :param plan: a :class:`SegmentPlan` of ``idx`` (reuse it across calls with the same index map)
+    :return: ``[B, C, n_segments]`` float32"""
+    if not isinstance(grad, torch.Tensor):
+        raise TypeError("grad must be a torch.Tensor, got %r" % type(grad))
+    if grad.dtype != torch.float32:
+        raise TypeError("grad must be float32, got %s" % grad.dtype)
+    if grad.dim() not in (3, 4) or grad.numel() == 0:
+        raise ValueError("grad must be a non-empty [B, C, P] or [B, C, h, w], got %s" % (tuple(grad.shape),))
+    _need_cuda(grad, "grad")
+    B, Cc = int(grad.shape[0]), int(grad.shape[1])
+    g = grad.contiguous().reshape(B, Cc, -1)
+    if plan is None:
+        plan = SegmentPlan(idx, n_segments)
+    elif not isinstance(plan, SegmentPlan):
+        raise TypeError("plan must be a SegmentPlan, got %r" % type(plan))
+    if (plan.B, plan.P, plan.NA) != (B, g.shape[2], int(n_segments)):
+        raise ValueError("plan is for B=%d, P=%d, n_segments=%d; grad has B=%d, P=%d and n_segments=%d"
+                         % (plan.B, plan.P, plan.NA, B, g.shape[2], int(n_segments)))
+    if plan.device != grad.device:
+        raise ValueError("plan lives on %s, grad on %s" % (plan.device, grad.device))
+    out = torch.empty((B, Cc, plan.NA), dtype=torch.float32, device=grad.device)
+    with torch.cuda.device(grad.device):
+        check(lib.ffb6d_segment_sum(g.data_ptr(), plan.data.data_ptr(), plan.nbytes, B, Cc, plan.P, plan.NA,
+                                    out.data_ptr(), _stream(grad.device)))
+    return out
+
+
 def att_pool(f1, f2, att):
     """Attentive-pooling core of RandLA's ``Att_pooling`` (models/RandLA/RandLANet.py:245-248):
     ``sum_k cat(f1, f2) * softmax(att, dim=3)`` over the neighbour axis.

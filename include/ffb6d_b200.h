@@ -308,6 +308,23 @@ int ffb6d_act_bwd(const float *z, const float *grad_y, int64_t n, int act, float
 int ffb6d_fusion_mlp_wgrad(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2,
                            int64_t B, int64_t Co, int64_t P, float *grad_w, ffb6d_stream_t stream);
 
+/* Backward of the gathered addend of the restructured fusion stage (ffb6d_fusion_mlp_fwd_ex with addend):
+ * the transpose of the K = 1 pixel -> point gather, a deterministic segment sum
+ *   out[b, c, s] = sum over pixels p with idx[b, p] = s of grad[b, c, p]
+ * ffb6d_segment_plan turns idx [B,P] (int32 / int64, values in [0, NA); other values belong to no segment) into a
+ * CSR per frame in `plan` (device, 16-byte aligned, ffb6d_segment_plan_bytes(B, P, NA) bytes; 0 for bad sizes):
+ * int32 offsets [NA+1], then the pixels of every segment in ascending order.  ffb6d_segment_sum reads
+ * grad [B,C,P] f32 (NCHW) and writes out [B,C,NA] f32 (NCS) with a plan made for the same B, P, NA.
+ * Every output element is written exactly once (no atomics on out; an empty segment gets 0.0); the sum runs in
+ * fp64 in plan order and is rounded once to fp32.  No allocation, no host synchronisation (capturable in a CUDA
+ * graph); bit-identical from run to run and from replay to replay.  Sizes, null pointers, plan bytes and
+ * alignment are checked before any launch (FFB6D_ERR_INVALID, text in ffb6d_last_error). */
+size_t ffb6d_segment_plan_bytes(int64_t B, int64_t P, int64_t NA);
+int ffb6d_segment_plan(const void *idx, int idx_is_i64, int64_t B, int64_t P, int64_t NA, void *plan,
+                       size_t plan_bytes, ffb6d_stream_t stream);
+int ffb6d_segment_sum(const float *grad, const void *plan, size_t plan_bytes, int64_t B, int64_t C, int64_t P,
+                      int64_t NA, float *out, ffb6d_stream_t stream);
+
 /*
  * Attentive pooling core of RandLA's Att_pooling (models/RandLA/RandLANet.py:243-248):
  *   out[b,c,n] = sum_k f[b,c,n,k] * softmax_k(att[b,c,n,:])[k],   f = cat(f1, f2) along channels

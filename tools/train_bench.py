@@ -32,6 +32,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--batch", type=int, default=0)
     ap.add_argument("--profile", action="store_true", help="print the per-kernel GPU time of one step (CUPTI) to stderr")
+    ap.add_argument("--restructured", action="store_true",
+                    help="run the pixel branch of every fusion as W1 . rgb + (W2 . p2r)[idx] (no interpolated maps)")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -50,7 +52,7 @@ def main():
     n_classes, n_kps = (2, 8) if args.config == 3 else (22, 8)
     N0 = 12288
     torch.manual_seed(0)
-    model = FFB6DFusionNet(n_classes=n_classes, n_pts=N0, n_kps=n_kps).to(dev).train()
+    model = FFB6DFusionNet(n_classes=n_classes, n_pts=N0, n_kps=n_kps, restructured=args.restructured).to(dev).train()
     n_params = sum(p.numel() for p in model.parameters())
     net = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local_rank], output_device=local_rank,
                                                     find_unused_parameters=False) if world > 1 else model
@@ -95,6 +97,7 @@ def main():
     torch.cuda.synchronize()
     if world > 1:
         dist.barrier()
+    torch.cuda.reset_peak_memory_stats(dev)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     t0 = time.perf_counter()
     e0.record()
@@ -106,6 +109,7 @@ def main():
     if world > 1:
         dist.barrier()
     ms = max(e0.elapsed_time(e1), wall)
+    peak_mb = torch.cuda.max_memory_allocated(dev) / 1e6      # over the timed steps
     (ms,) = max_over_ranks([ms], device=dev)
     if args.profile and rank == 0:
         import collections
@@ -135,7 +139,9 @@ def main():
                 "value": world * B * N0 * args.steps / (ms / 1e3), "unit": "points/s", "n_gpus": world,
                 "batch_per_gpu": B, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
                 "params": n_params, "grad_allreduce_bytes": 4 * n_params if world > 1 else 0, "loss": float(loss.detach()),
-                "finite": finite, "dtype": "f32", "data": "synthetic", "scaling": "weak"}
+                "finite": finite, "dtype": "f32", "data": "synthetic", "scaling": "weak",
+                "restructured": args.restructured, "max_memory_allocated_mb": peak_mb,
+                "gpu": torch.cuda.get_device_name(dev)}
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
