@@ -76,6 +76,15 @@ def _load():
         "ffb6d_segment_plan_bytes": (sz, [i64, i64, i64]),
         "ffb6d_segment_plan": (ci, [vp, ci, i64, i64, i64, vp, sz, vp]),
         "ffb6d_segment_sum": (ci, [vp, vp, sz, i64, i64, i64, i64, vp, vp]),
+        "ffb6d_segment_csr_bytes": (sz, [i64, i64, i64]),
+        "ffb6d_segment_csr": (ci, [vp, ci, i64, i64, i64, vp, sz, vp]),
+        "ffb6d_segment_sum_csr": (ci, [vp, vp, sz, i64, i64, i64, i64, vp, vp]),
+        "ffb6d_gather_max_bwd_det_workspace_bytes": (sz, [i64, i64, i64, i64, ci]),
+        "ffb6d_gather_max_bwd_det": (ci, [vp, vp, ci, vp, i64, i64, i64, i64, ci, ci, vp, sz, vp, vp]),
+        "ffb6d_gather_neighbour_bwd_det_workspace_bytes": (sz, [i64, i64, i64, ci]),
+        "ffb6d_gather_neighbour_bwd_det": (ci, [vp, vp, ci, i64, i64, i64, i64, ci, vp, sz, vp, vp]),
+        "ffb6d_fusion_mlp_wgrad_det_workspace_bytes": (sz, [i64, i64, i64, i64, i64]),
+        "ffb6d_fusion_mlp_wgrad_det": (ci, [vp, vp, i64, vp, i64, i64, i64, i64, vp, sz, vp, vp]),
         "ffb6d_att_pool_bwd": (ci, [vp, i64, vp, i64, vp, vp, i64, i64, ci, vp, vp, vp, vp]),
         "ffb6d_lfa_att_pool_fused": (ci, [vp, vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i64, ci, i64, i64, fp, vp, vp]),
         "ffb6d_att_pool_fwd": (ci, [vp, i64, vp, i64, vp, i64, i64, ci, vp, vp]),

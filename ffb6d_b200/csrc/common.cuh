@@ -74,6 +74,11 @@ static inline int num_sms() { return device_info().num_sms; }
 // train.cu: weight gradient of narrow layers (used by ffb6d_fusion_mlp_wgrad, fusion_mlp.cu)
 int wgrad_small_launch(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2, int64_t B, int64_t Co,
                        int64_t P, float *grad_w, cudaStream_t st);
+// ... and of ffb6d_fusion_mlp_wgrad_det: its split count (SM count dependent), and the launch that stores each split's
+// partial into part + split * Co * (C1 + C2)
+int64_t wgrad_small_splits(int64_t B, int64_t P);
+int wgrad_small_det_launch(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2, int64_t B,
+                           int64_t Co, int64_t P, float *part, cudaStream_t st);
 
 // Experiment switches, read ONCE per process (never in a launch path; results never depend on them).
 struct Env {

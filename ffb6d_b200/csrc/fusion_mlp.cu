@@ -353,9 +353,12 @@ fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__re
 // added into round-to-nearest fp32 register sums.  Split-K over the grid's z axis: every CTA owns a run of
 // (frame, 32-point) k-tiles and adds its 128x128 partial to dW with fp32 atomics (dW is zero-filled by the
 // entry point), like cuDNN's own wgrad: summation order is not deterministic, values agree to fp32 round-off.
-__global__ void __launch_bounds__(MLP_THREADS, 1)
-fusion_wgrad_kernel(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
-                    float *__restrict__ dw, int Co, int P, int tiles_per_frame, int total_tiles, int tiles_per_split)
+// DET (fusion_wgrad_det_kernel, ffb6d_fusion_mlp_wgrad_det): the same CTA stores its partial into its own slice
+// dw + blockIdx.z * Co * Ci instead; wgrad_split_reduce_kernel adds the slices in split order.
+template <bool DET>
+__device__ __forceinline__ void
+fusion_wgrad_body(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
+                  float *__restrict__ dw, int Co, int P, int tiles_per_frame, int total_tiles, int tiles_per_split)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31, wg = tid >> 7;
@@ -425,6 +428,7 @@ fusion_wgrad_kernel(const float *__restrict__ dz, const float *__restrict__ x1, 
     }
     drain(acc, sum);
     const int row0 = m0 + 64 * wg + 16 * (wid & 3) + (lane >> 2), col0 = n0 + 2 * (lane & 3);
+    if (DET) dw += (size_t)blockIdx.z * Co * Ci;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int gm = row0 + 8 * h;
@@ -435,9 +439,52 @@ fusion_wgrad_kernel(const float *__restrict__ dz, const float *__restrict__ x1, 
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
                 const int gn = col0 + 8 * i + u;
-                if (gn < Ci) atomicAdd(row + gn, sum[4 * i + 2 * h + u]);
+                if (gn < Ci) {
+                    if (DET)
+                        row[gn] = sum[4 * i + 2 * h + u];
+                    else
+                        atomicAdd(row + gn, sum[4 * i + 2 * h + u]);
+                }
             }
     }
+}
+
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+fusion_wgrad_kernel(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
+                    float *__restrict__ dw, int Co, int P, int tiles_per_frame, int total_tiles, int tiles_per_split)
+{
+    fusion_wgrad_body<false>(dz, x1, C1, x2, C2, dw, Co, P, tiles_per_frame, total_tiles, tiles_per_split);
+}
+
+// dw = the workspace of ffb6d_fusion_mlp_wgrad_det: one [Co, Ci] slice per split
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+fusion_wgrad_det_kernel(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2,
+                        int C2, float *__restrict__ dw, int Co, int P, int tiles_per_frame, int total_tiles, int tiles_per_split)
+{
+    fusion_wgrad_body<true>(dz, x1, C1, x2, C2, dw, Co, P, tiles_per_frame, total_tiles, tiles_per_split);
+}
+
+// dw[i] = the fp64 sum of part[s * n + i] over s = 0 .. nsplit-1 in that order, rounded once
+__global__ void __launch_bounds__(256)
+wgrad_split_reduce_kernel(const float *__restrict__ part, int nsplit, long long n, float *__restrict__ dw)
+{
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    double acc = 0.0;
+    for (int s = 0; s < nsplit; ++s) acc += (double)__ldg(part + (size_t)s * n + i);
+    dw[i] = (float)acc;
+}
+
+// split count of fusion_wgrad_kernel (a function of the shape and the SM count only)
+static int64_t wgrad_splits(int64_t B, int64_t Co, int64_t Ci, int64_t P, int64_t &per)
+{
+    const int64_t tpf = ceil_div(P, TK), total = B * tpf;
+    const int64_t tiles = ceil_div(Ci, TN) * ceil_div(Co, TM);
+    // split K so that the grid fills the SMs about twice, but keep at least 8 k-tiles (one chunk pair) per CTA
+    int64_t splits = std::max<int64_t>(1, std::min<int64_t>(ceil_div(2 * (int64_t)num_sms(), tiles), ceil_div(total, 8)));
+    if (splits > 65535) splits = 65535;
+    per = ceil_div(total, splits);
+    return ceil_div(total, per);
 }
 
 }  // namespace ffb6d
@@ -559,15 +606,71 @@ extern "C" int ffb6d_fusion_mlp_wgrad(const float *grad_z, const float *x1, int6
     FFB6D_OPTIN_SMEM(fusion_wgrad_kernel, MLP_SMEM);
     const int64_t tpf = ceil_div(P, TK), total = B * tpf;
     FFB6D_CHECK_ARG(total < (1ll << 31), "fusion_mlp_wgrad: B * P too large");
-    const int64_t tiles = ceil_div(Ci, TN) * ceil_div(Co, TM);
-    // split K so that the grid fills the SMs about twice, but keep at least 8 k-tiles (one chunk pair) per CTA
-    int64_t splits = std::max<int64_t>(1, std::min<int64_t>(ceil_div(2 * (int64_t)num_sms(), tiles), ceil_div(total, 8)));
-    if (splits > 65535) splits = 65535;
-    const int64_t per = ceil_div(total, splits);
-    splits = ceil_div(total, per);
+    int64_t per = 0;
+    const int64_t splits = wgrad_splits(B, Co, Ci, P, per);
     dim3 grid((unsigned)ceil_div(Ci, TN), (unsigned)ceil_div(Co, TM), (unsigned)splits);
     fusion_wgrad_kernel<<<grid, MLP_THREADS, MLP_SMEM, st>>>(grad_z, x1, (int)C1, C2 ? x2 : nullptr, (int)C2, grad_w, (int)Co, (int)P,
                                                     (int)tpf, (int)total, (int)per);
     FFB6D_LAUNCH_OK("fusion_wgrad_kernel");
+    return FFB6D_OK;
+}
+
+static bool wgrad_det_sizes_ok(int64_t C1, int64_t C2, int64_t B, int64_t Co, int64_t P)
+{
+    return B >= 1 && C1 >= 1 && C2 >= 0 && Co >= 1 && P >= 1 && B < 65536 && Co <= 65535ll * TM && C1 + C2 <= 65535ll * TN &&
+           P < (1ll << 31) && B * ceil_div(P, TK) < (1ll << 31);
+}
+
+extern "C" size_t ffb6d_fusion_mlp_wgrad_det_workspace_bytes(int64_t C1, int64_t C2, int64_t B, int64_t Co, int64_t P)
+{
+    if (!wgrad_det_sizes_ok(C1, C2, B, Co, P)) return 0;
+    const int64_t Ci = C1 + C2;
+    int64_t per = 0;
+    const int64_t splits = (Co <= 64 && Ci <= 64) ? wgrad_small_splits(B, P) : wgrad_splits(B, Co, Ci, P, per);
+    return align_up((size_t)splits * Co * Ci * sizeof(float), 16);
+}
+
+extern "C" int ffb6d_fusion_mlp_wgrad_det(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2,
+                                          int64_t B, int64_t Co, int64_t P, void *workspace, size_t workspace_bytes,
+                                          float *grad_w, ffb6d_stream_t stream)
+{
+    FFB6D_CHECK_ARG(B >= 0 && C1 >= 1 && C2 >= 0 && Co >= 1 && P >= 0, "fusion_mlp_wgrad_det: bad size");
+    FFB6D_CHECK_ARG(B < 65536 && Co <= 65535ll * TM && C1 + C2 <= 65535ll * TN && P < (1ll << 31),
+                    "fusion_mlp_wgrad_det: size too large");
+    FFB6D_CHECK_ARG(grad_w, "fusion_mlp_wgrad_det: null grad_w");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t Ci = C1 + C2;
+    if (B == 0 || P == 0) {
+        FFB6D_CUDA(cudaMemsetAsync(grad_w, 0, (size_t)Co * Ci * sizeof(float), st));
+        return FFB6D_OK;
+    }
+    FFB6D_CHECK_ARG(wgrad_det_sizes_ok(C1, C2, B, Co, P), "fusion_mlp_wgrad_det: B * P too large");
+    FFB6D_CHECK_ARG(grad_z && x1 && (C2 == 0 || x2) && workspace, "fusion_mlp_wgrad_det: null pointer");
+    FFB6D_CHECK_ARG(((reinterpret_cast<uintptr_t>(grad_z) | reinterpret_cast<uintptr_t>(x1) | reinterpret_cast<uintptr_t>(x2) |
+                      reinterpret_cast<uintptr_t>(grad_w)) & 3) == 0,
+                    "fusion_mlp_wgrad_det: grad_z, x1, x2 and grad_w must be 4-byte aligned");
+    FFB6D_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "fusion_mlp_wgrad_det: workspace must be 16-byte aligned");
+    const size_t need = ffb6d_fusion_mlp_wgrad_det_workspace_bytes(C1, C2, B, Co, P);
+    FFB6D_CHECK_ARG(workspace_bytes >= need, "fusion_mlp_wgrad_det: workspace too small (%zu bytes required, %zu given)", need,
+                    workspace_bytes);
+    float *part = (float *)workspace;
+    int64_t splits;
+    if (Co <= 64 && Ci <= 64) {
+        splits = wgrad_small_splits(B, P);
+        const int rc = wgrad_small_det_launch(grad_z, x1, C1, x2, C2, B, Co, P, part, st);
+        if (rc != FFB6D_OK) return rc;
+    } else {
+        FFB6D_OPTIN_SMEM(fusion_wgrad_det_kernel, MLP_SMEM);
+        int64_t per = 0;
+        splits = wgrad_splits(B, Co, Ci, P, per);
+        dim3 grid((unsigned)ceil_div(Ci, TN), (unsigned)ceil_div(Co, TM), (unsigned)splits);
+        fusion_wgrad_det_kernel<<<grid, MLP_THREADS, MLP_SMEM, st>>>(grad_z, x1, (int)C1, C2 ? x2 : nullptr, (int)C2, part,
+                                                                     (int)Co, (int)P, (int)ceil_div(P, TK),
+                                                                     (int)(B * ceil_div(P, TK)), (int)per);
+        FFB6D_LAUNCH_OK("fusion_wgrad_det_kernel");
+    }
+    const long long n = (long long)Co * Ci;
+    wgrad_split_reduce_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(part, (int)splits, n, grad_w);
+    FFB6D_LAUNCH_OK("wgrad_split_reduce_kernel");
     return FFB6D_OK;
 }

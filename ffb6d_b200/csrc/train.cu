@@ -286,10 +286,12 @@ att_pool_bwd_kernel(const float *__restrict__ f1, int C1, const float *__restric
 constexpr int WS_TP = 64;    // positions per slab
 // T = tile edge (16, 32, 64: the smallest that holds Co and Ci); a thread owns a (T/16) x (T/16) block of dW and
 // walks the slab four positions at a time with 128-bit shared-memory loads.
-template <int T>
-__global__ void __launch_bounds__(256)
-wgrad_small_kernel(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
-                   float *__restrict__ dw, int Co, int P, int B, int slabs_per_cta)
+// DET (wgrad_small_det_kernel): the CTA stores its whole partial, zeros included, into its own slice
+// dw + blockIdx.x * Co * Ci instead of adding it.
+template <int T, bool DET>
+__device__ __forceinline__ void
+wgrad_small_body(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
+                 float *__restrict__ dw, int Co, int P, int B, int slabs_per_cta)
 {
     constexpr int R = T / 16;                    // rows of dz / x per thread
     constexpr int LD = WS_TP + 4;                // row stride: 16-byte aligned rows, conflict-free 128-bit loads
@@ -330,13 +332,34 @@ wgrad_small_kernel(const float *__restrict__ dz, const float *__restrict__ x1, i
                     acc[i][j] = fmaf(a[i].x, c[j].x, fmaf(a[i].y, c[j].y, fmaf(a[i].z, c[j].z, fmaf(a[i].w, c[j].w, acc[i][j]))));
         }
     }
+    if (DET) dw += (size_t)blockIdx.x * Co * Ci;
 #pragma unroll
     for (int i = 0; i < R; ++i)
 #pragma unroll
         for (int j = 0; j < R; ++j) {
             const int co = R * ty + i, ci = R * tx + j;
-            if (co < Co && ci < Ci && acc[i][j] != 0.f) atomicAdd(dw + (size_t)co * Ci + ci, acc[i][j]);
+            if (DET) {
+                if (co < Co && ci < Ci) dw[(size_t)co * Ci + ci] = acc[i][j];
+            } else if (co < Co && ci < Ci && acc[i][j] != 0.f) {
+                atomicAdd(dw + (size_t)co * Ci + ci, acc[i][j]);
+            }
         }
+}
+
+template <int T>
+__global__ void __launch_bounds__(256)
+wgrad_small_kernel(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
+                   float *__restrict__ dw, int Co, int P, int B, int slabs_per_cta)
+{
+    wgrad_small_body<T, false>(dz, x1, C1, x2, C2, dw, Co, P, B, slabs_per_cta);
+}
+
+template <int T>
+__global__ void __launch_bounds__(256)
+wgrad_small_det_kernel(const float *__restrict__ dz, const float *__restrict__ x1, int C1, const float *__restrict__ x2,
+                       int C2, float *__restrict__ part, int Co, int P, int B, int slabs_per_cta)
+{
+    wgrad_small_body<T, true>(dz, x1, C1, x2, C2, part, Co, P, B, slabs_per_cta);
 }
 
 static void split_plan(int64_t C, int64_t P, int &chunk, int &nsplit)
@@ -349,14 +372,42 @@ static void split_plan(int64_t C, int64_t P, int &chunk, int &nsplit)
     nsplit = (int)ceil_div(P, ch);
 }
 
+// slabs per CTA and CTAs of the narrow-layer weight gradient: about four CTAs per SM
+static int wgrad_small_per(int64_t B, int64_t P)
+{
+    const long long slabs = ceil_div(P, WS_TP) * B;
+    return (int)std::max<long long>(1, ceil_div(slabs, 4ll * num_sms()));
+}
+
+int64_t wgrad_small_splits(int64_t B, int64_t P)
+{
+    return ceil_div(ceil_div(P, WS_TP) * B, wgrad_small_per(B, P));
+}
+
+// ffb6d_fusion_mlp_wgrad_det's narrow layers: the same CTAs, each storing its partial into its slice of part
+int wgrad_small_det_launch(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2, int64_t B,
+                           int64_t Co, int64_t P, float *part, cudaStream_t st)
+{
+    const int per = wgrad_small_per(B, P);
+    const unsigned grid = (unsigned)wgrad_small_splits(B, P);
+    const int64_t m = std::max<int64_t>(Co, C1 + C2);
+    if (m <= 16)
+        wgrad_small_det_kernel<16><<<grid, 256, 0, st>>>(grad_z, x1, (int)C1, C2 ? x2 : nullptr, (int)C2, part, (int)Co, (int)P, (int)B, per);
+    else if (m <= 32)
+        wgrad_small_det_kernel<32><<<grid, 256, 0, st>>>(grad_z, x1, (int)C1, C2 ? x2 : nullptr, (int)C2, part, (int)Co, (int)P, (int)B, per);
+    else
+        wgrad_small_det_kernel<64><<<grid, 256, 0, st>>>(grad_z, x1, (int)C1, C2 ? x2 : nullptr, (int)C2, part, (int)Co, (int)P, (int)B, per);
+    FFB6D_LAUNCH_OK("wgrad_small_det_kernel");
+    return FFB6D_OK;
+}
+
 // narrow layers (Co, Ci <= 64) of ffb6d_fusion_mlp_wgrad: CUDA-core streaming reduction
 int wgrad_small_launch(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2, int64_t B, int64_t Co,
                       int64_t P, float *grad_w, cudaStream_t st_in)
 {
     cudaStream_t st = st_in;
-    const long long slabs = ceil_div(P, WS_TP) * B;
-    const int per = (int)std::max<long long>(1, ceil_div(slabs, 4ll * num_sms()));
-    const unsigned grid = (unsigned)ceil_div(slabs, per);
+    const int per = wgrad_small_per(B, P);
+    const unsigned grid = (unsigned)wgrad_small_splits(B, P);
     const int64_t m = std::max<int64_t>(Co, C1 + C2);
     if (m <= 16)
         wgrad_small_kernel<16><<<grid, 256, 0, st>>>(grad_z, x1, (int)C1, C2 ? x2 : nullptr, (int)C2, grad_w, (int)Co, (int)P, (int)B, per);

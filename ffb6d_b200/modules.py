@@ -14,7 +14,9 @@ Both modes run on the CUDA library:
 * ``train()``: batch-statistics BatchNorm and autograd -- forward = GEMM (wgmma) + ``ffb6d_bn_train_fwd``
   (running statistics updated like ``nn.BatchNorm2d``); backward = ``ffb6d_bn_train_bwd``, weight gradient
   ``ffb6d_fusion_mlp_wgrad`` (wgmma, split-K), input gradient = the forward GEMM with the transposed
-  weight; neighbour gathers and attentive pooling have their own backward kernels.
+  weight; neighbour gathers and attentive pooling have their own backward kernels.  Under
+  ``torch.use_deterministic_algorithms(True)`` (or, for the weight gradients only, ``torch.backends.cudnn.deterministic``)
+  the backwards that add with atomics take their run-to-run deterministic paths (:func:`ops.deterministic_backward`).
 
 A layer accepts its input as one tensor or as the two halves of a concat (``layer(x1, x2)`` ==
 ``layer(torch.cat((x1, x2), 1))`` without materialising the concat, models/ffb6d.py:251-262).
@@ -102,10 +104,18 @@ def _bn_act_bwd(z, gy, stats, B, Co, P, act, slope, has_bn):
 
 
 def _wgrad(dz, x1, x2, B, Co, P):
-    """dW [Co, C1+C2] = sum over frames of dz [B, Co, P] . cat(x1, x2)^T (``ffb6d_fusion_mlp_wgrad``)."""
+    """dW [Co, C1+C2] = sum over frames of dz [B, Co, P] . cat(x1, x2)^T (``ffb6d_fusion_mlp_wgrad``; under
+    :func:`ffb6d_b200.ops.deterministic_backward` ``ffb6d_fusion_mlp_wgrad_det``, the splits added in a fixed order)."""
     C1, C2 = x1.shape[1], (x2.shape[1] if x2 is not None else 0)
     gw = torch.empty((Co, C1 + C2), dtype=torch.float32, device=dz.device)
     with torch.cuda.device(dz.device):
+        if ops.deterministic_backward(weight_grad=True):
+            nbytes = int(lib.ffb6d_fusion_mlp_wgrad_det_workspace_bytes(C1, C2, B, Co, P))
+            ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dz.device)
+            check(lib.ffb6d_fusion_mlp_wgrad_det(dz.data_ptr(), x1.data_ptr(), C1,
+                                                 x2.data_ptr() if x2 is not None else None, C2, B, Co, P, ws.data_ptr(),
+                                                 nbytes, gw.data_ptr(), ops._stream(dz.device)))
+            return gw
         check(lib.ffb6d_fusion_mlp_wgrad(dz.data_ptr(), x1.data_ptr(), C1, x2.data_ptr() if x2 is not None else None,
                                          C2, B, Co, P, gw.data_ptr(), ops._stream(dz.device)))
     return gw

@@ -32,6 +32,19 @@ def _need_cuda(t, name):
         raise RuntimeError("%s must be a CUDA tensor: ffb6d_b200 has no CPU path" % name)
 
 
+def deterministic_backward(weight_grad=False):
+    """Whether a backward should take its deterministic path, decided when the backward runs (as torch decides for
+    its own ops).  ``torch.use_deterministic_algorithms(True)`` turns it on for every backward of this package that
+    otherwise adds with atomics (gathers, neighbour gathers, layer weight gradients).  With ``weight_grad=True`` --
+    the 1x1 layers, which stand in for cuDNN convolutions -- ``torch.backends.cudnn.deterministic`` does too: it is
+    the flag the reference's ``--deterministic`` sets.  Like ``torch.gather``'s backward, the gathers do not follow
+    ``cudnn.deterministic`` alone.  The deterministic paths write every output once, in a fixed order, and are
+    bit-identical from run to run; the default paths are unchanged."""
+    if torch.are_deterministic_algorithms_enabled():
+        return True
+    return bool(weight_grad) and bool(torch.backends.cudnn.deterministic)
+
+
 def _idx_arg(idx, name):
     if idx.dtype not in _IDX:
         raise TypeError("%s must be int32 or int64, got %s" % (name, idx.dtype))
@@ -218,20 +231,50 @@ class _GatherMax(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, gout):
         f3, idx_c = ctx.saved_tensors
-        layout = ctx.layout
-        B, Cc, S = f3.shape
-        Q, K = idx_c.shape[1], idx_c.shape[2]
-        if layout == LAYOUT_NCS:
-            g = gout.contiguous()
-            gf = torch.empty((B, Cc, S), dtype=torch.float32, device=f3.device)
-        else:
-            g = gout.transpose(1, 2).contiguous().transpose(1, 2)   # dense [B,Q,C] storage
-            gf = torch.empty((B, S, Cc), dtype=torch.float32, device=f3.device).transpose(1, 2)
-        with torch.cuda.device(f3.device):
-            check(lib.ffb6d_gather_max_bwd(f3.data_ptr(), idx_c.data_ptr(),
-                                           int(idx_c.dtype == torch.int64), g.data_ptr(), B, Cc, S,
-                                           Q, K, layout, gf.data_ptr(), _stream(f3.device)))
-        return gf, None
+        return _gather_max_bwd(f3, idx_c, gout, ctx.layout), None
+
+
+def _gather_max_bwd(f3, idx_c, gout, layout):
+    """The gradient of :class:`_GatherMax` w.r.t. ``f3`` (in f3's layout): ``ffb6d_gather_max_bwd`` (fp32 atomics), or
+    under :func:`deterministic_backward` a segment sum over the CSR of the index (``ffb6d_gather_max_bwd_det``)."""
+    B, Cc, S = f3.shape
+    Q, K = idx_c.shape[1], idx_c.shape[2]
+    if layout == LAYOUT_NCS:
+        g = gout.contiguous()
+        gf = torch.empty((B, Cc, S), dtype=torch.float32, device=f3.device)
+    else:
+        g = gout.transpose(1, 2).contiguous().transpose(1, 2)   # dense [B,Q,C] storage
+        gf = torch.empty((B, S, Cc), dtype=torch.float32, device=f3.device).transpose(1, 2)
+    if deterministic_backward():
+        if K == 1 and layout == LAYOUT_NCS and _counter_plan_fits(Q, S):
+            return segment_sum(g, None, S, plan=SegmentPlan(idx_c.reshape(B, Q), S))
+        _gather_max_bwd_det(f3, idx_c, g, layout, gf)
+        return gf
+    with torch.cuda.device(f3.device):
+        check(lib.ffb6d_gather_max_bwd(f3.data_ptr(), idx_c.data_ptr(),
+                                       int(idx_c.dtype == torch.int64), g.data_ptr(), B, Cc, S,
+                                       Q, K, layout, gf.data_ptr(), _stream(f3.device)))
+    return gf
+
+
+def _counter_plan_fits(P, NA):
+    """True when the (segment, 1024-entry tile) counters of :class:`SegmentPlan` take no more room than the
+    linear :class:`SegmentCSR`: few segments, as in the p2r maps.  Both give the same CSR, so this choice changes
+    speed only, never a result."""
+    return NA * -(-P // 1024) <= P + NA
+
+
+def _gather_max_bwd_det(f3, idx_c, g, layout, gf):
+    """``ffb6d_gather_max_bwd_det`` into ``gf`` (the backward of :class:`_GatherMax` without atomics)."""
+    B, Cc, S = f3.shape
+    Q, K = idx_c.shape[1], idx_c.shape[2]
+    dev = f3.device
+    with torch.cuda.device(dev):
+        nbytes = int(lib.ffb6d_gather_max_bwd_det_workspace_bytes(B, Cc, S, Q, K))
+        ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+        check(lib.ffb6d_gather_max_bwd_det(f3.data_ptr(), idx_c.data_ptr(), int(idx_c.dtype == torch.int64),
+                                           g.data_ptr(), B, Cc, S, Q, K, layout, ws.data_ptr(), nbytes,
+                                           gf.data_ptr(), _stream(dev)))
 
 
 def _gather_max(feature, idx3):
@@ -327,6 +370,14 @@ class _GatherNeighbour(torch.autograd.Function):
         N, K = idx_c.shape[1], idx_c.shape[2]
         g = gout.contiguous()
         gpc = torch.empty((B, S, D), dtype=torch.float32, device=g.device)
+        if deterministic_backward():
+            with torch.cuda.device(g.device):
+                nbytes = int(lib.ffb6d_gather_neighbour_bwd_det_workspace_bytes(B, S, N, K))
+                ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=g.device)
+                check(lib.ffb6d_gather_neighbour_bwd_det(g.data_ptr(), idx_c.data_ptr(), int(idx_c.dtype == torch.int64),
+                                                         B, S, D, N, K, ws.data_ptr(), nbytes, gpc.data_ptr(),
+                                                         _stream(g.device)))
+            return gpc, None
         with torch.cuda.device(g.device):
             check(lib.ffb6d_gather_neighbour_bwd(g.data_ptr(), idx_c.data_ptr(),
                                                  int(idx_c.dtype == torch.int64), B, S, D, N, K,
@@ -489,6 +540,7 @@ def fusion_mlp(x1, x2, weight, scale, shift, relu=True, negative_slope=None, add
 class SegmentPlan:
     """The pixels of every segment of a ``[B, P]`` index map, grouped per segment in ascending order
     (``ffb6d_segment_plan``): what :func:`segment_sum` reads.  Build it once per index map."""
+    _bytes, _build, _sum = "ffb6d_segment_plan_bytes", "ffb6d_segment_plan", "ffb6d_segment_sum"
 
     def __init__(self, idx, n_segments):
         if not isinstance(idx, torch.Tensor):
@@ -503,19 +555,38 @@ class SegmentPlan:
         idx_c, i64 = _idx_arg(idx.reshape(idx.shape[0], -1), "idx")
         self.B, self.P, self.NA = int(idx_c.shape[0]), int(idx_c.shape[1]), int(n_segments)
         self.device = idx_c.device
-        self.nbytes = int(lib.ffb6d_segment_plan_bytes(self.B, self.P, self.NA))
+        self.nbytes = int(getattr(lib, self._bytes)(self.B, self.P, self.NA))
         if self.nbytes == 0:
             raise ValueError("no segment plan for B=%d, P=%d, n_segments=%d" % (self.B, self.P, self.NA))
         self.data = torch.empty(self.nbytes, dtype=torch.uint8, device=self.device)
         with torch.cuda.device(self.device):
-            check(lib.ffb6d_segment_plan(idx_c.data_ptr(), i64, self.B, self.P, self.NA, self.data.data_ptr(),
-                                         self.nbytes, _stream(self.device)))
+            check(getattr(lib, self._build)(idx_c.data_ptr(), i64, self.B, self.P, self.NA, self.data.data_ptr(),
+                                            self.nbytes, _stream(self.device)))
+
+    def csr(self):
+        """``(offsets [B, n_segments+1], entries [B, P])`` int32 views of the plan; entries past
+        ``offsets[b, -1]`` (positions with an out-of-range index) are unspecified."""
+        words = self.data.view(torch.int32).view(self.B, -1)
+        return words[:, :self.NA + 1], words[:, self.NA + 1:self.NA + 1 + self.P]
+
+
+class SegmentCSR(SegmentPlan):
+    """The same CSR as :class:`SegmentPlan`, built in work and memory linear in P + n_segments
+    (``ffb6d_segment_csr``: counts, a device-wide scan, atomic placement, a sort per segment) where SegmentPlan
+    keeps n_segments x ceil(P/1024) counters.  For index maps with many segments: the gathers of a training step."""
+    _bytes, _build, _sum = "ffb6d_segment_csr_bytes", "ffb6d_segment_csr", "ffb6d_segment_sum_csr"
 
 
 def segment_plan(idx, n_segments):
     """Plan the segment sum of the index map ``idx [B, P]`` / ``[B, P, 1]`` (int32 or int64 CUDA, values in
     ``[0, n_segments)``; others belong to no segment).  Returns a :class:`SegmentPlan`."""
     return SegmentPlan(idx, n_segments)
+
+
+def segment_csr(idx, n_segments):
+    """:func:`segment_plan` in work and memory linear in P + n_segments; returns a :class:`SegmentCSR`, which
+    :func:`segment_sum` takes as its ``plan``."""
+    return SegmentCSR(idx, n_segments)
 
 
 def segment_sum(grad, idx, n_segments, plan=None):
@@ -525,7 +596,8 @@ def segment_sum(grad, idx, n_segments, plan=None):
 
     :param grad: ``[B, C, P]`` or ``[B, C, h, w]`` (h * w = P) float32 CUDA
     :param idx: ``[B, P]`` or ``[B, P, 1]`` int32 / int64; ignored when ``plan`` is given
-    :param plan: a :class:`SegmentPlan` of ``idx`` (reuse it across calls with the same index map)
+    :param plan: a :class:`SegmentPlan` or :class:`SegmentCSR` of ``idx`` (reuse it across calls with the same
+      index map); without one, a SegmentPlan is built
     :return: ``[B, C, n_segments]`` float32"""
     if not isinstance(grad, torch.Tensor):
         raise TypeError("grad must be a torch.Tensor, got %r" % type(grad))
@@ -547,8 +619,8 @@ def segment_sum(grad, idx, n_segments, plan=None):
         raise ValueError("plan lives on %s, grad on %s" % (plan.device, grad.device))
     out = torch.empty((B, Cc, plan.NA), dtype=torch.float32, device=grad.device)
     with torch.cuda.device(grad.device):
-        check(lib.ffb6d_segment_sum(g.data_ptr(), plan.data.data_ptr(), plan.nbytes, B, Cc, plan.P, plan.NA,
-                                    out.data_ptr(), _stream(grad.device)))
+        check(getattr(lib, plan._sum)(g.data_ptr(), plan.data.data_ptr(), plan.nbytes, B, Cc, plan.P, plan.NA,
+                                      out.data_ptr(), _stream(grad.device)))
     return out
 
 

@@ -194,7 +194,7 @@ const char *ffb6d_gather_kernel_name(int64_t B, int64_t C, int64_t S, int64_t Q,
  * Backward of the above as autograd defines it for gather + max: grad_feat is
  * zero-filled, then grad_out[b,c,q] is added at the arg-max neighbour (the first
  * maximal k).  fp32 atomic adds: summation order is not deterministic, exactly
- * as the reference's torch.gather backward on CUDA.
+ * as the reference's torch.gather backward on CUDA (ffb6d_gather_max_bwd_det below is the deterministic one).
  */
 int ffb6d_gather_max_bwd(const float *feat, const void *idx, int idx_is_i64,
                          const float *grad_out,
@@ -324,6 +324,46 @@ int ffb6d_segment_plan(const void *idx, int idx_is_i64, int64_t B, int64_t P, in
                        size_t plan_bytes, ffb6d_stream_t stream);
 int ffb6d_segment_sum(const float *grad, const void *plan, size_t plan_bytes, int64_t B, int64_t C, int64_t P,
                       int64_t NA, float *out, ffb6d_stream_t stream);
+
+/* Deterministic backward (what a caller runs when torch.use_deterministic_algorithms(True) is set; the atomic
+ * entry points above and below stay as they are).  None of these allocates or synchronises with the host: they can
+ * be captured in a CUDA graph, and their results are bit-identical from run to run and from replay to replay.
+ * Sizes, null pointers, alignment, workspace bytes and idx_is_i64 are checked before any launch (FFB6D_ERR_INVALID).
+ *
+ * ffb6d_segment_csr builds the CSR of ffb6d_segment_plan -- int32 offsets [NA+1], then the entries of every segment
+ * in ascending position; out-of-range indices belong to no segment -- in work and memory linear in P + NA (the
+ * plan above keeps NA x ceil(P/1024) counters).  Frame b starts at byte b * ffb6d_segment_csr_bytes(1, P, NA) of
+ * `plan` (16-byte aligned); scratch follows the entries.  ffb6d_segment_sum_csr is ffb6d_segment_sum on that
+ * layout (same kernel, same results). */
+size_t ffb6d_segment_csr_bytes(int64_t B, int64_t P, int64_t NA);
+int ffb6d_segment_csr(const void *idx, int idx_is_i64, int64_t B, int64_t P, int64_t NA, void *plan,
+                      size_t plan_bytes, ffb6d_stream_t stream);
+int ffb6d_segment_sum_csr(const float *grad, const void *plan, size_t plan_bytes, int64_t B, int64_t C, int64_t P,
+                          int64_t NA, float *out, ffb6d_stream_t stream);
+/* ffb6d_gather_max_bwd without atomics: grad_feat[b,c,s] = the sum of grad_out[b,c,q] over the rows q whose
+ * arg-max neighbour (the rule of ffb6d_gather_max_bwd: a NaN wins, else the first strict maximum) is s.  A CSR of
+ * idx flattened to [B, Q*K] and, for K > 1, a uint8 arg-max map go into `workspace` (16-byte aligned,
+ * ffb6d_gather_max_bwd_det_workspace_bytes; 0 for bad sizes); the sum runs in fp64 in ascending (q, k) and is
+ * rounded once; every element of grad_feat is written once (0.0 where nothing lands).  Layouts as the atomic one. */
+size_t ffb6d_gather_max_bwd_det_workspace_bytes(int64_t B, int64_t C, int64_t S, int64_t Q, int K);
+int ffb6d_gather_max_bwd_det(const float *feat, const void *idx, int idx_is_i64, const float *grad_out,
+                             int64_t B, int64_t C, int64_t S, int64_t Q, int K, int layout, void *workspace,
+                             size_t workspace_bytes, float *grad_feat, ffb6d_stream_t stream);
+/* ffb6d_gather_neighbour_bwd without atomics: the CSR of idx [B, N*K] and the segment sum over the channels of
+ * grad_out [B,N,K,D]; workspace: ffb6d_gather_neighbour_bwd_det_workspace_bytes(B, S, N, K) bytes. */
+size_t ffb6d_gather_neighbour_bwd_det_workspace_bytes(int64_t B, int64_t S, int64_t N, int K);
+int ffb6d_gather_neighbour_bwd_det(const float *grad_out, const void *idx, int idx_is_i64, int64_t B, int64_t S,
+                                   int64_t D, int64_t N, int K, void *workspace, size_t workspace_bytes,
+                                   float *grad_pc, ffb6d_stream_t stream);
+/* ffb6d_fusion_mlp_wgrad without atomics: the same CTAs, tiles, numerics and split count, but each split stores
+ * its partial dW into its own slice of `workspace`, and wgrad_split_reduce_kernel adds the slices in split order in
+ * fp64 and rounds once.  The split count depends on the shape and on the SM count of the current device (never on
+ * timing), so ffb6d_fusion_mlp_wgrad_det_workspace_bytes(C1, C2, B, Co, P) must be asked on the device that runs
+ * the call, and results are bit-identical between runs on GPUs with the same SM count. */
+size_t ffb6d_fusion_mlp_wgrad_det_workspace_bytes(int64_t C1, int64_t C2, int64_t B, int64_t Co, int64_t P);
+int ffb6d_fusion_mlp_wgrad_det(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2,
+                               int64_t B, int64_t Co, int64_t P, void *workspace, size_t workspace_bytes,
+                               float *grad_w, ffb6d_stream_t stream);
 
 /*
  * Attentive pooling core of RandLA's Att_pooling (models/RandLA/RandLANet.py:243-248):

@@ -34,6 +34,10 @@ def main():
     ap.add_argument("--profile", action="store_true", help="print the per-kernel GPU time of one step (CUPTI) to stderr")
     ap.add_argument("--restructured", action="store_true",
                     help="run the pixel branch of every fusion as W1 . rgb + (W2 . p2r)[idx] (no interpolated maps)")
+    ap.add_argument("--deterministic", action="store_true",
+                    help="torch.use_deterministic_algorithms(True, warn_only=True): every backward of the model takes its "
+                         "run-to-run deterministic path (warn_only: torch's own nll_loss2d forward in the loss has no "
+                         "deterministic CUDA kernel and would raise)")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -43,6 +47,8 @@ def main():
     from ffb6d_b200.synthetic import make_batch
     from ffb6d_b200.dist import frame_shard, max_over_ranks
 
+    if args.deterministic:
+        torch.use_deterministic_algorithms(True, warn_only=True)
     rank, local_rank, world = (int(os.environ.get(k, d)) for k, d in (("RANK", 0), ("LOCAL_RANK", 0), ("WORLD_SIZE", 1)))
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
@@ -140,7 +146,7 @@ def main():
                 "batch_per_gpu": B, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
                 "params": n_params, "grad_allreduce_bytes": 4 * n_params if world > 1 else 0, "loss": float(loss.detach()),
                 "finite": finite, "dtype": "f32", "data": "synthetic", "scaling": "weak",
-                "restructured": args.restructured, "max_memory_allocated_mb": peak_mb,
+                "restructured": args.restructured, "deterministic": args.deterministic, "max_memory_allocated_mb": peak_mb,
                 "gpu": torch.cuda.get_device_name(dev)}
         print(json.dumps(line))
     if world > 1:
