@@ -71,6 +71,10 @@ def _load():
         "ffb6d_bn_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_bn_train_fwd": (ci, [vp, i64, i64, i64, vp, vp, fp, fp, vp, vp, ci, fp, vp, vp, vp, sz, vp]),
         "ffb6d_bn_train_bwd": (ci, [vp, vp, vp, i64, i64, i64, ci, fp, vp, vp, vp, vp, sz, vp]),
+        "ffb6d_bn_sync_moments": (ci, [vp, i64, i64, i64, vp, vp, sz, vp]),
+        "ffb6d_bn_sync_fwd": (ci, [vp, i64, i64, i64, vp, i64, vp, vp, fp, fp, vp, vp, ci, fp, vp, vp, vp, vp]),
+        "ffb6d_bn_sync_bwd_sums": (ci, [vp, vp, vp, i64, i64, i64, ci, fp, vp, vp, vp, vp, sz, vp]),
+        "ffb6d_bn_sync_bwd": (ci, [vp, vp, vp, i64, i64, i64, vp, i64, vp, ci, fp, vp, vp, sz, vp]),
         "ffb6d_act_bwd": (ci, [vp, vp, i64, ci, fp, vp, vp]),
         "ffb6d_fusion_mlp_wgrad": (ci, [vp, vp, i64, vp, i64, i64, i64, i64, vp, vp]),
         "ffb6d_segment_plan_bytes": (sz, [i64, i64, i64]),

@@ -208,6 +208,98 @@ act_bwd_kernel(const float *__restrict__ z, const float *__restrict__ g, long lo
         dz[i] = act_grad(__ldg(g + i), __ldg(z + i), act, slope);
 }
 
+// ------------------------------------------------------------------ BatchNorm over several ranks (torch's SyncBatchNorm)
+// Each rank reduces its own values with bn_stats_kernel / bn_bwd_reduce_kernel, the caller gathers one fp64 row per
+// rank, and every rank combines the same gathered rows in rank order: all ranks hold bit-identical statistics.
+
+// row = (n, mean[C], M2[C]) of this rank: mean = k + A/n and M2 = sum (z - mean)^2 = Q - A^2/n about
+// bn_stats_kernel's pivot k; a constant channel has A = Q = 0, so M2 = 0 exactly.
+__global__ void __launch_bounds__(BN_THREADS)
+bn_moments_kernel(const double *__restrict__ partial, const float *__restrict__ z, int C, int P, int nsplit, double n,
+                  double *__restrict__ row)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double A = 0.0, Q = 0.0;
+    for (int s = 0; s < nsplit; ++s) {
+        A += partial[((size_t)c * nsplit + s) * 2];
+        Q += partial[((size_t)c * nsplit + s) * 2 + 1];
+    }
+    if (c == 0) row[0] = n;
+    row[1 + c] = (double)z[(size_t)c * P] + A / n;
+    const double m2 = Q - A * (A / n);
+    row[1 + C + c] = m2 > 0.0 ? m2 : 0.0;
+}
+
+// Chan's parallel combination of the W gathered rows [W][2C+1], in rank order:
+//     n = n_a + n_b,  delta = mean_b - mean_a,  mean_a += delta * n_b / n,  M2_a += M2_b + delta^2 * n_a * n_b / n
+// then stats and the running statistics as bn_finalize_kernel, from the global mean, M2 / n and the global count,
+// which goes to *count for the backward.
+__global__ void __launch_bounds__(BN_THREADS)
+bn_sync_finalize_kernel(const double *__restrict__ rows, int W, int C, float eps, float momentum,
+                        const float *__restrict__ gamma, const float *__restrict__ beta, float *__restrict__ running_mean,
+                        float *__restrict__ running_var, float4 *__restrict__ stats, double *__restrict__ count)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    const size_t ld = 2 * (size_t)C + 1;
+    double n = rows[0], mean = rows[1 + c], m2 = rows[1 + C + c];
+    for (int w = 1; w < W; ++w) {
+        const double *r = rows + (size_t)w * ld;
+        const double nb = r[0], nn = n + nb, d = r[1 + c] - mean;
+        mean += d * (nb / nn);
+        m2 += r[1 + C + c] + d * d * (n * nb / nn);
+        n = nn;
+    }
+    if (c == 0) *count = n;
+    double var = m2 / n;                // biased, as BatchNorm normalises with
+    if (var < 0.0) var = 0.0;
+    const float invstd = (float)(1.0 / sqrt(var + (double)eps));
+    const float g = gamma ? gamma[c] : 1.f;
+    stats[c] = make_float4((float)mean, invstd, g * invstd, beta ? beta[c] : 0.f);
+    if (running_mean) running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)mean;
+    if (running_var) {
+        const double unbiased = n > 1.0 ? m2 / (n - 1.0) : var;
+        running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unbiased;
+    }
+}
+
+// this rank's (sum g'[C], sum g' * xhat[C]) in fp64 from bn_bwd_reduce_kernel's partials; grad_beta / grad_gamma
+// are the same sums rounded (they stay local: DDP's gradient all-reduce adds them over the ranks)
+__global__ void __launch_bounds__(BN_THREADS)
+bn_sync_bwd_local_kernel(const double *__restrict__ partial, int C, int nsplit, double *__restrict__ row,
+                         float *__restrict__ grad_gamma, float *__restrict__ grad_beta)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double A = 0.0, Q = 0.0;
+    for (int s = 0; s < nsplit; ++s) {
+        A += partial[((size_t)c * nsplit + s) * 2];
+        Q += partial[((size_t)c * nsplit + s) * 2 + 1];
+    }
+    row[c] = A;
+    row[C + c] = Q;
+    if (grad_beta) grad_beta[c] = (float)A;
+    if (grad_gamma) grad_gamma[c] = (float)Q;
+}
+
+// sums[c] = (sum g', sum g' * xhat) / n over the gathered rows [W][2C], added in rank order, divided once by the
+// global count: bn_bwd_apply_kernel then runs with inv_n = 1
+__global__ void __launch_bounds__(BN_THREADS)
+bn_sync_bwd_combine_kernel(const double *__restrict__ rows, int W, int C, const double *__restrict__ count,
+                           float2 *__restrict__ sums)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double A = 0.0, Q = 0.0;
+    for (int w = 0; w < W; ++w) {
+        A += rows[(size_t)w * 2 * C + c];
+        Q += rows[(size_t)w * 2 * C + C + c];
+    }
+    const double n = *count;
+    sums[c] = make_float2((float)(A / n), (float)(Q / n));
+}
+
 // ------------------------------------------------------------------ attentive pooling backward
 // forward: out[b,c,n] = sum_k f[k] * s[k], s = softmax_k(att)   (models/RandLA/RandLANet.py:245-248)
 // backward: df[k] = g * s[k];  datt[k] = s[k] * g * (f[k] - out).  One thread per (b, c, n); with KT = 16 the
@@ -487,6 +579,105 @@ int ffb6d_bn_train_bwd(const float *z, const float *grad_y, const float *stats, 
     FFB6D_LAUNCH_OK("bn_bwd_apply_kernel");
     return FFB6D_OK;
 }
+
+#define FFB6D_BN_SIZES(name)                                                                                      \
+    FFB6D_CHECK_ARG(B >= 1 && C >= 1 && P >= 1 && B < 65536 && C <= 65535 && P < (1ll << 31) && B * C < (1ll << 31), \
+                    name ": bad size")
+#define FFB6D_ALIGNED(p, a) ((reinterpret_cast<uintptr_t>(p) & ((a) - 1)) == 0)
+
+int ffb6d_bn_sync_moments(const float *z, int64_t B, int64_t C, int64_t P, double *moments, void *workspace,
+                          size_t workspace_bytes, ffb6d_stream_t stream)
+{
+    FFB6D_BN_SIZES("bn_sync_moments");
+    FFB6D_CHECK_ARG(z && moments && workspace, "bn_sync_moments: null pointer");
+    FFB6D_CHECK_ARG(FFB6D_ALIGNED(moments, 8), "bn_sync_moments: moments must be 8-byte aligned");
+    FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_sync_moments: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    int chunk, nsplit;
+    split_plan(C, P, chunk, nsplit);
+    double *partial = (double *)workspace;
+    bn_stats_kernel<<<dim3((unsigned)nsplit, (unsigned)C), BN_THREADS, 0, st>>>(z, (int)B, (int)C, (int)P, chunk, nsplit, partial);
+    FFB6D_LAUNCH_OK("bn_stats_kernel");
+    bn_moments_kernel<<<(unsigned)ceil_div(C, BN_THREADS), BN_THREADS, 0, st>>>(partial, z, (int)C, (int)P, nsplit,
+                                                                               (double)B * (double)P, moments);
+    FFB6D_LAUNCH_OK("bn_moments_kernel");
+    return FFB6D_OK;
+}
+
+int ffb6d_bn_sync_fwd(const float *z, int64_t B, int64_t C, int64_t P, const double *gathered, int64_t W,
+                      const float *gamma, const float *beta, float eps, float momentum, float *running_mean,
+                      float *running_var, int act, float negative_slope, float *stats, double *count, float *y,
+                      ffb6d_stream_t stream)
+{
+    FFB6D_BN_SIZES("bn_sync_fwd");
+    FFB6D_CHECK_ARG(W >= 1 && W <= 65536, "bn_sync_fwd: W=%lld outside [1, 65536]", (long long)W);
+    FFB6D_CHECK_ARG(z && gathered && stats && count && y, "bn_sync_fwd: null pointer");
+    FFB6D_CHECK_ARG(act >= 0 && act <= 2, "bn_sync_fwd: act=%d", act);
+    FFB6D_CHECK_ARG(FFB6D_ALIGNED(stats, 16), "bn_sync_fwd: stats must be 16-byte aligned");
+    FFB6D_CHECK_ARG(FFB6D_ALIGNED(gathered, 8) && FFB6D_ALIGNED(count, 8),
+                    "bn_sync_fwd: gathered and count must be 8-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    bn_sync_finalize_kernel<<<(unsigned)ceil_div(C, BN_THREADS), BN_THREADS, 0, st>>>(
+        gathered, (int)W, (int)C, eps, momentum, gamma, beta, running_mean, running_var, (float4 *)stats, count);
+    FFB6D_LAUNCH_OK("bn_sync_finalize_kernel");
+    const unsigned gx = (unsigned)std::min<int64_t>(ceil_div(P, 4 * BN_THREADS), 64);
+    bn_apply_kernel<<<dim3((unsigned)(B * C), gx), BN_THREADS, 0, st>>>(z, (const float4 *)stats, (int)C, (int)P, act,
+                                                                        negative_slope, y);
+    FFB6D_LAUNCH_OK("bn_apply_kernel");
+    return FFB6D_OK;
+}
+
+int ffb6d_bn_sync_bwd_sums(const float *z, const float *grad_y, const float *stats, int64_t B, int64_t C, int64_t P,
+                           int act, float negative_slope, double *sums, float *grad_gamma, float *grad_beta,
+                           void *workspace, size_t workspace_bytes, ffb6d_stream_t stream)
+{
+    FFB6D_BN_SIZES("bn_sync_bwd_sums");
+    FFB6D_CHECK_ARG(z && grad_y && stats && sums && workspace, "bn_sync_bwd_sums: null pointer");
+    FFB6D_CHECK_ARG(act >= 0 && act <= 2, "bn_sync_bwd_sums: act=%d", act);
+    FFB6D_CHECK_ARG(FFB6D_ALIGNED(stats, 16), "bn_sync_bwd_sums: stats must be 16-byte aligned");
+    FFB6D_CHECK_ARG(FFB6D_ALIGNED(sums, 8), "bn_sync_bwd_sums: sums must be 8-byte aligned");
+    FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_sync_bwd_sums: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    int chunk, nsplit;
+    split_plan(C, P, chunk, nsplit);
+    double *partial = (double *)workspace;
+    bn_bwd_reduce_kernel<<<dim3((unsigned)nsplit, (unsigned)C), BN_THREADS, 0, st>>>(
+        z, grad_y, (const float4 *)stats, (int)B, (int)C, (int)P, chunk, nsplit, act, negative_slope, partial);
+    FFB6D_LAUNCH_OK("bn_bwd_reduce_kernel");
+    bn_sync_bwd_local_kernel<<<(unsigned)ceil_div(C, BN_THREADS), BN_THREADS, 0, st>>>(partial, (int)C, nsplit, sums,
+                                                                                      grad_gamma, grad_beta);
+    FFB6D_LAUNCH_OK("bn_sync_bwd_local_kernel");
+    return FFB6D_OK;
+}
+
+int ffb6d_bn_sync_bwd(const float *z, const float *grad_y, const float *stats, int64_t B, int64_t C, int64_t P,
+                      const double *gathered, int64_t W, const double *count, int act, float negative_slope,
+                      float *grad_z, void *workspace, size_t workspace_bytes, ffb6d_stream_t stream)
+{
+    FFB6D_BN_SIZES("bn_sync_bwd");
+    FFB6D_CHECK_ARG(W >= 1 && W <= 65536, "bn_sync_bwd: W=%lld outside [1, 65536]", (long long)W);
+    FFB6D_CHECK_ARG(z && grad_y && stats && gathered && count && grad_z && workspace, "bn_sync_bwd: null pointer");
+    FFB6D_CHECK_ARG(act >= 0 && act <= 2, "bn_sync_bwd: act=%d", act);
+    FFB6D_CHECK_ARG(FFB6D_ALIGNED(stats, 16), "bn_sync_bwd: stats must be 16-byte aligned");
+    FFB6D_CHECK_ARG(FFB6D_ALIGNED(gathered, 8) && FFB6D_ALIGNED(count, 8),
+                    "bn_sync_bwd: gathered and count must be 8-byte aligned");
+    FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_sync_bwd: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    int chunk, nsplit;
+    split_plan(C, P, chunk, nsplit);
+    float2 *sums = (float2 *)((char *)workspace + align_up((size_t)C * nsplit * 2 * sizeof(double), 256));
+    bn_sync_bwd_combine_kernel<<<(unsigned)ceil_div(C, BN_THREADS), BN_THREADS, 0, st>>>(gathered, (int)W, (int)C, count,
+                                                                                        sums);
+    FFB6D_LAUNCH_OK("bn_sync_bwd_combine_kernel");
+    const unsigned gx = (unsigned)std::min<int64_t>(ceil_div(P, BN_THREADS), 64);
+    bn_bwd_apply_kernel<<<dim3((unsigned)(B * C), gx), BN_THREADS, 0, st>>>(
+        z, grad_y, (const float4 *)stats, sums, (int)C, (int)P, 1.f, act, negative_slope, grad_z);
+    FFB6D_LAUNCH_OK("bn_bwd_apply_kernel");
+    return FFB6D_OK;
+}
+
+#undef FFB6D_BN_SIZES
+#undef FFB6D_ALIGNED
 
 int ffb6d_act_bwd(const float *z, const float *grad_y, int64_t n, int act, float negative_slope, float *grad_z,
                   ffb6d_stream_t stream)

@@ -1,9 +1,24 @@
 """Multi-GPU plumbing of the hot path: frames are independent (every KNN / gather stays inside
 one batch item: NN/knn_.cxx:109-113, models/ffb6d.py:172-174), so ranks take disjoint frame
 ranges and the only cross-rank traffic is the timing reduction of bench.py.  No data-path
-collective exists ("replicas / weak scaling", SURVEY.md §8e)."""
+collective exists ("replicas / weak scaling", SURVEY.md §8e).  Training is the one opt-in exception: a
+model converted with ``nn.SyncBatchNorm.convert_sync_batchnorm`` gathers each BatchNorm layer's per-rank
+moments and gradient sums with :func:`all_gather_rows` (ffb6d_b200.modules)."""
 import torch
 import torch.distributed as dist
+
+
+def all_gather_rows(row, group, world):
+    """``[world, n]``: the 1-D ``row`` of every rank of ``group`` in rank order.  ``all_gather_into_tensor``, or the
+    list form on gloo, which lacks it (as torch's SyncBatchNorm does).  A gather rather than an all-reduce: the
+    caller combines the rows in rank order, so the result does not depend on the backend's reduction order."""
+    if dist.get_backend(group) == "gloo":
+        parts = [torch.empty_like(row) for _ in range(world)]
+        dist.all_gather(parts, row, group=group)
+        return torch.stack(parts)
+    out = torch.empty((world, row.numel()), dtype=row.dtype, device=row.device)
+    dist.all_gather_into_tensor(out, row, group=group)
+    return out
 
 
 def frame_shard(frames_per_rank, rank, world):

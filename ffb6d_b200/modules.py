@@ -17,6 +17,9 @@ Both modes run on the CUDA library:
   weight; neighbour gathers and attentive pooling have their own backward kernels.  Under
   ``torch.use_deterministic_algorithms(True)`` (or, for the weight gradients only, ``torch.backends.cudnn.deterministic``)
   the backwards that add with atomics take their run-to-run deterministic paths (:func:`ops.deterministic_backward`).
+  After ``nn.SyncBatchNorm.convert_sync_batchnorm(model)`` a training-mode layer under an initialised process group
+  of more than one rank normalises with the statistics of every rank's batch, as ``nn.SyncBatchNorm`` does
+  (``ffb6d_bn_sync_*``, one all-gather per layer and direction; :meth:`_ConvBase._bn_sync`).
 
 A layer accepts its input as one tensor or as the two halves of a concat (``layer(x1, x2)`` ==
 ``layer(torch.cat((x1, x2), 1))`` without materialising the concat, models/ffb6d.py:251-262).
@@ -26,10 +29,11 @@ fusion's nearest interpolation, and never builds the interpolated map.
 import math
 
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 import torch.nn.functional as F_
 
-from . import fusion, ops
+from . import dist as dist_, fusion, ops
 from ._lib import lib, check
 
 _ACT_NONE, _ACT_RELU, _ACT_LEAKY = 0, 1, 2
@@ -61,29 +65,46 @@ def _gemm(x1, x2, w2d):
     return ops.fusion_mlp(x1, x2, w2d, one, zero, relu=False)
 
 
-def _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn):
+def _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn, sync=None):
     """y = act(BatchNorm with batch statistics(z)) (``ffb6d_bn_train_fwd``, also updates the running statistics) or,
-    without BatchNorm, y = act(z).  Returns ``(y, stats)``; ``stats`` [Co, 4] is what :func:`_bn_act_bwd` reads."""
+    without BatchNorm, y = act(z).  Returns ``(y, stats, count)``; ``stats`` [Co, 4] and ``count`` are what
+    :func:`_bn_act_bwd` reads.  With ``sync = (group, world)`` the statistics are those of the batches of every rank of
+    ``group`` (torch's SyncBatchNorm): this rank's moments (``ffb6d_bn_sync_moments``), an all-gather, the rank-ordered
+    combination (``ffb6d_bn_sync_fwd``); ``count`` [1] fp64 is then the global count, else None."""
     if not has_bn:
         if act == _ACT_RELU:
-            return torch.relu(z), None
-        return (F_.leaky_relu(z, slope) if act == _ACT_LEAKY else z), None
+            return torch.relu(z), None, None
+        return (F_.leaky_relu(z, slope) if act == _ACT_LEAKY else z), None, None
     stats = torch.empty((Co, 4), dtype=torch.float32, device=z.device)
     y = torch.empty_like(z)
     nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
     ws = torch.empty(nbytes, dtype=torch.uint8, device=z.device)
+    gamma_p = gamma.data_ptr() if gamma is not None else None
+    beta_p = beta.data_ptr() if beta is not None else None
+    rm_p = running_mean.data_ptr() if running_mean is not None else None
+    rv_p = running_var.data_ptr() if running_var is not None else None
     with torch.cuda.device(z.device):
-        check(lib.ffb6d_bn_train_fwd(
-            z.data_ptr(), B, Co, P, gamma.data_ptr() if gamma is not None else None,
-            beta.data_ptr() if beta is not None else None, float(eps), float(momentum),
-            running_mean.data_ptr() if running_mean is not None else None,
-            running_var.data_ptr() if running_var is not None else None, int(act), float(slope),
-            stats.data_ptr(), y.data_ptr(), ws.data_ptr(), nbytes, ops._stream(z.device)))
-    return y, stats
+        if sync is None:
+            check(lib.ffb6d_bn_train_fwd(
+                z.data_ptr(), B, Co, P, gamma_p, beta_p, float(eps), float(momentum), rm_p, rv_p, int(act), float(slope),
+                stats.data_ptr(), y.data_ptr(), ws.data_ptr(), nbytes, ops._stream(z.device)))
+            return y, stats, None
+        group, world = sync
+        row = torch.empty(2 * Co + 1, dtype=torch.float64, device=z.device)
+        check(lib.ffb6d_bn_sync_moments(z.data_ptr(), B, Co, P, row.data_ptr(), ws.data_ptr(), nbytes,
+                                        ops._stream(z.device)))
+        rows = dist_.all_gather_rows(row, group, world)
+        count = torch.empty(1, dtype=torch.float64, device=z.device)
+        check(lib.ffb6d_bn_sync_fwd(
+            z.data_ptr(), B, Co, P, rows.data_ptr(), world, gamma_p, beta_p, float(eps), float(momentum), rm_p, rv_p,
+            int(act), float(slope), stats.data_ptr(), count.data_ptr(), y.data_ptr(), ops._stream(z.device)))
+    return y, stats, count
 
 
-def _bn_act_bwd(z, gy, stats, B, Co, P, act, slope, has_bn):
-    """Backward of :func:`_bn_act_fwd`: ``(dz, dgamma, dbeta)``; dgamma / dbeta are None without BatchNorm."""
+def _bn_act_bwd(z, gy, stats, B, Co, P, act, slope, has_bn, sync=None, count=None):
+    """Backward of :func:`_bn_act_fwd`: ``(dz, dgamma, dbeta)``; dgamma / dbeta are None without BatchNorm.  With
+    ``sync`` (and the forward's ``count``) dz uses the sums of every rank (``ffb6d_bn_sync_bwd_sums``, an all-gather,
+    ``ffb6d_bn_sync_bwd``); dgamma / dbeta stay this rank's, for the gradient all-reduce of DDP to add."""
     dev = z.device
     with torch.cuda.device(dev):
         if has_bn:
@@ -92,9 +113,20 @@ def _bn_act_bwd(z, gy, stats, B, Co, P, act, slope, has_bn):
             gbeta = torch.empty(Co, dtype=torch.float32, device=dev)
             nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
             ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            check(lib.ffb6d_bn_train_bwd(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
-                                         ggamma.data_ptr(), gbeta.data_ptr(), dz.data_ptr(), ws.data_ptr(), nbytes,
-                                         ops._stream(dev)))
+            if sync is None:
+                check(lib.ffb6d_bn_train_bwd(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
+                                             ggamma.data_ptr(), gbeta.data_ptr(), dz.data_ptr(), ws.data_ptr(), nbytes,
+                                             ops._stream(dev)))
+                return dz, ggamma, gbeta
+            group, world = sync
+            row = torch.empty(2 * Co, dtype=torch.float64, device=dev)
+            check(lib.ffb6d_bn_sync_bwd_sums(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
+                                             row.data_ptr(), ggamma.data_ptr(), gbeta.data_ptr(), ws.data_ptr(), nbytes,
+                                             ops._stream(dev)))
+            rows = dist_.all_gather_rows(row, group, world)
+            check(lib.ffb6d_bn_sync_bwd(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, rows.data_ptr(), world,
+                                        count.data_ptr(), act, slope, dz.data_ptr(), ws.data_ptr(), nbytes,
+                                        ops._stream(dev)))
             return dz, ggamma, gbeta
         if act != _ACT_NONE:
             dz = torch.empty_like(z)
@@ -125,7 +157,8 @@ class _ConvBnActTrain(torch.autograd.Function):
     """conv1x1(cat(x1, x2)) -> [BatchNorm with batch statistics] -> activation, with its backward."""
 
     @staticmethod
-    def forward(ctx, x1, x2, weight, bias, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn):
+    def forward(ctx, x1, x2, weight, bias, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn,
+                sync=None):
         x1 = x1.contiguous()
         x2 = x2.contiguous() if x2 is not None else None
         B, C1 = x1.shape[0], x1.shape[1]
@@ -138,17 +171,19 @@ class _ConvBnActTrain(torch.autograd.Function):
         else:
             z = _gemm(x1, x2, w2d)
         P = z.numel() // (B * Co)
-        y, stats = _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn)
-        ctx.save_for_backward(x1, x2, w2d, z, stats, gamma)
+        y, stats, count = _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope,
+                                      has_bn, sync)
+        ctx.sync = sync
+        ctx.save_for_backward(x1, x2, w2d, z, stats, gamma, count)
         ctx.meta = (B, C1, C2, Co, P, int(act), float(slope), bool(has_bn), bias is not None, tuple(weight.shape))
         return y
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, gy):
-        x1, x2, w2d, z, stats, gamma = ctx.saved_tensors
+        x1, x2, w2d, z, stats, gamma, count = ctx.saved_tensors
         B, C1, C2, Co, P, act, slope, has_bn, has_bias, wshape = ctx.meta
-        dz, ggamma, gbeta = _bn_act_bwd(z, gy.contiguous(), stats, B, Co, P, act, slope, has_bn)
+        dz, ggamma, gbeta = _bn_act_bwd(z, gy.contiguous(), stats, B, Co, P, act, slope, has_bn, ctx.sync, count)
         gw = gbias = None
         if ctx.needs_input_grad[2]:
             gw = _wgrad(dz, x1, x2, B, Co, P).reshape(wshape)
@@ -162,7 +197,7 @@ class _ConvBnActTrain(torch.autograd.Function):
             gx2 = _gemm(dz, None, w2d[:, C1:].t().contiguous()).reshape(x2.shape)
         if gamma is None:
             ggamma = None
-        return gx1, gx2, gw, gbias, ggamma, gbeta, None, None, None, None, None, None, None
+        return gx1, gx2, gw, gbias, ggamma, gbeta, None, None, None, None, None, None, None, None
 
 
 class _InterpConvBnActTrain(torch.autograd.Function):
@@ -176,7 +211,8 @@ class _InterpConvBnActTrain(torch.autograd.Function):
     ascending pixel order (``ffb6d_segment_sum``), so the gradients are bit-identical from run to run."""
 
     @staticmethod
-    def forward(ctx, x1, p, idx, weight, bias, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn):
+    def forward(ctx, x1, p, idx, weight, bias, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn,
+                sync=None):
         x1, p = x1.contiguous(), p.contiguous()
         B, C1 = x1.shape[0], x1.shape[1]
         C2, NA = p.shape[1], p.shape[2]
@@ -187,19 +223,21 @@ class _InterpConvBnActTrain(torch.autograd.Function):
         zp = ops.fusion_mlp(p, None, w2, one, zero, relu=False, out_channels_last=True)          # [B, N', Co]
         z = ops.fusion_mlp(x1, None, w1, one, bias if bias is not None else zero, relu=False, add=zp, add_idx=idx)
         P = z.numel() // (B * Co)
-        y, stats = _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope, has_bn)
+        y, stats, count = _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, momentum, act, slope,
+                                      has_bn, sync)
+        ctx.sync = sync
         # dZ feeds dW2 and dp only: without either, the backward needs no plan
         ctx.plan = ops.segment_plan(idx, NA) if (ctx.needs_input_grad[1] or ctx.needs_input_grad[3]) else None
-        ctx.save_for_backward(x1, p, w1, w2, z, stats, gamma)
+        ctx.save_for_backward(x1, p, w1, w2, z, stats, gamma, count)
         ctx.meta = (B, C1, C2, Co, P, NA, int(act), float(slope), bool(has_bn), bias is not None, tuple(weight.shape))
         return y
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, gy):
-        x1, p, w1, w2, z, stats, gamma = ctx.saved_tensors
+        x1, p, w1, w2, z, stats, gamma, count = ctx.saved_tensors
         B, C1, C2, Co, P, NA, act, slope, has_bn, has_bias, wshape = ctx.meta
-        dz, ggamma, gbeta = _bn_act_bwd(z, gy.contiguous(), stats, B, Co, P, act, slope, has_bn)
+        dz, ggamma, gbeta = _bn_act_bwd(z, gy.contiguous(), stats, B, Co, P, act, slope, has_bn, ctx.sync, count)
         dz = dz.reshape(B, Co, P)
         dzp = ops.segment_sum(dz, None, NA, plan=ctx.plan) if ctx.plan is not None else None     # [B, Co, N']
         gx1 = gp = gw = gbias = None
@@ -214,7 +252,7 @@ class _InterpConvBnActTrain(torch.autograd.Function):
             gp = _gemm(dzp, None, w2.t().contiguous()).reshape(p.shape)
         if gamma is None:
             ggamma = None
-        return gx1, gp, None, gw, gbias, ggamma, gbeta, None, None, None, None, None, None, None
+        return gx1, gp, None, gw, gbias, ggamma, gbeta, None, None, None, None, None, None, None, None
 
 
 class _BNWrap(nn.Sequential):
@@ -285,11 +323,24 @@ class _ConvBase(nn.Module):
             self._packed = (ver, ops.fusion_mlp_pack(self._conv.weight.detach()), scale, shift)
         return self._packed[1:]
 
-    def _train_momentum(self, x):
-        """Training-mode BatchNorm bookkeeping before a forward, as nn.BatchNorm2d does it: rejects one value per
-        channel, counts the batch, returns the momentum to update the running statistics with."""
+    def _bn_sync(self):
+        """``(process group, world size)`` when the training-mode BatchNorm normalises with the statistics of every
+        rank, decided as ``nn.SyncBatchNorm.forward`` does: the layer is training, its BatchNorm is an
+        ``nn.SyncBatchNorm``, torch.distributed is initialised, and the group (``process_group``, or WORLD) has more
+        than one rank.  None otherwise: the layer's own batch, today's kernels."""
         bn = self._bn
-        if x.shape[0] * math.prod(x.shape[2:]) == 1:     # as torch's BatchNorm in training
+        if not (self.training and isinstance(bn, nn.SyncBatchNorm) and dist.is_available() and dist.is_initialized()):
+            return None
+        group = bn.process_group if bn.process_group is not None else dist.group.WORLD
+        world = dist.get_world_size(group)
+        return (group, world) if world > 1 else None
+
+    def _train_momentum(self, x, sync=None):
+        """Training-mode BatchNorm bookkeeping before a forward, as nn.BatchNorm2d does it: rejects one value per
+        channel (unless synchronised over several ranks, as nn.SyncBatchNorm), counts the batch, returns the momentum
+        to update the running statistics with."""
+        bn = self._bn
+        if sync is None and x.shape[0] * math.prod(x.shape[2:]) == 1:     # as torch's BatchNorm in training
             raise ValueError("Expected more than 1 value per channel when training, got input size %s"
                              % (torch.Size((x.shape[0], bn.num_features) + tuple(x.shape[2:])),))
         if bn.track_running_stats and bn.num_batches_tracked is not None:
@@ -317,9 +368,10 @@ class _ConvBase(nn.Module):
         need_grad = torch.is_grad_enabled() and (x.requires_grad or conv.weight.requires_grad or
                                                  (x2 is not None and x2.requires_grad))
         if self.training and bn is not None:
-            momentum = self._train_momentum(x)
+            sync = self._bn_sync()
+            momentum = self._train_momentum(x, sync)
             return _ConvBnActTrain.apply(x, x2, conv.weight, None, bn.weight, bn.bias, bn.running_mean, bn.running_var,
-                                         bn.eps, momentum, self.act, self.slope, True)
+                                         bn.eps, momentum, self.act, self.slope, True, sync)
         if need_grad and bn is None:
             return _ConvBnActTrain.apply(x, x2, conv.weight, conv.bias, None, None, None, None, 0.0, 0.0, self.act,
                                          self.slope, False)
@@ -373,9 +425,10 @@ class Conv2d(_ConvBase):
         idx = interp_idx.reshape(B, h * w)
         need_grad = torch.is_grad_enabled() and (x1.requires_grad or p.requires_grad or conv.weight.requires_grad)
         if self.training and bn is not None:
-            momentum = self._train_momentum(x1)
+            sync = self._bn_sync()
+            momentum = self._train_momentum(x1, sync)
             return _InterpConvBnActTrain.apply(x1, p, idx, conv.weight, None, bn.weight, bn.bias, bn.running_mean,
-                                               bn.running_var, bn.eps, momentum, self.act, self.slope, True)
+                                               bn.running_var, bn.eps, momentum, self.act, self.slope, True, sync)
         if need_grad and bn is None:
             return _InterpConvBnActTrain.apply(x1, p, idx, conv.weight, conv.bias, None, None, None, None, 0.0, 0.0,
                                                self.act, self.slope, False)

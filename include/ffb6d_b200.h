@@ -301,6 +301,33 @@ int ffb6d_bn_train_fwd(const float *z, int64_t B, int64_t C, int64_t P, const fl
 int ffb6d_bn_train_bwd(const float *z, const float *grad_y, const float *stats, int64_t B, int64_t C, int64_t P,
                        int act, float negative_slope, float *grad_gamma, float *grad_beta, float *grad_z,
                        void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+/* The same BatchNorm with the statistics of the batch of every rank of a process group (torch's
+ * nn.SyncBatchNorm).  The caller gathers one fp64 row per rank between the two halves of each direction:
+ *   forward   ffb6d_bn_sync_moments  z -> moments [2C+1] = (n, mean[C], M2[C]) of this rank's B*P values
+ *             (all-gather the rows in rank order into gathered [W][2C+1])
+ *             ffb6d_bn_sync_fwd      combines the W rows in rank order in fp64 (Chan's parallel formula), writes
+ *                                    stats, the running statistics (unbiased variance of the global count) and the
+ *                                    global count *count (device, fp64), then y as ffb6d_bn_train_fwd
+ *   backward  ffb6d_bn_sync_bwd_sums z, grad_y, stats -> sums [2C] = (sum g'[C], sum g' * xhat[C]) of this rank,
+ *                                    and this rank's grad_gamma / grad_beta (left to the caller's gradient all-reduce)
+ *             (all-gather the rows into gathered [W][2C])
+ *             ffb6d_bn_sync_bwd      adds the W rows in rank order in fp64, divides by *count once, writes grad_z
+ * Every rank combines the same rows in the same order, so all ranks hold bit-identical stats and running
+ * statistics.  No allocation, no host synchronisation.  workspace: ffb6d_bn_workspace_bytes(C, P); moments, sums,
+ * gathered and count 8-byte aligned, stats 16-byte aligned; 1 <= W <= 65536.  A rank with no values is not
+ * supported (B, P >= 1). */
+int ffb6d_bn_sync_moments(const float *z, int64_t B, int64_t C, int64_t P, double *moments,
+                          void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+int ffb6d_bn_sync_fwd(const float *z, int64_t B, int64_t C, int64_t P, const double *gathered, int64_t W,
+                      const float *gamma, const float *beta, float eps, float momentum, float *running_mean,
+                      float *running_var, int act, float negative_slope, float *stats, double *count, float *y,
+                      ffb6d_stream_t stream);
+int ffb6d_bn_sync_bwd_sums(const float *z, const float *grad_y, const float *stats, int64_t B, int64_t C, int64_t P,
+                           int act, float negative_slope, double *sums, float *grad_gamma, float *grad_beta,
+                           void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+int ffb6d_bn_sync_bwd(const float *z, const float *grad_y, const float *stats, int64_t B, int64_t C, int64_t P,
+                      const double *gathered, int64_t W, const double *count, int act, float negative_slope,
+                      float *grad_z, void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
 /* grad_z = grad_y * act'(z) for a layer with an activation but no BatchNorm. */
 int ffb6d_act_bwd(const float *z, const float *grad_y, int64_t n, int act, float negative_slope, float *grad_z,
                   ffb6d_stream_t stream);

@@ -3,11 +3,14 @@
 fusion + heads (ffb6d_b200.model.FFB6DFusionNet: everything of FFB6D.forward except the ResNet/PSPNet image
 backbone, whose stage outputs are synthetic leaf tensors) under DistributedDataParallel, one process per GPU,
 NCCL gradient all-reduce -- the reference's recipe (train_ycb.py:536-539, 596-599).  BatchNorm statistics are per
-GPU (the reference additionally converts to apex SyncBN, train_ycb.py:568; BASELINE.json's north_star keeps NCCL
-"only for the DDP gradient allreduce", so the cross-rank statistics exchange is not part of this path).
+GPU by default (BASELINE.json's north_star keeps NCCL "only for the DDP gradient allreduce").  ``--syncbn`` converts
+the model with nn.SyncBatchNorm.convert_sync_batchnorm before the DDP wrap, as the reference converts to apex SyncBN
+(train_ycb.py:568): every BatchNorm then normalises with the statistics of the global batch, one all-gather per
+BatchNorm layer and direction.
 
     python tools/train_bench.py --config 3                      (1 GPU)
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 tools/train_bench.py --config 3
+    python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tools/train_bench.py --config 3 --syncbn
 
 Config 3: LineMOD-shaped (2 classes, 8 keypoints + centre), batch 8 per GPU, forward + backward.
 Config 4: YCB-shaped (22 classes), batch 4 per GPU, forward + backward + Adam step ("end-to-end train step").
@@ -38,6 +41,9 @@ def main():
                     help="torch.use_deterministic_algorithms(True, warn_only=True): every backward of the model takes its "
                          "run-to-run deterministic path (warn_only: torch's own nll_loss2d forward in the loss has no "
                          "deterministic CUDA kernel and would raise)")
+    ap.add_argument("--syncbn", action="store_true",
+                    help="nn.SyncBatchNorm.convert_sync_batchnorm(model) before the DDP wrap: BatchNorm statistics of the "
+                         "global batch (the reference's convert_syncbn_model, train_ycb.py:568)")
     args = ap.parse_args()
     import numpy as np
     import torch
@@ -59,6 +65,8 @@ def main():
     N0 = 12288
     torch.manual_seed(0)
     model = FFB6DFusionNet(n_classes=n_classes, n_pts=N0, n_kps=n_kps, restructured=args.restructured).to(dev).train()
+    if args.syncbn:
+        model = torch.nn.SyncBatchNorm.convert_sync_batchnorm(model)
     n_params = sum(p.numel() for p in model.parameters())
     net = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local_rank], output_device=local_rank,
                                                     find_unused_parameters=False) if world > 1 else model
@@ -146,7 +154,7 @@ def main():
                 "batch_per_gpu": B, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
                 "params": n_params, "grad_allreduce_bytes": 4 * n_params if world > 1 else 0, "loss": float(loss.detach()),
                 "finite": finite, "dtype": "f32", "data": "synthetic", "scaling": "weak",
-                "restructured": args.restructured, "deterministic": args.deterministic, "max_memory_allocated_mb": peak_mb,
+                "restructured": args.restructured, "deterministic": args.deterministic, "syncbn": args.syncbn, "max_memory_allocated_mb": peak_mb,
                 "gpu": torch.cuda.get_device_name(dev)}
         print(json.dumps(line))
     if world > 1:
