@@ -7,24 +7,11 @@
 // cloud per frame is neither shipped to the GPU nor materialised on it; the host sends the depth
 // map (1.2 MB) and `choose` (48 KB).
 //
-// Arithmetic is the reference's, which numpy evaluates in float64 (integer pixel grid minus a
-// float64 intrinsic): x = ((col - cx) * d) / fx, y = ((row - cy) * d) / fy, z = d, each multiplied by
-// the validity mask (d > 1e-8 ? 1 : 0 -- holes become signed zeros), then rounded once to float32
-// where the reference casts (`cld.astype(np.float32)`, NN/knn.pyx:95-96).
-#include "common.cuh"
+// Arithmetic is the reference's, which numpy evaluates in float64 (backproject.cuh), rounded once to
+// float32 where the reference casts (`cld.astype(np.float32)`, NN/knn.pyx:95-96).
+#include "backproject.cuh"
 
 namespace ffb6d {
-
-__device__ __forceinline__ void backproject_px(const float *__restrict__ depth, int W, int row, int col,
-                                               double fx, double fy, double cx, double cy, float *o)
-{
-    const float d = __ldg(depth + (size_t)row * W + col);
-    const double msk = (d > 1e-8f) ? 1.0 : 0.0;
-    const double dd = (double)d;
-    o[0] = __double2float_rn(__dmul_rn(__ddiv_rn(__dmul_rn((double)col - cx, dd), fx), msk));
-    o[1] = __double2float_rn(__dmul_rn(__ddiv_rn(__dmul_rn((double)row - cy, dd), fy), msk));
-    o[2] = __double2float_rn(__dmul_rn(dd, msk));
-}
 
 // flat work list per frame: [0,N) sampled points, then the stride-2, -4, -8 sub-grids
 __global__ void __launch_bounds__(256)

@@ -707,14 +707,17 @@ def backproject(depth, K, choose):
     if depth.dim() != 3 or depth.dtype != torch.float32:
         raise ValueError("depth must be float32 [B,H,W], got %s %s" % (depth.dtype, tuple(depth.shape)))
     depth = depth.contiguous()
-    B, H, W = depth.shape
-    dev = depth.device
+    intr_d, per_frame = _intrinsics_arg(K, depth.shape[0], depth.device)
+    return _backproject(depth, intr_d, per_frame, choose)
+
+
+def _intrinsics_arg(K, B, dev):
+    """``K`` as :func:`backproject` takes it -> ``(float64 (fx, fy, cx, cy) [4] or [B,4] on dev, per_frame)``."""
     if isinstance(K, torch.Tensor) and K.is_cuda:
         # (fx, fy, cx, cy) already on the device: [4] shared or [B,4] (no host copy: graph-capturable)
         if K.dtype != torch.float64 or K.shape not in ((4,), (B, 4)):
             raise ValueError("device intrinsics must be float64 [4] or [B,4] = (fx, fy, cx, cy)")
-        intr_d, per_frame = K.contiguous(), int(K.dim() == 2)
-        return _backproject(depth, intr_d, per_frame, choose)
+        return K.contiguous(), int(K.dim() == 2)
     Kn = np.asarray(K, dtype=np.float64)
     if Kn.shape == (3, 3):
         intr = np.array([Kn[0, 0], Kn[1, 1], Kn[0, 2], Kn[1, 2]], np.float64)
@@ -724,7 +727,73 @@ def backproject(depth, K, choose):
         per_frame = 1
     else:
         raise ValueError("K must be [3,3] or [B,3,3], got %s" % (Kn.shape,))
-    return _backproject(depth, torch.from_numpy(intr).to(dev), per_frame, choose)
+    return torch.from_numpy(intr).to(dev), per_frame
+
+
+def point_item(depth_m, K, choose, rgb, labels, nrm_map, obj_cls, obj_kps, obj_ctr):
+    """The sampled points' input features and pose-training targets on the GPU (``ffb6d_point_item``): the half of
+    the datasets' ``get_item`` that reads ``choose`` (datasets/ycb/ycb_dataset.py:237-247 and ``get_pose_gt_info``
+    :348-386; datasets/linemod/linemod_dataset.py:284-293, 398-436), bit-identical to the reference.
+
+    :param depth_m: ``[B,H,W]`` float32 CUDA, metres (``dpt_m``); :param K: camera matrix as :func:`backproject`
+      takes it
+    :param choose: ``[B,1,N]`` or ``[B,N]`` int32 / int64 CUDA flat pixel indices
+    :param rgb: ``[B,H,W,3]`` uint8; :param labels: ``[B,H,W]`` uint8 label image
+    :param nrm_map: ``[B,H,W,3]`` float32, or float64 (rounded once to float32, as the reference's concat + cast does)
+    :param obj_cls: ``[B,n_obj]`` int32 class id per object slot (< 0: empty slot)
+    :param obj_kps: ``[B,n_obj,n_kps,3]`` float64 posed keypoints; :param obj_ctr: ``[B,n_obj,3]`` float64 posed centres
+      (the tables of :func:`ffb6d_b200.item.pose_gt_objects`)
+    :return: ``(cld_rgb_nrm [B,9,N] f32, labels [B,N] i32, kp_targ_ofst [B,N,n_kps,3] f32, ctr_targ_ofst [B,N,3] f32)``
+    """
+    tensors = ((depth_m, "depth_m"), (choose, "choose"), (rgb, "rgb"), (labels, "labels"), (nrm_map, "nrm_map"),
+               (obj_cls, "obj_cls"), (obj_kps, "obj_kps"), (obj_ctr, "obj_ctr"))
+    for t, name in tensors:
+        if not isinstance(t, torch.Tensor):
+            raise TypeError("%s must be a torch.Tensor, got %r" % (name, type(t)))
+    if depth_m.dim() != 3 or depth_m.dtype != torch.float32:
+        raise ValueError("depth_m must be float32 [B,H,W], got %s %s" % (depth_m.dtype, tuple(depth_m.shape)))
+    B, H, W = depth_m.shape
+    if choose.dtype not in _IDX:
+        raise ValueError("choose must be int32 or int64, got %s" % choose.dtype)
+    if not (choose.dim() == 2 or (choose.dim() == 3 and choose.shape[1] == 1)) or choose.shape[0] != B:
+        raise ValueError("choose must be [B,1,N] or [B,N], got %s" % (tuple(choose.shape),))
+    if rgb.dtype != torch.uint8 or tuple(rgb.shape) != (B, H, W, 3):
+        raise ValueError("rgb must be uint8 [B,H,W,3] = %s, got %s %s" % ((B, H, W, 3), rgb.dtype, tuple(rgb.shape)))
+    if labels.dtype != torch.uint8 or tuple(labels.shape) != (B, H, W):
+        raise ValueError("labels must be uint8 [B,H,W], got %s %s" % (labels.dtype, tuple(labels.shape)))
+    if nrm_map.dtype not in (torch.float32, torch.float64) or tuple(nrm_map.shape) != (B, H, W, 3):
+        raise ValueError("nrm_map must be float32 or float64 [B,H,W,3], got %s %s" % (nrm_map.dtype, tuple(nrm_map.shape)))
+    if obj_cls.dtype != torch.int32 or obj_cls.dim() != 2 or obj_cls.shape[0] != B:
+        raise ValueError("obj_cls must be int32 [B,n_obj], got %s %s" % (obj_cls.dtype, tuple(obj_cls.shape)))
+    n_obj = obj_cls.shape[1]
+    if obj_kps.dtype != torch.float64 or obj_kps.dim() != 4 or tuple(obj_kps.shape[:2]) != (B, n_obj) \
+            or obj_kps.shape[3] != 3:
+        raise ValueError("obj_kps must be float64 [B,n_obj,n_kps,3], got %s %s" % (obj_kps.dtype, tuple(obj_kps.shape)))
+    n_kps = obj_kps.shape[2]
+    if obj_ctr.dtype != torch.float64 or tuple(obj_ctr.shape) != (B, n_obj, 3):
+        raise ValueError("obj_ctr must be float64 [B,n_obj,3], got %s %s" % (obj_ctr.dtype, tuple(obj_ctr.shape)))
+    for t, name in tensors:
+        _need_cuda(t, name)
+        if t.device != depth_m.device:
+            raise ValueError("%s is on %s, depth_m on %s" % (name, t.device, depth_m.device))
+    dev = depth_m.device
+    intr_d, per_frame = _intrinsics_arg(K, B, dev)
+    ch = choose.reshape(B, -1).to(torch.int32).contiguous()
+    N = ch.shape[1]
+    nrm = nrm_map.to(torch.float32).contiguous()
+    cld_rgb_nrm = torch.empty((B, 9, N), dtype=torch.float32, device=dev)
+    labels_pt = torch.empty((B, N), dtype=torch.int32, device=dev)
+    kp_targ_ofst = torch.empty((B, N, n_kps, 3), dtype=torch.float32, device=dev)
+    ctr_targ_ofst = torch.empty((B, N, 3), dtype=torch.float32, device=dev)
+    args = [t.contiguous() for t in (depth_m, rgb, labels, obj_cls, obj_kps, obj_ctr)]
+    depth_c, rgb_c, labels_c, cls_c, kps_c, ctr_c = args
+    with torch.cuda.device(dev):
+        check(lib.ffb6d_point_item(depth_c.data_ptr(), B, H, W, intr_d.data_ptr(), per_frame, ch.data_ptr(), N,
+                                   rgb_c.data_ptr(), labels_c.data_ptr(), nrm.data_ptr(), cls_c.data_ptr(),
+                                   kps_c.data_ptr(), ctr_c.data_ptr(), n_obj, n_kps, cld_rgb_nrm.data_ptr(),
+                                   labels_pt.data_ptr(), kp_targ_ofst.data_ptr(), ctr_targ_ofst.data_ptr(),
+                                   _stream(dev)))
+    return cld_rgb_nrm, labels_pt, kp_targ_ofst, ctr_targ_ofst
 
 
 def sample_valid_pixels(depth, n_points, seed=0, min_depth=1e-8, return_count=False):

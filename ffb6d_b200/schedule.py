@@ -289,3 +289,63 @@ def build_ffb6d_indices_from_raw_depth(dpt_raw, cam_scale, K, n_points, seed=0, 
     inputs["choose"] = choose
     inputs["dpt_map_m"] = depth_m
     return inputs
+
+
+# the datasets' get_item returns None below this many valid pixels and the loader draws another frame
+# (ycb_dataset.py:219, linemod_dataset.py:266)
+MIN_VALID_PIXELS = 400
+_OBJECT_KEYS = ("RTs", "kp_3ds", "ctr_3ds", "cls_ids", "obj_cls", "obj_kps", "obj_ctr")
+
+
+def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points, seed=0, fill=True,
+                     min_valid=MIN_VALID_PIXELS, k=K_NEIGH, index_dtype=torch.int32, streams=None):
+    """The datasets' ``get_item`` for a batch on the GPU, from the decoded images to every ``item_dict`` key.
+
+    ``fill=True`` is YCB (datasets/ycb/ycb_dataset.py:204-336): depth completion of the raw depth, ``msk_dp``,
+    sampling, ``dpt_m`` and the 22 searches (as :func:`build_ffb6d_indices_from_raw_depth`).  ``fill=False`` is
+    LineMOD (datasets/linemod/linemod_dataset.py:251-386): the raw ``dpt_mm`` as it is, with ``cam_scale`` 1000.
+    Then :func:`ffb6d_b200.ops.point_item` builds ``cld_rgb_nrm``, ``labels`` and the offset targets of the
+    sampled points.  The points are drawn by :func:`ffb6d_b200.ops.sample_valid_pixels` with ``seed``: the
+    reference's distribution, not numpy's random stream.
+
+    :param dpt: ``[B,H,W]`` ``torch.uint16`` CUDA, the depth PNGs' raw values
+    :param cam_scale: raw units per metre (YCB ``meta['factor_depth']``, LineMOD 1000), used as float32
+    :param K: camera matrix as :func:`ffb6d_b200.ops.backproject` takes it
+    :param rgb: ``[B,H,W,3]`` uint8; :param labels: ``[B,H,W]`` uint8 label image
+    :param nrm_map: ``[B,H,W,3]`` float32 / float64 normal map (computed by the caller, see INTEGRATION.md)
+    :param objects: the per-object arrays of :func:`ffb6d_b200.item.pose_gt_objects`, as a dict of ``[B,...]``
+      arrays or tensors (what a DataLoader collates) or a list of B per-frame dicts
+    :param min_valid: frames with fewer valid depth pixels are flagged ``valid = False``: the reference returns
+      ``None`` for them and draws another frame, which a device batch cannot do, so the trainer masks them
+    :return: dict with the reference's keys ``rgb [B,3,H,W]`` uint8, ``cld_rgb_nrm [B,9,N]``, ``choose [B,1,N]``,
+      ``labels [B,N]``, ``rgb_labels [B,H,W]`` int32, ``dpt_map_m [B,H,W]``, ``RTs``, ``kp_targ_ofst [B,N,n_kps,3]``,
+      ``ctr_targ_ofst [B,N,3]``, ``cls_ids``, ``ctr_3ds``, ``kp_3ds``, the tensors of :func:`build_ffb6d_indices`,
+      and ``valid [B]`` bool
+    """
+    import numpy as np
+    from .ops import _fill_depth, sample_valid_pixels, point_item
+    if not isinstance(dpt, torch.Tensor) or dpt.dim() != 3 or dpt.dtype != torch.uint16:
+        raise ValueError("dpt must be a [B,H,W] torch.uint16 CUDA tensor")
+    dev = dpt.device
+    if fill:
+        filled, depth_m = _fill_depth(dpt, cam_scale)
+        choose, n_valid = sample_valid_pixels(filled, n_points, seed=seed, min_depth=MSK_DP_THRESHOLD,
+                                              return_count=True)
+    else:
+        # dpt_m = dpt_mm.astype(np.float32) / cam_scale; msk_dp = dpt_mm > 1e-6 is dpt_m > 0
+        cs = float(np.float32(cam_scale))
+        if not (cs > 0.0 and np.isfinite(cs)):
+            raise ValueError("cam_scale must be positive and finite, got %r" % (cam_scale,))
+        depth_m = dpt.to(torch.float32) / torch.tensor(cs, dtype=torch.float32, device=dev)
+        choose, n_valid = sample_valid_pixels(depth_m, n_points, seed=seed, min_depth=0.0, return_count=True)
+    if isinstance(objects, (list, tuple)):
+        objects = {key: np.stack([np.asarray(o[key]) for o in objects]) for key in _OBJECT_KEYS}
+    obj = {key: torch.as_tensor(objects[key]).to(dev) for key in _OBJECT_KEYS}
+    item = build_ffb6d_indices_from_depth(depth_m, K, choose, k=k, index_dtype=index_dtype, streams=streams)
+    cld_rgb_nrm, labels_pt, kp_targ_ofst, ctr_targ_ofst = point_item(
+        depth_m, K, choose, rgb, labels, nrm_map, obj["obj_cls"], obj["obj_kps"], obj["obj_ctr"])
+    item.update(rgb=rgb.permute(0, 3, 1, 2).contiguous(), cld_rgb_nrm=cld_rgb_nrm, choose=choose, labels=labels_pt,
+                rgb_labels=labels.to(torch.int32), dpt_map_m=depth_m, RTs=obj["RTs"], kp_targ_ofst=kp_targ_ofst,
+                ctr_targ_ofst=ctr_targ_ofst, cls_ids=obj["cls_ids"], ctr_3ds=obj["ctr_3ds"], kp_3ds=obj["kp_3ds"],
+                valid=n_valid >= int(min_valid))
+    return item

@@ -15,6 +15,8 @@ INTRINSICS = {
     "linemod": np.array([[572.4114, 0., 325.2611], [0., 573.57043, 242.04899], [0., 0., 1.]]),
     "ycb_K1": np.array([[1066.778, 0., 312.9869], [0., 1067.487, 241.3109], [0., 0., 1.]],
                        np.float32).astype(np.float64),
+    "ycb_K2": np.array([[1077.836, 0., 323.7872], [0., 1078.189, 279.6921], [0., 0., 1.]],
+                       np.float32).astype(np.float64),
 }
 
 
@@ -99,6 +101,70 @@ def fill_test_frames():
         "special_values": sv,
         "empty_top": make_raw_depth(3, h=37, w=91, empty_rows=5, empty_cols=(0, 40, 90)),
         "tiny": make_raw_depth(4, h=3, w=4, hole_frac=0.3, block_holes=0),
+    }
+
+
+def _rotation(rs):
+    q, r = np.linalg.qr(rs.randn(3, 3))
+    q = q * np.sign(np.diag(r))
+    return q if np.linalg.det(q) > 0 else -q
+
+
+def make_item_frame(seed, h=480, w=640, dataset="ycb", n_kps=8, cls_ids=(1, 5, 9), blobs=(1, 5, 9),
+                    hole_frac=0.1, nrm_dtype=np.float32, intrinsics=None):
+    """The decoded images and pose metadata of one dataset item, seeded: what ``get_item`` reads from disk.
+
+    * ``raw [H,W] uint16``: raw depth (YCB 1e4, LineMOD 1e3 units per metre) around 0.8-1.4 m, ``hole_frac`` of
+      the pixels missing;
+    * ``rgb [H,W,3] uint8``; ``nrm [H,W,3]`` unit normals in ``nrm_dtype``;
+    * ``labels [H,W] uint8``: background 0 and one elliptic blob per entry of ``blobs`` (later blobs paint over
+      earlier ones); a class in ``cls_ids`` without a blob is an object with no points, a blob class not in
+      ``cls_ids`` a label absent from the object list, a repeated class in ``cls_ids`` a duplicated object;
+    * ``poses``: YCB ``meta['poses']`` ``[3,4,n]``, LineMOD ``RT [3,4]``; ``cls_ids``; per object the mesh
+      keypoints ``kps [n_kps,3]`` and centre ``ctrs [3]`` of its class (float64, metres, a few cm across);
+    * ``K`` (the dataset's intrinsics, float32 for YCB as the reference's config holds them) and ``cam_scale``.
+    LineMOD frames hold one object of class 1 (``cls_ids=(1,)``, ``blobs=(1,)``)."""
+    rs = np.random.RandomState(seed)
+    ys, xs = np.mgrid[:h, :w]
+    d = 1.1 + 0.3 * np.sin(xs / 57.0) * np.cos(ys / 43.0) + 0.02 * rs.rand(h, w)
+    cam_scale = 10000.0 if dataset == "ycb" else 1000.0
+    raw = np.round(d * cam_scale).astype(np.uint16)
+    raw[rs.rand(h, w) < hole_frac] = 0
+    rgb = rs.randint(0, 256, (h, w, 3)).astype(np.uint8)
+    nrm = rs.normal(size=(h, w, 3))
+    nrm = (nrm / np.linalg.norm(nrm, axis=2, keepdims=True)).astype(nrm_dtype)
+    labels = np.zeros((h, w), np.uint8)
+    for c in blobs:
+        cy, cx = rs.uniform(0.1, 0.9) * h, rs.uniform(0.1, 0.9) * w
+        ry, rx = rs.uniform(0.08, 0.3) * h, rs.uniform(0.08, 0.3) * w
+        labels[((ys - cy) / ry) ** 2 + ((xs - cx) / rx) ** 2 < 1.0] = c
+    n = len(cls_ids)
+    Rt = [np.concatenate((_rotation(rs), rs.uniform(-0.2, 0.2, (3, 1)) + [[0.0], [0.0], [1.0]]), axis=1)
+          for _ in range(n)]
+    poses = np.stack(Rt, axis=2) if dataset == "ycb" else Rt[0]
+    mesh = {c: (rs.uniform(-0.08, 0.08, (n_kps, 3)), rs.uniform(-0.01, 0.01, 3)) for c in sorted(set(cls_ids))}
+    kps = [mesh[c][0] for c in cls_ids]
+    ctrs = [mesh[c][1] for c in cls_ids]
+    if intrinsics is None:
+        intrinsics = "ycb_K1" if dataset == "ycb" else "linemod"
+    K = INTRINSICS[intrinsics].astype(np.float32) if dataset == "ycb" else INTRINSICS[intrinsics]
+    return dict(raw=raw, rgb=rgb, nrm=nrm, labels=labels, poses=poses, cls_ids=np.array(cls_ids, np.uint32),
+                kps=kps, ctrs=ctrs, K=K, cam_scale=cam_scale)
+
+
+def item_test_frames():
+    """The frames of tests/golden/item_cases.npz by name, with the item shape each is sampled at:
+    ``{name: (frame, dataset, n_points, n_objects)}``.  Two full 480x640 frames at 12288 points (YCB with 8
+    keypoints, LineMOD with 16) and two small ones: a YCB frame with fewer valid pixels than points (the 'wrap'
+    padding), an absent label, an object without points and a duplicated class id; a LineMOD frame with a point
+    count that is no multiple of the kernel's tile."""
+    return {
+        "ycb_full": (make_item_frame(101, n_kps=8, cls_ids=(2, 7, 11, 7), blobs=(2, 7, 11, 4)), "ycb", 12288, 22),
+        "lm_full": (make_item_frame(102, dataset="linemod", n_kps=16, cls_ids=(1,), blobs=(1,)), "linemod", 12288, 2),
+        "ycb_small": (make_item_frame(103, h=24, w=40, n_kps=16, cls_ids=(3, 6, 3, 20), blobs=(3, 6, 9), hole_frac=0.4,
+                                      intrinsics="ycb_K2"), "ycb", 700, 22),
+        "lm_small": (make_item_frame(104, h=30, w=36, dataset="linemod", n_kps=8, cls_ids=(1,), blobs=(1,),
+                                     nrm_dtype=np.float64), "linemod", 500, 2),
     }
 
 

@@ -440,6 +440,33 @@ int ffb6d_backproject(const float *depth, int64_t B, int64_t H, int64_t W,
                       float *cld, float *pyr2, float *pyr4, float *pyr8, ffb6d_stream_t stream);
 
 /*
+ * The sampled points' network input and pose-training targets: the part of the datasets' get_item that reads
+ * `choose` (datasets/ycb/ycb_dataset.py:237-247 with get_pose_gt_info :348-386; datasets/linemod/
+ * linemod_dataset.py:284-293, 398-436).  For point p of frame b at pixel px = choose[b,p]:
+ *   cld_rgb_nrm [B,9,N] f32: channels 0-2 the point of ffb6d_backproject (same float64 arithmetic, rounded once:
+ *                            bitwise equal to its cld), 3-5 rgb[px] as float, 6-8 nrm[px]
+ *   labels_pt   [B,N] i32:   labels[px]
+ *   kp_targ_ofst [B,N,n_kps,3], ctr_targ_ofst [B,N,3] f32: the float64 point minus obj_kps[b,i] / obj_ctr[b,i],
+ *                            rounded once, for i the LAST slot with obj_cls[b,i] == labels[px]; +0.0 where none is
+ *   depth_m [B,H,W] f32 metres, intrinsics as ffb6d_backproject, choose [B,N] int32 (trusted, as there);
+ *   rgb [B,H,W,3] u8; labels [B,H,W] u8; nrm [B,H,W,3] f32; obj_cls [B,n_obj] i32 class id per slot (< 0: empty);
+ *   obj_kps [B,n_obj,n_kps,3] f64 and obj_ctr [B,n_obj,3] f64 posed keypoints and centres.
+ * 1 <= n_kps <= FFB6D_ITEM_MAX_KPS, 1 <= n_obj <= FFB6D_ITEM_MAX_OBJ.  Sizes, null pointers and alignment are
+ * checked before any launch (FFB6D_ERR_INVALID).  No allocation, no host synchronisation (capturable in a CUDA
+ * graph); deterministic.
+ */
+#define FFB6D_ITEM_MAX_KPS 32
+#define FFB6D_ITEM_MAX_OBJ 256
+int ffb6d_point_item(const float *depth_m, int64_t B, int64_t H, int64_t W,
+                     const double *intrinsics, int intrinsics_per_frame,
+                     const int *choose, int64_t N,
+                     const uint8_t *rgb, const uint8_t *labels, const float *nrm,
+                     const int *obj_cls, const double *obj_kps, const double *obj_ctr,
+                     int64_t n_obj, int64_t n_kps,
+                     float *cld_rgb_nrm, int *labels_pt, float *kp_targ_ofst, float *ctr_targ_ofst,
+                     ffb6d_stream_t stream);
+
+/*
  * Valid-pixel compaction + seeded point sampling on the device: replaces the reference's CPU recipe
  * (datasets/ycb/ycb_dataset.py:218-235: `nonzero()` of the depth mask, a random subset of N valid pixels --
  * or all of them repeated cyclically ('wrap') when fewer exist --, then a random permutation).
