@@ -260,69 +260,70 @@ gather_max_ncs_direct_kernel(const float *__restrict__ feat, const IdxT *__restr
 // a handful of 32-byte sectors instead of 32 (lanes along the query axis would scatter every
 // lane into its own sector); the max over the group is a log2(K)-step shuffle reduction.  Results
 // are collected in a [channel][query] shared-memory tile and written out coalesced.
+// A CTA takes one query per lane group (256 / K queries) and issues the loads of all its channels
+// before the first shuffle: eight loads in flight per thread, and short CTAs.  (H100: 10-20 % less
+// time on the sparse r2p gathers than 32 queries per CTA in rounds of four channels.)
+constexpr int KLANE_CH = 8;           // channels per CTA: many CTAs per frame keep ONE frame's rows in L2
+                                      // (ncu: with 64 channels per CTA twelve frames were in flight,
+                                      // 235 MB of rows thrashed the L2 and DRAM read them twice)
+
 template <typename IdxT, int KT>
 __global__ void __launch_bounds__(256)
 gather_max_ncs_klane_kernel(const float *__restrict__ feat, const IdxT *__restrict__ idx,
                             float *__restrict__ out, int C, int S, int Q)
 {
-    constexpr int TQ = 32;            // queries per CTA tile (one 128-byte output segment per channel)
-    constexpr int QPW = 32 / KT;      // queries per warp at a time
-    constexpr int CCH = 8;            // channels per CTA: many CTAs per frame keep ONE frame's rows in L2
-                                      // (ncu: with 64 channels per CTA twelve frames were in flight,
-                                      // 235 MB of rows thrashed the L2 and DRAM read them twice)
-    __shared__ float tile[CCH][TQ + 1];
+    constexpr int TQ = 256 / KT;      // queries per CTA: one per lane group
+    __shared__ float tile[KLANE_CH][TQ + 1];
     const int b = blockIdx.z;
     const int q_tile = blockIdx.x * TQ;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int grp = lane / KT, kl = lane % KT;
-    const float *fb = feat + (size_t)b * C * S;
-    for (int c0 = blockIdx.y * CCH; c0 < C; c0 += gridDim.y * CCH) {
-        const int cc = min(CCH, C - c0);
-        for (int ql = wid * QPW + grp; ql < TQ; ql += 8 * QPW) {
-            const int q = q_tile + ql;
-            const bool on = q < Q;
-            const int id = on ? (int)__ldg(idx + ((size_t)b * Q + q) * KT + kl) : 0;
-            const float *src = fb + (size_t)c0 * S + id;
-            for (int c = 0; c < cc; c += 4) {   // four independent loads in flight
-                float v[4];
+    const int ql = threadIdx.x / KT, kl = threadIdx.x % KT;
+    const int q = q_tile + ql;
+    const bool on = q < Q;
+    const int c0 = blockIdx.y * KLANE_CH;
+    const int cc = min(KLANE_CH, C - c0);
+    const int id = on ? (int)__ldg(idx + ((size_t)b * Q + q) * KT + kl) : 0;
+    const float *src = feat + ((size_t)b * C + c0) * S + id;
+    float v[KLANE_CH];
 #pragma unroll
-                for (int u = 0; u < 4; ++u) v[u] = (c + u < cc) ? __ldg(src + (size_t)(c + u) * S) : 0.f;
+    for (int c = 0; c < KLANE_CH; ++c) v[c] = (c < cc) ? __ldg(src + (size_t)c * S) : 0.f;
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
+    for (int c = 0; c < KLANE_CH; ++c) {
 #pragma unroll
-                    for (int o = KT / 2; o > 0; o >>= 1) v[u] = max_nan(v[u], __shfl_xor_sync(0xffffffffu, v[u], o));
-                    if (kl == 0 && c + u < cc) tile[c + u][ql] = v[u];
-                }
-            }
-        }
-        __syncthreads();
-        for (int t = threadIdx.x; t < cc * TQ; t += blockDim.x) {
-            const int c = t / TQ, ql = t % TQ;
-            if (q_tile + ql < Q) out[((size_t)b * C + c0 + c) * Q + q_tile + ql] = tile[c][ql];
-        }
-        __syncthreads();
+        for (int o = KT / 2; o > 0; o >>= 1) v[c] = max_nan(v[c], __shfl_xor_sync(0xffffffffu, v[c], o));
+        if (kl == 0 && c < cc) tile[c][ql] = v[c];
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < cc * TQ; t += blockDim.x) {
+        const int c = t / TQ, qt = t % TQ;
+        if (q_tile + qt < Q) out[((size_t)b * C + c0 + c) * Q + q_tile + qt] = tile[c][qt];
     }
 }
 
-// K == 1 with long rows (the `choose` gather): eight channels per thread, loads first
+// K == 1 with long rows (the `choose` gather): two channels per thread, loads first.  The picks are
+// scattered, so nearly every load misses to its own HBM line; two channels per thread make many short
+// CTAs, which keep more lines in flight than fewer CTAs with more loads each (H100, B = 32: 0.55 ms
+// against 0.60 ms with four channels and 0.64 ms with eight).
+constexpr int G1_CH = 2;
+
 template <typename IdxT>
 __global__ void __launch_bounds__(256)
 gather1_ncs_direct_kernel(const float *__restrict__ feat, const IdxT *__restrict__ idx,
                           float *__restrict__ out, int C, int S, int Q)
 {
     const int b = blockIdx.z;
-    const int c0 = blockIdx.y * 8;
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= Q) return;
     const int id = (int)__ldg(idx + (size_t)b * Q + q);
-    const float *src = feat + ((size_t)b * C + c0) * S + id;
-    float *dst = out + ((size_t)b * C + c0) * Q + q;
-    float v[8];
+    for (int c0 = blockIdx.y * G1_CH; c0 < C; c0 += gridDim.y * G1_CH) {   // grid.y is capped at 65535
+        const float *src = feat + ((size_t)b * C + c0) * S + id;
+        float *dst = out + ((size_t)b * C + c0) * Q + q;
+        float v[G1_CH];
 #pragma unroll
-    for (int c = 0; c < 8; ++c) v[c] = (c0 + c < C) ? __ldg(src + (size_t)c * S) : 0.f;
+        for (int c = 0; c < G1_CH; ++c) v[c] = (c0 + c < C) ? __ldg(src + (size_t)c * S) : 0.f;
 #pragma unroll
-    for (int c = 0; c < 8; ++c)
-        if (c0 + c < C) __stcs(dst + (size_t)c * Q, v[c]);
+        for (int c = 0; c < G1_CH; ++c)
+            if (c0 + c < C) __stcs(dst + (size_t)c * Q, v[c]);
+    }
 }
 
 // ------------------------------------------------------------------ NSC (channels last)
@@ -713,12 +714,12 @@ static int launch_ncs(const float *feat, const IdxT *idx, float *out, int64_t B,
                                       (int)q_per_cta);
         FFB6D_LAUNCH_OK("gather_max_ncs_staged_kernel");
     } else if (KT == 1) {
-        dim3 grid((unsigned)ceil_div(Q, 256), (unsigned)ceil_div(C, 8), (unsigned)B);
+        dim3 grid((unsigned)ceil_div(Q, 256), (unsigned)std::min<int64_t>(ceil_div(C, G1_CH), 65535), (unsigned)B);
         gather1_ncs_direct_kernel<IdxT><<<grid, 256, 0, st>>>(feat, idx, out, (int)C, (int)S, (int)Q);
         FFB6D_LAUNCH_OK("gather1_ncs_direct_kernel");
     } else if ((KT == 8 || KT == 16 || KT == 32) && !env().gather_direct) {
         if constexpr (KT == 8 || KT == 16 || KT == 32) {
-            dim3 grid((unsigned)ceil_div(Q, 32), (unsigned)std::min<int64_t>(ceil_div(C, 8), 65535), (unsigned)B);
+            dim3 grid((unsigned)ceil_div(Q, 256 / KT), (unsigned)ceil_div(C, KLANE_CH), (unsigned)B);
             gather_max_ncs_klane_kernel<IdxT, KT><<<grid, 256, 0, st>>>(feat, idx, out, (int)C, (int)S, (int)Q);
             FFB6D_LAUNCH_OK("gather_max_ncs_klane_kernel");
         }
