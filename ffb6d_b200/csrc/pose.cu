@@ -291,8 +291,13 @@ __global__ void best_fit_kernel(const float *__restrict__ A, const float *__rest
             for (int q = p + 1; q < 3; ++q) {
                 double al = 0, be = 0, ga = 0;
                 for (int r = 0; r < 3; ++r) al += H[r][p] * H[r][p], be += H[r][q] * H[r][q], ga += H[r][p] * H[r][q];
-                if (fabs(ga) <= 1e-300 || fabs(ga) <= 1e-17 * sqrt(al * be)) continue;
-                off = fmax(off, fabs(ga) / sqrt(al * be));
+                // a pair is done when its columns are orthogonal to working precision, or when one of them is
+                // negligible next to the other (norm ratio <= 1e-15, below the rank cut-off `tiny` further down, so
+                // its direction is never used: rotating it only spins on rounding noise).  sqrt(al) * sqrt(be),
+                // not sqrt(al * be): the product underflows to 0 for spreads of float32 subnormals.
+                const double nrm = sqrt(al) * sqrt(be);
+                if (fabs(ga) <= 1e-17 * nrm || fmin(al, be) <= 1e-30 * fmax(al, be)) continue;
+                off = fmax(off, fabs(ga) / nrm);
                 const double zeta = (be - al) / (2.0 * ga);
                 const double tt = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
                 const double cs = 1.0 / sqrt(1.0 + tt * tt), sn = cs * tt;
@@ -314,12 +319,25 @@ __global__ void best_fit_kernel(const float *__restrict__ A, const float *__rest
     double U[3][3], W[3][3];
     for (int k = 0; k < 3; ++k)
         for (int r = 0; r < 3; ++r) W[r][k] = V[r][ord[k]];
+    // U = H V / S where a singular value is above `tiny`; the rest of the basis is completed so that U stays
+    // orthonormal: rank 3 none, rank 2 (coplanar) U2 = U0 x U1, rank 1 (collinear, or M = 2) U1 = the coordinate
+    // axis least aligned with U0 made orthogonal to it, then U2 = U0 x U1, rank 0 (all points identical) the
+    // identity.  Below rank 3 the fit is not unique: any such completion gives a proper rotation (after the
+    // reflection flip) that reaches the least-squares minimum, as every choice of numpy's SVD does.
     const double tiny = 1e-12 * fmax(sg[ord[0]], 1e-300);
     for (int k = 0; k < 2; ++k)
         for (int r = 0; r < 3; ++r) U[r][k] = sg[ord[k]] > tiny ? H[r][ord[k]] / sg[ord[k]] : (r == k ? 1.0 : 0.0);
+    if (sg[ord[0]] > tiny && sg[ord[1]] <= tiny) {
+        int k = 0;
+        for (int r = 1; r < 3; ++r)
+            if (fabs(U[r][0]) < fabs(U[k][0])) k = r;
+        for (int r = 0; r < 3; ++r) U[r][1] = (r == k ? 1.0 : 0.0) - U[k][0] * U[r][0];      // Gram-Schmidt of e_k
+        const double nu = sqrt(U[0][1] * U[0][1] + U[1][1] * U[1][1] + U[2][1] * U[2][1]);    // >= sqrt(2/3)
+        for (int r = 0; r < 3; ++r) U[r][1] /= nu;
+    }
     if (sg[ord[2]] > tiny)
         for (int r = 0; r < 3; ++r) U[r][2] = H[r][ord[2]] / sg[ord[2]];
-    else {                                           // coplanar keypoints: complete the basis
+    else {                                           // rank <= 2: complete the basis
         U[0][2] = U[1][0] * U[2][1] - U[2][0] * U[1][1];
         U[1][2] = U[2][0] * U[0][1] - U[0][0] * U[2][1];
         U[2][2] = U[0][0] * U[1][1] - U[1][0] * U[0][1];

@@ -152,6 +152,98 @@ def make_item_frame(seed, h=480, w=640, dataset="ycb", n_kps=8, cls_ids=(1, 5, 9
                 kps=kps, ctrs=ctrs, K=K, cam_scale=cam_scale)
 
 
+def _far_votes(rs, n, anchors, min_dist=0.25, sep=0.0):
+    """``n`` uniform votes at least ``min_dist`` from every anchor and ``sep`` from each other: nonsense that sits
+    near no refinement or bandwidth boundary, and (with ``sep`` = 0.2 m) too far from anything to move under a
+    0.04 m Gaussian kernel, so a mean shift over it stops after a few rounds."""
+    out = []
+    while len(out) < n:
+        v = rs.uniform(-0.7, 0.7, 3) + [0.0, 0.0, 1.0]
+        if np.linalg.norm(np.asarray(anchors) - v, axis=1).min() >= min_dist and \
+                (not out or np.linalg.norm(np.asarray(out) - v, axis=1).min() >= sep):
+            out.append(v)
+    return np.array(out)
+
+
+def make_pose_frame(seed, n_kps=8):
+    """The network's per-point predictions for one frame, seeded: what ``cal_frame_poses`` reads.
+
+    Four classes and background, 2000 points, class radii 8, 12, 10, 8 cm (``cls_radius``, indexed by ``cls - 1``;
+    a fifth entry of 6 cm exists only so that indexing by ``cls`` is a wrong answer rather than an IndexError).
+    Objects 1-3 are 150, 520 and 430 points; their points vote the object's centre and keypoints with 4 mm noise,
+    5 % of them nonsense far from everything (none of class 1's centre votes).  Groups placed so that every rule of
+    the centre-clustering refinement and of the centre-label filter moves some keypoint by millimetres:
+
+    * 40 points of object 2 labelled 3: centre votes at object 2's centre, keypoint votes 1.8 cm off object 2's
+      keypoints.  Refinement gives them to class 2, whose keypoints they pull.
+    * 30 points labelled 3 whose centre votes lie 7.2 cm from object 1's centre (between 0.8 r of class 1, 6.4 cm,
+      and 0.8 r of classes 2 and 3, 9.6 and 8 cm), keypoint votes 1.8 cm off object 3's keypoints.  They stay in
+      class 3, where the centre-label filter drops them; kept, they pull class 3's keypoints.
+    * 60 background points (class 0) whose centre votes lie 1.5 cm from object 2's centre and keypoint votes 2 cm
+      off its keypoints: refinement must leave them alone (it only relabels object points).
+    * class 4: a bit-exact copy of class 1's points (one object segmented twice).  Both vote the same centre, the
+      distance tie goes to the lower class id, and refinement leaves class 4 without points.
+
+    The other background points vote nonsense.  Returns ``pcld [N,3]``, ``mask [N] int64``, ``ctr_of [1,N,3]``,
+    ``kp_of [n_kps,N,3]`` (float32), ``mesh {cls: [n_kps+1,3] float64}`` (centre last), ``cls_radius`` and
+    ``poses {cls: [3,4]}`` the votes were made from."""
+    rs = np.random.RandomState(seed)
+    counts = {1: 150, 2: 520, 3: 430}
+    radius = [0.08, 0.12, 0.10, 0.08, 0.06]
+    mesh, poses, ctr_cam, kps_cam = {}, {}, {}, {}
+    ctr_choices = [np.array([-0.25, 0.0, 1.0]), np.array([0.05, 0.15, 0.9]), np.array([0.25, -0.15, 1.1])]
+    for c in (1, 2, 3):
+        mesh[c] = np.concatenate((rs.uniform(-0.08, 0.08, (n_kps, 3)), rs.uniform(-0.01, 0.01, (1, 3))))
+        t = ctr_choices[c - 1] + rs.uniform(-0.03, 0.03, 3)
+        poses[c] = np.concatenate((_rotation(rs), t[:, None]), axis=1)
+        cam = mesh[c] @ poses[c][:, :3].T + poses[c][:, 3]
+        kps_cam[c], ctr_cam[c] = cam[:n_kps], cam[n_kps]
+    anchors = np.concatenate([np.concatenate((kps_cam[c], ctr_cam[c][None])) for c in (1, 2, 3)])
+
+    def votes(n, target, nonsense=0.05):
+        v = target + rs.normal(0, 0.004, (n, 3))
+        bad = rs.rand(n) < nonsense
+        if bad.any():
+            v[bad] = _far_votes(rs, int(bad.sum()), anchors, sep=0.2)
+        return v
+
+    def group(n, label, ctr_target, ctr_noise, kps_target):
+        pts.append(ctr_target + rs.normal(0, 0.03, (n, 3)))
+        lab.append(np.full(n, label))
+        ctr_v.append(ctr_target + rs.normal(0, ctr_noise, (n, 3)))
+        kp_v.append(np.stack([kps_target[k] + rs.normal(0, 0.004, (n, 3)) for k in range(n_kps)]))
+
+    pts, lab, ctr_v, kp_v = [], [], [], []
+    for c in (1, 2, 3):
+        n = counts[c]
+        pts.append(ctr_cam[c] + rs.normal(0, 0.03, (n, 3)))
+        lab.append(np.full(n, c))
+        ctr_v.append(votes(n, ctr_cam[c], 0.0 if c == 1 else 0.05))
+        kp_v.append(np.stack([votes(n, kps_cam[c][k]) for k in range(n_kps)]))
+    group(40, 3, ctr_cam[2], 0.004, kps_cam[2] + [0.015, -0.01, 0.0])                 # mislabelled object 2
+    group(30, 3, ctr_cam[1] + [-0.072, 0.0, 0.0], 0.0015, kps_cam[3] + [0.0, 0.015, -0.01])   # between radii
+    group(60, 0, ctr_cam[2] + [0.0, 0.0, 0.015], 0.004, kps_cam[2] + [-0.012, 0.0, 0.016])    # background
+    nb = 2000 - sum(len(p) for p in pts) - counts[1]
+    pts.append(rs.uniform(-0.5, 0.5, (nb, 3)) + [0.0, 0.0, 1.0])
+    lab.append(np.zeros(nb, np.int64))
+    ctr_v.append(_far_votes(rs, nb, anchors))
+    kp_v.append(np.stack([_far_votes(rs, nb, anchors) for _ in range(n_kps)]))
+    pcld = np.concatenate(pts).astype(np.float32)
+    mask = np.concatenate(lab).astype(np.int64)
+    ctr_of = (pcld - np.concatenate(ctr_v)).astype(np.float32)[None]
+    kp_of = (pcld[None] - np.concatenate(kp_v, axis=1)).astype(np.float32)
+    perm = rs.permutation(len(pcld))
+    pcld, mask, ctr_of, kp_of = pcld[perm], mask[perm], ctr_of[:, perm], kp_of[:, perm]
+    # class 4: a copy of class 1's points, in the same order, appended at the end
+    one = np.flatnonzero(mask == 1)
+    pcld = np.concatenate((pcld, pcld[one]))
+    mask = np.concatenate((mask, np.full(len(one), 4)))
+    ctr_of = np.concatenate((ctr_of, ctr_of[:, one]), axis=1)
+    kp_of = np.concatenate((kp_of, kp_of[:, one]), axis=1)
+    mesh[4], poses[4] = mesh[1], poses[1]
+    return dict(pcld=pcld, mask=mask, ctr_of=ctr_of, kp_of=kp_of, mesh=mesh, cls_radius=radius, poses=poses)
+
+
 def item_test_frames():
     """The frames of tests/golden/item_cases.npz by name, with the item shape each is sampled at:
     ``{name: (frame, dataset, n_points, n_objects)}``.  Two full 480x640 frames at 12288 points (YCB with 8

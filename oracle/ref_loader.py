@@ -194,3 +194,49 @@ def pose_functions():
                 fns[n] = ns[n]
         _pose_fns = fns
     return _pose_fns
+
+
+class _Stub:
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+def frame_pose_functions(mesh_kps, cls_radius):
+    """{'cal_frame_poses', 'cal_frame_poses_lm'} (utils/pvn3d_eval_utils_kpls.py:65-160, 220-284) executed from
+    the reference's own source text on the CPU, with the module-level objects they read stubbed: ``config.ycb_r_lst``
+    = ``cls_radius``; ``cls_lst[i]`` = ``i + 1`` and ``bs_utils.get_kps`` / ``get_ctr`` = the rows of
+    ``mesh_kps[cls_id]`` ``[n_kps+1,3]`` (centre last); ``bs_utils_lm`` the same, keyed by ``obj_id``;
+    ``MeanShiftTorch`` and ``best_fit_transform`` the reference's own (:func:`pose_functions`).  The functions
+    call ``.cuda()``: run them under :func:`cuda_is_identity`."""
+    if not reference_sources_present():
+        raise RuntimeError("reference sources not found under %s" % REF_ROOT)
+    import torch
+    base = pose_functions()
+    path = os.path.join(REF_ROOT, "ffb6d", "utils", "pvn3d_eval_utils_kpls.py")
+    bs = _Stub(get_kps=lambda cls, kp_type="farthest", ds_type="ycb": mesh_kps[int(cls)][:-1].copy(),
+               get_ctr=lambda cls, ds_type="ycb": mesh_kps[int(cls)][-1].copy())
+    ns = {"torch": torch, "np": np, "config": _Stub(ycb_r_lst=list(cls_radius)), "bs_utils": bs, "bs_utils_lm": bs,
+          "cls_lst": list(range(1, len(cls_radius) + 1)), "MeanShiftTorch": base["MeanShiftTorch"],
+          "best_fit_transform": base["best_fit_transform"]}
+    with open(path) as fh:
+        tree = ast.parse(fh.read())
+    names = ("cal_frame_poses", "cal_frame_poses_lm")
+    for node in tree.body:
+        if isinstance(node, ast.FunctionDef) and node.name in names:
+            exec(compile(ast.Module(body=[node], type_ignores=[]), path, "exec"), ns)
+    return {n: ns[n] for n in names}
+
+
+class cuda_is_identity:
+    """Context manager: ``Tensor.cuda()`` returns the tensor itself (the reference's eval code on the CPU)."""
+
+    def __enter__(self):
+        import torch
+        self._saved = torch.Tensor.cuda
+        torch.Tensor.cuda = lambda self, *a, **k: self
+        return self
+
+    def __exit__(self, *exc):
+        import torch
+        torch.Tensor.cuda = self._saved
+        return False

@@ -426,6 +426,32 @@ def pose_cases():
     return out
 
 
+POSE_FRAME_SEED = 0
+
+
+def pose_frame_cases():
+    """Outputs of the reference's cal_frame_poses / cal_frame_poses_lm (executed from its source on the CPU, module
+    objects stubbed: oracle/ref_loader.frame_pose_functions) on ffb6d_b200.synthetic.make_pose_frame(0); the inputs
+    are regenerated by the tests and tied to this fixture by their sha256."""
+    from ffb6d_b200.synthetic import make_pose_frame
+    from oracle.pose_oracle import FRAME_VARIANTS, frame_input_sha256
+    fr = make_pose_frame(POSE_FRAME_SEED)
+    fns = R.frame_pose_functions(fr["mesh"], fr["cls_radius"])
+    t = [torch.from_numpy(fr[k]) for k in ("pcld", "mask", "ctr_of", "kp_of")]
+    out = {"input_sha256": np.array(frame_input_sha256(fr)), "seed": np.array(POSE_FRAME_SEED)}
+    with R.cuda_is_identity():
+        for name, use_ctr, flt in FRAME_VARIANTS:
+            ids, poses, kps = fns["cal_frame_poses"](*t, use_ctr, 5, flt, None, None)
+            out[name + "/ids"] = np.asarray(ids, np.int64)
+            out[name + "/poses"] = np.stack(poses)
+            for c, k in zip(ids, kps):
+                out["%s/kps_%d" % (name, c)] = np.asarray(k)
+        lm = [fns["cal_frame_poses_lm"](*t, True, 2, True, 1)[0],
+              fns["cal_frame_poses_lm"](t[0], torch.zeros_like(t[1]), *t[2:], True, 2, True, 1)[0]]
+        out["lm/poses"] = np.stack(lm)
+    return out
+
+
 STRESS_SIZES = (4096, 40960, 131072)
 STRESS_ROWS = 1024          # seeded sample of query rows kept per stress-sweep search
 
@@ -501,7 +527,8 @@ def main():
     if len(sys.argv) > 2 and sys.argv[1] == "--only":      # regenerate one fixture file
         which = sys.argv[2]
         fn = {"lfa": lfa_cases, "knn": knn_cases, "gather": gather_cases, "grid": grid_cases, "train": train_cases,
-              "fusion": fusion_cases, "pose": pose_cases, "refcheck": refcheck_cases}[which]
+              "fusion": fusion_cases, "pose": pose_cases, "pose_frame": pose_frame_cases,
+              "refcheck": refcheck_cases}[which]
         np.savez_compressed(os.path.join(OUT, which + "_cases.npz"), **fn())
         print("rewrote", which + "_cases.npz")
         return
@@ -512,6 +539,7 @@ def main():
     np.savez_compressed(os.path.join(OUT, "fusion_cases.npz"), **fusion_cases())
     np.savez_compressed(os.path.join(OUT, "train_cases.npz"), **train_cases())
     np.savez_compressed(os.path.join(OUT, "pose_cases.npz"), **pose_cases())
+    np.savez_compressed(os.path.join(OUT, "pose_frame_cases.npz"), **pose_frame_cases())
     np.savez_compressed(os.path.join(OUT, "refcheck_cases.npz"), **refcheck_cases())
     dig = {"generator": "ffb6d_b200.synthetic.make_frame", "frames": {}}
     for seed, n in ((0, 12288), (1, 12288), (2, 3072)):
