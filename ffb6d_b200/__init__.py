@@ -16,6 +16,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   ``get_item`` from the raw depth PNG to the 22 index tensors.
 * :func:`build_ffb6d_item` -- the datasets' whole ``get_item`` for a batch on the GPU (:func:`point_item` builds
   the sampled points' input and pose targets; :func:`pose_gt_objects` is the per-object half that stays on the host).
+* :func:`rgb_add_noise`, :func:`add_real_back` -- the datasets' synthetic-frame augmentation
+  (datasets/ycb/ycb_dataset.py:79-163, datasets/linemod/linemod_dataset.py:114-186) on the GPU; the scalar draws stay
+  in the worker (:mod:`ffb6d_b200.augment`).
 * :mod:`ffb6d_b200.pose` -- ``MeanShiftTorch``, ``best_fit_transform``, ``cal_frame_poses(_lm)``
   (utils/meanshift_pytorch.py:27-57, utils/pvn3d_eval_utils_kpls.py:28-160, 220-284): keypoint voting on the GPU.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
@@ -32,13 +35,14 @@ import importlib
 _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbour", "relative_pos_encoding",
         "choose_gather", "grid_sub_sampling", "KnnGrid", "backproject", "fusion_mlp", "fusion_mlp_pack",
         "PackedWeight", "fold_batchnorm", "att_pool", "sample_valid_pixels", "check_indices", "mean_shift_fit", "best_fit_transform",
-        "fill_missing", "segment_plan", "segment_sum", "point_item")
+        "fill_missing", "segment_plan", "segment_sum", "point_item", "rgb_add_noise", "add_real_back",
+        "aug_noise_field")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "_lib")
 
 __all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM) + ["randla", "modules", "fusion", "pose", "DataProcessing"]
 

@@ -1011,3 +1011,113 @@ def best_fit_transform(A, B):
     with torch.cuda.device(A.device):
         check(lib.ffb6d_best_fit_transform(A.data_ptr(), B.data_ptr(), G, M, T.data_ptr(), _stream(A.device)))
     return T[0] if single else T
+
+
+def _aug_image(t, name, shape=None, dtype=torch.uint8):
+    _need_cuda(t, name)
+    if t.dtype != dtype or (shape is not None and tuple(t.shape) != tuple(shape)):
+        raise ValueError("%s must be %s %s, got %s %s" % (name, dtype, shape, t.dtype, tuple(t.shape)))
+    return t.contiguous()
+
+
+def rgb_add_noise(rgb, plan, seed, noise=None):
+    """The datasets' ``rgb_add_noise`` (datasets/ycb/ycb_dataset.py:107-143, linemod_dataset.py:142-164) for a batch
+    on the GPU (``ffb6d_rgb_add_noise``).
+
+    :param rgb: ``[B,H,W,3]`` uint8 CUDA, H, W >= 32 (the channel roles are the reference's: it feeds RGB data to
+      ``COLOR_BGR2HSV``)
+    :param plan: ``[B, REC_LEN]`` float64 numpy records of :func:`ffb6d_b200.augment.draw_rgb_noise`
+    :param seed: key of the per-pixel normal draws (frame b of the batch, the record's pass); use one seed per batch
+    :param noise: optional ``[2,B,H,W,3]`` float64 CUDA normals to use instead of the generator's (the first for
+      ``gaussian_noise``, the second for YCB's ``normal(0, 7)``), e.g. to replay numpy's stream
+    :return: ``[B,H,W,3]`` uint8
+    """
+    from . import augment as A
+    _need_cuda(rgb, "rgb")
+    if rgb.dtype != torch.uint8 or rgb.dim() != 4 or rgb.shape[3] != 3:
+        raise ValueError("rgb must be uint8 [B,H,W,3], got %s %s" % (rgb.dtype, tuple(rgb.shape)))
+    B, H, W, _ = rgb.shape
+    plan = np.ascontiguousarray(plan, dtype=np.float64)
+    if plan.shape != (B, A.REC_LEN):
+        raise ValueError("plan must be float64 [B, %d] = [%d, %d], got %s" % (A.REC_LEN, B, A.REC_LEN, plan.shape))
+    if not (0 <= int(seed) < 1 << 64):
+        raise ValueError("seed must fit 64 bits, got %r" % (seed,))
+    dev = rgb.device
+    if noise is not None:
+        noise = _aug_image(noise, "noise", (2, B, H, W, 3), torch.float64)
+        if noise.device != dev:
+            raise ValueError("noise is on %s, rgb on %s" % (noise.device, dev))
+    src = rgb.contiguous()
+    plan_d = torch.from_numpy(plan).to(dev)
+    out = torch.empty_like(src)
+    work = torch.empty_like(src)
+    with torch.cuda.device(dev):
+        check(lib.ffb6d_rgb_add_noise(src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), int(seed),
+                                      None if noise is None else noise.data_ptr(), out.data_ptr(), work.data_ptr(),
+                                      _stream(dev)))
+    return out
+
+
+def add_real_back(rgb, labels, dpt, back_rgb, back_labels, back_dpt, apply_rgb=None, dataset="ycb", active=None):
+    """The datasets' ``add_real_back`` (datasets/ycb/ycb_dataset.py:145-163, linemod_dataset.py:166-186) for a batch
+    on the GPU (``ffb6d_add_real_back``), after the worker has loaded the background frames.
+
+    :param rgb: ``[B,H,W,3]`` uint8; :param labels: ``[B,H,W]`` uint8 (the frame's labels; 0 is background)
+    :param dpt: ``[B,H,W]`` uint16 raw depth (YCB ``dpt_um``; LineMOD ``dpt_mm.astype(np.uint16)``)
+    :param back_rgb: ``[B,H,W,3]`` uint8; :param back_labels: ``[B,H,W]`` or ``[B,H,W,3]`` uint8 (the background
+      frame's label image, YCB, or mask, LineMOD); :param back_dpt: ``[B,H,W]`` uint16
+    :param apply_rgb: LineMOD: per-frame bools, the ``rand() < 0.6`` draw (YCB always composes the colour image)
+    :param dataset: ``'ycb'`` or ``'linemod'``; :param active: per-frame bools, frames that go through
+      ``add_real_back`` at all (default: every frame); the others pass through unchanged
+    :return: ``(rgb [B,H,W,3] uint8, dpt [B,H,W] uint16)``; the composed depth is uint16 and feeds
+      :func:`fill_missing` as it is
+    """
+    if dataset not in ("ycb", "linemod"):
+        raise ValueError("dataset must be 'ycb' or 'linemod', got %r" % (dataset,))
+    _need_cuda(rgb, "rgb")
+    if rgb.dtype != torch.uint8 or rgb.dim() != 4 or rgb.shape[3] != 3:
+        raise ValueError("rgb must be uint8 [B,H,W,3], got %s %s" % (rgb.dtype, tuple(rgb.shape)))
+    B, H, W, _ = rgb.shape
+    labels = _aug_image(labels, "labels", (B, H, W))
+    dpt = _aug_image(dpt, "dpt", (B, H, W), torch.uint16)
+    back_rgb = _aug_image(back_rgb, "back_rgb", (B, H, W, 3))
+    _need_cuda(back_labels, "back_labels")
+    if back_labels.dim() == 3:
+        back_labels = back_labels[..., None]
+    ch = back_labels.shape[-1] if back_labels.dim() == 4 else 0
+    back_labels = _aug_image(back_labels, "back_labels", (B, H, W, ch if ch in (1, 3) else -1))
+    back_dpt = _aug_image(back_dpt, "back_dpt", (B, H, W), torch.uint16)
+    for t, name in ((labels, "labels"), (dpt, "dpt"), (back_rgb, "back_rgb"), (back_labels, "back_labels"),
+                    (back_dpt, "back_dpt")):
+        if t.device != rgb.device:
+            raise ValueError("%s is on %s, rgb on %s" % (name, t.device, rgb.device))
+    act = np.ones(B, bool) if active is None else np.asarray(active, bool).reshape(-1)
+    if dataset == "ycb":
+        col = np.ones(B, bool) if apply_rgb is None else np.asarray(apply_rgb, bool).reshape(-1)
+    else:
+        if apply_rgb is None:
+            raise ValueError("LineMOD needs apply_rgb (the frame's rand() < 0.6 draw)")
+        col = np.asarray(apply_rgb, bool).reshape(-1)
+    if act.shape != (B,) or col.shape != (B,):
+        raise ValueError("apply_rgb and active must have one entry per frame (%d)" % B)
+    dev = rgb.device
+    mode = torch.from_numpy((act * (1 + 2 * col)).astype(np.uint8)).to(dev)
+    src = rgb.contiguous()
+    rgb_out = torch.empty_like(src)
+    dpt_out = torch.empty_like(dpt)
+    with torch.cuda.device(dev):
+        check(lib.ffb6d_add_real_back(src.data_ptr(), labels.data_ptr(), dpt.data_ptr(), back_rgb.data_ptr(),
+                                      back_labels.data_ptr(), ch, back_dpt.data_ptr(), mode.data_ptr(),
+                                      0 if dataset == "ycb" else 1, B, H, W, rgb_out.data_ptr(), dpt_out.data_ptr(),
+                                      _stream(dev)))
+    return rgb_out, dpt_out
+
+
+def aug_noise_field(seed, B, H, W, stage, device="cuda"):
+    """The ``[B,H,W,3]`` float64 normals that :func:`rgb_add_noise` draws for ``(seed, frame, stage)``; stage
+    ``2*pass`` is ``gaussian_noise``'s, ``2*pass + 1`` YCB's ``normal(0, 7)``'s (``ffb6d_aug_noise_field``)."""
+    out = torch.empty((B, H, W, 3), dtype=torch.float64, device=device)
+    _need_cuda(out, "out")
+    with torch.cuda.device(out.device):
+        check(lib.ffb6d_aug_noise_field(int(seed), B, H, W, int(stage), out.data_ptr(), _stream(out.device)))
+    return out

@@ -272,3 +272,43 @@ def image_pyramid_np(dpt_xyz):
     H, W, _ = dpt_xyz.shape
     return {sr: np.ascontiguousarray(dpt_xyz[:(H // sr) * sr:sr, :(W // sr) * sr:sr, :].reshape(-1, 3))
             for sr in (1, 2, 4, 8)}
+
+
+def make_aug_frame(seed, h=40, w=48, dataset="ycb", mask_channels=1):
+    """A seeded frame and background frame for the augmentation (``rgb_add_noise`` / ``add_real_back``).
+
+    The colour image mixes smooth gradients with noise and has bands of special pixels: saturated (S = 255 at
+    V = 255 and below), grey (S = 0), black and white.  ``labels`` marks object blobs (YCB class ids, LineMOD 0/1);
+    ``raw`` is uint16 depth with holes.  The background has its own colour, depth (with holes) and label image:
+    YCB class ids, or a LineMOD 0/255 mask with ``mask_channels`` channels."""
+    rs = np.random.RandomState(seed)
+    yy, xx = np.mgrid[:h, :w].astype(np.float64)
+    base = np.stack([128 + 127 * np.sin(xx / 7.0 + k) * np.cos(yy / 5.0 - k) for k in range(3)], -1)
+    rgb = np.clip(base + rs.randn(h, w, 3) * 20, 0, 255).astype(np.uint8)
+    specials = np.array([[255, 0, 0], [0, 255, 0], [0, 0, 255], [255, 255, 0], [200, 0, 90], [128, 128, 128],
+                         [37, 37, 37], [0, 0, 0], [255, 255, 255], [255, 254, 255], [1, 0, 0], [254, 255, 0]],
+                        np.uint8)
+    rgb[0, : len(specials)] = specials
+    rgb[h // 2, -len(specials):] = specials[::-1]
+    rgb[-1, :] = rs.randint(0, 256, (w, 3)).astype(np.uint8)
+    cls = rs.randint(1, 22, 3) if dataset == "ycb" else np.ones(3, np.int64)
+    labels = np.zeros((h, w), np.uint8)
+    for c in cls:
+        cy, cx, r = rs.randint(0, h), rs.randint(0, w), rs.randint(4, 10)
+        labels[(yy - cy) ** 2 + (xx - cx) ** 2 < r * r] = c
+    raw = (5000 + 3000 * rs.rand(h, w)).astype(np.uint16)
+    raw[rs.rand(h, w) < 0.3] = 0
+    back_rgb = rs.randint(0, 256, (h, w, 3)).astype(np.uint8)
+    back_dpt = (4000 + 4000 * rs.rand(h, w)).astype(np.uint16)
+    back_dpt[rs.rand(h, w) < 0.2] = 0
+    blob = (yy - h / 3) ** 2 + (xx - w / 2) ** 2 < (min(h, w) / 4) ** 2
+    if dataset == "ycb":
+        back_labels = np.where(blob, rs.randint(1, 22), 0).astype(np.uint8)
+        back_labels[rs.rand(h, w) < 0.05] = 3
+    else:
+        m = np.where(blob, 255, 0).astype(np.uint8)
+        m[rs.rand(h, w) < 0.05] = 254
+        back_labels = m if mask_channels == 1 else np.repeat(m[..., None], 3, 2)
+        if mask_channels == 3:
+            back_labels[..., 1] = 255 - back_labels[..., 1]      # only channel 0 may matter
+    return dict(rgb=rgb, labels=labels, raw=raw, back_rgb=back_rgb, back_labels=back_labels, back_dpt=back_dpt)

@@ -550,6 +550,42 @@ int ffb6d_grid_subsample_host(const float *points, size_t N,
                               float *sub_points, float *sub_features, int *sub_classes,
                               size_t *M_out);
 
+/*
+ * Synthetic-frame augmentation (datasets/ycb/ycb_dataset.py:79-163, datasets/linemod/linemod_dataset.py:114-186).
+ *
+ * ffb6d_rgb_add_noise: the datasets' rgb_add_noise for a batch, rgb [B,H,W,3] u8 -> out [B,H,W,3] u8 (out may
+ *   equal rgb).  Each frame has a float64 record of FFB6D_AUG_REC_LEN slots (layout: ffb6d_b200/augment.py) drawn on
+ *   the host: HSV factors, the sharpen 3x3, the motion-blur kernel (a x a, a <= FFB6D_AUG_MAX_KSIZE), the Gaussian
+ *   blur's fixed-point taps and the noise flags.  plan_host [B,REC_LEN] is what is validated (layout version, flags,
+ *   kernel sizes, taps); plan_dev holds the same bytes on the device and is what the kernels read.  The normal draws
+ *   are Philox4x32-10 of (seed, frame b, stage 2*pass / 2*pass+1, pixel, channel), or, when noise is not NULL, the
+ *   given [2,B,H,W,3] f64 fields.  work: B*H*W*3 bytes of device scratch, aliasing neither rgb nor out.  Given the
+ *   record and the same normals the output is bitwise OpenCV's and numpy's, except that filter2D takes a DFT path
+ *   for kernels of 130 or more taps (a >= 12), where OpenCV may differ by 1 (DESIGN.md §4.14).
+ * ffb6d_add_real_back: add_real_back for a batch.  mode [B] u8 (device): bit 0 composes the depth
+ *   (dpt where dpt > 0, else back_dpt where the background pixel is kept, else 0), bit 1 with bit 0 also the colour
+ *   (back_rgb where labels == 0 and the background pixel is kept, 0 where it is not).  The background keeps a pixel
+ *   where back_labels <= 0 (YCB) or back_labels[...,0] < 255 (LineMOD).  labels [B,H,W] u8, back_labels
+ *   [B,H,W,back_label_channels] u8 (1 or 3), dpt / back_dpt / dpt_out [B,H,W] u16.  Outputs may equal inputs.
+ * ffb6d_aug_noise_field: out [B,H,W,3] f64 = the normals ffb6d_rgb_add_noise draws for (seed, frame, stage).
+ * All three need H, W >= 32, check sizes and null pointers before any launch (FFB6D_ERR_INVALID), allocate nothing and
+ * do not synchronise the host (capturable in a CUDA graph); they are deterministic.
+ */
+#define FFB6D_AUG_VERSION 1
+#define FFB6D_AUG_REC_LEN 1024
+#define FFB6D_AUG_MAX_KSIZE 30
+#define FFB6D_AUG_YCB 0
+#define FFB6D_AUG_LINEMOD 1
+int ffb6d_rgb_add_noise(const uint8_t *rgb, int64_t B, int64_t H, int64_t W,
+                        const double *plan_host, const double *plan_dev, uint64_t seed, const double *noise,
+                        uint8_t *out, uint8_t *work, ffb6d_stream_t stream);
+int ffb6d_add_real_back(const uint8_t *rgb, const uint8_t *labels, const uint16_t *dpt,
+                        const uint8_t *back_rgb, const uint8_t *back_labels, int back_label_channels,
+                        const uint16_t *back_dpt, const uint8_t *mode, int dataset,
+                        int64_t B, int64_t H, int64_t W, uint8_t *rgb_out, uint16_t *dpt_out, ffb6d_stream_t stream);
+int ffb6d_aug_noise_field(uint64_t seed, int64_t B, int64_t H, int64_t W, int stage, double *out,
+                          ffb6d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
