@@ -110,7 +110,7 @@ def test_knn_empty_and_tiny(cuda, algo):
     assert got.shape == (1, 5, 3) and (got == 0).all()
 
 
-@pytest.mark.parametrize("frame", ["seed0_n12288", "seed2_n3072"])
+@pytest.mark.parametrize("frame", ["seed0_n12288", "seed1_n12288", "seed2_n3072"])
 def test_schedule_digest_full_frame(cuda, frame):
     """build_ffb6d_indices on a full 480x640 / 12288-point frame == the reference's 22 arrays
     (sha256 of the int32 arrays produced by the reference's compiled KNN)."""
