@@ -18,7 +18,8 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   the sampled points' input and pose targets; :func:`pose_gt_objects` is the per-object half that stays on the host).
 * :func:`rgb_add_noise`, :func:`add_real_back` -- the datasets' synthetic-frame augmentation
   (datasets/ycb/ycb_dataset.py:79-163, datasets/linemod/linemod_dataset.py:114-186) on the GPU; the scalar draws stay
-  in the worker (:mod:`ffb6d_b200.augment`).
+  in the worker (:mod:`ffb6d_b200.augment`).  :func:`color_jitter` -- the datasets' ``trancolor``
+  (torchvision ``ColorJitter``) on the GPU, from plans of :func:`ffb6d_b200.augment.draw_color_jitter`.
 * :mod:`ffb6d_b200.pose` -- ``MeanShiftTorch``, ``best_fit_transform``, ``cal_frame_poses(_lm)``
   (utils/meanshift_pytorch.py:27-57, utils/pvn3d_eval_utils_kpls.py:28-160, 220-284): keypoint voting on the GPU.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
@@ -36,7 +37,7 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "choose_gather", "grid_sub_sampling", "KnnGrid", "backproject", "fusion_mlp", "fusion_mlp_pack",
         "PackedWeight", "fold_batchnorm", "att_pool", "sample_valid_pixels", "check_indices", "mean_shift_fit", "best_fit_transform",
         "fill_missing", "segment_plan", "segment_sum", "point_item", "rgb_add_noise", "add_real_back",
-        "aug_noise_field")
+        "aug_noise_field", "color_jitter")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")

@@ -11,6 +11,9 @@ The per-pixel normal draws (``rng.randn(*img.shape)`` in ``gaussian_noise``, ``n
 are NOT drawn here: the device draws them from a counter-based generator keyed by (seed, frame, stage, pixel,
 channel).  They have numpy's distribution but not numpy's stream, and the positions of ``rng`` after a frame
 therefore differ from the reference's, which would also have consumed 3*H*W normals per noise stage.
+
+:func:`draw_color_jitter` draws the datasets' ``ColorJitter`` (``trancolor``) from torch's generator, as torchvision
+does, and returns the plans that :func:`ffb6d_b200.ops.color_jitter` applies on the GPU.
 """
 import math
 
@@ -188,6 +191,31 @@ def draw_rgb_noise(rng, dataset, pass_=0):
         if rng.rand() > 0.8:
             rec[I_FINAL] = 1          # (and np.random.normal(0, 7, (H, W, 3)) here)
     return rec
+
+
+JITTER_PLAN_LEN = 8     # include/ffb6d_b200.h FFB6D_JITTER_PLAN_LEN
+# torchvision's ColorJitter(0.2, 0.2, 0.2, 0.05) ranges, formed as its _check_input forms them
+JITTER_RANGES = ((1 - 0.2, 1 + 0.2), (1 - 0.2, 1 + 0.2), (1 - 0.2, 1 + 0.2), (-0.05, 0.05))
+
+
+def draw_color_jitter(n, generator=None):
+    """The draws of the datasets' ``self.trancolor = transforms.ColorJitter(0.2, 0.2, 0.2, 0.05)``
+    (ycb_dataset.py:34, 190-193; linemod_dataset.py:35, 220-223) for ``n`` frames, frame after frame.
+
+    Consumes ``generator`` (default: torch's default CPU generator) exactly as ``ColorJitter.get_params`` does:
+    ``randperm(4)``, then four ``torch.empty(1).uniform_(lo, hi)``.  Plain torch on the CPU, no torchvision.
+
+    :return: ``[n, JITTER_PLAN_LEN]`` float64 plans for :func:`ffb6d_b200.ops.color_jitter`: slots 0-3 the order of
+      the ops (0 brightness, 1 contrast, 2 saturation, 3 hue), slots 4-7 the brightness, contrast, saturation and hue
+      factors as torchvision holds them (float32 draws widened to float64)
+    """
+    import torch
+    plan = np.zeros((int(n), JITTER_PLAN_LEN), np.float64)
+    for i in range(int(n)):
+        plan[i, :4] = torch.randperm(4, generator=generator).numpy()
+        for k, (lo, hi) in enumerate(JITTER_RANGES):
+            plan[i, 4 + k] = float(torch.empty(1).uniform_(lo, hi, generator=generator))
+    return plan
 
 
 def draw_frame_augmentation(rng, dataset, n_real, rnd_typ="syn"):

@@ -1113,6 +1113,47 @@ def add_real_back(rgb, labels, dpt, back_rgb, back_labels, back_dpt, apply_rgb=N
     return rgb_out, dpt_out
 
 
+def color_jitter(rgb, plan, active=None):
+    """The datasets' ``trancolor`` (torchvision ``ColorJitter(0.2, 0.2, 0.2, 0.05)`` on the PIL image,
+    datasets/ycb/ycb_dataset.py:190-193, linemod_dataset.py:220-223) for a batch on the GPU
+    (``ffb6d_color_jitter``); bitwise what torchvision 0.26 with Pillow 12.2 computes.
+
+    :param rgb: ``[B,H,W,3]`` uint8 CUDA
+    :param plan: ``[B, JITTER_PLAN_LEN]`` float64 plans of :func:`ffb6d_b200.augment.draw_color_jitter`; every
+      frame's plan is validated, an inactive frame's too
+    :param active: per-frame bools (a sequence, or a tensor), frames to jitter (default: every frame); the others,
+      e.g. frames the dataset does not jitter, pass through unchanged
+    :return: ``[B,H,W,3]`` uint8
+    """
+    from . import augment as A
+    _need_cuda(rgb, "rgb")
+    if rgb.dtype != torch.uint8 or rgb.dim() != 4 or rgb.shape[3] != 3:
+        raise ValueError("rgb must be uint8 [B,H,W,3], got %s %s" % (rgb.dtype, tuple(rgb.shape)))
+    B, H, W, _ = rgb.shape
+    plan = np.ascontiguousarray(plan, dtype=np.float64)
+    if plan.shape != (B, A.JITTER_PLAN_LEN):
+        raise ValueError("plan must be float64 [B, %d] = [%d, %d], got %s"
+                         % (A.JITTER_PLAN_LEN, B, A.JITTER_PLAN_LEN, plan.shape))
+    dev = rgb.device
+    if active is None:
+        act = torch.ones(B, dtype=torch.uint8, device=dev)
+    else:
+        act = active if isinstance(active, torch.Tensor) else torch.from_numpy(np.asarray(active, bool))
+        if tuple(act.shape) != (B,):
+            raise ValueError("active must have one entry per frame (%d), got %s" % (B, tuple(act.shape)))
+        act = act.to(device=dev, dtype=torch.uint8).contiguous()
+    src = rgb.contiguous()
+    out = torch.empty_like(src)
+    if B * H * W == 0:
+        return out
+    plan_d = torch.from_numpy(plan).to(dev)
+    work = torch.empty(B, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.ffb6d_color_jitter(src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), act.data_ptr(),
+                                     out.data_ptr(), work.data_ptr(), _stream(dev)))
+    return out
+
+
 def aug_noise_field(seed, B, H, W, stage, device="cuda"):
     """The ``[B,H,W,3]`` float64 normals that :func:`rgb_add_noise` draws for ``(seed, frame, stage)``; stage
     ``2*pass`` is ``gaussian_noise``'s, ``2*pass + 1`` YCB's ``normal(0, 7)``'s (``ffb6d_aug_noise_field``)."""

@@ -586,6 +586,26 @@ int ffb6d_add_real_back(const uint8_t *rgb, const uint8_t *labels, const uint16_
 int ffb6d_aug_noise_field(uint64_t seed, int64_t B, int64_t H, int64_t W, int stage, double *out,
                           ffb6d_stream_t stream);
 
+/*
+ * Colour jitter of training frames: torchvision's ColorJitter(0.2, 0.2, 0.2, 0.05) on a PIL RGB image
+ * (datasets/ycb/ycb_dataset.py:34, 190-193; datasets/linemod/linemod_dataset.py:35, 220-223), bitwise as
+ * torchvision 0.26 with Pillow 12.2 computes it (DESIGN.md §4.15).
+ *   rgb [B,H,W,3] u8 -> out [B,H,W,3] u8 (out may equal rgb, but may not overlap it otherwise).
+ *   plan_host / plan_dev [B,FFB6D_JITTER_PLAN_LEN] f64, the same bytes on the host (validated) and on the device
+ *   (read by the kernels): slots 0-3 the order of the ops (a permutation of 0 brightness, 1 contrast, 2 saturation,
+ *   3 hue), slots 4-7 the brightness, contrast and saturation factors (finite, >= 0, <= FLT_MAX) and the hue
+ *   factor (|hue| <= 0.5), as ColorJitter.get_params draws them (ffb6d_b200/augment.py draw_color_jitter).
+ *   active [B] u8 (device): frames with 0 are copied through unchanged.
+ *   work [B] int64 (device, 8-byte aligned, overlapping neither image): the frames' sums of L, zeroed by the call.
+ * 1 <= B < 65536, 1 <= H, W < 2^20, H*W*3 < 2^31.  Sizes, null pointers, alignment and every plan are checked before
+ * any launch (FFB6D_ERR_INVALID).  A memset and two launches; no allocation, no host synchronisation (capturable in a
+ * CUDA graph); deterministic.
+ */
+#define FFB6D_JITTER_PLAN_LEN 8
+int ffb6d_color_jitter(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, const double *plan_host,
+                       const double *plan_dev, const uint8_t *active, uint8_t *out, int64_t *work,
+                       ffb6d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
