@@ -22,6 +22,8 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   (torchvision ``ColorJitter``) on the GPU, from plans of :func:`ffb6d_b200.augment.draw_color_jitter`.
 * :mod:`ffb6d_b200.pose` -- ``MeanShiftTorch``, ``best_fit_transform``, ``cal_frame_poses(_lm)``
   (utils/meanshift_pytorch.py:27-57, utils/pvn3d_eval_utils_kpls.py:28-160, 220-284): keypoint voting on the GPU.
+* :mod:`ffb6d_b200.loss` -- ``FocalLoss``, ``of_l1_loss``, ``OFLoss`` (models/loss.py:12-90) and
+  :func:`~ffb6d_b200.loss.ffb6d_loss`, ``model_fn``'s loss block, masked by the batch's valid frames.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -43,9 +45,9 @@ _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "augment", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "loss", "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM) + ["randla", "modules", "fusion", "pose", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM) + ["randla", "modules", "fusion", "pose", "loss", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched

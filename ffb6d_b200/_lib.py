@@ -107,6 +107,11 @@ def _load():
         "ffb6d_add_real_back": (ci, [vp, vp, vp, vp, vp, ci, vp, vp, ci, i64, i64, i64, vp, vp, vp]),
         "ffb6d_aug_noise_field": (ci, [C.c_uint64, i64, i64, i64, ci, vp, vp]),
         "ffb6d_color_jitter": (ci, [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp]),
+        "ffb6d_loss_workspace_bytes": (sz, [i64, i64, i64]),
+        "ffb6d_focal_loss_fwd": (ci, [vp, ci, vp, ci, vp, i64, i64, i64, fp, vp, ci, vp, vp, vp, vp, vp, sz, vp]),
+        "ffb6d_focal_loss_bwd": (ci, [vp, ci, vp, ci, vp, i64, i64, i64, fp, vp, ci, vp, vp, vp, vp, vp]),
+        "ffb6d_of_l1_loss_fwd": (ci, [vp, vp, vp, ci, vp, i64, i64, i64, vp, vp, vp, sz, vp]),
+        "ffb6d_of_l1_loss_bwd": (ci, [vp, vp, vp, ci, vp, i64, i64, i64, vp, vp, vp, vp]),
         "ffb6d_grid_subsample_host": (ci, [vp, sz, vp, sz, vp, sz, fp, vp, vp, vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():

@@ -1162,3 +1162,132 @@ def aug_noise_field(seed, B, H, W, stage, device="cuda"):
     with torch.cuda.device(out.device):
         check(lib.ffb6d_aug_noise_field(int(seed), B, H, W, int(stage), out.data_ptr(), _stream(out.device)))
     return out
+
+
+# --------------------------------------------------------------------------- training loss
+def _loss_labels(labels, B, N, dev):
+    _need_cuda(labels, "labels")
+    if labels.dtype not in _IDX:
+        raise TypeError("labels must be int32 or int64, got %s" % labels.dtype)
+    if labels.numel() != B * N or labels.device != dev:
+        raise ValueError("labels must hold %d x %d values on %s, got %s on %s"
+                         % (B, N, dev, tuple(labels.shape), labels.device))
+    return labels.reshape(B, N).contiguous(), int(labels.dtype == torch.int64)
+
+
+def _loss_valid(valid, B, dev):
+    """``valid`` as the kernels read it: None, or ``[B]`` uint8 on ``dev`` (a bool / integer tensor is converted on
+    the device, without a host synchronisation)."""
+    if valid is None:
+        return None
+    v = valid if isinstance(valid, torch.Tensor) else torch.as_tensor(np.asarray(valid, bool))
+    if v.numel() != B:
+        raise ValueError("valid must have one entry per frame (%d), got %s" % (B, tuple(v.shape)))
+    return v.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
+
+
+def _loss_workspace(B, N, n_kps, dev):
+    nbytes = lib.ffb6d_loss_workspace_bytes(B, N, n_kps)
+    if nbytes == 0:
+        raise ValueError("loss: unsupported size B=%d N=%d n_kps=%d" % (B, N, n_kps))
+    return torch.empty(nbytes, dtype=torch.uint8, device=dev)
+
+
+def _f32(t, name, shape):
+    _need_cuda(t, name)
+    if t.dtype != torch.float32 or tuple(t.shape) != tuple(shape):
+        raise ValueError("%s must be float32 %s, got %s %s" % (name, tuple(shape), t.dtype, tuple(t.shape)))
+    return t.contiguous()
+
+
+def focal_loss_fwd(logits, labels, valid=None, gamma=0.0, alpha=None, size_average=True, layout=0):
+    """FocalLoss forward (models/loss.py:12-43) on ``logits [B,C,N]`` (``layout=0``) or ``[B,N,C]`` (``layout=1``)
+    float32 CUDA, ``labels [B,N]`` int32 / int64, ``valid [B]`` or None, ``alpha [C]`` float32 CUDA or None
+    (``ffb6d_focal_loss_fwd``, one call).  :return: ``(loss [], acc [], count [] int64, lse [B,N])``"""
+    _need_cuda(logits, "logits")
+    if logits.dim() != 3 or logits.dtype != torch.float32 or layout not in (0, 1):
+        raise ValueError("logits must be float32 [B,C,N] (layout 0) or [B,N,C] (layout 1), got %s %s"
+                         % (logits.dtype, tuple(logits.shape)))
+    x = logits.contiguous()
+    B, C, N = (x.shape[0], x.shape[2], x.shape[1]) if layout else x.shape
+    dev = x.device
+    lab, is64 = _loss_labels(labels, B, N, dev)
+    v = _loss_valid(valid, B, dev)
+    if alpha is not None:
+        alpha = _f32(alpha, "alpha", alpha.shape)
+        if alpha.dim() != 1 or alpha.numel() < C or alpha.device != dev:
+            raise ValueError("alpha must be a [>= C] float32 tensor on %s" % dev)
+    ws = _loss_workspace(B, N, 1, dev)
+    out = torch.empty(2, dtype=torch.float32, device=dev)
+    count = torch.empty((), dtype=torch.int64, device=dev)
+    lse = torch.empty((B, N), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.ffb6d_focal_loss_fwd(x.data_ptr(), layout, lab.data_ptr(), is64, None if v is None else v.data_ptr(),
+                                       B, C, N, float(gamma), None if alpha is None else alpha.data_ptr(),
+                                       int(bool(size_average)), out.data_ptr(), out.data_ptr() + 4, count.data_ptr(),
+                                       lse.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
+    return out[0], out[1], count, lse
+
+
+def focal_loss_bwd(logits, labels, valid, gamma, alpha, size_average, lse, count, grad_loss, layout=0):
+    """FocalLoss backward (``ffb6d_focal_loss_bwd``, one launch): the gradient of the logits, in their layout, from
+    the forward's ``lse`` and ``count`` and the upstream gradient ``grad_loss`` (a one-element CUDA tensor)."""
+    x = logits.contiguous()
+    B, C, N = (x.shape[0], x.shape[2], x.shape[1]) if layout else x.shape
+    dev = x.device
+    lab, is64 = _loss_labels(labels, B, N, dev)
+    v = _loss_valid(valid, B, dev)
+    lse = _f32(lse, "lse", (B, N))
+    g = grad_loss.to(torch.float32).reshape(1).contiguous()
+    grad = torch.empty_like(x)
+    with torch.cuda.device(dev):
+        check(lib.ffb6d_focal_loss_bwd(x.data_ptr(), layout, lab.data_ptr(), is64, None if v is None else v.data_ptr(),
+                                       B, C, N, float(gamma), None if alpha is None else alpha.data_ptr(),
+                                       int(bool(size_average)), lse.data_ptr(), count.data_ptr(), g.data_ptr(),
+                                       grad.data_ptr(), _stream(dev)))
+    return grad
+
+
+def _of_args(pred, targ, labels, valid):
+    _need_cuda(pred, "pred_ofsts")
+    if pred.dim() != 4 or pred.shape[3] != 3 or pred.dtype != torch.float32:
+        raise ValueError("pred_ofsts must be float32 [B,n_kps,N,3], got %s %s" % (pred.dtype, tuple(pred.shape)))
+    B, K, N, _ = pred.shape
+    _need_cuda(targ, "kp_targ_ofst")
+    if targ.numel() != B * N * K * 3 or targ.dtype != torch.float32 or targ.device != pred.device:
+        raise ValueError("kp_targ_ofst must be float32 [B,N,n_kps,3] = [%d,%d,%d,3] on %s, got %s %s"
+                         % (B, N, K, pred.device, targ.dtype, tuple(targ.shape)))
+    lab, is64 = _loss_labels(labels, B, N, pred.device)
+    return pred.contiguous(), targ.reshape(B, N, K, 3).contiguous(), lab, is64, _loss_valid(valid, B, pred.device)
+
+
+def of_l1_loss_fwd(pred, targ, labels, valid=None):
+    """of_l1_loss forward with ``normalize=True`` (models/loss.py:46-74; ``ffb6d_of_l1_loss_fwd``, one call):
+    ``pred [B,n_kps,N,3]``, ``targ [B,N,n_kps,3]`` float32 CUDA.  :return: ``(loss [B,n_kps], count [B])``"""
+    p, t, lab, is64, v = _of_args(pred, targ, labels, valid)
+    B, K, N, _ = p.shape
+    dev = p.device
+    ws = _loss_workspace(B, N, K, dev)
+    out = torch.empty((B, K), dtype=torch.float32, device=dev)
+    count = torch.empty(B, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.ffb6d_of_l1_loss_fwd(p.data_ptr(), t.data_ptr(), lab.data_ptr(), is64,
+                                       None if v is None else v.data_ptr(), B, K, N, out.data_ptr(), count.data_ptr(),
+                                       ws.data_ptr(), ws.numel(), _stream(dev)))
+    return out, count
+
+
+def of_l1_loss_bwd(pred, targ, labels, valid, count, grad_out):
+    """of_l1_loss backward (``ffb6d_of_l1_loss_bwd``, one launch): the gradient of ``pred`` for an upstream
+    ``grad_out [B,n_kps]``, from the forward's ``count``."""
+    p, t, lab, is64, v = _of_args(pred, targ, labels, valid)
+    B, K, N, _ = p.shape
+    dev = p.device
+    count = _f32(count, "count", (B,))
+    g = _f32(grad_out.to(torch.float32), "grad_out", (B, K))
+    grad = torch.empty_like(p)
+    with torch.cuda.device(dev):
+        check(lib.ffb6d_of_l1_loss_bwd(p.data_ptr(), t.data_ptr(), lab.data_ptr(), is64,
+                                       None if v is None else v.data_ptr(), B, K, N, count.data_ptr(), g.data_ptr(),
+                                       grad.data_ptr(), _stream(dev)))
+    return grad

@@ -606,6 +606,49 @@ int ffb6d_color_jitter(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, cons
                        const double *plan_dev, const uint8_t *active, uint8_t *out, int64_t *work,
                        ffb6d_stream_t stream);
 
+/*
+ * FFB6D's training loss (models/loss.py:12-90, combined as train_ycb.py:237-253): FocalLoss and the offset L1 loss
+ * of_l1_loss / OFLoss, each with an optional per-frame mask valid [B] u8 (device; NULL: every frame).  A frame with
+ * valid[b] == 0 adds nothing to any sum or count and gets zero gradients, so every output equals the reference's on
+ * the sub-batch of valid frames.  Labels [B,N] int32 or int64 (labels_is_i64).
+ *
+ * ffb6d_focal_loss_fwd: logits [B,C,N] (layout 0, the head's) or [B,N,C] (layout 1: the reference's reshaped rows,
+ *   e.g. an [M,C] input as B = 1, N = M); 1 <= C <= 256; gamma finite, >= 0; alpha [C] f32 (device) or NULL.
+ *   pt = exp(logpt) is a constant of the backward, as the reference's Variable(logpt.data.exp()).  Writes the loss
+ *   (mean over the M counted points when size_average, else the sum), acc = (arg-max == label) / M with the lowest
+ *   index winning ties, count = M (int64, for the backward) and lse [B,N] (0 on masked frames).  With M = 0 (every
+ *   frame masked) loss and acc are 0 and the backward writes zeros.  A label outside [0, C) is not read through: its
+ *   term and its gradients are NaN.  workspace: ffb6d_loss_workspace_bytes(B, N, any n_kps), 16-byte aligned.
+ * ffb6d_focal_loss_bwd: grad_logits (same layout) from the saved lse and count and the upstream grad_loss [1]
+ *   (device): dz_j = g_t [j == t] - exp(z_j - lse) g_t, g_t = -(1 - pt)^gamma alpha[t] g / M (g when not
+ *   size_average).  One launch.
+ * ffb6d_of_l1_loss_fwd: pred [B,n_kps,N,3] (the head's layout), targ [B,N,n_kps,3] (the item's layout),
+ *   w_n = labels[b,n] > 0; 1 <= n_kps <= FFB6D_ITEM_MAX_KPS.  out [B,n_kps] = S_bk / (float(cnt_b) + 1e-3f) with
+ *   S_bk = sum_n sum_c w_n |pred - targ| (fp64) and cnt_b = sum_n w_n, saved in count [B] f32 (0 on masked frames,
+ *   whose out is 0).  workspace: ffb6d_loss_workspace_bytes(B, N, n_kps), 16-byte aligned.
+ * ffb6d_of_l1_loss_bwd: grad_pred [B,n_kps,N,3] = (g_bk / (count_b + 1e-3f)) * w_n * sign(pred - targ) in fp32,
+ *   sign(0) = 0, for any upstream grad_out [B,n_kps] (device): bitwise the reference's autograd.  One launch.
+ * 1 <= B < 65536, 1 <= N < 2^31 - 128.  Sizes, null pointers and alignment are checked before any launch
+ * (FFB6D_ERR_INVALID; a short workspace FFB6D_ERR_WORKSPACE).  A forward is two launches (partials per CTA, then
+ * one finalize that adds them in a fixed order); no allocation, no host synchronisation (capturable in a CUDA
+ * graph), no atomics (deterministic).  ffb6d_loss_workspace_bytes returns 0 for sizes the calls reject.
+ */
+size_t ffb6d_loss_workspace_bytes(int64_t B, int64_t N, int64_t n_kps);
+int ffb6d_focal_loss_fwd(const float *logits, int layout, const void *labels, int labels_is_i64,
+                         const uint8_t *valid, int64_t B, int64_t C, int64_t N, float gamma, const float *alpha,
+                         int size_average, float *loss, float *acc, int64_t *count, float *lse,
+                         void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+int ffb6d_focal_loss_bwd(const float *logits, int layout, const void *labels, int labels_is_i64,
+                         const uint8_t *valid, int64_t B, int64_t C, int64_t N, float gamma, const float *alpha,
+                         int size_average, const float *lse, const int64_t *count, const float *grad_loss,
+                         float *grad_logits, ffb6d_stream_t stream);
+int ffb6d_of_l1_loss_fwd(const float *pred, const float *targ, const void *labels, int labels_is_i64,
+                         const uint8_t *valid, int64_t B, int64_t n_kps, int64_t N, float *out, float *count,
+                         void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+int ffb6d_of_l1_loss_bwd(const float *pred, const float *targ, const void *labels, int labels_is_i64,
+                         const uint8_t *valid, int64_t B, int64_t n_kps, int64_t N, const float *count,
+                         const float *grad_out, float *grad_pred, ffb6d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,6 +14,10 @@ BatchNorm layer and direction.
 
 Config 3: LineMOD-shaped (2 classes, 8 keypoints + centre), batch 8 per GPU, forward + backward.
 Config 4: YCB-shaped (22 classes), batch 4 per GPU, forward + backward + Adam step ("end-to-end train step").
+``--loss ffb6d`` trains with FFB6D's loss (ffb6d_b200.loss.ffb6d_loss: 2 FocalLoss(gamma=2) + OFLoss(kp) + OFLoss(ctr),
+train_ycb.py:237-253) on item-shaped targets (labels [B,N], kp_targ_ofst [B,N,n_kps,3], ctr_targ_ofst [B,N,3]) with
+every fourth frame marked invalid; the default is the stand-in (cross_entropy + plain L1 means), so earlier numbers stay
+comparable.  With ``--loss ffb6d``, ``--deterministic`` sets torch.use_deterministic_algorithms(True) without warn_only.
 Every step also rebuilds the 22 KNN index tensors on the device from the step's cloud (the reference does this on
 the CPU in DataLoader workers).  One JSON line on stdout (rank 0): points/s = GPUs * B * 12288 / t_step, time =
 max over ranks of CUDA-event time.
@@ -40,7 +44,9 @@ def main():
     ap.add_argument("--deterministic", action="store_true",
                     help="torch.use_deterministic_algorithms(True, warn_only=True): every backward of the model takes its "
                          "run-to-run deterministic path (warn_only: torch's own nll_loss2d forward in the loss has no "
-                         "deterministic CUDA kernel and would raise)")
+                         "deterministic CUDA kernel and would raise; with --loss ffb6d, without warn_only)")
+    ap.add_argument("--loss", default="standin", choices=["standin", "ffb6d"],
+                    help="standin: cross_entropy + plain L1 means (default); ffb6d: FFB6D's loss with a valid mask")
     ap.add_argument("--syncbn", action="store_true",
                     help="nn.SyncBatchNorm.convert_sync_batchnorm(model) before the DDP wrap: BatchNorm statistics of the "
                          "global batch (the reference's convert_syncbn_model, train_ycb.py:568)")
@@ -54,7 +60,7 @@ def main():
     from ffb6d_b200.dist import frame_shard, max_over_ranks
 
     if args.deterministic:
-        torch.use_deterministic_algorithms(True, warn_only=True)
+        torch.use_deterministic_algorithms(True, warn_only=args.loss == "standin")
     rank, local_rank, world = (int(os.environ.get(k, d)) for k, d in (("RANK", 0), ("LOCAL_RANK", 0), ("WORLD_SIZE", 1)))
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
@@ -83,6 +89,13 @@ def main():
     labels = torch.randint(0, n_classes, (B, N0), generator=g, device=dev)
     kp_t = torch.randn((B, n_kps, N0, 3), generator=g, device=dev)
     ctr_t = torch.randn((B, 1, N0, 3), generator=g, device=dev)
+    if args.loss == "ffb6d":
+        from ffb6d_b200.loss import ffb6d_loss
+        lab_i = labels.to(torch.int32)
+        lab_i[torch.rand((B, N0), generator=g, device=dev) < 0.6] = 0          # background, as in a real frame
+        item_t = {"labels": lab_i, "kp_targ_ofst": torch.randn((B, N0, n_kps, 3), generator=g, device=dev),
+                  "ctr_targ_ofst": torch.randn((B, N0, 3), generator=g, device=dev),
+                  "valid": torch.arange(B, device=dev) % 4 != 1}                 # frames below 400 valid pixels
 
     def step():
         with torch.no_grad():
@@ -97,10 +110,13 @@ def main():
             for p in model.parameters():
                 p.grad = None
         out = net(inputs, rgb_feats)
-        loss = (torch.nn.functional.cross_entropy(out["pred_rgbd_segs"], labels) * 2.0
-                + (out["pred_kp_ofs"] - kp_t).abs().mean() + (out["pred_ctr_ofs"] - ctr_t).abs().mean()
-                # the fused image maps feed the (absent) CNN stages: a stand-in term keeps their layers in the graph
-                + sum(r.mean() for r in out["fused_rgb"]) * 1e-3)
+        if args.loss == "ffb6d":
+            loss = ffb6d_loss(out, item_t, valid=item_t["valid"])[0]
+        else:
+            loss = (torch.nn.functional.cross_entropy(out["pred_rgbd_segs"], labels) * 2.0
+                    + (out["pred_kp_ofs"] - kp_t).abs().mean() + (out["pred_ctr_ofs"] - ctr_t).abs().mean())
+        # the fused image maps feed the (absent) CNN stages: a stand-in term keeps their layers in the graph
+        loss = loss + sum(r.mean() for r in out["fused_rgb"]) * 1e-3
         loss.backward()
         if opt is not None:
             opt.step()
@@ -154,7 +170,9 @@ def main():
                 "batch_per_gpu": B, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
                 "params": n_params, "grad_allreduce_bytes": 4 * n_params if world > 1 else 0, "loss": float(loss.detach()),
                 "finite": finite, "dtype": "f32", "data": "synthetic", "scaling": "weak",
-                "restructured": args.restructured, "deterministic": args.deterministic, "syncbn": args.syncbn, "max_memory_allocated_mb": peak_mb,
+                "restructured": args.restructured, "deterministic": args.deterministic,
+                "deterministic_warn_only": args.deterministic and args.loss == "standin", "loss_kind": args.loss,
+                "syncbn": args.syncbn, "max_memory_allocated_mb": peak_mb,
                 "gpu": torch.cuda.get_device_name(dev)}
         print(json.dumps(line))
     if world > 1:
