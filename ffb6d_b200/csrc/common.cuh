@@ -45,6 +45,15 @@ void count_launch(int n = 1);
     } while (0)
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// torch.max semantics: NaN if either operand is NaN (fmaxf returns the other operand).  Also the ReLU of the
+// epilogues, max_nan(y, 0): torch.relu(NaN) is NaN, and a NaN input must not come out of a layer as 0.
+__device__ __forceinline__ float max_nan(float m, float v)
+{
+    float r;   // FMNMX.NAN
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(m), "f"(v));
+    return r;
+}
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // Per-device facts, cached per device ordinal (a process may drive several GPUs: function attributes

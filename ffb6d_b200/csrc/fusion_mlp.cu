@@ -56,12 +56,24 @@ __device__ __forceinline__ float to_tf32(float x)
     return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
 
+// x = hi + lo.  For a NaN the integer add of to_tf32 can carry the high mantissa bits out of the exponent and wrap
+// it to +-0 (0x7FFFFFFF, the NaN the GPU's own arithmetic produces, among them), and x - hi is NaN for every
+// non-finite x, whose to_tf32 wraps too: an upstream NaN would vanish from the layer.  hi = fma(x - hi, 0, hi)
+// restores it (one FMA-pipe op; hi itself for finite x), so a NaN input comes out NaN, and so does +-inf
+// (inf - inf).
+__device__ __forceinline__ void split1(float x, float &hi, float &lo)
+{
+    const float h = to_tf32(x), d = x - h;
+    lo = to_tf32(d);
+    hi = __fmaf_rn(d, 0.f, h);
+}
+
 __device__ __forceinline__ void split4(const float4 v, float4 &hi, float4 &lo)
 {
-    hi.x = to_tf32(v.x); lo.x = to_tf32(v.x - hi.x);
-    hi.y = to_tf32(v.y); lo.y = to_tf32(v.y - hi.y);
-    hi.z = to_tf32(v.z); lo.z = to_tf32(v.z - hi.z);
-    hi.w = to_tf32(v.w); lo.w = to_tf32(v.w - hi.w);
+    split1(v.x, hi.x, lo.x);
+    split1(v.y, hi.y, lo.y);
+    split1(v.z, hi.z, lo.z);
+    split1(v.w, hi.w, lo.w);
 }
 
 // K-major, no-swizzle (layout type 0) wgmma shared-memory matrix descriptor: start address, LBO = next
@@ -325,7 +337,7 @@ fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__re
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
                 y[u] = __fadd_rn(__fmul_rn(y[u], sc), sh);
-                if (act == 1) y[u] = fmaxf(y[u], 0.f);
+                if (act == 1) y[u] = max_nan(y[u], 0.f);
                 else if (act == 2) y[u] = (y[u] > 0.f) ? y[u] : __fmul_rn(y[u], slope);
             }
             if (ocol) {

@@ -25,13 +25,7 @@
 
 namespace ffb6d {
 
-// torch.max semantics: NaN propagates; first maximal element wins the arg-max
-__device__ __forceinline__ float max_nan(float m, float v)
-{
-    float r;   // FMNMX.NAN: NaN if either operand is NaN, like torch.max
-    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(m), "f"(v));
-    return r;
-}
+// torch.max semantics (max_nan, common.cuh): NaN propagates; first maximal element wins the arg-max
 
 template <typename IdxT, int KT>
 __device__ __forceinline__ void load_ids(const IdxT *__restrict__ ip, int K, int (&id)[KT > 0 ? KT : 1])

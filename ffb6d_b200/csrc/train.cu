@@ -101,7 +101,7 @@ bn_finalize_kernel(const double *__restrict__ partial, const float *__restrict__
 
 __device__ __forceinline__ float act_fwd(float y, int act, float slope)
 {
-    if (act == 1) return fmaxf(y, 0.f);
+    if (act == 1) return max_nan(y, 0.f);
     if (act == 2) return y > 0.f ? y : y * slope;
     return y;
 }

@@ -62,15 +62,28 @@ def test_dilated_res_block_matches_reference(cuda, name):
 
 
 def test_att_pool_against_torch(cuda):
+    """The kernels for K = 8, 16, 32 and the generic one (K = 1, 2, 7, 33, 64); at K = 16 also an f1 that starts
+    4 bytes past a 16-byte boundary (the element-wise loads) and logits of +-60, where the softmax saturates."""
     g = torch.Generator().manual_seed(3)
-    for (B, C1, C2, N, K) in ((2, 16, 16, 50, 16), (1, 5, 0, 33, 7), (1, 8, 8, 20, 32)):
-        f1 = torch.randn(B, C1, N, K, generator=g).cuda()
+    for (B, C1, C2, N, K, offset, logits) in ((2, 16, 16, 50, 16, 0, "randn"), (1, 5, 0, 33, 7, 0, "randn"),
+                                              (1, 8, 8, 20, 32, 0, "randn"), (2, 6, 3, 40, 1, 0, "randn"),
+                                              (2, 4, 4, 30, 2, 0, "randn"), (2, 8, 8, 50, 8, 0, "randn"),
+                                              (1, 5, 3, 20, 33, 0, "randn"), (1, 8, 0, 25, 64, 0, "randn"),
+                                              (2, 16, 16, 100, 16, 1, "randn"), (2, 16, 16, 300, 16, 0, "pm60"),
+                                              (1, 8, 8, 40, 8, 0, "pm60"), (1, 4, 4, 20, 33, 0, "pm60")):
+        f1 = torch.randn(offset + B * C1 * N * K, generator=g).cuda()[offset:].view(B, C1, N, K)
+        assert (f1.data_ptr() % 16 != 0) == bool(offset)
         f2 = torch.randn(B, C2, N, K, generator=g).cuda() if C2 else None
-        att = (torch.randn(B, C1 + C2, N, K, generator=g) * 3).cuda()
+        if logits == "randn":
+            att = torch.randn(B, C1 + C2, N, K, generator=g) * 3
+        else:
+            sign = torch.where(torch.rand(B, C1 + C2, N, K, generator=g) < 0.5, -1.0, 1.0)
+            att = 60 * sign + torch.randn(B, C1 + C2, N, K, generator=g)
+        att = att.cuda()
         fs = torch.cat((f1, f2), 1) if f2 is not None else f1
         want = torch.sum(fs.double() * torch.softmax(att.double(), dim=3), dim=3, keepdim=True)   # RandLANet.py:245-248
         got = F.att_pool(f1, f2, att)
-        close(got.cpu().numpy(), want.cpu().numpy(), "att_pool %s" % ((B, C1, C2, N, K),))
+        close(got.cpu().numpy(), want.cpu().numpy(), "att_pool %s offset=%d %s" % ((B, C1, C2, N, K), offset, logits))
 
 
 def test_relative_pos_encoding_channel_major(cuda):

@@ -10,6 +10,7 @@ import torch.nn.functional as Fn
 from ffb6d_b200.model import FFB6DFusionNet
 from ffb6d_b200.schedule import build_ffb6d_indices
 from ffb6d_b200.synthetic import make_batch
+from oracle import lfa_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -59,27 +60,15 @@ class TorchRef:
 
     def att_pool(self, pre, fs):                    # RandLANet.py:243-250
         w = self.p[pre + ".fc.weight"]
-        att = torch.einsum("oc,bcnk->bonk", w.reshape(w.shape[0], -1), fs)
-        agg = torch.sum(fs * torch.softmax(att, dim=3), dim=3, keepdim=True)
+        agg = lfa_oracle.att_pool(fs, torch.einsum("oc,bcnk->bonk", w.reshape(w.shape[0], -1), fs))
         return self.rconv(pre + ".mlp", agg)
 
     def block(self, pre, feature, xyz, idx):        # RandLANet.py:170-234
-        B, N, K = idx.shape
         f_pc = self.rconv(pre + ".mlp1", feature)
-        nb = torch.gather(xyz, 1, idx.reshape(B, -1, 1).expand(-1, -1, 3).long()).reshape(B, N, K, 3)
-        tile = xyz.unsqueeze(2).expand(-1, -1, K, -1)
-        rel = tile - nb
-        dis = torch.sqrt(torch.sum(rel ** 2, dim=-1, keepdim=True))
-        f_xyz = torch.cat([dis, rel, tile, nb], dim=-1).permute(0, 3, 1, 2)
-        f_xyz = self.rconv(pre + ".lfa.mlp1", f_xyz)
-
-        def gather_cm(f):
-            d = f.shape[1]
-            return torch.gather(f.squeeze(3), 2, idx.reshape(B, 1, -1).expand(-1, d, -1).long()).reshape(B, d, N, K)
-
-        agg = self.att_pool(pre + ".lfa.att_pooling_1", torch.cat([gather_cm(f_pc), f_xyz], 1))
+        f_xyz = self.rconv(pre + ".lfa.mlp1", lfa_oracle.relative_pos_encoding(xyz, idx))
+        agg = self.att_pool(pre + ".lfa.att_pooling_1", torch.cat([lfa_oracle.gather_cm(f_pc, idx), f_xyz], 1))
         f_xyz = self.rconv(pre + ".lfa.mlp2", f_xyz)
-        agg = self.att_pool(pre + ".lfa.att_pooling_2", torch.cat([gather_cm(agg), f_xyz], 1))
+        agg = self.att_pool(pre + ".lfa.att_pooling_2", torch.cat([lfa_oracle.gather_cm(agg, idx), f_xyz], 1))
         return Fn.leaky_relu(self.rconv(pre + ".mlp2", agg, None) + self.rconv(pre + ".shortcut", feature, None), 0.2)
 
     def fuse(self, tag, i, rgb0, p0, p2r_idx, r2p_idx):      # models/ffb6d.py:245-263

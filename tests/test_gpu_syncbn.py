@@ -141,6 +141,35 @@ def test_bn_sync_vs_float64(cuda, C, P, act, slope, eps, momentum, dist):
         close_fp32(dz[:, cc], gz64[:, cc], gz32[:, cc], what + " constant channel dz")
 
 
+@pytest.mark.parametrize("act,slope", [(0, 0.0), (1, 0.0), (2, 0.2)], ids=["none", "relu", "leaky"])
+def test_bn_sync_nan_on_one_rank_gives_nan_everywhere(cuda, act, slope):
+    """A NaN in one rank's shard makes the combined statistics of its channel NaN, and that channel NaN on every
+    rank, as torch's batch_norm -> activation over the whole batch gives: the ReLU must not turn it into zeros."""
+    C, P = 8, 1000
+    W = len(SHARDS)
+    g = torch.Generator(device=cuda).manual_seed(5)
+    shard = [torch.randn(s, C, P, generator=g, device=cuda) for s in SHARDS]
+    shard[1][0, 2, 17] = float("nan")
+    want = act_fn(act, slope)(F_.batch_norm(torch.cat(shard), None, None, None, None, True, 0.1, 1e-5))
+    assert torch.isnan(want[:, 2]).all() and not torch.isnan(want[:, :2]).any()
+    nbytes = int(lib.ffb6d_bn_workspace_bytes(C, P))
+    st = _stream(cuda)
+    ws = [torch.empty(nbytes, dtype=torch.uint8, device=cuda) for _ in range(W)]
+    rows = torch.empty(W, 2 * C + 1, dtype=torch.float64, device=cuda)
+    for r in range(W):
+        check(lib.ffb6d_bn_sync_moments(shard[r].data_ptr(), SHARDS[r], C, P, rows[r].data_ptr(), ws[r].data_ptr(), nbytes, st))
+    gamma, beta = torch.ones(C, device=cuda), torch.zeros(C, device=cuda)
+    for r in range(W):
+        rm, rv = torch.zeros(C, device=cuda), torch.ones(C, device=cuda)
+        stats, count, y = torch.empty(C, 4, device=cuda), torch.empty(1, dtype=torch.float64, device=cuda), torch.empty_like(shard[r])
+        check(lib.ffb6d_bn_sync_fwd(shard[r].data_ptr(), SHARDS[r], C, P, rows.data_ptr(), W, gamma.data_ptr(),
+                                    beta.data_ptr(), 1e-5, 0.1, rm.data_ptr(), rv.data_ptr(), act, slope,
+                                    stats.data_ptr(), count.data_ptr(), y.data_ptr(), st))
+        lo = sum(SHARDS[:r])
+        assert torch.equal(torch.isnan(y), torch.isnan(want[lo:lo + SHARDS[r]])), "rank %d act=%d: %d NaN outputs, torch %d" % (
+            r, act, int(torch.isnan(y).sum()), int(torch.isnan(want[lo:lo + SHARDS[r]]).sum()))
+
+
 # ------------------------------------------------------------------ the modules over a process group
 STACK_B, STACK_N, STACK_K, STACK_NA = 4, 256, 8, 100
 

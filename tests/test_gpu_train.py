@@ -472,6 +472,23 @@ def test_bn_momentum_none_is_a_cumulative_average(cuda):
                           "momentum=None step %d running_var" % step)
 
 
+@pytest.mark.parametrize("activation", [nn.ReLU(), nn.LeakyReLU(0.2), None], ids=["relu", "leaky", "none"])
+def test_nan_input_in_training_gives_nan(cuda, activation):
+    """One NaN in the input of a training-mode layer makes every channel's batch statistics NaN.  torch's
+    batch_norm -> relu then gives NaN everywhere; the layer must too, not a finite (all-zero) output that hides
+    the poisoned batch."""
+    torch.manual_seed(0)
+    layer = M.Conv2d(16, 8, bn=True, activation=activation).cuda().train()
+    twin = torch_twin(layer, activation).cuda().train()
+    x = torch.randn(2, 16, 30, 40, device=cuda)
+    x[1, 3, 7, 9] = float("nan")
+    with torch.no_grad():
+        want = twin(x)
+        got = layer(x)
+    assert torch.isnan(want).all()
+    assert torch.isnan(got).all(), "%d of %d outputs are not NaN" % (int((~torch.isnan(got)).sum()), got.numel())
+
+
 def test_one_value_per_channel_is_rejected_in_training(cuda):
     """As torch's BatchNorm: training statistics over one value per channel raise ValueError."""
     torch.manual_seed(0)
