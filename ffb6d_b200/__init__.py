@@ -24,6 +24,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   (utils/meanshift_pytorch.py:27-57, utils/pvn3d_eval_utils_kpls.py:28-160, 220-284): keypoint voting on the GPU.
 * :mod:`ffb6d_b200.loss` -- ``FocalLoss``, ``of_l1_loss``, ``OFLoss`` (models/loss.py:12-90) and
   :func:`~ffb6d_b200.loss.ffb6d_loss`, ``model_fn``'s loss block, masked by the batch's valid frames.
+* :mod:`ffb6d_b200.cnn` -- the ResNet34-PSPNet image branch (models/cnn/extractors.py, models/cnn/pspnet.py) in
+  torch, with :func:`psp_pool`, :func:`psp_bottleneck` and :func:`conv1x1_log_softmax` on the GPU for its PSP head
+  and ``final`` at inference; ``ffb6d_b200.model.FFB6D`` is the whole network.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -39,15 +42,15 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "choose_gather", "grid_sub_sampling", "KnnGrid", "backproject", "fusion_mlp", "fusion_mlp_pack",
         "PackedWeight", "fold_batchnorm", "att_pool", "sample_valid_pixels", "check_indices", "mean_shift_fit", "best_fit_transform",
         "fill_missing", "segment_plan", "segment_sum", "point_item", "rgb_add_noise", "add_real_back",
-        "aug_noise_field", "color_jitter")
+        "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "augment", "loss", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM) + ["randla", "modules", "fusion", "pose", "loss", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched

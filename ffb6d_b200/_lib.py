@@ -112,6 +112,9 @@ def _load():
         "ffb6d_focal_loss_bwd": (ci, [vp, ci, vp, ci, vp, i64, i64, i64, fp, vp, ci, vp, vp, vp, vp, vp]),
         "ffb6d_of_l1_loss_fwd": (ci, [vp, vp, vp, ci, vp, i64, i64, i64, vp, vp, vp, sz, vp]),
         "ffb6d_of_l1_loss_bwd": (ci, [vp, vp, vp, ci, vp, i64, i64, i64, vp, vp, vp, vp]),
+        "ffb6d_psp_pool": (ci, [vp, i64, i64, i64, i64, vp, vp]),
+        "ffb6d_psp_bottleneck_fwd": (ci, [vp, i64, i64, i64, i64, vp, vp, i64, vp, vp, vp]),
+        "ffb6d_conv1x1_log_softmax_fwd": (ci, [vp, i64, i64, i64, vp, vp, i64, vp, vp]),
         "ffb6d_grid_subsample_host": (ci, [vp, sz, vp, sz, vp, sz, fp, vp, vp, vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():

@@ -203,19 +203,20 @@ fusion_mlp_pack_kernel(const float *__restrict__ w, int Co, int Ci, int nk, int 
     dst[TILE_BYTES / 16 + r] = lo;
 }
 
-__global__ void __launch_bounds__(MLP_THREADS, 1)
-fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
-                         const unsigned char *__restrict__ wpack, const float *__restrict__ scale,
-                         const float *__restrict__ shift, float *__restrict__ out, int Co, int P, int act,
-                         float slope, MlpEpilogue ep)
+// The product of the packed-weight kernels (fusion_mlp_packed_kernel here, and the PSP head's kernels of psp.cu):
+// sum = this warpgroup's 64 x 128 part of the CTA tile W[m0 .., :] * [X1; X2][:, n0 ..] of one frame, rounded as
+// described at the top of the file.  xb1 / xb2: the frame's inputs (NCHW, [C1, P] and [C2, P]); wsrc: the packed
+// blocks of the CTA's 128-row tile; vec: 16-byte vector loads are allowed (P % 4 == 0, inputs aligned).  Uses the
+// whole dynamic shared memory (MLP_SMEM); a caller that reuses it afterwards synchronises the CTA first.
+__device__ __forceinline__ void packed_mainloop(unsigned char *smem, const float *__restrict__ xb1, int C1,
+                                                const float *__restrict__ xb2, int C2,
+                                                const unsigned char *__restrict__ wsrc, int P, int n0, bool vec,
+                                                float (&sum)[64])
 {
-    extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t *full_a = reinterpret_cast<uint64_t *>(smem + NST * STAGE_BYTES);
     const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31, wg = tid >> 7;
-    const int b = blockIdx.z, m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
     const int Ci = C1 + C2;
     const int nk = (Ci + TK - 1) / TK;
-    const unsigned char *wsrc = wpack + (size_t)blockIdx.y * nk * PACK_BLOCK_BYTES;
     auto fetch_a = [&](int kt) {
         const int st = kt % NST;
         const uint32_t bar = smem_u32(full_a + st);
@@ -231,11 +232,6 @@ fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__re
     __syncthreads();
     if (tid == 0) fetch_a(0);
 
-    const float *xb1 = x1 + (size_t)b * C1 * P;
-    const float *xb2 = x2 ? x2 + (size_t)b * C2 * P : nullptr;
-    const bool vec = ((P & 3) == 0) && ((reinterpret_cast<uintptr_t>(xb1) & 15) == 0) &&
-                     (!xb2 || (reinterpret_cast<uintptr_t>(xb2) & 15) == 0) &&
-                     ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
     // X tile (32 k x 128 n): warp -> K chunk kg (4 k rows), lane -> 4 n (128-bit loads); a thread ends up
     // with whole 16-byte (n; k..k+3) slots of the K-major layout
     const int kg = wid, nl = 4 * lane;
@@ -289,7 +285,7 @@ fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__re
         }
     };
 
-    float acc[64], sum[64];
+    float acc[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = sum[i] = 0.f;
     float4 rb[4];
@@ -307,6 +303,25 @@ fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__re
         wgmma_wait<1>();   // the MMAs of k-tile kt - 1 are done
     }
     drain(acc, sum);
+}
+
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__restrict__ x2, int C2,
+                         const unsigned char *__restrict__ wpack, const float *__restrict__ scale,
+                         const float *__restrict__ shift, float *__restrict__ out, int Co, int P, int act,
+                         float slope, MlpEpilogue ep)
+{
+    extern __shared__ __align__(1024) unsigned char smem[];
+    const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const int b = blockIdx.z, m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
+    const int nk = (C1 + C2 + TK - 1) / TK;
+    const float *xb1 = x1 + (size_t)b * C1 * P;
+    const float *xb2 = x2 ? x2 + (size_t)b * C2 * P : nullptr;
+    const bool vec = ((P & 3) == 0) && ((reinterpret_cast<uintptr_t>(xb1) & 15) == 0) &&
+                     (!xb2 || (reinterpret_cast<uintptr_t>(xb2) & 15) == 0) &&
+                     ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+    float sum[64];
+    packed_mainloop(smem, xb1, C1, xb2, C2, wpack + (size_t)blockIdx.y * nk * PACK_BLOCK_BYTES, P, n0, vec, sum);
 
     // accumulator fragment of m64n128: register 4i + 2h + c holds row 16 w + lane / 4 + 8 h,
     // column 8 i + 2 (lane % 4) + c of the warpgroup's 64 x 128 tile
@@ -355,6 +370,223 @@ fusion_mlp_packed_kernel(const float *__restrict__ x1, int C1, const float *__re
     }
 }
 
+// ===================================================================== PSP head (eval, DESIGN.md 4.17)
+// Bottleneck of PSPModule restructured (models/cnn/pspnet.py:24-31):
+//     out = relu( W_f * f + bias + sum_s up_s(T_s) ),   T_s = (W_s C_s) pool_s(f),   s = 1, 2, 3, 6
+// The product W_f * f is the packed main loop over the C feature channels only; the epilogue adds the
+// align_corners=False bilinear taps of the four prior tables T (channels-last, [B, s*s, Co] per scale, one after the
+// other), the bias and the ReLU.  The upsampled priors and the 5C-channel concat are never written.
+constexpr int PSP_NS = 4;
+__constant__ int c_psp_size[PSP_NS] = {1, 2, 3, 6};
+__constant__ int c_psp_off[PSP_NS] = {0, 1, 5, 14};   // first bin of each scale among the 50
+
+// one output coordinate's two source taps along one axis (torch upsample_bilinear2d, align_corners=False)
+struct PspTap {
+    int i0, i1;
+    float l0, l1;
+};
+
+__device__ __forceinline__ PspTap psp_tap(int dst, int out_size, int in_size)
+{
+    // area_pixel_compute_source_index: src = (in / out) * (dst + 0.5) - 0.5, clamped at 0; in double like the
+    // float64 reference, so that the tap index agrees with it wherever src is not within round-off of an integer
+    double src = (double)in_size / (double)out_size * ((double)dst + 0.5) - 0.5;
+    if (src < 0.0) src = 0.0;
+    PspTap t;
+    t.i0 = min((int)src, in_size - 1);
+    t.i1 = t.i0 + ((t.i0 < in_size - 1) ? 1 : 0);
+    const double l1 = src - (double)t.i0;
+    t.l1 = (float)l1;
+    t.l0 = (float)(1.0 - l1);
+    return t;
+}
+
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+psp_bottleneck_kernel(const float *__restrict__ x, int C, const unsigned char *__restrict__ wpack,
+                      const float *__restrict__ bias, const float *__restrict__ table, float *__restrict__ out, int Co,
+                      int H, int W, int B)
+{
+    extern __shared__ __align__(1024) unsigned char smem[];
+    const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const int b = blockIdx.z, m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
+    const int P = H * W;
+    const int nk = (C + TK - 1) / TK;
+    const float *xb = x + (size_t)b * C * P;
+    const bool vec = ((P & 3) == 0) && ((reinterpret_cast<uintptr_t>(xb) & 15) == 0) &&
+                     ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+    float sum[64];
+    packed_mainloop(smem, xb, C, nullptr, 0, wpack + (size_t)blockIdx.y * nk * PACK_BLOCK_BYTES, P, n0, vec, sum);
+    __syncthreads();   // both warpgroups are past their last MMA: the stages are free
+
+    // taps of every output row (scale-major, [4][H]) and column ([4][W])
+    PspTap *tap_y = reinterpret_cast<PspTap *>(smem), *tap_x = tap_y + PSP_NS * H;
+    for (int t = tid; t < PSP_NS * (H + W); t += MLP_THREADS) {
+        if (t < PSP_NS * H)
+            tap_y[t] = psp_tap(t % H, H, c_psp_size[t / H]);
+        else
+            tap_x[t - PSP_NS * H] = psp_tap((t - PSP_NS * H) % W, W, c_psp_size[(t - PSP_NS * H) / W]);
+    }
+    __syncthreads();
+
+    const int row0 = m0 + 64 * wg + 16 * (wid & 3) + (lane >> 2), col0 = n0 + 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < TN / 8; ++i) {
+        const int gn0 = col0 + 8 * i;
+        if (gn0 >= P) continue;
+        // the two pixels of this fragment column pair: their four scales' tap rows and columns
+        int oy0[2][PSP_NS], oy1[2][PSP_NS], ox0[2][PSP_NS], ox1[2][PSP_NS];
+        float ly0[2][PSP_NS], ly1[2][PSP_NS], lx0[2][PSP_NS], lx1[2][PSP_NS];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            const int gn = min(gn0 + u, P - 1), py = gn / W, px = gn - py * W;
+#pragma unroll
+            for (int k = 0; k < PSP_NS; ++k) {
+                const PspTap ty = tap_y[k * H + py], tx = tap_x[k * W + px];
+                const int s = c_psp_size[k];
+                // bin (iy, ix) of scale k, frame b: row (B * off_k + b * s * s + iy * s + ix) of the table
+                const int base = B * c_psp_off[k] + b * s * s;
+                oy0[u][k] = base + ty.i0 * s;
+                oy1[u][k] = base + ty.i1 * s;
+                ox0[u][k] = tx.i0;
+                ox1[u][k] = tx.i1;
+                ly0[u][k] = ty.l0;
+                ly1[u][k] = ty.l1;
+                lx0[u][k] = tx.l0;
+                lx1[u][k] = tx.l1;
+            }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int gm = row0 + 8 * h;
+            if (gm >= Co) continue;
+            const float bs = __ldg(bias + gm);
+            const float *tc = table + gm;   // channels-last: the 8 rows of a warp read 32 contiguous bytes
+            float y[2];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                float prior = 0.f;
+#pragma unroll
+                for (int k = 0; k < PSP_NS; ++k) {
+                    // torch's order: h0lambda * (w0lambda * t00 + w1lambda * t01) + h1lambda * (...); every tap is
+                    // read, so a NaN at a zero-weight tap propagates as it does in torch
+                    const float t00 = __ldg(tc + (size_t)(oy0[u][k] + ox0[u][k]) * Co);
+                    const float t01 = __ldg(tc + (size_t)(oy0[u][k] + ox1[u][k]) * Co);
+                    const float t10 = __ldg(tc + (size_t)(oy1[u][k] + ox0[u][k]) * Co);
+                    const float t11 = __ldg(tc + (size_t)(oy1[u][k] + ox1[u][k]) * Co);
+                    const float r0 = __fadd_rn(__fmul_rn(lx0[u][k], t00), __fmul_rn(lx1[u][k], t01));
+                    const float r1 = __fadd_rn(__fmul_rn(lx0[u][k], t10), __fmul_rn(lx1[u][k], t11));
+                    prior = __fadd_rn(prior, __fadd_rn(__fmul_rn(ly0[u][k], r0), __fmul_rn(ly1[u][k], r1)));
+                }
+                y[u] = max_nan(__fadd_rn(__fadd_rn(sum[4 * i + 2 * h + u], prior), bs), 0.f);
+            }
+            float *orow = out + ((size_t)b * Co + gm) * P;
+            if (vec && gn0 + 1 < P) {
+                *reinterpret_cast<float2 *>(orow + gn0) = make_float2(y[0], y[1]);
+            } else {
+#pragma unroll
+                for (int u = 0; u < 2; ++u)
+                    if (gn0 + u < P) orow[gn0 + u] = y[u];
+            }
+        }
+    }
+}
+
+// `final` of PSPNet (models/cnn/pspnet.py:108-112): 1x1 conv + bias + LogSoftmax over the channels, Co <= 128, so every
+// channel of a pixel is in the CTA's one 128-row tile.  The max and the sum of exponentials over the channels are
+// reduced in the epilogue (registers -> shuffles across the 8 rows of a warp -> shared memory across the 8 warps), and
+// the map is read once and written once.
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+conv1x1_log_softmax_kernel(const float *__restrict__ x, int Ci, const unsigned char *__restrict__ wpack,
+                           const float *__restrict__ bias, float *__restrict__ out, int Co, int P)
+{
+    extern __shared__ __align__(1024) unsigned char smem[];
+    const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31, wg = tid >> 7;
+    const int b = blockIdx.z, n0 = blockIdx.x * TN;
+    const float *xb = x + (size_t)b * Ci * P;
+    const bool vec = ((P & 3) == 0) && ((reinterpret_cast<uintptr_t>(xb) & 15) == 0) &&
+                     ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+    float sum[64];
+    packed_mainloop(smem, xb, Ci, nullptr, 0, wpack, P, n0, vec, sum);
+    __syncthreads();   // the stages are free
+
+    float *red = reinterpret_cast<float *>(smem);   // [8 warps][128 columns]
+    float *colv = red + 8 * TN;                      // [128]: the column's max, then its max + log(sum)
+    const int row0 = 64 * wg + 16 * (wid & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+    float bs[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) bs[h] = (row0 + 8 * h < Co) ? __ldg(bias + row0 + 8 * h) : 0.f;
+#pragma unroll
+    for (int i = 0; i < TN / 8; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int u = 0; u < 2; ++u) sum[4 * i + 2 * h + u] = __fadd_rn(sum[4 * i + 2 * h + u], bs[h]);
+
+    // max over the channels (NaN if any is NaN, torch's max)
+#pragma unroll
+    for (int i = 0; i < TN / 8; ++i)
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            float m = -INFINITY;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                if (row0 + 8 * h < Co) m = max_nan(m, sum[4 * i + 2 * h + u]);
+            m = max_nan(m, __shfl_xor_sync(0xffffffffu, m, 4));
+            m = max_nan(m, __shfl_xor_sync(0xffffffffu, m, 8));
+            m = max_nan(m, __shfl_xor_sync(0xffffffffu, m, 16));
+            if (lane < 4) red[wid * TN + 8 * i + c0 + u] = m;
+        }
+    __syncthreads();
+    if (tid < TN) {
+        float m = red[tid];
+        for (int w = 1; w < 8; ++w) m = max_nan(m, red[w * TN + tid]);
+        colv[tid] = m;
+    }
+    __syncthreads();
+    // sum of exp(y - max) over the channels
+#pragma unroll
+    for (int i = 0; i < TN / 8; ++i)
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            const float m = colv[8 * i + c0 + u];
+            float s = 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                if (row0 + 8 * h < Co) s = __fadd_rn(s, expf(__fsub_rn(sum[4 * i + 2 * h + u], m)));
+            s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 4));
+            s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 8));
+            s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 16));
+            if (lane < 4) red[wid * TN + 8 * i + c0 + u] = s;
+        }
+    __syncthreads();
+    if (tid < TN) {
+        float s = 0.f;
+        for (int w = 0; w < 8; ++w) s = __fadd_rn(s, red[w * TN + tid]);
+        red[tid] = logf(s);   // row 0 of red is read by no one else any more
+    }
+    __syncthreads();
+    // out = y - max - log(sum), as torch's log_softmax
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int gm = row0 + 8 * h;
+        if (gm >= Co) continue;
+        float *orow = out + ((size_t)b * Co + gm) * P;
+#pragma unroll
+        for (int i = 0; i < TN / 8; ++i) {
+            const int c = 8 * i + c0, gn = n0 + c;
+            float y[2];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) y[u] = __fsub_rn(__fsub_rn(sum[4 * i + 2 * h + u], colv[c + u]), red[c + u]);
+            if (vec && gn + 1 < P) {
+                *reinterpret_cast<float2 *>(orow + gn) = make_float2(y[0], y[1]);
+            } else {
+#pragma unroll
+                for (int u = 0; u < 2; ++u)
+                    if (gn + u < P) orow[gn + u] = y[u];
+            }
+        }
+    }
+}
 
 // ===================================================================== weight gradient (training)
 // dW[co, ci] = sum_b sum_p dZ[b, co, p] * X[b, ci, p],  X = [X1; X2]  (backward of the 1x1 conv w.r.t. its
@@ -684,5 +916,40 @@ extern "C" int ffb6d_fusion_mlp_wgrad_det(const float *grad_z, const float *x1, 
     const long long n = (long long)Co * Ci;
     wgrad_split_reduce_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(part, (int)splits, n, grad_w);
     FFB6D_LAUNCH_OK("wgrad_split_reduce_kernel");
+    return FFB6D_OK;
+}
+
+extern "C" int ffb6d_psp_bottleneck_fwd(const float *x, int64_t B, int64_t C, int64_t H, int64_t W, const void *packed,
+                                        const float *bias, int64_t Co, const float *table, float *out,
+                                        ffb6d_stream_t stream)
+{
+    FFB6D_CHECK_ARG(B >= 1 && C >= 1 && H >= 1 && W >= 1 && Co >= 1, "psp_bottleneck_fwd: bad size");
+    FFB6D_CHECK_ARG(B < 65536 && Co <= 65535ll * TM && C < (1ll << 31) && H + W <= 3072 && H * W < (1ll << 31) &&
+                        B * 50 * Co < (1ll << 31),
+                    "psp_bottleneck_fwd: size too large");
+    FFB6D_CHECK_ARG(x && packed && bias && table && out, "psp_bottleneck_fwd: null pointer");
+    FFB6D_CHECK_ARG((reinterpret_cast<uintptr_t>(packed) & 15) == 0, "psp_bottleneck_fwd: packed must be 16-byte aligned");
+    FFB6D_OPTIN_SMEM(psp_bottleneck_kernel, MLP_SMEM);
+    dim3 grid((unsigned)ceil_div(H * W, TN), (unsigned)ceil_div(Co, TM), (unsigned)B);
+    psp_bottleneck_kernel<<<grid, MLP_THREADS, MLP_SMEM, (cudaStream_t)stream>>>(
+        x, (int)C, (const unsigned char *)packed, bias, table, out, (int)Co, (int)H, (int)W, (int)B);
+    FFB6D_LAUNCH_OK("psp_bottleneck_kernel");
+    return FFB6D_OK;
+}
+
+extern "C" int ffb6d_conv1x1_log_softmax_fwd(const float *x, int64_t B, int64_t Ci, int64_t P, const void *packed,
+                                             const float *bias, int64_t Co, float *out, ffb6d_stream_t stream)
+{
+    FFB6D_CHECK_ARG(B >= 1 && Ci >= 1 && P >= 1 && Co >= 1, "conv1x1_log_softmax_fwd: bad size");
+    FFB6D_CHECK_ARG(Co <= TM, "conv1x1_log_softmax_fwd: Co = %lld, at most %d channels", (long long)Co, TM);
+    FFB6D_CHECK_ARG(B < 65536 && Ci < (1ll << 31) && P < (1ll << 31), "conv1x1_log_softmax_fwd: size too large");
+    FFB6D_CHECK_ARG(x && packed && bias && out, "conv1x1_log_softmax_fwd: null pointer");
+    FFB6D_CHECK_ARG((reinterpret_cast<uintptr_t>(packed) & 15) == 0,
+                    "conv1x1_log_softmax_fwd: packed must be 16-byte aligned");
+    FFB6D_OPTIN_SMEM(conv1x1_log_softmax_kernel, MLP_SMEM);
+    dim3 grid((unsigned)ceil_div(P, TN), 1u, (unsigned)B);
+    conv1x1_log_softmax_kernel<<<grid, MLP_THREADS, MLP_SMEM, (cudaStream_t)stream>>>(
+        x, (int)Ci, (const unsigned char *)packed, bias, out, (int)Co, (int)P);
+    FFB6D_LAUNCH_OK("conv1x1_log_softmax_kernel");
     return FFB6D_OK;
 }

@@ -12,11 +12,17 @@ The image branch enters through ``rgb_feats``: the eight tensors the CNN stages 
 ``rgb_stage_fn`` a caller can instead run its own CNN stage on the fused map, exactly where the reference does.
 
 Used by ``tools/train_bench.py`` for BASELINE configs 3-4 (forward + backward under DDP, synthetic data).
+
+``FFB6D`` is the whole network: ``FFB6DFusionNet`` plus the ResNet34-PSPNet image branch of :mod:`ffb6d_b200.cnn`
+driven through ``rgb_stage_fn``, with every name of the reference's state dict (``load_reference_checkpoint`` loads
+its trainer's checkpoints with ``strict=True``).
 """
+import os
+
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import cnn, ops
 from . import tables as T
 from .modules import Conv1d, Conv2d, Dilated_res_block, RandLAConv1d, RandLAConv2d
 
@@ -150,3 +156,68 @@ class FFB6DFusionNet(nn.Module):
         shapes += [(batch, T.UP_RGB_OC[i], h // T.RGB_UP_SR[i], w // T.RGB_UP_SR[i]) for i in range(3)]
         shapes.append((batch, T.UP_RGB_OC[2], h, w))
         return shapes
+
+
+class FFB6D(FFB6DFusionNet):
+    """The whole network of models/ffb6d.py: :class:`FFB6DFusionNet` plus the ResNet34-PSPNet image branch
+    (:mod:`ffb6d_b200.cnn`) under the reference's names ``cnn_pre_stages``, ``cnn_ds_stages`` and ``cnn_up_stages``, so
+    a reference checkpoint loads with ``strict=True`` (:func:`load_reference_checkpoint`).
+
+    ``forward(inputs)`` takes the reference's dict with ``inputs['rgb'] [B,3,H,W]`` float and returns its
+    ``end_points`` (plus ``fused_rgb``, as :class:`FFB6DFusionNet`).  The image branch runs where the reference runs
+    it: stage 0 is ``cnn_ds_stages[0](cnn_pre_stages(rgb))``, stages 1-3 take the previous fused map through
+    ``cnn_ds_stages[j]``, stages 4-7 through ``cnn_up_stages[j - 4]``.
+
+    * Training mode, or whenever autograd needs the image branch: its torch modules (cuDNN, batch statistics, active
+      dropout), as the reference.
+    * Eval mode without autograd: the PSP head (:meth:`ffb6d_b200.cnn.PSPModule.forward_fused`) and both uses of
+      ``final`` (:meth:`ffb6d_b200.cnn.Final.forward_fused`) run on this package's kernels; the trunk and the
+      ``PSPUpsample`` stages stay on cuDNN."""
+
+    def __init__(self, n_classes, n_pts=12288, n_kps=8, restructured=False):
+        super().__init__(n_classes=n_classes, n_pts=n_pts, n_kps=n_kps, restructured=restructured)
+        self.cnn_pre_stages, self.cnn_ds_stages, self.cnn_up_stages = cnn.image_branch()
+
+    def _image_needs_grad(self, rgb):
+        return torch.is_grad_enabled() and (rgb.requires_grad or any(
+            p.requires_grad for m in (self.cnn_pre_stages, self.cnn_ds_stages, self.cnn_up_stages) for p in m.parameters()))
+
+    def forward(self, inputs, end_points=None):
+        rgb = inputs["rgb"]
+        fused = not self.training and not self._image_needs_grad(rgb)
+        final = self.cnn_up_stages[2][0]
+
+        def stage(j, prev):
+            if j == 0:
+                return self.cnn_ds_stages[0](self.cnn_pre_stages(rgb))
+            if fused and j == 3:
+                return self.cnn_ds_stages[3][0].forward_fused(prev)              # psp (+ drop_1, identity in eval)
+            if fused and j == 6:
+                return final.forward_fused(prev)
+            if fused and j == 7:
+                return final.forward_fused(self.cnn_up_stages[3][0](prev))      # up_3, then final
+            return (self.cnn_ds_stages[j] if j < 4 else self.cnn_up_stages[j - 4])(prev)
+
+        out = super().forward(inputs, rgb_stage_fn=stage)
+        if end_points is not None:
+            end_points.update(out)
+            return end_points
+        return out
+
+
+def load_reference_checkpoint(model, path_or_dict):
+    """Load what the reference's training script saves (train_ycb.py:130-178) into ``model`` with ``strict=True``:
+    a path to a ``torch.save``'d checkpoint or the object itself, either ``{'model_state': state_dict, ...}`` or a bare
+    state dict, with or without the ``module.`` prefix of a (Distributed)DataParallel model.  Returns the result of
+    ``load_state_dict``."""
+    ck = path_or_dict
+    if isinstance(ck, (str, os.PathLike)):
+        ck = torch.load(ck, map_location="cpu", weights_only=False)
+    if isinstance(ck, dict) and "model_state" in ck:
+        ck = ck["model_state"]
+    if ck is None:
+        raise ValueError("the checkpoint holds no model_state")
+    keys = list(ck.keys())
+    if keys and all(k.startswith("module.") for k in keys):
+        ck = {k[len("module."):]: v for k, v in ck.items()}
+    return model.load_state_dict(ck, strict=True)

@@ -1291,3 +1291,106 @@ def of_l1_loss_bwd(pred, targ, labels, valid, count, grad_out):
                                        None if v is None else v.data_ptr(), B, K, N, count.data_ptr(), g.data_ptr(),
                                        grad.data_ptr(), _stream(dev)))
     return grad
+
+
+# --------------------------------------------------------------------------- PSP head of the image branch (eval)
+PSP_SIZES = (1, 2, 3, 6)
+_PSP_BINS = sum(s * s for s in PSP_SIZES)     # 50
+
+
+def _f32_map(x, name):
+    _need_cuda(x, name)
+    if x.dtype != torch.float32 or x.dim() != 4:
+        raise ValueError("%s must be float32 [B,C,H,W], got %s %s" % (name, x.dtype, tuple(x.shape)))
+    return x.contiguous()
+
+
+def psp_pool(x):
+    """``[AdaptiveAvgPool2d(s)(x) for s in (1, 2, 3, 6)]`` (the priors of PSPModule, models/cnn/pspnet.py:19-28) in
+    one read of ``x [B,C,H,W]`` float32 CUDA (``ffb6d_psp_pool``).  :return: four ``[B,C,s,s]`` tensors, views of one
+    buffer in the block order :func:`psp_bottleneck` reads."""
+    xc = _f32_map(x, "x")
+    B, C, H, W = xc.shape
+    out = torch.empty(_PSP_BINS * B * C, dtype=torch.float32, device=xc.device)
+    with torch.cuda.device(xc.device):
+        check(lib.ffb6d_psp_pool(xc.data_ptr(), B, C, H, W, out.data_ptr(), _stream(xc.device)))
+    views, off = [], 0
+    for s in PSP_SIZES:
+        views.append(out[off:off + B * C * s * s].view(B, C, s, s))
+        off += B * C * s * s
+    return views
+
+
+class PSPWeights:
+    """PSPModule's weights packed for :func:`psp_bottleneck`: with the bottleneck weight split by input block,
+    ``W = [W_1|W_2|W_3|W_6|W_f]``, the stage convs ``C_s`` are folded into ``M_s = W_s C_s`` (computed in fp64, then
+    packed), and ``W_f`` is packed as it is.  Build it once per weight version (inference)."""
+
+    def __init__(self, stage_weights, weight, bias):
+        _need_cuda(weight, "weight")
+        w = weight.detach().reshape(weight.shape[0], -1)
+        C = stage_weights[0].shape[0]
+        if len(stage_weights) != len(PSP_SIZES) or w.shape[1] != (len(PSP_SIZES) + 1) * C:
+            raise ValueError("PSPWeights: %d stage convs [C, C] and a [Co, %d C] bottleneck expected"
+                             % (len(PSP_SIZES), len(PSP_SIZES) + 1))
+        self.C, self.Co = int(C), int(w.shape[0])
+        self.stages = [PackedWeight((w[:, i * C:(i + 1) * C].double() @ cs.detach().reshape(C, C).double()).float())
+                       for i, cs in enumerate(stage_weights)]
+        self.feat = PackedWeight(w[:, len(PSP_SIZES) * C:])
+        self.bias = bias.detach().float().contiguous()
+        self.one = torch.ones(self.Co, dtype=torch.float32, device=w.device)
+        self.zero = torch.zeros(self.Co, dtype=torch.float32, device=w.device)
+        self.device = w.device
+
+
+def psp_pack(stage_weights, weight, bias):
+    """:class:`PSPWeights` from the four stage convs' weights ``[C,C,1,1]``, the bottleneck's weight
+    ``[Co,5C,1,1]`` and its bias ``[Co]``."""
+    return PSPWeights(stage_weights, weight, bias)
+
+
+def psp_bottleneck(x, pooled, weights):
+    """``relu(bottleneck(cat(up_1(C_1 p_1), .., up_6(C_6 p_6), x)))`` of PSPModule (models/cnn/pspnet.py:24-31) without
+    the upsampled priors or the concat: ``relu(W_f x + b + sum_s up_s(T_s))``, ``T_s = M_s p_s``.  The four ``T_s``
+    are packed GEMMs on the 50 pooled columns (``ffb6d_fusion_mlp_fwd_ex``, channels-last into one table), the rest
+    is ``ffb6d_psp_bottleneck_fwd``.  :param x: ``[B,C,H,W]`` float32 CUDA; :param pooled: :func:`psp_pool` of ``x``;
+    :param weights: :class:`PSPWeights`.  :return: ``[B,Co,H,W]``"""
+    xc = _f32_map(x, "x")
+    B, C, H, W = xc.shape
+    if C != weights.C or weights.device != xc.device:
+        raise ValueError("psp weights take %d channels on %s, x has %d on %s" % (weights.C, weights.device, C, xc.device))
+    Co = weights.Co
+    table = torch.empty(_PSP_BINS * B * Co, dtype=torch.float32, device=xc.device)
+    out = torch.empty((B, Co, H, W), dtype=torch.float32, device=xc.device)
+    st = _stream(xc.device)
+    with torch.cuda.device(xc.device):
+        off = 0
+        for s, p, pk in zip(PSP_SIZES, pooled, weights.stages):
+            if tuple(p.shape) != (B, C, s, s) or not p.is_contiguous() or p.dtype != torch.float32:
+                raise ValueError("pooled must be psp_pool(x)")
+            check(lib.ffb6d_fusion_mlp_fwd_ex(p.data_ptr(), C, None, 0, pk.data.data_ptr(), weights.one.data_ptr(),
+                                              weights.zero.data_ptr(), B, Co, s * s, 0, 0.0, None, None, 0, 0,
+                                              LAYOUT_NSC, table.data_ptr() + 4 * off * Co, st))
+            off += B * s * s
+        check(lib.ffb6d_psp_bottleneck_fwd(xc.data_ptr(), B, C, H, W, weights.feat.data.data_ptr(),
+                                           weights.bias.data_ptr(), Co, table.data_ptr(), out.data_ptr(), st))
+    return out
+
+
+def conv1x1_log_softmax(x, weight, bias):
+    """``log_softmax(conv1x1(x, weight, bias), dim=1)`` in one tensor-core kernel (``ffb6d_conv1x1_log_softmax_fwd``):
+    PSPNet's ``final`` (models/cnn/pspnet.py:108-112).  :param x: ``[B,Ci,H,W]`` float32 CUDA; :param weight:
+    ``[Co,Ci(,1,1)]`` or its :class:`PackedWeight`, Co <= 128; :param bias: ``[Co]``.  :return: ``[B,Co,H,W]``"""
+    xc = _f32_map(x, "x")
+    B, Ci, H, W = xc.shape
+    packed = weight if isinstance(weight, PackedWeight) else PackedWeight(weight)
+    if packed.Ci != Ci or packed.device != xc.device:
+        raise ValueError("weight takes %d channels on %s, x has %d on %s" % (packed.Ci, packed.device, Ci, xc.device))
+    b = bias.detach().float().contiguous()
+    if b.numel() != packed.Co or b.device != xc.device:
+        raise ValueError("bias must have %d elements on %s" % (packed.Co, xc.device))
+    out = torch.empty((B, packed.Co, H, W), dtype=torch.float32, device=xc.device)
+    with torch.cuda.device(xc.device):
+        check(lib.ffb6d_conv1x1_log_softmax_fwd(xc.data_ptr(), B, Ci, H * W, packed.data.data_ptr(), b.data_ptr(),
+                                                packed.Co, out.data_ptr(), _stream(xc.device)))
+    return out

@@ -649,6 +649,32 @@ int ffb6d_of_l1_loss_bwd(const float *pred, const float *targ, const void *label
                          const uint8_t *valid, int64_t B, int64_t n_kps, int64_t N, const float *count,
                          const float *grad_out, float *grad_pred, ffb6d_stream_t stream);
 
+/*
+ * The PSP head of FFB6D's image branch at inference (models/cnn/pspnet.py:7-31, 108-112; DESIGN.md §4.17).
+ *
+ * ffb6d_psp_pool: AdaptiveAvgPool2d at the sizes 1, 2, 3 and 6 of x [B,C,H,W] f32 in one read, with torch's bins
+ *   (bin i of s over n: [floor(i n / s), ceil((i + 1) n / s)), overlapping where s does not divide n).  out holds the
+ *   50 B C bins scale-major: [B,C,1,1], [B,C,2,2], [B,C,3,3], [B,C,6,6] one after the other, each block equal to
+ *   adaptive_avg_pool2d(x, s).  Sums in fp64.  1 <= B, C; B C < 2^31; 1 <= H <= 1024; 1 <= W < 2^24.  One launch.
+ * ffb6d_psp_bottleneck_fwd: out [B,Co,H,W] = relu(W_f x + bias + sum_s up_s(T_s)), the bottleneck of PSPModule with
+ *   its concat split by input block (W = [W_1|W_2|W_3|W_6|W_f]) and the stage convs moved behind the pooling:
+ *   T_s = W_s C_s pool_s(x).  packed = ffb6d_fusion_mlp_pack of W_f [Co, C]; bias [Co]; table [B*50, Co] f32, the
+ *   four T_s channels-last, in the block order of ffb6d_psp_pool ([B, s*s, Co] for s = 1, 2, 3, 6, e.g. made by
+ *   ffb6d_fusion_mlp_fwd_ex with out_layout FFB6D_LAYOUT_NSC).  up_s is torch's bilinear upsampling with
+ *   align_corners=False, all four taps read (a NaN at a zero-weight tap propagates, as in torch).  3xTF32 on wgmma,
+ *   like the fusion layers.  1 <= B < 65536; H + W <= 3072; B * 50 * Co < 2^31.  One launch.
+ * ffb6d_conv1x1_log_softmax_fwd: out [B,Co,P] = log_softmax(W x + bias, dim=1) for x [B,Ci,P] f32, packed =
+ *   ffb6d_fusion_mlp_pack of W [Co, Ci], bias [Co]; 1 <= Co <= 128 (every channel of a pixel in one output tile).
+ *   out = y - max - log(sum exp(y - max)) per pixel, NaN / +-inf propagate as torch's log_softmax.  One launch.
+ * All three check sizes and null pointers before any launch (FFB6D_ERR_INVALID); no allocation, no host
+ * synchronisation (capturable in a CUDA graph), no atomics.
+ */
+int ffb6d_psp_pool(const float *x, int64_t B, int64_t C, int64_t H, int64_t W, float *out, ffb6d_stream_t stream);
+int ffb6d_psp_bottleneck_fwd(const float *x, int64_t B, int64_t C, int64_t H, int64_t W, const void *packed,
+                             const float *bias, int64_t Co, const float *table, float *out, ffb6d_stream_t stream);
+int ffb6d_conv1x1_log_softmax_fwd(const float *x, int64_t B, int64_t Ci, int64_t P, const void *packed,
+                                  const float *bias, int64_t Co, float *out, ffb6d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
