@@ -26,7 +26,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   :func:`~ffb6d_b200.loss.ffb6d_loss`, ``model_fn``'s loss block, masked by the batch's valid frames.
 * :mod:`ffb6d_b200.cnn` -- the ResNet34-PSPNet image branch (models/cnn/extractors.py, models/cnn/pspnet.py) in
   torch, with :func:`psp_pool`, :func:`psp_bottleneck` and :func:`conv1x1_log_softmax` on the GPU for its PSP head
-  and ``final`` at inference; ``ffb6d_b200.model.FFB6D`` is the whole network.
+  and ``final`` at inference, and their adjoints (:func:`psp_bottleneck_bwd`, :func:`psp_pool_bwd`,
+  :func:`log_softmax_bwd`, :func:`upsample_bilinear2d_bwd`) for deterministic training;
+  ``ffb6d_b200.model.FFB6D`` is the whole network.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -42,7 +44,8 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "choose_gather", "grid_sub_sampling", "KnnGrid", "backproject", "fusion_mlp", "fusion_mlp_pack",
         "PackedWeight", "fold_batchnorm", "att_pool", "sample_valid_pixels", "check_indices", "mean_shift_fit", "best_fit_transform",
         "fill_missing", "segment_plan", "segment_sum", "point_item", "rgb_add_noise", "add_real_back",
-        "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax")
+        "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax",
+        "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")

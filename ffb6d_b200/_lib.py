@@ -115,6 +115,10 @@ def _load():
         "ffb6d_psp_pool": (ci, [vp, i64, i64, i64, i64, vp, vp]),
         "ffb6d_psp_bottleneck_fwd": (ci, [vp, i64, i64, i64, i64, vp, vp, i64, vp, vp, vp]),
         "ffb6d_conv1x1_log_softmax_fwd": (ci, [vp, i64, i64, i64, vp, vp, i64, vp, vp]),
+        "ffb6d_psp_bottleneck_bwd": (ci, [vp, vp, i64, i64, i64, i64, vp, vp, vp, vp]),
+        "ffb6d_psp_pool_bwd": (ci, [vp, i64, i64, i64, i64, vp, vp]),
+        "ffb6d_log_softmax_bwd": (ci, [vp, vp, i64, i64, i64, vp, vp]),
+        "ffb6d_upsample_bilinear2d_bwd": (ci, [vp, i64, i64, i64, i64, i64, i64, vp, vp]),
         "ffb6d_grid_subsample_host": (ci, [vp, sz, vp, sz, vp, sz, fp, vp, vp, vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():

@@ -14,8 +14,12 @@ What the reference's code does, and these modules therefore do too:
   ResNet (conv ``normal_(0, sqrt(2 / n))`` with n = k*k*out_channels, BatchNorm 1 / 0), the head with torch's defaults.
 
 The modules' ``forward`` is the reference's, on any device and dtype.  :meth:`PSPModule.forward_fused` and
-:meth:`Final.forward_fused` are the inference paths on this package's kernels (:func:`ffb6d_b200.ops.psp_bottleneck`,
-:func:`ffb6d_b200.ops.conv1x1_log_softmax`); :class:`ffb6d_b200.model.FFB6D` takes them in eval mode.
+:meth:`Final.forward_fused` are the same on this package's kernels (:func:`ffb6d_b200.ops.psp_bottleneck`,
+:func:`ffb6d_b200.ops.conv1x1_log_softmax`); :class:`ffb6d_b200.model.FFB6D` takes them in eval mode.  They are
+differentiable: under autograd their backward is the adjoint kernels of DESIGN.md §4.18, which add in a fixed order and
+so follow ``torch.use_deterministic_algorithms(True)``, where torch's adaptive-average-pool and bilinear backwards
+raise.  :meth:`PSPUpsample.forward_fused` is the module with its x2 upsampling's backward on
+:func:`ffb6d_b200.ops.upsample_bilinear2d_bwd`.  ``FFB6D(fused_image_head=True)`` trains through all three.
 """
 import math
 
@@ -104,9 +108,9 @@ class PSPModule(nn.Module):
         return self.relu(self.bottleneck(torch.cat(priors, 1)))
 
     def forward_fused(self, feats):
-        """The same at inference on the package's kernels (no autograd): one pooling pass, the stage convs folded
-        into the bottleneck's blocks, and a bottleneck GEMM over the input's channels only whose epilogue adds the
-        upsampled priors (DESIGN.md §4.17)."""
+        """The same on the package's kernels: one pooling pass, the stage convs folded into the bottleneck's blocks,
+        and a bottleneck GEMM over the input's channels only whose epilogue adds the upsampled priors (DESIGN.md
+        §4.17).  Differentiable (:class:`_PSPFused`, DESIGN.md §4.18); the output is the same either way."""
         from . import ops
         if tuple(tuple(st[0].output_size) for st in self.stages) != tuple((s, s) for s in PSP_SIZES):
             raise ValueError("forward_fused: the kernels pool at the sizes %s only" % (PSP_SIZES,))
@@ -114,7 +118,64 @@ class PSPModule(nn.Module):
         if self._packed is None or self._packed[0] != ver:
             self._packed = (ver, ops.psp_pack([st[1].weight for st in self.stages], self.bottleneck.weight,
                                               self.bottleneck.bias))
+        params = [st[1].weight for st in self.stages] + [self.bottleneck.weight, self.bottleneck.bias]
+        if _needs_grad(feats, params):
+            return _PSPFused.apply(feats, self._packed[1], *params)
         return ops.psp_bottleneck(feats, ops.psp_pool(feats), self._packed[1])
+
+
+def _needs_grad(x, params):
+    return torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))
+
+
+class _PSPFused(torch.autograd.Function):
+    """PSPModule on the kernels, with its backward (DESIGN.md §4.18).  With ``M_s = W_s C_s``, ``p_s = pool_s(x)``,
+    ``T_s = M_s p_s`` and ``out = relu(W_f x + b + sum_s up_s(T_s))``:
+
+    * ``grad_z`` and every ``dT_s`` in one launch (:func:`ops.psp_bottleneck_bwd`);
+    * ``dW_f = sum_b grad_z x^T`` (:func:`modules._wgrad`, ordered under deterministic mode), ``db = sum grad_z``;
+    * ``dM_s = sum_b dT_s p_s^T``, ``dW_s = dM_s C_s^T``, ``dC_s = W_s^T dM_s``, ``dp_s = M_s^T dT_s`` (small; fp64);
+    * ``dx = W_f^T grad_z`` (the forward GEMM on the transposed block), then ``+= pool^T(dp)``
+      (:func:`ops.psp_pool_bwd`)."""
+
+    @staticmethod
+    def forward(ctx, x, packed, c1, c2, c3, c6, weight, bias):
+        from . import ops
+        x = x.contiguous()
+        pooled = ops.psp_pool(x)
+        out = ops.psp_bottleneck(x, pooled, packed)
+        ctx.save_for_backward(x, out, weight, c1, c2, c3, c6, *pooled)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad):
+        from . import modules, ops
+        x, out, weight = ctx.saved_tensors[:3]
+        cs, pooled = ctx.saved_tensors[3:7], ctx.saved_tensors[7:]
+        B, C, H, W = x.shape
+        Co = out.shape[1]
+        gz, table, gsum = ops.psp_bottleneck_bwd(grad.contiguous(), out)
+        w = weight.detach().reshape(Co, -1)
+        gw, gcs, gp = [], [], []
+        row = 0
+        for i, (s, cw, p) in enumerate(zip(PSP_SIZES, cs, pooled)):
+            n = s * s
+            dT = table[row:row + B * n].view(B, n, Co).double()
+            row += B * n
+            ws, cm = w[:, i * C:(i + 1) * C].double(), cw.detach().reshape(C, C).double()
+            dM = torch.einsum("bno,bcn->oc", dT, p.reshape(B, C, n).double())
+            gw.append((dM @ cm.t()).float())
+            gcs.append((ws.t() @ dM).float().reshape(cw.shape))
+            gp.append(torch.einsum("oc,bno->bcn", ws @ cm, dT).float().reshape(B, C, s, s))
+        gw.append(modules._wgrad(gz, x, None, B, Co, H * W))
+        gweight = torch.cat(gw, 1).reshape(weight.shape)
+        gbias = gsum.double().sum(0).float()
+        gx = None
+        if ctx.needs_input_grad[0]:
+            gx = modules._gemm(gz, None, w[:, len(PSP_SIZES) * C:].t().contiguous()).reshape(x.shape)
+            ops.psp_pool_bwd(gp, gx)
+        return (gx, None, *gcs, gweight, gbias)
 
 
 class PSPUpsample(nn.Module):
@@ -129,6 +190,15 @@ class PSPUpsample(nn.Module):
     def forward(self, x):
         return self.conv(x)
 
+    def forward_fused(self, x):
+        """The same modules, with the x2 upsampling's backward on :func:`ffb6d_b200.ops.upsample_bilinear2d_bwd`
+        (torch's forward; a backward that adds in a fixed order).  The conv, BatchNorm and PReLU stay torch's."""
+        from . import ops
+        up, conv, bn, act = self.conv
+        if up.mode != "bilinear" or not up.align_corners or up.size is not None:
+            raise ValueError("forward_fused: bilinear upsampling with align_corners=True by a scale factor only")
+        return act(bn(conv(ops.upsample_bilinear2d(x, up.scale_factor))))
+
 
 class Final(nn.Sequential):
     """PSPNet's ``final``: ``Conv2d(64, 64, 1)`` and a LogSoftmax over the channels (state-dict keys ``0.weight``,
@@ -139,13 +209,45 @@ class Final(nn.Sequential):
         self._packed = None      # (parameter versions, ops.PackedWeight) of forward_fused
 
     def forward_fused(self, x):
-        """The same at inference in one kernel (``ffb6d_conv1x1_log_softmax_fwd``; no autograd)."""
+        """The same in one kernel (``ffb6d_conv1x1_log_softmax_fwd``).  Differentiable (:class:`_FinalFused`); the
+        output is the same either way."""
         from . import ops
         conv = self[0]
         ver = _version((conv.weight, conv.bias))
         if self._packed is None or self._packed[0] != ver:
             self._packed = (ver, ops.fusion_mlp_pack(conv.weight.detach()))
+        if _needs_grad(x, (conv.weight, conv.bias)):
+            return _FinalFused.apply(x, self._packed[1], conv.weight, conv.bias)
         return ops.conv1x1_log_softmax(x, self._packed[1], conv.bias)
+
+
+class _FinalFused(torch.autograd.Function):
+    """``final`` on the kernel, with its backward: ``dz`` = the log-softmax backward (:func:`ops.log_softmax_bwd`),
+    then ``dW = sum_b dz x^T`` (:func:`modules._wgrad`), ``db = sum dz`` and ``dx = W^T dz`` (the forward GEMM on
+    the transposed weight).  ``final`` is used twice per step; autograd adds the two uses' gradients."""
+
+    @staticmethod
+    def forward(ctx, x, packed, weight, bias):
+        from . import ops
+        x = x.contiguous()
+        out = ops.conv1x1_log_softmax(x, packed, bias)
+        ctx.save_for_backward(x, out, weight)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad):
+        from . import modules, ops
+        x, out, weight = ctx.saved_tensors
+        B, Co = out.shape[0], out.shape[1]
+        dz = ops.log_softmax_bwd(grad.contiguous(), out)
+        gw = modules._wgrad(dz, x, None, B, Co, out.numel() // (B * Co)).reshape(weight.shape)
+        # per-plane sums first: torch.sum(..., dtype=float64) would make a float64 copy of dz (1.3 GB at B = 8, 480x640)
+        gb = dz.sum(dim=(2, 3)).double().sum(0).float()
+        gx = None
+        if ctx.needs_input_grad[0]:
+            gx = modules._gemm(dz, None, weight.detach().reshape(Co, -1).t().contiguous()).reshape(x.shape)
+        return gx, None, gw, gb
 
 
 class PSPNet34(nn.Module):

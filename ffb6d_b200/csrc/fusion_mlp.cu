@@ -32,6 +32,7 @@
 //     into round-to-nearest fp32 register sums
 //   * epilogue: scale/shift/activation in registers, stores along the point axis (NCHW output)
 #include "common.cuh"
+#include "psp.cuh"
 
 #include <algorithm>
 #include <stdlib.h>
@@ -380,26 +381,7 @@ constexpr int PSP_NS = 4;
 __constant__ int c_psp_size[PSP_NS] = {1, 2, 3, 6};
 __constant__ int c_psp_off[PSP_NS] = {0, 1, 5, 14};   // first bin of each scale among the 50
 
-// one output coordinate's two source taps along one axis (torch upsample_bilinear2d, align_corners=False)
-struct PspTap {
-    int i0, i1;
-    float l0, l1;
-};
-
-__device__ __forceinline__ PspTap psp_tap(int dst, int out_size, int in_size)
-{
-    // area_pixel_compute_source_index: src = (in / out) * (dst + 0.5) - 0.5, clamped at 0; in double like the
-    // float64 reference, so that the tap index agrees with it wherever src is not within round-off of an integer
-    double src = (double)in_size / (double)out_size * ((double)dst + 0.5) - 0.5;
-    if (src < 0.0) src = 0.0;
-    PspTap t;
-    t.i0 = min((int)src, in_size - 1);
-    t.i1 = t.i0 + ((t.i0 < in_size - 1) ? 1 : 0);
-    const double l1 = src - (double)t.i0;
-    t.l1 = (float)l1;
-    t.l0 = (float)(1.0 - l1);
-    return t;
-}
+// psp_tap (psp.cuh): one output coordinate's two source taps along one axis, shared with the adjoint in psp.cu
 
 __global__ void __launch_bounds__(MLP_THREADS, 1)
 psp_bottleneck_kernel(const float *__restrict__ x, int C, const unsigned char *__restrict__ wpack,

@@ -172,11 +172,19 @@ class FFB6D(FFB6DFusionNet):
       dropout), as the reference.
     * Eval mode without autograd: the PSP head (:meth:`ffb6d_b200.cnn.PSPModule.forward_fused`) and both uses of
       ``final`` (:meth:`ffb6d_b200.cnn.Final.forward_fused`) run on this package's kernels; the trunk and the
-      ``PSPUpsample`` stages stay on cuDNN."""
+      ``PSPUpsample`` stages stay on cuDNN.
+    * ``fused_image_head=True`` (a plain attribute like ``restructured``; it may be switched on a built or loaded
+      model and does not change the state dict): whenever autograd needs the image branch, the PSP head, the x2
+      upsampling of ``up_1`` / ``up_2`` / ``up_3`` and both uses of ``final`` run their ``forward_fused`` paths,
+      whose backwards are this package's kernels (DESIGN.md §4.18).  Their backwards add in a fixed order, so the
+      whole network trains under ``torch.use_deterministic_algorithms(True)``, where torch's adaptive-average-pool
+      and bilinear-upsampling backwards raise.  The trunk, the 3x3 convs, BatchNorms and PReLUs of ``PSPUpsample``
+      and the dropouts stay torch modules (the CUDA RNG is drawn as on the torch path).  Off by default."""
 
-    def __init__(self, n_classes, n_pts=12288, n_kps=8, restructured=False):
+    def __init__(self, n_classes, n_pts=12288, n_kps=8, restructured=False, fused_image_head=False):
         super().__init__(n_classes=n_classes, n_pts=n_pts, n_kps=n_kps, restructured=restructured)
         self.cnn_pre_stages, self.cnn_ds_stages, self.cnn_up_stages = cnn.image_branch()
+        self.fused_image_head = bool(fused_image_head)
 
     def _image_needs_grad(self, rgb):
         return torch.is_grad_enabled() and (rgb.requires_grad or any(
@@ -184,12 +192,25 @@ class FFB6D(FFB6DFusionNet):
 
     def forward(self, inputs, end_points=None):
         rgb = inputs["rgb"]
-        fused = not self.training and not self._image_needs_grad(rgb)
+        needs_grad = self._image_needs_grad(rgb)
+        fused = not self.training and not needs_grad
+        train_fused = self.fused_image_head and needs_grad
         final = self.cnn_up_stages[2][0]
+        up = self.cnn_up_stages
 
         def stage(j, prev):
             if j == 0:
                 return self.cnn_ds_stages[0](self.cnn_pre_stages(rgb))
+            if train_fused and j == 3:
+                psp, drop_1 = self.cnn_ds_stages[3]
+                return drop_1(psp.forward_fused(prev))
+            if train_fused and j in (4, 5):
+                ups, drop_2 = up[j - 4]
+                return drop_2(ups.forward_fused(prev))
+            if train_fused and j == 6:
+                return final.forward_fused(prev)
+            if train_fused and j == 7:
+                return final.forward_fused(up[3][0].forward_fused(prev))
             if fused and j == 3:
                 return self.cnn_ds_stages[3][0].forward_fused(prev)              # psp (+ drop_1, identity in eval)
             if fused and j == 6:

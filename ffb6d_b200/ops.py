@@ -1394,3 +1394,96 @@ def conv1x1_log_softmax(x, weight, bias):
         check(lib.ffb6d_conv1x1_log_softmax_fwd(xc.data_ptr(), B, Ci, H * W, packed.data.data_ptr(), b.data_ptr(),
                                                 packed.Co, out.data_ptr(), _stream(xc.device)))
     return out
+
+
+# --------------------------------------------------------------------------- PSP head of the image branch (training)
+def psp_bottleneck_bwd(grad_out, out):
+    """Backward of :func:`psp_bottleneck` (``ffb6d_psp_bottleneck_bwd``, one launch) from ``grad_out`` and the forward's
+    ``out`` ``[B,Co,H,W]`` float32 CUDA.  :return: ``(grad_z [B,Co,H,W], grad_table [B*50, Co], grad_sum [B, Co])``:
+    the gradient of the bottleneck's pre-ReLU sum (torch's ReLU backward on ``out``), that of the prior table in the
+    forward's layout (block ``s`` is ``[B, s*s, Co]``, in the order of :data:`PSP_SIZES`), and the per-frame sums of
+    ``grad_z`` (the bias gradient is their sum over the frames)."""
+    o = _f32_map(out, "out")
+    B, Co, H, W = o.shape
+    g = _f32(grad_out, "grad_out", o.shape)
+    if g.device != o.device:
+        raise ValueError("grad_out and out must be on the same device")
+    gz = torch.empty_like(o)
+    table = torch.empty((_PSP_BINS * B, Co), dtype=torch.float32, device=o.device)
+    gsum = torch.empty((B, Co), dtype=torch.float32, device=o.device)
+    with torch.cuda.device(o.device):
+        check(lib.ffb6d_psp_bottleneck_bwd(g.data_ptr(), o.data_ptr(), B, Co, H, W, gz.data_ptr(), table.data_ptr(),
+                                           gsum.data_ptr(), _stream(o.device)))
+    return gz, table, gsum
+
+
+def psp_pool_bwd(grad_pooled, grad_x):
+    """Adjoint of :func:`psp_pool` (``ffb6d_psp_pool_bwd``, one launch), accumulated: ``grad_x [B,C,H,W]`` float32 CUDA
+    (contiguous; updated in place and returned) ``+= sum_s pool_s^T(grad_pooled[s])``.  :param grad_pooled: the four
+    ``[B,C,s,s]`` gradients of :func:`psp_pool`'s outputs, or one flat buffer in its block order."""
+    gx = _f32_map(grad_x, "grad_x")
+    if gx.data_ptr() != grad_x.data_ptr():
+        raise ValueError("grad_x must be contiguous (it is updated in place)")
+    B, C, H, W = gx.shape
+    if isinstance(grad_pooled, torch.Tensor):
+        gp = _f32(grad_pooled, "grad_pooled", (_PSP_BINS * B * C,))
+    else:
+        parts = [_f32(p, "grad_pooled[%d]" % i, (B, C, s, s)) for i, (s, p) in enumerate(zip(PSP_SIZES, grad_pooled))]
+        if len(parts) != len(PSP_SIZES):
+            raise ValueError("grad_pooled must hold %d tensors" % len(PSP_SIZES))
+        gp = torch.cat([p.reshape(-1) for p in parts])
+    if gp.device != gx.device:
+        raise ValueError("grad_pooled and grad_x must be on the same device")
+    with torch.cuda.device(gx.device):
+        check(lib.ffb6d_psp_pool_bwd(gp.data_ptr(), B, C, H, W, gx.data_ptr(), _stream(gx.device)))
+    return grad_x
+
+
+def log_softmax_bwd(grad_out, out):
+    """Backward of ``log_softmax(dim=1)`` from its result ``out`` and ``grad_out`` ``[B,C,...]`` float32 CUDA
+    (``ffb6d_log_softmax_bwd``, one launch): ``grad_out - exp(out) * grad_out.sum(1, keepdim=True)``."""
+    _need_cuda(out, "out")
+    if out.dtype != torch.float32 or out.dim() < 2:
+        raise ValueError("out must be float32 [B,C,...], got %s %s" % (out.dtype, tuple(out.shape)))
+    o = out.contiguous()
+    g = _f32(grad_out, "grad_out", o.shape)
+    if g.device != o.device:
+        raise ValueError("grad_out and out must be on the same device")
+    B, C = o.shape[0], o.shape[1]
+    gi = torch.empty_like(o)
+    with torch.cuda.device(o.device):
+        check(lib.ffb6d_log_softmax_bwd(g.data_ptr(), o.data_ptr(), B, C, o.numel() // (B * C), gi.data_ptr(),
+                                        _stream(o.device)))
+    return gi
+
+
+def upsample_bilinear2d_bwd(grad_out, input_size):
+    """Backward of ``F.interpolate(x, mode="bilinear", align_corners=True)`` (``ffb6d_upsample_bilinear2d_bwd``, one
+    launch): ``grad_out [B,C,Ho,Wo]`` float32 CUDA, ``input_size = (Hi, Wi)``.  :return: ``grad_in [B,C,Hi,Wi]``"""
+    g = _f32_map(grad_out, "grad_out")
+    B, C, Ho, Wo = g.shape
+    Hi, Wi = (int(v) for v in input_size)
+    gi = torch.empty((B, C, Hi, Wi), dtype=torch.float32, device=g.device)
+    with torch.cuda.device(g.device):
+        check(lib.ffb6d_upsample_bilinear2d_bwd(g.data_ptr(), B, C, Hi, Wi, Ho, Wo, gi.data_ptr(), _stream(g.device)))
+    return gi
+
+
+class _UpsampleBilinear2d(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, scale_factor):
+        ctx.in_size = tuple(x.shape[2:])
+        return torch.nn.functional.interpolate(x, scale_factor=scale_factor, mode="bilinear", align_corners=True)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad):
+        return upsample_bilinear2d_bwd(grad.contiguous(), ctx.in_size), None
+
+
+def upsample_bilinear2d(x, scale_factor=2):
+    """``F.interpolate(x, scale_factor=scale_factor, mode="bilinear", align_corners=True)`` (``nn.Upsample`` of
+    PSPUpsample, models/cnn/pspnet.py:36-48) with a deterministic backward: the forward is torch's, the backward
+    :func:`upsample_bilinear2d_bwd`.  :param x: ``[B,C,H,W]`` float32 CUDA."""
+    _f32_map(x, "x")
+    return _UpsampleBilinear2d.apply(x, scale_factor)

@@ -675,6 +675,37 @@ int ffb6d_psp_bottleneck_fwd(const float *x, int64_t B, int64_t C, int64_t H, in
 int ffb6d_conv1x1_log_softmax_fwd(const float *x, int64_t B, int64_t Ci, int64_t P, const void *packed,
                                   const float *bias, int64_t Co, float *out, ffb6d_stream_t stream);
 
+/*
+ * The backward of the PSP head and of PSPUpsample's upsampling, for training (DESIGN.md §4.18).  All four check
+ * sizes, null pointers and 4-byte alignment before any launch (FFB6D_ERR_INVALID); one launch each, no allocation,
+ * no host synchronisation (capturable in a CUDA graph), no atomics: every output element is written once, its sum
+ * taken in a fixed order, so results are bit-identical from run to run (torch.use_deterministic_algorithms).
+ *
+ * ffb6d_psp_bottleneck_bwd: backward of ffb6d_psp_bottleneck_fwd from grad_out and the forward's out [B,Co,H,W]:
+ *   grad_z = threshold_backward(grad_out, out, 0) (0 where out <= 0, grad_out elsewhere, as torch's ReLU backward on
+ *   its result); grad_table [B*50, Co], laid out as the forward's table, = the adjoint of sum_s up_s(T_s) applied to
+ *   grad_z, with the forward's taps, every tap's product added (weight 0 too); grad_sum [B*Co] = the sum of each
+ *   (frame, channel) plane of grad_z (the bias gradient is its sum over the frames).  Sums in fp64.
+ *   1 <= B, Co; H, W <= 1024 with H*104 + (H + W)*64 <= 227 KB of shared memory; B Co < 2^31.
+ * ffb6d_psp_pool_bwd: adjoint of ffb6d_psp_pool: grad_x [B,C,H,W] += sum over the bins of the four sizes that contain
+ *   a pixel of grad_pooled[bin] / area(bin), grad_pooled in ffb6d_psp_pool's block order.  grad_x must hold a value
+ *   (e.g. the bottleneck's input gradient W_f^T grad_z); the sum is in fp64, rounded once into it.
+ *   H <= 1024, W <= 16384, B C < 2^31.
+ * ffb6d_log_softmax_bwd: grad_in = grad_out - exp(out) * sum_c grad_out per pixel, for out, grad_out [B,C,P]
+ *   (channel stride P; torch's _log_softmax_backward_data, NaN / +-inf propagating as there).  B < 65536.
+ * ffb6d_upsample_bilinear2d_bwd: backward of upsample_bilinear2d(align_corners=True) from grad_out [B,C,Ho,Wo] to
+ *   grad_in [B,C,Hi,Wi] (written, not added), with torch's float taps (scale = (float)(in-1)/(out-1), 0 when out == 1),
+ *   weight-0 taps included.  Every size < 2^24.
+ */
+int ffb6d_psp_bottleneck_bwd(const float *grad_out, const float *out, int64_t B, int64_t Co, int64_t H, int64_t W,
+                             float *grad_z, float *grad_table, float *grad_sum, ffb6d_stream_t stream);
+int ffb6d_psp_pool_bwd(const float *grad_pooled, int64_t B, int64_t C, int64_t H, int64_t W, float *grad_x,
+                       ffb6d_stream_t stream);
+int ffb6d_log_softmax_bwd(const float *grad_out, const float *out, int64_t B, int64_t C, int64_t P, float *grad_in,
+                          ffb6d_stream_t stream);
+int ffb6d_upsample_bilinear2d_bwd(const float *grad_out, int64_t B, int64_t C, int64_t Hi, int64_t Wi, int64_t Ho,
+                                  int64_t Wo, float *grad_in, ffb6d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,11 +8,25 @@
 * ``train_step``: forward + ``ffb6d_loss`` + backward in training mode at BASELINE config 3's shape (LineMOD:
   2 classes, B = 8, 12288 points; the image branch runs its torch modules in training).
 
+With ``--train-arms`` it measures the training path instead (DESIGN.md §4.18), every arm alternated within each of
+``--reps`` repetitions, and prints the card's name and power limit first:
+
+* ``psp_train`` (B = 1, 8) and ``final240_train`` / ``final480_train`` (B = 8): forward + backward of the PSP block
+  and of both uses of ``final``, torch's modules against ``forward_fused`` (median of ``--iters`` graph replays), and
+  the peak memory one eager call of each allocates above what was allocated before it;
+* ``train_step_arm``: the config-3 step with ``fused_image_head`` off, on, and on under
+  ``torch.use_deterministic_algorithms(True)`` (median of max(3, ``--iters`` // 4) eager steps), each with
+  ``torch.cuda.max_memory_allocated``;
+* with ``--profile``, the CUDA time per kernel name of one step of each setting (``torch.profiler``).
+
 Prints one JSON line per measurement.  Usage: python tools/cnn_bench.py [--iters 20] [--batches 1,8] [--no-train]
+[--train-arms [--reps 3] [--profile]]
 """
 import argparse
+import contextlib
 import json
 import os
+import subprocess
 import sys
 
 import torch
@@ -108,12 +122,127 @@ def network(B, n_pts, train, n_classes=22):
     return model, inputs
 
 
+def card():
+    """The card's name and its power limit (read-only query)."""
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        q = "unavailable (%s)" % e
+    return {"gpu": torch.cuda.get_device_name(0), "nvidia_smi": q}
+
+
+def head_train_cases(B):
+    """(name, torch-module step, kernel step) of the PSP block and both uses of ``final``, forward + backward."""
+    dev = torch.device("cuda")
+    torch.manual_seed(0)
+    pre, ds, up = cnn.image_branch()
+    psp, final = ds[3][0].to(dev).train(), up[2][0].to(dev).train()
+    x = torch.relu(torch.randn(B, 512, 60, 80, device=dev)).requires_grad_(True)
+    g = torch.randn(B, 1024, 60, 80, device=dev)
+    y240 = torch.randn(B, 64, 240, 320, device=dev).requires_grad_(True)
+    y480 = torch.randn(B, 64, 480, 640, device=dev).requires_grad_(True)
+    g240, g480 = torch.randn_like(y240), torch.randn_like(y480)
+    params = list(psp.parameters()) + list(final.parameters())
+
+    def run(f):
+        def step():
+            for p in params + [x, y240, y480]:
+                p.grad = None
+            f()
+        return step
+    cases = [("psp_train", run(lambda: psp(x).backward(g)), run(lambda: psp.forward_fused(x).backward(g)))]
+    if B > 1:
+        cases += [("final240_train", run(lambda: final(y240).backward(g240)),
+                   run(lambda: final.forward_fused(y240).backward(g240))),
+                  ("final480_train", run(lambda: final(y480).backward(g480)),
+                   run(lambda: final.forward_fused(y480).backward(g480)))]
+    return cases
+
+
+def peak_extra_mb(fn):
+    """Peak memory one eager call allocates above what is allocated before it (MB)."""
+    torch.cuda.synchronize()
+    base = torch.cuda.memory_allocated()
+    torch.cuda.reset_peak_memory_stats()
+    fn()
+    torch.cuda.synchronize()
+    return round((torch.cuda.max_memory_allocated() - base) / 1e6, 1)
+
+
+@contextlib.contextmanager
+def deterministic(on):
+    saved = torch.are_deterministic_algorithms_enabled()
+    torch.use_deterministic_algorithms(on)
+    try:
+        yield
+    finally:
+        torch.use_deterministic_algorithms(saved)
+
+
+def train_arms(iters, reps, profile):
+    emit(**card(), cudnn_allow_tf32=torch.backends.cudnn.allow_tf32)
+    heads = {B: head_train_cases(B) for B in (1, 8)}
+    B = 8
+    model, inputs = network(B, 12288, True, n_classes=2)        # config 3: LineMOD-shaped, 8 frames
+    N = inputs["choose"].shape[-1]
+    item = {"labels": torch.randint(0, 2, (B, N), device="cuda", dtype=torch.int32),
+            "kp_targ_ofst": torch.randn(B, N, 8, 3, device="cuda"),
+            "ctr_targ_ofst": torch.randn(B, N, 3, device="cuda")}
+
+    def step():
+        model.zero_grad(set_to_none=True)
+        loss, _ = ffb6d_loss(model(inputs), item)
+        loss.backward()
+    settings = [("off", False, False), ("on", True, False), ("on_deterministic", True, True)]
+    for rep in range(reps):
+        for hb, cases in heads.items():
+            for name, ref, ker in cases:
+                t_ref, _ = graph_time(ref, iters)
+                t_ker, t_ker_min = graph_time(ker, iters)
+                emit(what=name, B=hb, rep=rep, torch_ms=round(t_ref, 4), kernels_ms=round(t_ker, 4),
+                     kernels_min_ms=round(t_ker_min, 4), speedup=round(t_ref / t_ker, 3),
+                     torch_peak_extra_MB=peak_extra_mb(ref), kernels_peak_extra_MB=peak_extra_mb(ker))
+        for label, flag, det in settings:
+            model.fused_image_head = flag
+            with deterministic(det):
+                step()
+                torch.cuda.synchronize()
+                torch.cuda.reset_peak_memory_stats()
+                t, tmin = eager_time(step, max(3, iters // 4))
+            emit(what="train_step_arm", fused_image_head=label, B=B, n_pts=12288, rep=rep, ms=round(t, 3),
+                 min_ms=round(tmin, 3), max_memory_allocated_GB=round(torch.cuda.max_memory_allocated() / 1e9, 3))
+    if profile:
+        from torch.profiler import ProfilerActivity, profile as prof
+        for label, flag, det in settings:
+            model.fused_image_head = flag
+            with deterministic(det):
+                step()
+                torch.cuda.synchronize()
+                with prof(activities=[ProfilerActivity.CUDA]) as p:
+                    step()
+                    torch.cuda.synchronize()
+            rows = {}
+            for e in p.key_averages():
+                if e.device_type == torch.autograd.DeviceType.CUDA or getattr(e, "self_device_time_total", 0) > 0:
+                    rows[e.key] = rows.get(e.key, 0.0) + getattr(e, "self_device_time_total", 0.0) / 1e3
+            top = sorted(rows.items(), key=lambda kv: -kv[1])[:25]
+            emit(what="train_step_profile", fused_image_head=label, total_cuda_ms=round(sum(rows.values()), 3),
+                 top_ms=[(k[:90], round(v, 3)) for k, v in top])
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--batches", default="1,8")
     ap.add_argument("--no-train", action="store_true")
+    ap.add_argument("--train-arms", action="store_true")
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--profile", action="store_true")
     a = ap.parse_args()
+    if a.train_arms:
+        train_arms(a.iters, a.reps, a.profile)
+        return
     emit(gpu=torch.cuda.get_device_name(0), cudnn_allow_tf32=torch.backends.cudnn.allow_tf32)
     for B in [int(b) for b in a.batches.split(",")]:
         head_blocks(B, a.iters)
