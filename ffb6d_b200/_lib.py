@@ -49,7 +49,6 @@ def _load():
         "ffb6d_knn_grid_build": (ci, [vp, i64, i64, ci, vp, sz, vp]),
         "ffb6d_knn_grid_query": (ci, [vp, vp, i64, i64, i64, ci, vp, ci, vp, sz, vp, sz, vp]),
         "ffb6d_knn_grid_query_organized": (ci, [vp, vp, i64, i64, i64, ci, vp, ci, vp, sz, vp, sz, i64, vp]),
-        "ffb6d_knn_subset_nn": (ci, [vp, vp, i64, i64, i64, vp, ci, vp, ci, vp, sz, vp]),
         "ffb6d_build_indices_workspace_bytes": (sz, [i64, i64, i64, i64, ci]),
         "ffb6d_build_indices": (ci, [vp, vp, vp, vp, i64, i64, i64, i64, ci, vp, ci, vp, sz, vp]),
         "ffb6d_knn_grid_tune": (None, [fp, ci]),

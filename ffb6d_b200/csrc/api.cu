@@ -58,16 +58,7 @@ const Env &env()
     static const Env e = [] {
         Env v;
         auto on = [](const char *n) { const char *x = getenv(n); return x && *x && strcmp(x, "0") != 0; };
-        v.gather_direct = on("FFB6D_GATHER_DIRECT");
         v.check_indices = on("FFB6D_CHECK_INDICES");
-        v.grid_thread_search = on("FFB6D_GRID_THREAD_SEARCH");
-        v.subset_nn = on("FFB6D_SUBSET_NN");
-        const char *x;
-        v.grid_scale = (x = getenv("FFB6D_GRID_SCALE")) ? (float)atof(x) : 1.0f;
-        v.grid_scale_k1 = (x = getenv("FFB6D_GRID_SCALE_K1")) ? (float)atof(x) : 2.5f;
-        v.grid_quantile = (x = getenv("FFB6D_GRID_QUANTILE")) ? atoi(x) : 17;
-        if (v.grid_quantile < 0) v.grid_quantile = 0;
-        if (v.grid_quantile > 31) v.grid_quantile = 31;
         return v;
     }();
     return e;
@@ -146,7 +137,7 @@ using namespace ffb6d;
 
 extern "C" {
 
-int ffb6d_version(void) { return 1; }
+int ffb6d_version(void) { return 2; }
 const char *ffb6d_last_error(void) { return g_err; }
 uint64_t ffb6d_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
@@ -230,21 +221,6 @@ int ffb6d_knn_grid_query_organized(const float *support, const float *query, int
     FFB6D_CHECK_ARG(support && query && idx_out && grid && scratch, "knn_grid_query: null pointer");
     return knn_grid_query(support, query, B, S, Q, K, idx_out, idx_is_i64, grid, grid_bytes, scratch,
                           scratch_bytes, (cudaStream_t)stream, query_width);
-}
-
-int ffb6d_knn_subset_nn(const float *support, const float *query, int64_t B, int64_t S, int64_t Q, const void *knn_idx,
-                        int K_list, void *idx_out, int idx_is_i64, void *scratch, size_t scratch_bytes,
-                        ffb6d_stream_t stream)
-{
-    FFB6D_CHECK_ARG(B >= 0 && S >= 1 && Q >= 0 && B < 65536 && S < (1ll << 31) && Q < (1ll << 31),
-                    "knn_subset_nn: bad size");
-    FFB6D_CHECK_ARG(S <= Q || Q == 0, "knn_subset_nn: the support (%lld rows) must be a row prefix of the %lld queries",
-                    (long long)S, (long long)Q);
-    FFB6D_CHECK_ARG(K_list >= 1 && K_list <= FFB6D_MAX_K, "knn_subset_nn: K_list=%d outside [1,%d]", K_list, FFB6D_MAX_K);
-    if (B == 0 || Q == 0) return FFB6D_OK;
-    FFB6D_CHECK_ARG(support && query && knn_idx && idx_out && scratch, "knn_subset_nn: null pointer");
-    return knn_subset_nn_from_knn(support, query, B, S, Q, knn_idx, K_list, idx_out, idx_is_i64, scratch, scratch_bytes,
-                                  (cudaStream_t)stream);
 }
 
 void ffb6d_knn_grid_tune(float cell_scale, int quantile) { knn_grid_tune(cell_scale, quantile); }

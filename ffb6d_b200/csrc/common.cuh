@@ -89,14 +89,9 @@ int64_t wgrad_small_splits(int64_t B, int64_t P);
 int wgrad_small_det_launch(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2, int64_t B,
                            int64_t Co, int64_t P, float *part, cudaStream_t st);
 
-// Experiment switches, read ONCE per process (never in a launch path; results never depend on them).
+// Debugging switches, read ONCE per process (never in a launch path; results never depend on them).
 struct Env {
-    bool gather_direct;     // FFB6D_GATHER_DIRECT=1: K-lane gathers through the older direct kernel
     bool check_indices;     // FFB6D_CHECK_INDICES=1: validate gather indices (synchronises; debugging aid)
-    bool grid_thread_search;
-    bool subset_nn;         // FFB6D_SUBSET_NN=1: ffb6d_build_indices reads cld_interp_idx{0,1} off the self searches (ffb6d_knn_subset_nn)
-    float grid_scale, grid_scale_k1;
-    int grid_quantile;
 };
 const Env &env();
 

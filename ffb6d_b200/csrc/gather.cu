@@ -671,7 +671,7 @@ static int launch_ncs(const float *feat, const IdxT *idx, float *out, int64_t B,
     const int64_t want = 4 * num_sms();   // CTAs to aim for
     // few queries against long rows (Q*K gathered elements << S): staging whole rows would read far
     // more than the ~5 sectors a query's K adjacent neighbours touch per row -> K-lane gather instead
-    const bool sparse_queries = (KT == 8 || KT == 16 || KT == 32) && Q * 40 < S && !env().gather_direct;
+    const bool sparse_queries = (KT == 8 || KT == 16 || KT == 32) && Q * 40 < S;
     if (row_bytes <= budget && !sparse_queries) {
         int CC = (int)(budget / row_bytes);
         if (CC > C) CC = (int)C;
@@ -711,12 +711,10 @@ static int launch_ncs(const float *feat, const IdxT *idx, float *out, int64_t B,
         dim3 grid((unsigned)ceil_div(Q, 256), (unsigned)std::min<int64_t>(ceil_div(C, G1_CH), 65535), (unsigned)B);
         gather1_ncs_direct_kernel<IdxT><<<grid, 256, 0, st>>>(feat, idx, out, (int)C, (int)S, (int)Q);
         FFB6D_LAUNCH_OK("gather1_ncs_direct_kernel");
-    } else if ((KT == 8 || KT == 16 || KT == 32) && !env().gather_direct) {
-        if constexpr (KT == 8 || KT == 16 || KT == 32) {
-            dim3 grid((unsigned)ceil_div(Q, 256 / KT), (unsigned)ceil_div(C, KLANE_CH), (unsigned)B);
-            gather_max_ncs_klane_kernel<IdxT, KT><<<grid, 256, 0, st>>>(feat, idx, out, (int)C, (int)S, (int)Q);
-            FFB6D_LAUNCH_OK("gather_max_ncs_klane_kernel");
-        }
+    } else if constexpr (KT == 8 || KT == 16 || KT == 32) {
+        dim3 grid((unsigned)ceil_div(Q, 256 / KT), (unsigned)ceil_div(C, KLANE_CH), (unsigned)B);
+        gather_max_ncs_klane_kernel<IdxT, KT><<<grid, 256, 0, st>>>(feat, idx, out, (int)C, (int)S, (int)Q);
+        FFB6D_LAUNCH_OK("gather_max_ncs_klane_kernel");
     } else {
         const int CC = 8;
         dim3 grid((unsigned)ceil_div(Q, 256), (unsigned)ceil_div(C, CC), (unsigned)B);
@@ -763,9 +761,9 @@ const char *ffb6d_gather_kernel_name(int64_t B, int64_t C, int64_t S, int64_t Q,
     const bool fits = (size_t)S * sizeof(float) <= budget;
     if (K == 1) return fits ? ((Q % 4 == 0) ? "gather1_ncs_staged_v4_kernel" : "gather_max_ncs_staged_kernel")
                             : "gather1_ncs_direct_kernel";
-    const bool sparse_queries = (K == 8 || K == 16 || K == 32) && Q * 40 < S && !env().gather_direct;
+    const bool sparse_queries = (K == 8 || K == 16 || K == 32) && Q * 40 < S;
     if (fits && !sparse_queries) return "gather_max_ncs_staged_kernel";
-    if ((K == 8 || K == 16 || K == 32) && !env().gather_direct) return "gather_max_ncs_klane_kernel";
+    if (K == 8 || K == 16 || K == 32) return "gather_max_ncs_klane_kernel";
     return "gather_max_ncs_direct_kernel";
 }
 

@@ -96,9 +96,4 @@ int knn_grid_query(const float *support, const float *query, int64_t B, int64_t 
                    void *idx_out, int idx_is_i64, const void *grid_mem, size_t grid_bytes,
                    void *scratch, size_t scratch_bytes, cudaStream_t st, int64_t query_width = 0);
 
-// nearest point of the row-prefix subset `support` = query[:, :S] for every query, read off the exact K-neighbour self
-// search `knn` [B,Q,KL] of `query`; rows without a subset member fall back to a full scan (knn_grid.cu, section H)
-int knn_subset_nn_from_knn(const float *support, const float *query, int64_t B, int64_t S, int64_t Q, const void *knn,
-                           int KL, void *idx_out, int idx_is_i64, void *scratch, size_t scratch_bytes, cudaStream_t st);
-
 }  // namespace ffb6d

@@ -1440,111 +1440,32 @@ grid_dup_copy_kernel(int Q, int K, const QueryState *__restrict__ state_all,
     }
 }
 
-// ------------------------------------------------------------------ H. nearest point of a row-PREFIX subset, read off a self search
-// The schedule asks, per cloud level i, for the nearest level-(i+1) point of every level-i point (cld_interp_idx{i},
-// ycb_dataset.py:280-282).  Level i+1 is the first N_{i+1} rows of level i (:278) and the K-neighbour self search of
-// level i (cld_nei_idx{i}) has just been computed: its rows are sorted by the total order (distance, index) over ALL
-// level-i points, so the first entry of a row with index < N_{i+1} IS the nearest subset point under the same total
-// order -- every subset point that is not in the row sorts after the row's last entry.  Only rows without such an
-// entry (0.75^16 = 1 % of the queries when the subset is a random quarter) need a search: they go to the full-scan
-// pass (one CTA per query).  No grid is needed.
-template <typename IdxT>
-__global__ void __launch_bounds__(256)
-subset_nn_from_knn_kernel(const IdxT *__restrict__ knn, int Q, int KL, int S, IdxT *__restrict__ idx_out,
-                          QueryState *state_all, int *__restrict__ ovf_all)
-{
-    const int b = blockIdx.y;
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= Q) return;
-    const IdxT *row = knn + ((size_t)b * Q + q) * KL;
-    const int kl = min(KL, Q);   // a level smaller than KL leaves (+inf, 0) fillers behind its Q real entries
-    for (int j = 0; j < kl; ++j) {
-        const IdxT v = __ldg(row + j);
-        if (v >= 0 && v < (IdxT)S) {
-            idx_out[(size_t)b * Q + q] = v;
-            return;
-        }
-    }
-    auto g = cooperative_groups::coalesced_threads();
-    int base = 0;
-    if (g.thread_rank() == 0) base = atomicAdd(&state_all[b].ovf_count, (int)g.size());
-    ovf_all[(size_t)b * Q + g.shfl(base, 0) + (int)g.thread_rank()] = q;
-}
-
-// support = the first S rows of `query` in every batch item ([B,S,3] contiguous copy), knn = the exact K-neighbour
-// self search of `query` ([B,Q,KL], rows sorted by (distance, index)); idx_out [B,Q,1]
-int knn_subset_nn_from_knn(const float *support, const float *query, int64_t B, int64_t S, int64_t Q, const void *knn,
-                           int KL, void *idx_out, int idx_is_i64, void *scratch, size_t scratch_bytes, cudaStream_t st)
-{
-    QueryScratch qs = carve_query(scratch, B, Q);
-    if (!scratch || scratch_bytes < qs.bytes) {
-        set_error("knn subset search: %zu bytes of scratch required, %zu given", qs.bytes, scratch_bytes);
-        return FFB6D_ERR_WORKSPACE;
-    }
-    FFB6D_CUDA(cudaMemsetAsync(qs.state, 0, (size_t)B * sizeof(QueryState), st));
-    dim3 grid((unsigned)ceil_div(Q, 256), (unsigned)B);
-    const int64_t per_item = std::max<int64_t>(1, 4 * num_sms() / B);
-    dim3 ogrid((unsigned)std::min<int64_t>(Q, per_item), (unsigned)B);
-    if (idx_is_i64) {
-        subset_nn_from_knn_kernel<long long><<<grid, 256, 0, st>>>((const long long *)knn, (int)Q, KL, (int)S,
-                                                                   (long long *)idx_out, qs.state, qs.ovf);
-        FFB6D_LAUNCH_OK("subset_nn_from_knn_kernel");
-        grid_overflow_warp_kernel<long long><<<ogrid, 256, 0, st>>>(support, query, (int)S, (int)Q, 1, qs.state, qs.ovf,
-                                                                    (long long *)idx_out);
-    } else {
-        subset_nn_from_knn_kernel<int><<<grid, 256, 0, st>>>((const int *)knn, (int)Q, KL, (int)S, (int *)idx_out, qs.state,
-                                                             qs.ovf);
-        FFB6D_LAUNCH_OK("subset_nn_from_knn_kernel");
-        grid_overflow_warp_kernel<int><<<ogrid, 256, 0, st>>>(support, query, (int)S, (int)Q, 1, qs.state, qs.ovf,
-                                                              (int *)idx_out);
-    }
-    FFB6D_LAUNCH_OK("grid_overflow_warp_kernel");
-    return FFB6D_OK;
-}
-
 // ------------------------------------------------------------------ host
-// cell-size knobs: defaults from the environment (read once, common.cuh Env), overridable by
-// ffb6d_knn_grid_tune* (tools/tune_grid.py); results never depend on them
-static bool g_force_thread_search = false;
+// cell-size knobs, overridable by ffb6d_knn_grid_tune* (tools/tune_grid.py); results never depend on them
 static float g_cell_scale = 1.0f;
 static float g_cell_scale_k1 = 2.5f;   // grids built for K = 1 searches (measured optimum 2 ... 2.8)
 static int g_quantile = 17;
-static std::atomic<bool> g_env_read{false};
-
-static void read_env()
-{
-    if (g_env_read.load(std::memory_order_acquire)) return;
-    const Env &e = env();
-    if (e.grid_scale > 0.f) g_cell_scale = e.grid_scale;
-    if (e.grid_scale_k1 > 0.f) g_cell_scale_k1 = e.grid_scale_k1;
-    g_force_thread_search = e.grid_thread_search;
-    g_quantile = e.grid_quantile;
-    g_env_read.store(true, std::memory_order_release);
-}
 
 void knn_grid_tune(float cell_scale, int quantile)
 {
-    read_env();
     if (cell_scale > 0.f) g_cell_scale = cell_scale;
     if (quantile >= 0) g_quantile = std::min(31, quantile);
 }
 
 void knn_grid_tune_k1(float cell_scale_k1)
 {
-    read_env();
     if (cell_scale_k1 > 0.f) g_cell_scale_k1 = cell_scale_k1;
 }
 
-template <int KCAP, typename IdxT>
+template <typename IdxT>
 static int launch_search(const float *support, const float *query, int64_t B, int64_t S, int64_t Q,
                          int K, void *idx_out, const GridStore &w, const QueryScratch &qs, int64_t query_width,
                          cudaStream_t st)
 {
     const bool self = (support == query) && (S == Q);
-    const bool warp = K >= 2 && K <= 32 && !g_force_thread_search;
+    const bool warp = K >= 2 && K <= 32;
     FFB6D_CUDA(cudaMemsetAsync(qs.state, 0, (size_t)B * sizeof(QueryState), st));
-    const bool organised = K == 1 && !self && query_width >= 8 && Q % query_width == 0 && Q / query_width >= 4 &&
-                           !g_force_thread_search;
+    const bool organised = K == 1 && !self && query_width >= 8 && Q % query_width == 0 && Q / query_width >= 4;
     bool far_sentinels = false;
     if (organised) {   // queries are an image: one warp per 8x4 pixel tile
         const int64_t tiles_x = ceil_div(query_width, 8), tiles = tiles_x * ceil_div(Q / query_width, 4);
@@ -1568,14 +1489,12 @@ static int launch_search(const float *support, const float *query, int64_t B, in
         else
             grid_search_warp_kernel<IdxT, false><<<wgrid, 256, 0, st>>>(
                 query, (int)S, (int)Q, K, w.params, w.cursor, w.maxc, w.sorted, (IdxT *)idx_out, qs.state, qs.ovf);
-    } else {
+    } else {   // one thread per query: unorganised K = 1 queries and K > 32
         dim3 grid((unsigned)ceil_div(Q, 128), (unsigned)B);
-        if (self)
-            grid_search_kernel<KCAP, IdxT, true><<<grid, 128, 0, st>>>(
-                query, (int)S, (int)Q, K, w.params, w.cursor, w.maxc, w.sorted, (IdxT *)idx_out, qs.state, qs.ovf);
-        else
-            grid_search_kernel<KCAP, IdxT, false><<<grid, 128, 0, st>>>(
-                query, (int)S, (int)Q, K, w.params, w.cursor, w.maxc, w.sorted, (IdxT *)idx_out, qs.state, qs.ovf);
+        const auto kernel = K == 1 ? (self ? grid_search_kernel<1, IdxT, true> : grid_search_kernel<1, IdxT, false>)
+                                   : (self ? grid_search_kernel<64, IdxT, true> : grid_search_kernel<64, IdxT, false>);
+        kernel<<<grid, 128, 0, st>>>(query, (int)S, (int)Q, K, w.params, w.cursor, w.maxc, w.sorted, (IdxT *)idx_out,
+                                     qs.state, qs.ovf);
     }
     FFB6D_LAUNCH_OK("grid_search_kernel");
     const int64_t per_item = std::max<int64_t>(1, 4 * num_sms() / B);
@@ -1589,10 +1508,10 @@ static int launch_search(const float *support, const float *query, int64_t B, in
             grid_far_fill_kernel<IdxT><<<fgrid, 256, 0, st>>>((int)Q, qs.state, (IdxT *)idx_out);
             FFB6D_LAUNCH_OK("grid_far_fill_kernel");
         }
-    } else {
-        constexpr int OT = (KCAP >= 32) ? 64 : 128;
+    } else {   // K > 32
+        constexpr int OT = 64;
         dim3 ogrid((unsigned)std::min<int64_t>(ceil_div(Q, OT), per_item), (unsigned)B);
-        grid_overflow_kernel<KCAP, OT, 1024, IdxT><<<ogrid, OT, 0, st>>>(
+        grid_overflow_kernel<64, OT, 1024, IdxT><<<ogrid, OT, 0, st>>>(
             support, query, (int)S, (int)Q, K, qs.state, qs.ovf, (IdxT *)idx_out);
         FFB6D_LAUNCH_OK("grid_overflow_kernel");
         dim3 dgrid((unsigned)std::min<int64_t>(ceil_div(Q * K, 256), per_item), (unsigned)B);
@@ -1602,24 +1521,10 @@ static int launch_search(const float *support, const float *query, int64_t B, in
     return FFB6D_OK;
 }
 
-template <typename IdxT>
-static int launch_search_k(const float *support, const float *query, int64_t B, int64_t S, int64_t Q,
-                           int K, void *idx_out, const GridStore &w, const QueryScratch &qs, int64_t query_width,
-                           cudaStream_t st)
-{
-    if (K == 1) return launch_search<1, IdxT>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
-    if (K <= 4) return launch_search<4, IdxT>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
-    if (K <= 8) return launch_search<8, IdxT>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
-    if (K <= 16) return launch_search<16, IdxT>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
-    if (K <= 32) return launch_search<32, IdxT>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
-    return launch_search<64, IdxT>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
-}
-
 // Build the grid of `support` for searches of about K neighbours (K only tunes the cell size).
 int knn_grid_build(const float *support, int64_t B, int64_t S, int K, void *grid_mem,
                    size_t grid_bytes, cudaStream_t st)
 {
-    read_env();
     GridStore w = carve_grid(grid_mem, B, S);
     if (!grid_mem || grid_bytes < w.bytes) {
         set_error("knn grid build: %zu bytes of grid storage required, %zu given", w.bytes, grid_bytes);
@@ -1638,7 +1543,6 @@ int knn_grid_query(const float *support, const float *query, int64_t B, int64_t 
                    void *idx_out, int idx_is_i64, const void *grid_mem, size_t grid_bytes,
                    void *scratch, size_t scratch_bytes, cudaStream_t st, int64_t query_width)
 {
-    read_env();
     GridStore w = carve_grid(const_cast<void *>(grid_mem), B, S);
     QueryScratch qs = carve_query(scratch, B, Q);
     if (!grid_mem || grid_bytes < w.bytes || !scratch || scratch_bytes < qs.bytes) {
@@ -1646,8 +1550,8 @@ int knn_grid_query(const float *support, const float *query, int64_t B, int64_t 
                   scratch_bytes, qs.bytes);
         return FFB6D_ERR_WORKSPACE;
     }
-    if (idx_is_i64) return launch_search_k<long long>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
-    return launch_search_k<int>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
+    if (idx_is_i64) return launch_search<long long>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
+    return launch_search<int>(support, query, B, S, Q, K, idx_out, w, qs, query_width, st);
 }
 
 int knn_grid_launch(const float *support, const float *query, int64_t B, int64_t S, int64_t Q, int K,

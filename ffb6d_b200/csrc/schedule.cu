@@ -200,15 +200,7 @@ extern "C" int ffb6d_build_indices(const float *cld, const float *img2, const fl
             const int64_t Q = size_of(z, d.qry_kind, d.qry_id);
             const float *qry = set_ptr(d.qry_kind, d.qry_id);
             int rc;
-            // FFB6D_SUBSET_NN=1 (off by default, like in the Python scheduler): cld_interp_idx{i} (call 4i+1: nearest
-            // level-(i+1) point of every level-i point) is read off cld_nei_idx{i} (call 4i, finished above on this
-            // stream): level i+1 is a row prefix of level i (knn_grid.cu, section H)
-            const bool from_self = env().subset_nn && d.K == 1 && K >= 8 && d.sup_kind == 0 && d.qry_kind == 0 && d.sup_id == d.qry_id + 1 &&
-                                   j == 4 * d.qry_id + 1 && done[4 * d.qry_id] && knn_grid_workspace_bytes(B, S, Q, 1) > 0;
-            if (from_self)
-                rc = knn_subset_nn_from_knn(sup, qry, B, S, Q, out[4 * d.qry_id], K, out[j], idx_is_i64, scratch,
-                                            knn_grid_query_bytes(B, Q), st);
-            else if (use_grid)
+            if (use_grid)
                 rc = knn_grid_query(sup, qry, B, S, Q, d.K, out[j], idx_is_i64, grid, knn_grid_store_bytes(B, S), scratch,
                                     knn_grid_query_bytes(B, Q), st, d.qry_kind == 1 ? W / d.qry_id : 0);
             else

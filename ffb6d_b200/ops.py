@@ -169,34 +169,6 @@ def knn_uses_grid(B, S, Q, k):
     return int(lib.ffb6d_knn_workspace_bytes(B, S, Q, int(k))) > 0
 
 
-def subset_nn_from_knn(support, query_pts, knn_idx):
-    """``cld_interp_idx{i}`` read off ``cld_nei_idx{i}`` (``ffb6d_knn_subset_nn``): the nearest point of ``support``
-    for every query, when ``support [B,S,3]`` is the first S rows of ``query_pts [B,Q,3]`` (cloud level i+1 is a row
-    prefix of level i, datasets/ycb/ycb_dataset.py:278) and ``knn_idx [B,Q,K]`` is the K-neighbour self search of
-    ``query_pts`` (:275-277).  The first entry of a row that is < S is the answer (rows are ordered by (distance,
-    index) over all of ``query_pts``); the ~0.75**K of the rows without one get a full scan.  Returns ``[B,Q,1]`` in
-    the dtype of ``knn_idx``; identical to ``knn_search(support, query_pts, 1)``."""
-    _need_cuda(support, "support")
-    _need_cuda(query_pts, "query_pts")
-    _need_cuda(knn_idx, "knn_idx")
-    sup, qry = support.contiguous().float(), query_pts.contiguous().float()
-    if sup.dim() != 3 or qry.dim() != 3 or sup.shape[2] != 3 or qry.shape[2] != 3 or sup.shape[0] != qry.shape[0]:
-        raise ValueError("expected support [B,S,3] and query [B,Q,3]")
-    B, S, Q = sup.shape[0], sup.shape[1], qry.shape[1]
-    if knn_idx.dim() != 3 or knn_idx.shape[0] != B or knn_idx.shape[1] != Q or knn_idx.dtype not in _IDX:
-        raise ValueError("knn_idx must be an int32 / int64 [B,Q,K] tensor, got %s %s" % (tuple(knn_idx.shape), knn_idx.dtype))
-    if S < 1 or S > Q:
-        raise ValueError("the support (%d rows) must be a non-empty row prefix of the %d queries" % (S, Q))
-    knn = knn_idx.contiguous()
-    out = torch.empty((B, Q, 1), dtype=knn.dtype, device=sup.device)
-    with torch.cuda.device(sup.device):
-        sb = int(lib.ffb6d_knn_grid_query_bytes(B, Q))
-        scratch = torch.empty(max(sb, 1), dtype=torch.uint8, device=sup.device)
-        check(lib.ffb6d_knn_subset_nn(sup.data_ptr(), qry.data_ptr(), B, S, Q, knn.data_ptr(), int(knn.shape[2]),
-                                      out.data_ptr(), int(knn.dtype == torch.int64), scratch.data_ptr(), sb, _stream(sup.device)))
-    return out
-
-
 # --------------------------------------------------------------------------- gather + max
 def _layout_of(f3):
     """f3: [B,C,S] view.  Returns (tensor, layout) with tensor dense in that layout."""

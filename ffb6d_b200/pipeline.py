@@ -29,20 +29,11 @@ class FusionPass:
         self.device = torch.device(device)
         self.layout = layout
         self.index_dtype = index_dtype
-        import os
-        # FFB6D_STREAM_PRIO="s,g": CUDA priorities of the search / gather streams (experiment switch; lower = higher)
-        prio = [int(x) for x in os.environ.get("FFB6D_STREAM_PRIO", "0,0").split(",")]
-        self.streams = ([torch.cuda.Stream(device=self.device, priority=prio[0]) for _ in range(n_streams)]
-                        if n_streams > 1 else None)
+        self.streams = [torch.cuda.Stream(device=self.device) for _ in range(n_streams)] if n_streams > 1 else None
         # the gathers (HBM bound) get streams of their own: each waits only for its index tensor, so
         # it overlaps the searches (issue bound) that are still running
-        self.gstreams = ([torch.cuda.Stream(device=self.device, priority=prio[1])
-                          for _ in range(n_gather_streams or n_streams)] if n_streams > 1 else None)
-        # grid builds: latency-bound cluster kernels, spread over streams of their own (FFB6D_BUILD_STREAMS, default 0 = share the search streams)
-        nb = int(os.environ.get("FFB6D_BUILD_STREAMS", "0"))
-        bp = int(os.environ.get("FFB6D_BUILD_PRIO", "0"))
-        self.bstreams = ([torch.cuda.Stream(device=self.device, priority=bp) for _ in range(nb)]
-                         if (n_streams > 1 and nb > 0) else [])
+        self.gstreams = ([torch.cuda.Stream(device=self.device) for _ in range(n_gather_streams or n_streams)]
+                         if n_streams > 1 else None)
         self.gathers = S.gather_schedule(n_points, h, w)
         g = torch.Generator(device=self.device).manual_seed(seed)
         self.features = []
@@ -55,24 +46,18 @@ class FusionPass:
             self.features.append(f)
         # issue order of the searches: bytes of the gathers a search unlocks per unit of search work
         # (measured: a K = 16 query costs about 12 K = 1 queries)
-        import os
         unlocked = {}
         derived = S.derived_searches(S.knn_schedule(n_points, h, w, k))   # row slices of another search
         derived.update({c: p_ for c, (p_, f_) in S.derived_image_searches(S.knn_schedule(n_points, h, w, k), h, w).items()})
-        if k >= 8 and os.environ.get("FFB6D_SUBSET_NN", "0") == "1":   # cld_interp_idx{i} is read off cld_nei_idx{i} (schedule.py)
-            derived.update(S.derived_subset_searches(S.knn_schedule(n_points, h, w, k)))
         for op, key, C, Sz, Q, K in self.gathers:
             src = key.replace("cld_sub_idx", "cld_nei_idx")
             src = derived.get(src, src)
             unlocked[src] = unlocked.get(src, 0) + S.gather_alg_bytes(C, Sz, Q, K)
-        self.priority = None
-        if os.environ.get("FFB6D_SCHED", "unlock") == "unlock":   # "size": largest search first (3.63 vs 3.59 ms)
-            self.priority = {key: unlocked.get(key, 0) / float(S.set_size(q, n_points, h, w) * (12 if kk > 1 else 1))
-                             for key, s_, q, kk in S.knn_schedule(n_points, h, w, k)}
+        self.priority = {key: unlocked.get(key, 0) / float(S.set_size(q, n_points, h, w) * (12 if kk > 1 else 1))
+                         for key, s_, q, kk in S.knn_schedule(n_points, h, w, k)}
         # ... except the level-0 self search, the longest search of the pass: it needs only the level-0 grid, so it goes
         # first and the big p2r searches queue behind it (measured three times: -0.2 ... -0.6 % of the pass)
-        if self.priority is not None and os.environ.get("FFB6D_SELF_FIRST", "1") != "0":
-            self.priority["cld_nei_idx0"] = float("inf")
+        self.priority["cld_nei_idx0"] = float("inf")
         kb, gb = S.frame_alg_bytes(n_points, h, w, k)
         self.alg_bytes_per_frame = kb + gb
         self.knn_alg_bytes_per_frame = kb
@@ -81,8 +66,7 @@ class FusionPass:
     # -- the two halves of a pass ------------------------------------------------------
     def build_indices(self, cld, dpt_xyz, choose, timer=None, events=None):
         inputs = S.build_ffb6d_indices(cld, dpt_xyz, k=self.k, index_dtype=self.index_dtype,
-                                       timer=timer, streams=self.streams, events=events, priority=self.priority,
-                                       build_streams=self.bstreams)
+                                       timer=timer, streams=self.streams, events=events, priority=self.priority)
         inputs["choose"] = choose
         return inputs
 
@@ -136,7 +120,7 @@ class FusionPass:
                 # tell the caching allocator (inside a capture the graph's private pool keeps them alive)
                 inputs[key].record_stream(st)
                 outs[i].record_stream(main)
-        for st in (self.streams + self.gstreams + self.bstreams) if events is not None else gs:
+        for st in (self.streams + self.gstreams) if events is not None else gs:
             main.wait_stream(st)
         if events is not None:
             events.pop("_keepalive", None)   # every search has been joined: the grids may go
@@ -193,8 +177,7 @@ class FusionPass:
         cld, pyr = ops.backproject(depth, intr, choose)
         events = {} if self.streams is not None else None
         inputs = S.build_ffb6d_indices(cld, None, k=self.k, index_dtype=self.index_dtype, streams=self.streams,
-                                       pyramid=pyr, image_hw=(self.h, self.w), events=events, priority=self.priority,
-                                       build_streams=self.bstreams)
+                                       pyramid=pyr, image_hw=(self.h, self.w), events=events, priority=self.priority)
         inputs["choose"] = choose
         return inputs, self.run_gathers(inputs, events=events)
 

@@ -8,16 +8,14 @@ runs the index build on the GPU for a whole batch: xyz goes in, the same dict
 keys with the same shapes and dtypes (int32) come out, already on the device.
 """
 import contextlib
-import os
 
 import torch
 
-from .ops import knn_search, KnnGrid, knn_uses_grid, subset_nn_from_knn
+from .ops import knn_search, KnnGrid, knn_uses_grid
 
 from .tables import (RGB_DS_SR, RGB_UP_SR, PCLD_SUB_S_R, N_DS_LAYERS, N_UP_LAYERS, K_NEIGH,  # noqa: F401
                      DS_RGB_OC, DS_RNDLA_OC, UP_RGB_OC, UP_RNDLA_OC, knn_schedule, set_size, gather_schedule,
-                     fusion_mlp_schedule, knn_alg_bytes, gather_alg_bytes, frame_alg_bytes, derived_searches, derived_image_searches,
-                     derived_subset_searches)
+                     fusion_mlp_schedule, knn_alg_bytes, gather_alg_bytes, frame_alg_bytes, derived_searches, derived_image_searches)
 
 
 def image_pyramid(dpt_xyz, levels=(1, 2, 4, 8)):
@@ -32,7 +30,7 @@ def image_pyramid(dpt_xyz, levels=(1, 2, 4, 8)):
 
 
 def build_ffb6d_indices(cld, dpt_xyz=None, k=K_NEIGH, index_dtype=torch.int32, timer=None, streams=None,
-                        pyramid=None, image_hw=None, events=None, priority=None, build_streams=None):
+                        pyramid=None, image_hw=None, events=None, priority=None):
     """All neighbour-index tensors of the FFB6D fusion stack for a batch, on the GPU.
 
     :param cld: ``[B, N0, 3]`` float32 CUDA, the sampled (already shuffled) cloud
@@ -40,8 +38,6 @@ def build_ffb6d_indices(cld, dpt_xyz=None, k=K_NEIGH, index_dtype=torch.int32, t
       pass ``pyramid={2: [B,HW/4,3], 4: ..., 8: ...}`` + ``image_hw=(H, W)`` (what
       :func:`ffb6d_b200.ops.backproject` returns) and leave it None
     :param streams: optional list of side ``torch.cuda.Stream`` s to overlap the 22 searches on
-    :param build_streams: optional extra side streams for the grid builds (latency-bound cluster kernels that
-      co-run well); the caller joins them together with ``streams``
     :param priority: optional ``{index key: float}``; with ``streams`` the searches (and the grid
       builds they need) are issued in descending priority instead of descending size, so that the
       searches whose consumers are expensive finish first
@@ -89,35 +85,24 @@ def build_ffb6d_indices(cld, dpt_xyz=None, k=K_NEIGH, index_dtype=torch.int32, t
     groups = {}
     for key, s, q, kk in calls:
         groups.setdefault((s, kk), []).append((key, q))
-    # FFB6D_SUBSET_NN=1 (off by default: exact, but the pass is slower with it, DESIGN.md section 4.1): cld_interp_idx{i}
-    # (nearest level-(i+1) point of every level-i point) is read off cld_nei_idx{i} -- level i+1 is a row prefix of
-    # level i, so the first entry of a self-search row that is < N_{i+1} is the answer; only the rows without one
-    # (0.75^K of them) are searched (ops.subset_nn_from_knn).  Applies where the search would take the grid.
-    derived_sub = {c: p_ for c, p_ in derived_subset_searches(calls).items()
-                   if k >= 8 and os.environ.get("FFB6D_SUBSET_NN", "0") == "1"}
-    derived_sub = {c: p_ for c, p_ in derived_sub.items()
-                   if any(key == c and knn_uses_grid(B, sets[s].shape[1], sets[q].shape[1], kk) for key, s, q, kk in calls)}
     gridded = [g for g, members in groups.items()
-               if any(knn_uses_grid(B, sets[g[0]].shape[1], sets[q].shape[1], g[1]) for key_, q in members
-                      if key_ not in derived_sub)]
+               if any(knn_uses_grid(B, sets[g[0]].shape[1], sets[q].shape[1], g[1]) for key_, q in members)]
     grids = {}
     main = torch.cuda.current_stream(cld.device)
     par = streams is not None and timer is None
-    bstreams = list(build_streams) if (build_streams and par) else []
 
     def fork():
         if par:
-            for st in streams + bstreams:
+            for st in streams:
                 st.wait_stream(main)
 
     def join():
         if par:
-            for st in streams + bstreams:
+            for st in streams:
                 main.wait_stream(st)
 
-    def on(i, pool=None):
-        pool = pool or streams
-        return torch.cuda.stream(pool[i % len(pool)]) if par else contextlib.nullcontext()
+    def on(i):
+        return torch.cuda.stream(streams[i % len(streams)]) if par else contextlib.nullcontext()
 
     # Cloud level j is the first N_j rows of the shuffled cloud (ycb_dataset.py:278), so two searches of the same
     # support with the same K whose query sets are cloud levels answer the same questions on a prefix: the
@@ -150,7 +135,7 @@ def build_ffb6d_indices(cld, dpt_xyz=None, k=K_NEIGH, index_dtype=torch.int32, t
         order = sorted(calls, key=lambda c: -(sets[c[2]].shape[1] * c[3])) if par else calls
         build_order = sorted(gridded, key=lambda g: -sets[g[0]].shape[1])
     for i, g in enumerate(build_order):
-        with on(i, bstreams or None):
+        with on(i):
             if timer is not None:
                 timer.start("knn_build:%s%d:k%d" % (g[0][0], g[0][1], g[1]), 0)
             grids[g] = KnnGrid(sets[g[0]], g[1])
@@ -159,7 +144,7 @@ def build_ffb6d_indices(cld, dpt_xyz=None, k=K_NEIGH, index_dtype=torch.int32, t
             if par:
                 built[g] = torch.cuda.Event()
                 built[g].record()
-    order = [c for c in order if c[0] not in derived and c[0] not in derived_img and c[0] not in derived_sub]
+    order = [c for c in order if c[0] not in derived and c[0] not in derived_img]
     qsize = {key: sets[q].shape[1] for key, s, q, kk in calls}
     for i, (key, s, q, kk) in enumerate(order):
         sup, qry = sets[s], sets[q]
@@ -182,15 +167,6 @@ def build_ffb6d_indices(cld, dpt_xyz=None, k=K_NEIGH, index_dtype=torch.int32, t
                 n_sub = sets[("cld", lvl + 1)].shape[1]
                 inputs["cld_sub_idx%d" % lvl] = inputs[key][:, :n_sub, :].contiguous()
                 done.append("cld_sub_idx%d" % lvl)
-                child = "cld_interp_idx%d" % lvl
-                if derived_sub.get(child) == key:
-                    sub = sets[("cld", lvl + 1)]
-                    if timer is not None:
-                        timer.start("knn:" + child, knn_alg_bytes(sub.shape[1], qry.shape[1], 1) * B)
-                    inputs[child] = subset_nn_from_knn(sub, qry, inputs[key])
-                    if timer is not None:
-                        timer.stop()
-                    done.append(child)
             for child in children.get(key, ()):   # prefix slices instead of separate searches (see above)
                 inputs[child] = inputs[key][:, :qsize[child], :].contiguous()
                 done.append(child)

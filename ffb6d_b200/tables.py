@@ -60,19 +60,6 @@ def derived_searches(calls):
     return derived
 
 
-def derived_subset_searches(calls):
-    """``{child key: parent key}``: K = 1 searches of a cloud level into the NEXT level that can be read off the level's
-    K-neighbour self search: ``cld_interp_idx{i}`` (support cld_{i+1} = the first rows of cld_i, queries cld_i) from
-    ``cld_nei_idx{i}`` -- the first entry of a row that belongs to the prefix is the nearest prefix point
-    (:func:`ffb6d_b200.ops.subset_nn_from_knn`; rows without one are searched)."""
-    selfs = {q: key for key, s, q, kk in calls if s == q and s[0] == "cld" and kk > 1}
-    derived = {}
-    for key, s, q, kk in calls:
-        if kk == 1 and s[0] == "cld" and q[0] == "cld" and s[1] == q[1] + 1 and q in selfs:
-            derived[key] = selfs[q]
-    return derived
-
-
 def derived_image_searches(calls, h=480, w=640):
     """``{child key: (parent key, f)}``: searches whose QUERIES are an image level that is a strided subset of a
     finer level searched against the same support with the same K.  The stride-``sr`` pyramid level is

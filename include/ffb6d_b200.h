@@ -123,19 +123,6 @@ int ffb6d_knn_grid_query_organized(const float *support, const float *query,
                                    int64_t query_width, ffb6d_stream_t stream);
 
 /*
- * cld_interp_idx{i} (datasets/ycb/ycb_dataset.py:280-282: the nearest level-(i+1) point of every level-i point) read
- * off cld_nei_idx{i} (:275-277) instead of searched.  `query` [B,Q,3] is a cloud level, `support` [B,S,3] its first S
- * rows (the next level, :278), `knn_idx` [B,Q,K_list] the K-neighbour self search of `query` (rows ordered by
- * (distance, index), what ffb6d_knn_batch / ffb6d_knn_grid_query produce, same index dtype as idx_out).  The first
- * entry of a row that is < S is the nearest subset point under the same total order; rows without one are answered
- * by a full scan of the support.  idx_out [B,Q,1]; scratch: ffb6d_knn_grid_query_bytes(B, Q).  Results are identical
- * to ffb6d_knn_batch(support, query, ..., K = 1).
- */
-int ffb6d_knn_subset_nn(const float *support, const float *query, int64_t B, int64_t S, int64_t Q,
-                        const void *knn_idx, int K_list, void *idx_out, int idx_is_i64,
-                        void *scratch, size_t scratch_bytes, ffb6d_stream_t stream);
-
-/*
  * The whole index build of a batch in one call: the 22 searches of datasets/ycb/ycb_dataset.py:269-309
  * (== datasets/linemod/linemod_dataset.py:313-353) on `stream`, one grid per (support set, K class).
  *   cld  [B,N0,3]: the sampled, shuffled clouds; level i of the pyramid = the first N0/4^i rows (:278)

@@ -72,25 +72,6 @@ def knn_search(support_pts, query_pts, k):
     return knn_batch(support_pts, query_pts, k).astype(np.int32)
 
 
-def subset_nn_from_knn(knn_idx, n_sub, support, query):
-    """What ``ffb6d_knn_subset_nn`` must return, stated on the reference's own data flow: ``cld_interp_idx`` =
-    ``knn_search(sub_pts, cld, 1)`` with ``sub_pts = cld[:N//4]`` (datasets/ycb/ycb_dataset.py:278-282), given
-    ``knn_idx = knn_search(cld, cld, K)`` (:275-277, one frame, ``[Q,K]``): the first entry of a row that lies in the
-    prefix ``[0, n_sub)``, a K = 1 search of the prefix for the rows that have none.  Returns ``([Q,1], #searched)``."""
-    knn_idx = np.asarray(knn_idx)
-    out = np.empty((len(knn_idx), 1), knn_idx.dtype)
-    missed = []
-    for q, row in enumerate(knn_idx):
-        hit = row[row < n_sub]
-        if len(hit):
-            out[q, 0] = hit[0]
-        else:
-            missed.append(q)
-    if missed:
-        out[missed] = knn_search(np.asarray(support)[None], np.asarray(query)[missed][None], 1)[0]
-    return out, len(missed)
-
-
 def sqdist_of_indices(support, query, idx):
     """Reference-arithmetic squared distances of given neighbour indices [B,Q,K] (-1 when an
     index is out of range)."""

@@ -34,7 +34,7 @@ def test_header_symbols_exported():
 
 
 def test_version_and_error_text():
-    assert _lib.lib.ffb6d_version() == 1
+    assert _lib.lib.ffb6d_version() == 2
     assert isinstance(_lib.last_error(), str)
 
 

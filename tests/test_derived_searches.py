@@ -1,8 +1,8 @@
 """CPU: the searches the scheduler does not run are exactly slices of searches it does run.
 
-``tables.derived_searches`` (row prefixes: cloud level j = first rows of level i < j),
+``tables.derived_searches`` (row prefixes: cloud level j = first rows of level i < j) and
 ``tables.derived_image_searches`` (strided pixel subsets: image level 2s = every other pixel of every other row of
-level s) and ``tables.derived_subset_searches`` (nearest next-level point read off the level's self search) are checked on the point sets of a synthetic frame, and the index arrays the oracle computes for the child
+level s) are checked on the point sets of a synthetic frame, and the index arrays the oracle computes for the child
 searches are compared with the slices of the parents' arrays."""
 import numpy as np
 
@@ -54,28 +54,3 @@ def test_no_strided_derivation_for_indivisible_images():
     d = T.derived_image_searches(calls, 484, 644)                            # multiples of 4, not of 8
     assert set(d) == {"p2r_ds_nei_idx0"}
 
-
-def test_nearest_next_level_point_is_read_off_the_self_search():
-    """cld_interp_idx{i} == first entry of each cld_nei_idx{i} row that lies in level i+1 (a row prefix); rows without
-    one are searched.  Checked against the oracle's own K = 1 searches, on a plain frame, on a frame with duplicated
-    points (exact distance ties, like the datasets' wrap padding) and with a short neighbour list (many misses)."""
-    calls = T.knn_schedule(N_POINTS, H, W, 16)
-    sub = T.derived_subset_searches(calls)
-    assert sub == {"cld_interp_idx%d" % i: "cld_nei_idx%d" % i for i in range(4)}
-    by_key = {key: (s, q, kk) for key, s, q, kk in calls}
-    fr = make_frame(4, n_points=N_POINTS)
-    dup = fr["cld"].copy()
-    dup[1::5] = dup[0::5][: len(dup[1::5])]                                  # every fifth point duplicated: ties everywhere
-    for cld, k_list in ((fr["cld"], 16), (dup, 16), (fr["cld"], 3)):
-        sets = frame_point_sets(dict(fr, cld=cld), N_POINTS)
-        for child, parent in sub.items():
-            (s_c, q_c, k_c), (s_p, q_p, _) = by_key[child], by_key[parent]
-            assert k_c == 1 and s_p == q_p == q_c and s_c == ("cld", q_c[1] + 1)
-            n_sub = sets[s_c].shape[0]
-            assert np.array_equal(sets[s_c], sets[q_c][:n_sub])               # the support IS a row prefix of the queries
-            knn = O.knn_search(sets[q_c][None], sets[q_c][None], min(k_list, len(sets[q_c])))[0]
-            got, missed = O.subset_nn_from_knn(knn, n_sub, sets[s_c], sets[q_c])
-            want = O.knn_search(sets[s_c][None], sets[q_c][None], 1)[0]
-            assert np.array_equal(got, want), (child, k_list)
-            if k_list == 3 and len(sets[q_c]) >= 768:
-                assert missed > 0                                            # the fallback path was exercised

@@ -267,46 +267,6 @@ def test_knn_organised_queries_tile_path(cuda):
             assert np.array_equal(grid.query(tq, 1, out_dtype=dt, query_width=ww).cpu().numpy(), tiled)
 
 
-@pytest.mark.parametrize("k_list,dtype", [(16, torch.int32), (16, torch.int64), (3, torch.int32), (1, torch.int32)])
-def test_subset_nn_read_off_self_search(cuda, k_list, dtype):
-    """``ffb6d_knn_subset_nn`` (cld_interp_idx{i} read off cld_nei_idx{i}): bitwise the K = 1 search of the queries
-    into their row prefix -- random clouds, a batch item with duplicated points (ties), short lists (most rows miss
-    and take the full-scan pass), a level smaller than the list."""
-    rs = np.random.RandomState(k_list)
-    q = (rs.rand(3, 4096, 3) * np.array([1.0, 1.0, 0.1])).astype(np.float32)
-    q[1, 1::3] = q[1, 0::3][: len(q[1, 1::3])]
-    for n_q, n_sub in ((4096, 1024), (4096, 1), (12, 3)):
-        qry = torch.from_numpy(np.ascontiguousarray(q[:, :n_q])).cuda()
-        sup = qry[:, :n_sub].contiguous()
-        knn = F.knn_search(qry, qry, min(k_list, 64), out_dtype=dtype)
-        got = F.ops.subset_nn_from_knn(sup, qry, knn)
-        assert got.dtype == dtype and tuple(got.shape) == (3, n_q, 1)
-        want = F.knn_search(sup, qry, 1, out_dtype=dtype)
-        assert torch.equal(got, want), (n_q, n_sub)
-        assert np.array_equal(got.cpu().numpy(), O.knn_search(sup.cpu().numpy(), qry.cpu().numpy(), 1))
-    with pytest.raises(ValueError):
-        F.ops.subset_nn_from_knn(qry, qry[:, :2].contiguous(), knn[:, :2])     # support longer than the queries
-
-
-def test_scheduler_with_subset_derivation_equals_default(cuda, monkeypatch):
-    """FFB6D_SUBSET_NN=1 (cld_interp_idx{0,1} read off the self searches instead of searched; off by default because the
-    pass is slower with it) produces the same 22 + 4 tensors, sequentially and on side streams."""
-    from ffb6d_b200.synthetic import make_batch
-    batch = make_batch(range(50, 52), n_points=12288)
-    cld = torch.from_numpy(batch["cld"]).cuda()
-    xyz = torch.from_numpy(batch["dpt_xyz"]).cuda()
-    monkeypatch.setenv("FFB6D_SUBSET_NN", "0")
-    want = F.build_ffb6d_indices(cld, xyz)
-    monkeypatch.setenv("FFB6D_SUBSET_NN", "1")
-    streams = [torch.cuda.Stream() for _ in range(2)]
-    for st in (None, streams):
-        got = F.build_ffb6d_indices(cld, xyz, streams=st)
-        torch.cuda.synchronize()
-        assert set(got) == set(want)
-        for key in want:
-            assert torch.equal(got[key], want[key]), key
-
-
 @pytest.mark.parametrize("k", [2, 31, 32, 33, 64])
 def test_knn_all_k_paths(cuda, k):
     """warp-per-query (K <= 32) and thread-per-query (K > 32) searches, overflow paths included."""

@@ -2,8 +2,8 @@
 
 Under the default tuning nearly every query is certified within two rings, so most of the grid's
 code rarely runs in tests/test_gpu_knn.py: rings 3-4 and the ring jump, the new-shell scan of old
-rows, the cell-cap loop, the geometric fallbacks, the single-cell grid, the per-thread search for
-2 <= K <= 32, and overflow lists where the duplicate list (back) meets the plain one (front).  The
+rows, the cell-cap loop, the geometric fallbacks, the single-cell grid, and overflow lists where the
+duplicate list (back) meets the plain one (front).  The
 cases here drive the tuning knobs and the geometry onto those paths, read back the grid's
 ``GridParams`` and the query's ``QueryState`` to prove they got there, and require results
 bitwise equal to ``oracle.cpu_oracle.knn_search`` (fp32 reference arithmetic, ties in
@@ -11,8 +11,6 @@ bitwise equal to ``oracle.cpu_oracle.knn_search`` (fp32 reference arithmetic, ti
 import hashlib
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -20,7 +18,7 @@ import torch
 
 import ffb6d_b200 as F
 from ffb6d_b200._lib import lib, check
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
 from oracle import cpu_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -77,22 +75,6 @@ class Grid:
         return out.cpu().numpy(), scratch[: self.B * 16].cpu().numpy().view(QUERY_STATE)
 
 
-def _env_knobs():
-    """The knob values the library reads from FFB6D_GRID_* at start-up (api.cu env())."""
-    def num(name, default, cast):
-        v = os.environ.get(name)
-        if v is None:
-            return default
-        try:
-            return cast(v)
-        except ValueError:
-            return cast(0)
-    scale = num("FFB6D_GRID_SCALE", DEFAULTS[0], float)
-    scale_k1 = num("FFB6D_GRID_SCALE_K1", DEFAULTS[2], float)
-    quantile = min(max(num("FFB6D_GRID_QUANTILE", DEFAULTS[1], int), 0), 31)
-    return (scale if scale > 0 else DEFAULTS[0], quantile, scale_k1 if scale_k1 > 0 else DEFAULTS[2])
-
-
 def set_knobs(scale, quantile, scale_k1):
     lib.ffb6d_knn_grid_tune(float(scale), int(quantile))
     lib.ffb6d_knn_grid_tune_k1(float(scale_k1))
@@ -101,12 +83,12 @@ def set_knobs(scale, quantile, scale_k1):
 @pytest.fixture
 def knobs():
     """Sets the cell-size knobs for one test (documented defaults first) and always restores the
-    process's own values afterwards: the FFB6D_GRID_* variables where set, else the defaults."""
+    defaults afterwards."""
     set_knobs(*DEFAULTS)
     try:
         yield set_knobs
     finally:
-        set_knobs(*_env_knobs())
+        set_knobs(*DEFAULTS)
 
 
 def _width(Q):
@@ -444,7 +426,8 @@ def far_queries(rs, S=3000, Q=1536):
 
 def test_every_query_overflows(cuda, knobs):
     """The overflow lists full: every query overflows, the duplicates fill the list from the back and the
-    rest from the front until they meet; K > 32 takes the tiled overflow scan and the separate row copy."""
+    rest from the front until they meet (K = 1 without a row width: the per-thread search); K > 32 takes the
+    tiled overflow scan and the separate row copy."""
     rs = np.random.RandomState(10)
     sup, qry = far_queries(rs)
     Q = qry.shape[1]
@@ -520,42 +503,6 @@ def test_results_never_depend_on_the_tuning(cuda, knobs, frame_cases):
                     deep = int((kth > 3.001 * p["h"]).sum()) - int(st[0]["ovf"] + st[0]["dup"])
                     seen["deep"] = max(seen["deep"], deep)
     assert seen["single"] and seen["cap"] and seen["deep"] > 0, seen
-
-
-# ------------------------------------------------------------------------------------------ per-thread search
-THREAD_SCRIPT = r"""
-import sys
-sys.path[:0] = [%r, %r]
-import numpy as np, torch
-import test_gpu_knn_paths as T
-from oracle import cpu_oracle as O
-T.set_knobs(*T.DEFAULTS)
-rs = np.random.RandomState(10)
-sup, qry = T.far_queries(rs)
-T.run_all_kernels(sup, qry, (2, 4, 8, 16, 31, 32), 16, "thread search, all far")
-sup = T._lattice(16, 0.125, 0.0)
-T.run_all_kernels(sup[None], None, (2, 4, 8, 16, 31, 32), 16, "thread search, lattice self", tiled=False)
-base = T.face_cloud(1000.0, 1e-3, rs)
-p = T.Grid(torch.from_numpy(base[None]).cuda(), 8).params[0]
-q = T._snap(rs.rand(3072, 3) * (p["hi"] - p["lo"]) + p["lo"], p, rs)
-T.run_all_kernels(base[None], q[None], (2, 4, 8, 16, 31, 32), 8, "thread search, faces", tiled=False)
-# the organised K = 1 request no longer takes the tile kernel: its far duplicates go to the dup list
-sup, qry = T.far_queries(rs)
-g = T.Grid(torch.from_numpy(sup).cuda(), 1)
-got, st = g.query(torch.from_numpy(qry).cuda(), 1, query_width=32)
-assert np.array_equal(got, O.knn_search(sup, qry, 1))
-assert (st["dup"] > 0).all(), st
-print("thread search ok")
-"""
-
-
-def test_per_thread_search_for_small_k(cuda):
-    """FFB6D_GRID_THREAD_SEARCH=1 (read once per process, so in a child process) answers 2 <= K <= 32 with one
-    thread per query instead of the warp kernels, and K = 1 image queries without the tile kernel."""
-    env = dict(os.environ, FFB6D_GRID_THREAD_SEARCH="1")
-    r = subprocess.run([sys.executable, "-c", THREAD_SCRIPT % (ROOT, os.path.dirname(os.path.abspath(__file__)))],
-                       env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0 and "thread search ok" in r.stdout, (r.stdout[-2000:] + r.stderr[-4000:])
 
 
 # ------------------------------------------------------------------------------------------ the whole schedule
