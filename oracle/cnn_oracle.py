@@ -23,7 +23,7 @@ def _draw(key, shape, seed):
         return rs.uniform(0.5, 1.5, shape)
     if leaf == "running_mean":
         return rs.normal(0.0, 0.1, shape)
-    if len(shape) == 4:                                    # conv weight
+    if len(shape) in (3, 4):                               # conv weight (Conv1d, Conv2d)
         fan_in = int(np.prod(shape[1:]))
         return rs.normal(0.0, np.sqrt(2.0 / fan_in), shape)
     if len(shape) == 1 and shape[0] == 1:                  # PReLU slope

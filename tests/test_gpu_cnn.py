@@ -15,7 +15,7 @@ from ffb6d_b200.loss import ffb6d_loss
 from ffb6d_b200.model import FFB6D
 from ffb6d_b200.schedule import build_ffb6d_indices
 from ffb6d_b200.synthetic import make_batch
-from test_gpu_model import TorchRef, close
+from ffb6d_restatement import FullRef, close
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
@@ -163,54 +163,6 @@ def test_final_module_fused_matches(cuda):
 
 
 # ----------------------------------------------------------------------------------------------- whole network
-class FullRef(TorchRef):
-    """TorchRef with the image branch: float64 copies of the model's own ``cnn_*`` torch modules, run where
-    models/ffb6d.py runs them (the reference's order of operations)."""
-
-    def __init__(self, model, sd, n_kps):
-        super().__init__(sd, False, n_kps)
-        m64 = copy.deepcopy(model).double().eval()
-        self.pre, self.ds, self.up = m64.cnn_pre_stages, m64.cnn_ds_stages, m64.cnn_up_stages
-
-    def forward(self, inp, rgb):
-        with torch.no_grad():
-            p_emb = self.rconv("rndla_pre_stages", inp["cld_rgb_nrm"].to(self.dtype)).unsqueeze(3)
-            rgb_emb = self.pre(rgb.double())
-            ds_emb, fused = [], []
-            for i in range(4):
-                rgb0 = self.ds[i](rgb_emb)
-                f_enc = self.block("rndla_ds_stages.%d" % i, p_emb, inp["cld_xyz%d" % i].to(self.dtype),
-                                   inp["cld_nei_idx%d" % i])
-                p0 = self.random_sample(f_enc, inp["cld_sub_idx%d" % i])
-                if i == 0:
-                    ds_emb.append(f_enc)
-                rgb_emb, p_emb = self.fuse("ds", i, rgb0, p0, inp["p2r_ds_nei_idx%d" % i], inp["r2p_ds_nei_idx%d" % i])
-                ds_emb.append(p_emb)
-                fused.append(rgb_emb)
-            for i in range(3):
-                rgb0 = self.up[i](rgb_emb)
-                f_interp = self.nearest(p_emb, inp["cld_interp_idx%d" % (3 - i)])
-                p0 = self.rconv("rndla_up_stages.%d" % i, torch.cat([ds_emb[-i - 2], f_interp], 1))
-                rgb_emb, p_emb = self.fuse("up", i, rgb0, p0, inp["p2r_up_nei_idx%d" % i], inp["r2p_up_nei_idx%d" % i])
-                fused.append(rgb_emb)
-            f_interp = self.nearest(p_emb, inp["cld_interp_idx0"])
-            p_emb = self.rconv("rndla_up_stages.3", torch.cat([ds_emb[0], f_interp], 1)).squeeze(-1)
-            rgb = self.up[3](rgb_emb)
-            bs, di = rgb.shape[0], rgb.shape[1]
-            rgb_c = torch.gather(rgb.view(bs, di, -1), 2, inp["choose"].expand(-1, di, -1).long())
-            x0 = torch.cat([rgb_c, p_emb], 1)
-            outs = []
-            for head in ("rgbd_seg_layer", "kp_ofst_layer", "ctr_ofst_layer"):
-                x = x0
-                for j in range(3):
-                    x = self.conv("%s.%d" % (head, j), x, "normlayer", 1e-5, "relu")
-                outs.append(self.conv("%s.3" % head, x, "normlayer", 1e-5, None))
-        segs, kp, ctr = outs
-        kp = kp.view(bs, self.n_kps, 3, -1).permute(0, 1, 3, 2).contiguous()
-        ctr = ctr.view(bs, 1, 3, -1).permute(0, 1, 3, 2).contiguous()
-        return {"pred_rgbd_segs": segs, "pred_kp_ofs": kp, "pred_ctr_ofs": ctr, "fused_rgb": fused}
-
-
 def _network(B=2, h=120, w=160, n_pts=4096, seed=3, train=False):
     torch.manual_seed(seed)
     model = FFB6D(n_classes=22, n_pts=n_pts, n_kps=8).cuda()
@@ -264,7 +216,8 @@ def test_ffb6d_eval_matches_float64_restatement(cuda, monkeypatch):
     assert calls == {"psp": 1, "final": 2}, calls
     sd = {k: v.clone() for k, v in model.state_dict().items()}
     ref = FullRef(model, sd, 8)
-    want = ref.forward(inputs, inputs["rgb"])
+    with torch.no_grad():
+        want = ref.forward(inputs, inputs["rgb"])
     # the eval path without the kernels (autograd on): the image branch on its torch modules, in fp32
     with torch.enable_grad():
         out_t = model(inputs)

@@ -15,7 +15,7 @@ import torch.nn.functional as Fn
 from ffb6d_b200 import cnn, ops
 from ffb6d_b200.loss import ffb6d_loss
 from test_gpu_cnn import _network, same_nonfinite
-from test_gpu_model import close
+from ffb6d_restatement import close
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-import test_gpu_model
+from ffb6d_restatement import TorchRef, unit
 from test_gpu_train import close_fp32, WGRAD_CASES, WGRAD_CENTRED
 from ffb6d_b200 import ops
 from ffb6d_b200 import tables as T
@@ -441,15 +441,12 @@ def test_whole_network_bitwise_reproducible(cuda, restructured):
     for i, (x, y) in enumerate(zip(a[1], b[1])):
         assert torch.equal(x, y), "gradient of rgb_feats[%d] differs between two runs" % i
     # and the gradients meet tests/test_gpu_model.py's bounds against its float64 restatement
-    ref = test_gpu_model.TorchRef(s["sd"], True, 8)
-    ref32 = test_gpu_model.TorchRef(s["sd"], True, 8, dtype=torch.float32)
+    ref = TorchRef(s["sd"], True, 8)
+    ref32 = TorchRef(s["sd"], True, 8, dtype=torch.float32)
     rgb64 = [t.double().requires_grad_(True) for t in s["rgb"]]
     rgb32 = [t.clone().requires_grad_(True) for t in s["rgb"]]
     sum((v * g.double()).sum() for v, g in zip(flat(ref.forward(s["inputs"], rgb64)), go)).backward()
     sum((v * g).sum() for v, g in zip(flat(ref32.forward(s["inputs"], rgb32)), go)).backward()
-
-    def unit(name):
-        return name.rsplit(".conv.", 1)[0].rsplit(".normlayer.", 1)[0].rsplit(".bn.bn.", 1)[0].rsplit(".fc.", 1)[0]
 
     scale = {}
     for name in a[0]:

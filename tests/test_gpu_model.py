@@ -2,122 +2,15 @@
 203-337, on this package's kernels) against a plain-torch float64 restatement of the same lines built from the
 same state dict: forward values and, in training mode, the gradients of every parameter and of the image-branch
 inputs.  Index tensors come from build_ffb6d_indices (itself pinned to the reference elsewhere)."""
-import numpy as np
 import pytest
 import torch
-import torch.nn.functional as Fn
 
 from ffb6d_b200.model import FFB6DFusionNet
 from ffb6d_b200.schedule import build_ffb6d_indices
 from ffb6d_b200.synthetic import make_batch
-from oracle import lfa_oracle
+from ffb6d_restatement import TorchRef, close, unit
 
 pytestmark = pytest.mark.gpu
-
-
-class TorchRef:
-    """The reference's forward with torch ops only (float64), parameters taken from a state dict by the
-    reference's names.  ``train``: BatchNorm uses batch statistics."""
-
-    def __init__(self, sd, train, n_kps, dtype=torch.float64):
-        self.p = {k: v.detach().to(dtype).requires_grad_(v.dtype.is_floating_point and "running" not in k)
-                  for k, v in sd.items() if v.dtype.is_floating_point}
-        self.train, self.n_kps, self.dtype = train, n_kps, dtype
-
-    def conv(self, pre, x, bn_name, eps, act, slope=0.2):
-        w = self.p[pre + ".conv.weight"]
-        y = torch.einsum("oc,bc...->bo...", w.reshape(w.shape[0], -1), x)
-        if pre + ".conv.bias" in self.p:
-            y = y + self.p[pre + ".conv.bias"].view(1, -1, *([1] * (y.dim() - 2)))
-        b = pre + "." + bn_name + ".bn."
-        if b + "weight" in self.p:
-            y = Fn.batch_norm(y, self.p[b + "running_mean"].clone(), self.p[b + "running_var"].clone(), self.p[b + "weight"],
-                              self.p[b + "bias"], self.train, 0.1, eps)
-        if act == "relu":
-            y = torch.relu(y)
-        elif act == "leaky":
-            y = Fn.leaky_relu(y, slope)
-        return y
-
-    def fconv(self, pre, x):                        # fusion flavour
-        return self.conv(pre, x, "normlayer", 1e-5, "relu")
-
-    def rconv(self, pre, x, act="leaky"):           # RandLA flavour
-        return self.conv(pre, x, "bn", 1e-6, act)
-
-    @staticmethod
-    def random_sample(feature, idx):                # models/ffb6d.py:159-177
-        f = feature.squeeze(3) if feature.dim() == 4 else feature
-        B, d, K = f.shape[0], f.shape[1], idx.shape[-1]
-        g = torch.gather(f, 2, idx.reshape(B, 1, -1).expand(-1, d, -1).long())
-        return g.reshape(B, d, -1, K).max(dim=3, keepdim=True)[0]
-
-    @staticmethod
-    def nearest(feature, idx):                      # :179-194
-        f = feature.squeeze(3)
-        B, d = f.shape[0], f.shape[1]
-        return torch.gather(f, 2, idx.reshape(B, 1, -1).expand(-1, d, -1).long()).unsqueeze(3)
-
-    def att_pool(self, pre, fs):                    # RandLANet.py:243-250
-        w = self.p[pre + ".fc.weight"]
-        agg = lfa_oracle.att_pool(fs, torch.einsum("oc,bcnk->bonk", w.reshape(w.shape[0], -1), fs))
-        return self.rconv(pre + ".mlp", agg)
-
-    def block(self, pre, feature, xyz, idx):        # RandLANet.py:170-234
-        f_pc = self.rconv(pre + ".mlp1", feature)
-        f_xyz = self.rconv(pre + ".lfa.mlp1", lfa_oracle.relative_pos_encoding(xyz, idx))
-        agg = self.att_pool(pre + ".lfa.att_pooling_1", torch.cat([lfa_oracle.gather_cm(f_pc, idx), f_xyz], 1))
-        f_xyz = self.rconv(pre + ".lfa.mlp2", f_xyz)
-        agg = self.att_pool(pre + ".lfa.att_pooling_2", torch.cat([lfa_oracle.gather_cm(agg, idx), f_xyz], 1))
-        return Fn.leaky_relu(self.rconv(pre + ".mlp2", agg, None) + self.rconv(pre + ".shortcut", feature, None), 0.2)
-
-    def fuse(self, tag, i, rgb0, p0, p2r_idx, r2p_idx):      # models/ffb6d.py:245-263
-        bs, c, hr, wr = rgb0.shape
-        p2r = self.nearest(self.fconv("%s_fuse_p2r_pre_layers.%d" % (tag, i), p0), p2r_idx).view(bs, -1, hr, wr)
-        rgb = self.fconv("%s_fuse_p2r_fuse_layers.%d" % (tag, i), torch.cat((rgb0, p2r), 1))
-        r2p = self.random_sample(rgb0.reshape(bs, c, hr * wr, 1), r2p_idx)
-        r2p = self.fconv("%s_fuse_r2p_pre_layers.%d" % (tag, i), r2p)
-        return rgb, self.fconv("%s_fuse_r2p_fuse_layers.%d" % (tag, i), torch.cat((p0, r2p), 1))
-
-    def forward(self, inp, rgb_feats):
-        p_emb = self.rconv("rndla_pre_stages", inp["cld_rgb_nrm"].to(self.dtype)).unsqueeze(3)
-        ds_emb, fused = [], []
-        for i in range(4):
-            f_enc = self.block("rndla_ds_stages.%d" % i, p_emb, inp["cld_xyz%d" % i].to(self.dtype), inp["cld_nei_idx%d" % i])
-            p0 = self.random_sample(f_enc, inp["cld_sub_idx%d" % i])
-            if i == 0:
-                ds_emb.append(f_enc)
-            rgb, p_emb = self.fuse("ds", i, rgb_feats[i], p0, inp["p2r_ds_nei_idx%d" % i], inp["r2p_ds_nei_idx%d" % i])
-            ds_emb.append(p_emb)
-            fused.append(rgb)
-        for i in range(3):
-            f_interp = self.nearest(p_emb, inp["cld_interp_idx%d" % (3 - i)])
-            p0 = self.rconv("rndla_up_stages.%d" % i, torch.cat([ds_emb[-i - 2], f_interp], 1))
-            rgb, p_emb = self.fuse("up", i, rgb_feats[4 + i], p0, inp["p2r_up_nei_idx%d" % i], inp["r2p_up_nei_idx%d" % i])
-            fused.append(rgb)
-        f_interp = self.nearest(p_emb, inp["cld_interp_idx0"])
-        p_emb = self.rconv("rndla_up_stages.3", torch.cat([ds_emb[0], f_interp], 1)).squeeze(-1)
-        rgb = rgb_feats[7]
-        bs, di = rgb.shape[0], rgb.shape[1]
-        rgb_c = torch.gather(rgb.view(bs, di, -1), 2, inp["choose"].expand(-1, di, -1).long())
-        x0 = torch.cat([rgb_c, p_emb], 1)
-        outs = []
-        for head in ("rgbd_seg_layer", "kp_ofst_layer", "ctr_ofst_layer"):
-            x = x0
-            for j in range(3):
-                x = self.conv("%s.%d" % (head, j), x, "normlayer", 1e-5, "relu")
-            outs.append(self.conv("%s.3" % head, x, "normlayer", 1e-5, None))
-        segs, kp, ctr = outs
-        kp = kp.view(bs, self.n_kps, 3, -1).permute(0, 1, 3, 2).contiguous()
-        ctr = ctr.view(bs, 1, 3, -1).permute(0, 1, 3, 2).contiguous()
-        return {"pred_rgbd_segs": segs, "pred_kp_ofs": kp, "pred_ctr_ofs": ctr, "fused_rgb": fused}
-
-
-def close(got, want, what, tol):
-    got, want = got.detach().double().cpu().numpy(), want.detach().double().cpu().numpy()
-    scale = max(np.abs(want).max(), 1e-6)
-    err = np.abs(got - want).max()
-    assert err <= tol * scale, "%s: max abs err %.3e at scale %.3e (%.2e relative)" % (what, err, scale, err / scale)
 
 
 @pytest.mark.parametrize("train", [False, True], ids=["eval", "train"])
@@ -173,11 +66,7 @@ def test_fusion_net_matches_torch_restatement(cuda, train):
     want32 = ref32.forward(inputs, rgb32)
     sum((v * g_).sum() for (_, v), g_ in zip(flat(want32), go)).backward()
     # errors are measured against the gradient scale of the parameter's LAYER (largest gradient norm among the
-    # parameters of the same conv + BatchNorm unit): a BatchNorm bias gradient is a sum of terms that nearly
-    # cancel behind another BatchNorm, its own norm is no yardstick for round-off
-    def unit(name):
-        return name.rsplit(".conv.", 1)[0].rsplit(".normlayer.", 1)[0].rsplit(".bn.bn.", 1)[0].rsplit(".fc.", 1)[0]
-
+    # parameters of the same conv + BatchNorm unit, `unit`)
     scale_of = {}
     for name, _ in model.named_parameters():
         scale_of[unit(name)] = max(scale_of.get(unit(name), 1e-12), ref.p[name].grad.norm().item())

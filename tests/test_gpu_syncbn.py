@@ -405,7 +405,7 @@ def _check_fusion(res, cuda):
     """The whole network: rank-summed parameter gradients and per-rank input gradients against float64 TorchRef on
     the two-frame batch in one process, within test_gpu_model.py's bound (max(4x torch fp32, 2e-3)); two runs and both
     ranks' running statistics bit-identical."""
-    from test_gpu_model import TorchRef
+    from ffb6d_restatement import TorchRef
     for restructured in (False, True):
         runs = [r["fusion%d" % restructured] for r in res]
         what = "fusion restructured=%s" % restructured
