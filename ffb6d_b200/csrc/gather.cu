@@ -25,7 +25,11 @@
 
 namespace ffb6d {
 
-// torch.max semantics (max_nan, common.cuh): NaN propagates; first maximal element wins the arg-max
+// torch.max(dim) semantics: the value of the first NaN, else of the first maximal element, bit for bit.  `a` holds the
+// earlier neighbours, `b` later ones.  The backward's arg-max (gather_max_bwd_kernel, gather_argmax_kernel) follows
+// the same rule, so the forward's output is the feature the gradient goes to.  max.NaN.f32 (max_nan, common.cuh) would
+// not do: of -0.0 then +0.0 it returns +0.0, and of a NaN the canonical NaN, not the feature's payload.
+__device__ __forceinline__ float max_first(float a, float b) { return (b > a || (b != b && a == a)) ? b : a; }
 
 template <typename IdxT, int KT>
 __device__ __forceinline__ void load_ids(const IdxT *__restrict__ ip, int K, int (&id)[KT > 0 ? KT : 1])
@@ -124,14 +128,14 @@ gather_max_ncs_staged_kernel(const float *__restrict__ feat, const IdxT *__restr
                 const float *r = rows + c * S;
                 float m = r[id[0]];
 #pragma unroll
-                for (int k = 1; k < KT; ++k) m = max_nan(m, r[id[k]]);
+                for (int k = 1; k < KT; ++k) m = max_first(m, r[id[k]]);
                 dst[(size_t)c * Q + q] = m;
             }
         } else {
             for (int c = 0; c < cc; ++c) {
                 const float *r = rows + c * S;
                 float m = r[(int)__ldg(ip)];
-                for (int k = 1; k < K; ++k) m = max_nan(m, r[(int)__ldg(ip + k)]);
+                for (int k = 1; k < K; ++k) m = max_first(m, r[(int)__ldg(ip + k)]);
                 dst[(size_t)c * Q + q] = m;
             }
         }
@@ -226,8 +230,8 @@ gather_max_ncs_direct_kernel(const float *__restrict__ feat, const IdxT *__restr
             float m0 = v0[0], m1 = v1[0];
 #pragma unroll
             for (int k = 1; k < KT; ++k) {
-                m0 = max_nan(m0, v0[k]);
-                m1 = max_nan(m1, v1[k]);
+                m0 = max_first(m0, v0[k]);
+                m1 = max_first(m1, v1[k]);
             }
             dst[(size_t)c * Q + q] = m0;
             dst[(size_t)(c + 1) * Q + q] = m1;
@@ -236,14 +240,14 @@ gather_max_ncs_direct_kernel(const float *__restrict__ feat, const IdxT *__restr
             const float *r = src + (size_t)c * S;
             float m = __ldg(r + id[0]);
 #pragma unroll
-            for (int k = 1; k < KT; ++k) m = max_nan(m, __ldg(r + id[k]));
+            for (int k = 1; k < KT; ++k) m = max_first(m, __ldg(r + id[k]));
             dst[(size_t)c * Q + q] = m;
         }
     } else {
         for (int c = 0; c < cc; ++c) {
             const float *r = src + (size_t)c * S;
             float m = __ldg(r + (int)__ldg(ip));
-            for (int k = 1; k < K; ++k) m = max_nan(m, __ldg(r + (int)__ldg(ip + k)));
+            for (int k = 1; k < K; ++k) m = max_first(m, __ldg(r + (int)__ldg(ip + k)));
             dst[(size_t)c * Q + q] = m;
         }
     }
@@ -253,7 +257,9 @@ gather_max_ncs_direct_kernel(const float *__restrict__ feat, const IdxT *__restr
 // neighbours of ONE query.  Neighbours of a query are adjacent pixels, so a warp-wide load touches
 // a handful of 32-byte sectors instead of 32 (lanes along the query axis would scatter every
 // lane into its own sector); the max over the group is a log2(K)-step shuffle reduction.  Results
-// are collected in a [channel][query] shared-memory tile and written out coalesced.
+// are collected in a [channel][query] shared-memory tile and written out coalesced.  The shuffle steps go up from
+// distance 1, so each combines two adjacent ranges of neighbours in their order and lane 0 ends with the first NaN or
+// first maximum of all K (from distance K/2 down, lane 0 would compare {0, 8} with {4, 12}).
 // A CTA takes one query per lane group (256 / K queries) and issues the loads of all its channels
 // before the first shuffle: eight loads in flight per thread, and short CTAs.  (H100: 10-20 % less
 // time on the sparse r2p gathers than 32 queries per CTA in rounds of four channels.)
@@ -283,7 +289,10 @@ gather_max_ncs_klane_kernel(const float *__restrict__ feat, const IdxT *__restri
 #pragma unroll
     for (int c = 0; c < KLANE_CH; ++c) {
 #pragma unroll
-        for (int o = KT / 2; o > 0; o >>= 1) v[c] = max_nan(v[c], __shfl_xor_sync(0xffffffffu, v[c], o));
+        for (int o = 1; o < KT; o <<= 1) {   // blocks of o lanes; the one with bit o clear holds the earlier neighbours
+            const float u = __shfl_xor_sync(0xffffffffu, v[c], o);
+            v[c] = (kl & o) ? max_first(u, v[c]) : max_first(v[c], u);
+        }
         if (kl == 0 && c < cc) tile[c][ql] = v[c];
     }
     __syncthreads();
@@ -349,10 +358,10 @@ gather_max_nsc_kernel(const float *__restrict__ feat, const IdxT *__restrict__ i
                 const int s = __shfl_sync(0xffffffffu, (k < 32) ? my0 : my1, k & 31);
                 if (on) {
                     const float4 v = __ldg(reinterpret_cast<const float4 *>(base + (size_t)s * C + c));
-                    m.x = max_nan(m.x, v.x);
-                    m.y = max_nan(m.y, v.y);
-                    m.z = max_nan(m.z, v.z);
-                    m.w = max_nan(m.w, v.w);
+                    m.x = max_first(m.x, v.x);
+                    m.y = max_first(m.y, v.y);
+                    m.z = max_first(m.z, v.z);
+                    m.w = max_first(m.w, v.w);
                 }
             }
             if (on) *reinterpret_cast<float4 *>(o + c) = m;
@@ -365,7 +374,7 @@ gather_max_nsc_kernel(const float *__restrict__ feat, const IdxT *__restrict__ i
             float m = on ? __ldg(base + (size_t)s0 * C + c) : 0.f;
             for (int k = 1; k < K; ++k) {
                 const int s = __shfl_sync(0xffffffffu, (k < 32) ? my0 : my1, k & 31);
-                if (on) m = max_nan(m, __ldg(base + (size_t)s * C + c));
+                if (on) m = max_first(m, __ldg(base + (size_t)s * C + c));
             }
             if (on) o[c] = m;
         }

@@ -134,12 +134,13 @@ class TorchRef:
 class FullRef(TorchRef):
     """TorchRef with the image branch: float64 copies of the model's own ``cnn_*`` torch modules (``cnn``), run where
     models/ffb6d.py runs them (the reference's order of operations) on ``forward``'s second argument, the image.
-    ``train``: the image branch is in training mode too, except its dropouts, which stay off."""
+    ``train``: the image branch is in training mode too, except its dropouts, which stay off.  ``dtype``: float64, or
+    float32 for the yardstick of what float32 arithmetic in the reference's order reaches."""
 
-    def __init__(self, model, sd, n_kps, train=False):
-        super().__init__({k: v for k, v in sd.items() if not k.startswith("cnn_")}, train, n_kps)
-        self.cnn = copy.deepcopy(model).double().train(train)
-        self.cnn.load_state_dict({k: v.double() if v.dtype.is_floating_point else v for k, v in sd.items()})
+    def __init__(self, model, sd, n_kps, train=False, dtype=torch.float64):
+        super().__init__({k: v for k, v in sd.items() if not k.startswith("cnn_")}, train, n_kps, dtype=dtype)
+        self.cnn = copy.deepcopy(model).to(dtype).train(train)
+        self.cnn.load_state_dict({k: v.to(dtype) if v.dtype.is_floating_point else v for k, v in sd.items()})
         for m in self.cnn.modules():
             if isinstance(m, (torch.nn.Dropout, torch.nn.Dropout2d)):
                 m.eval()

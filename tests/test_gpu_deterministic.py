@@ -1,6 +1,8 @@
-"""GPU: the deterministic backward taken under torch's determinism switches.  The linear-size segment CSR against a
-stable torch.sort restatement (and the counter plan) at every gather shape of a 480x640 step; the gather + max
-backward without atomics against float64 by the arg-max rule of the atomic kernel; the split-ordered weight
+"""GPU: the gathers' backward under torch's determinism switches and without them.  The linear-size segment CSR
+against a stable torch.sort restatement (and the counter plan) at every gather shape of a 480x640 step; the gather +
+max backward, with and without atomics, against float64 by the arg-max rule of the atomic kernel at every gather of
+that step; the run-aggregating K = 1 backward at its edges; each forward kernel against the arg-max its backward
+picks, on ties, signed zeros and non-finite features; the split-ordered weight
 gradient against float64; bitwise repeatability over calls and CUDA-graph replays; which kernels a training step
 launches under each switch; and bit-identical training of the whole FFB6DFusionNet.  Inputs come from seeds."""
 import contextlib
@@ -14,7 +16,7 @@ from ffb6d_restatement import TorchRef, unit
 from test_gpu_train import close_fp32, WGRAD_CASES, WGRAD_CENTRED
 from ffb6d_b200 import ops
 from ffb6d_b200 import tables as T
-from ffb6d_b200._lib import lib, check, LAYOUT_NCS
+from ffb6d_b200._lib import lib, check, LAYOUT_NCS, LAYOUT_NSC
 from ffb6d_b200.model import FFB6DFusionNet
 from ffb6d_b200.schedule import build_ffb6d_indices
 from ffb6d_b200.synthetic import make_batch
@@ -110,9 +112,10 @@ def test_csr_edge_cases(cuda, case):
 
 
 # ------------------------------------------------------------------ gather + max backward
-def want_gather_bwd(f3, idx, gout):
-    """float64 scatter of gout onto the arg-max neighbour: a NaN wins, else the first strict maximum; reads of
-    out-of-range indices are clamped to row S-1 as in the kernels.  Returns (want, sum of |terms|, hit mask)."""
+def rule_argmax(f3, idx):
+    """The neighbour values ``[B, C, Q, K]`` of a gather + max and the arg-max k ``[B, C, Q]`` by the backward's rule:
+    the first NaN, else the first maximal value (so of a tie between -0.0 and +0.0 the first).  Reads of out-of-range
+    indices are clamped to row S-1 as in the kernels."""
     B, Cc, S = f3.shape
     Q, K = idx.shape[1], idx.shape[2]
     ix = idx.long()
@@ -123,15 +126,23 @@ def want_gather_bwd(f3, idx, gout):
     first_nan = torch.where(nan, ks, K).amin(-1)
     m = torch.where(nan, -float("inf"), vals).amax(-1, keepdim=True)
     first_max = torch.where(vals == m, ks, K).amin(-1)
-    kb = torch.where(nan.any(-1), first_nan, first_max)
-    s = ix.unsqueeze(1).expand(B, Cc, Q, K).gather(3, kb.unsqueeze(-1)).squeeze(-1)        # [B, C, Q]
+    return vals, torch.where(nan.any(-1), first_nan, first_max)
+
+
+def want_gather_bwd(f3, idx, gout):
+    """float64 scatter of gout onto the arg-max neighbour (:func:`rule_argmax`).  Returns (want, sum of |terms|,
+    number of terms) per element."""
+    B, Cc, S = f3.shape
+    Q, K = idx.shape[1], idx.shape[2]
+    _, kb = rule_argmax(f3, idx)
+    s = idx.long().unsqueeze(1).expand(B, Cc, Q, K).gather(3, kb.unsqueeze(-1)).squeeze(-1)        # [B, C, Q]
     ok = (s >= 0) & (s < S)
     sc = torch.where(ok, s, 0)
     g = torch.where(ok, gout.double(), 0.0)
     want = torch.zeros((B, Cc, S), dtype=torch.float64, device=f3.device).scatter_add_(2, sc, g)
     mag = torch.zeros_like(want).scatter_add_(2, sc, g.abs())
-    hit = torch.zeros_like(want).scatter_add_(2, sc, ok.double()) > 0
-    return want, mag, hit
+    cnt = torch.zeros_like(want).scatter_add_(2, sc, ok.double())
+    return want, mag, cnt
 
 
 def check_sum(out, want, mag, what):
@@ -140,6 +151,20 @@ def check_sum(out, want, mag, what):
     err = np.abs(out.double().cpu().numpy() - w)
     bad = err > bound
     assert not bad.any(), "%s: %d elements out of bound, worst err %.3e" % (what, int(bad.sum()), err[bad].max())
+
+
+def check_atomic_sum(out, want, mag, cnt, what):
+    """An fp32 sum of ``cnt`` terms in an unknown order: within (cnt - 1) * 2^-24 * sum(|terms|) of the float64 sum
+    (true of any order of additions), plus one ulp of the result.  An element no term reaches must stay 0."""
+    w = want.cpu().numpy()
+    ulp = np.spacing(np.abs(w).astype(np.float32)).astype(np.float64)
+    bound = np.maximum(cnt.cpu().numpy() - 1, 0) * 2.0 ** -24 * mag.cpu().numpy() + ulp
+    got = out.double().cpu().numpy()
+    err = np.abs(got - w)
+    bad = err > bound
+    assert not bad.any(), "%s: %d elements out of bound, worst err %.3e (bound there %.3e)" % (
+        what, int(bad.sum()), err[bad].max(), bound[bad][np.argmax(err[bad])])
+    assert not got[cnt.cpu().numpy() == 0].any(), what + ": gradient where no term lands"
 
 
 def gather_grad(f_values, idx, gout, layout, deterministic):
@@ -153,12 +178,16 @@ def gather_grad(f_values, idx, gout, layout, deterministic):
 
 
 def run_gather_case(f3, idx, gout, what):
-    want, mag, hit = want_gather_bwd(f3.double(), idx, gout)
+    """Both layouts: the deterministic path within check_sum's bound and bitwise repeatable, the atomic path within
+    the bound of an fp32 sum in unknown order; both write nowhere else."""
+    want, mag, cnt = want_gather_bwd(f3.double(), idx, gout)
+    hit = cnt > 0
     for layout in ("ncs", "nsc"):
         det = gather_grad(f3, idx, gout, layout, True)
         check_sum(det, want, mag, "%s %s" % (what, layout))
         assert torch.equal(det[~hit], torch.zeros_like(det[~hit])), what + ": gradient where no arg-max lands"
         atomic = gather_grad(f3, idx, gout, layout, False)
+        check_atomic_sum(atomic, want, mag, cnt, "%s %s atomic" % (what, layout))
         assert torch.equal(det != 0, atomic != 0), what + ": positions receiving gradient differ from the atomic path"
         assert torch.equal(det, gather_grad(f3, idx, gout, layout, True)), what + ": not bitwise repeatable"
 
@@ -175,6 +204,7 @@ def test_gather_max_bwd_det_at_step_shapes(cuda, g):
     f3 = torch.randn((B, Cc, S), generator=gen, device=cuda)
     gout = torch.randn((B, Cc, Q), generator=gen, device=cuda)
     run_gather_case(f3, idx, gout, key)
+    run_gather_case(f3, idx.long(), gout, key + " int64")
 
 
 @pytest.mark.parametrize("case", ["k_gt_s_duplicates", "nan_and_ties", "i64", "k1_choose"])
@@ -194,7 +224,8 @@ def test_gather_max_bwd_det_edge_cases(cuda, case):
 
 
 def test_nearest_interpolation_det_at_step_shapes(cuda):
-    """The K = 1 gathers of a step (interp, p2r, choose, the neighbour gathers): plan choice by shape, one CSR."""
+    """The K = 1 gathers of a step (interp, p2r, choose, the neighbour gathers): plan choice by shape, one CSR; and
+    the atomic paths (the run-aggregating kernel for NCS, the generic one for NSC) by value, int32 and int64."""
     ind = step_indices(cuda)
     cases = [(g[1], g[2], g[3], g[4]) for g in GATHERS if g[5] == 1] + [(k, 16, n, n * 16) for k, n in NEIGHBOURS]
     for key, Cc, S, Q in cases:
@@ -203,34 +234,154 @@ def test_nearest_interpolation_det_at_step_shapes(cuda):
         gen = torch.Generator(device=cuda).manual_seed(S + Q)
         f3 = torch.randn((B, Cc, S), generator=gen, device=cuda)
         gout = torch.randn((B, Cc, Q), generator=gen, device=cuda)
-        want, mag, _ = want_gather_bwd(f3.double(), idx, gout)
+        want, mag, cnt = want_gather_bwd(f3.double(), idx, gout)
         det = gather_grad(f3, idx, gout, "ncs", True)
         check_sum(det, want, mag, key)
         assert torch.equal(det, gather_grad(f3, idx, gout, "ncs", True)), key
+        for layout, ix in (("ncs", idx), ("ncs", idx.long()), ("nsc", idx)):
+            check_atomic_sum(gather_grad(f3, ix, gout, layout, False), want, mag, cnt,
+                             "%s %s %s atomic" % (key, layout, ix.dtype))
 
 
 def test_gather_neighbour_bwd_det(cuda):
+    """At the four RandLA levels, with the widths of the coordinates (3) and of the level's features: the
+    deterministic and the default (fp64 atomics, one rounding) backward within check_sum's bound."""
     gen = torch.Generator(device=cuda).manual_seed(7)
-    idx = step_indices(cuda)["cld_nei_idx1"]
-    B, N, K = idx.shape
-    for D in (3, 40):
-        pc = torch.randn((B, N, D), generator=gen, device=cuda, requires_grad=True)
-        gout = torch.randn((B, N, K, D), generator=gen, device=cuda)
-        grads = []
-        for det in (True, True, False):
-            pc.grad = None
-            with switches(algorithms=det):
-                ops.gather_neighbour(pc, idx).backward(gout)
-            grads.append(pc.grad.clone())
-        assert torch.equal(grads[0], grads[1])
-        want = torch.zeros((B, N, D), dtype=torch.float64, device=cuda)
-        mag = torch.zeros_like(want)
-        ix = idx.reshape(B, -1).long()
-        for b in range(B):
-            want[b].index_add_(0, ix[b], gout[b].reshape(-1, D).double())
-            mag[b].index_add_(0, ix[b], gout[b].reshape(-1, D).double().abs())
-        check_sum(grads[0], want, mag, "gather_neighbour D=%d" % D)
-        assert torch.equal(grads[0] != 0, grads[2] != 0)
+    for (key, _), width in zip(NEIGHBOURS, (16, 32, 64, 128)):
+        idx = step_indices(cuda)[key]
+        B, N, K = idx.shape
+        for D in (3, width):
+            pc = torch.randn((B, N, D), generator=gen, device=cuda, requires_grad=True)
+            gout = torch.randn((B, N, K, D), generator=gen, device=cuda)
+            grads = []
+            for det in (True, True, False):
+                pc.grad = None
+                with switches(algorithms=det):
+                    ops.gather_neighbour(pc, idx).backward(gout)
+                grads.append(pc.grad.clone())
+            assert torch.equal(grads[0], grads[1])
+            want = torch.zeros((B, N, D), dtype=torch.float64, device=cuda)
+            mag = torch.zeros_like(want)
+            ix = idx.reshape(B, -1).long()
+            for b in range(B):
+                want[b].index_add_(0, ix[b], gout[b].reshape(-1, D).double())
+                mag[b].index_add_(0, ix[b], gout[b].reshape(-1, D).double().abs())
+            check_sum(grads[0], want, mag, "gather_neighbour %s D=%d" % (key, D))
+            check_sum(grads[2], want, mag, "gather_neighbour %s D=%d atomic" % (key, D))
+            assert torch.equal(grads[0] != 0, grads[2] != 0)
+
+
+# ------------------------------------------------------------------ the run-aggregating K = 1 backward
+def runs(gen, n, longest, S, dev):
+    """``n`` indices in runs of 1..``longest`` equal keys, each run's key drawn from [0, S)."""
+    lengths = torch.randint(1, longest + 1, (n,), generator=gen, device=dev)
+    keys = torch.randint(0, S, (n,), generator=gen, device=dev)
+    return keys.repeat_interleave(lengths)[:n]
+
+
+RUN_CASES = {"runs_across_warps_and_ctas": (2, 5, 1000, 5000), "one_index_per_frame": (2, 3, 19200, 12288),
+             "alternating_keys": (2, 4, 300, 4099), "out_of_range_in_runs_i64": (2, 5, 700, 3000),
+             "q_not_multiple_of_32": (3, 7, 200, 1013), "c65536_generic": (1, 65536, 64, 300)}
+
+
+@pytest.mark.parametrize("case", list(RUN_CASES))
+def test_gather1_bwd_runs_edges(cuda, case):
+    """The default backward of a K = 1 NCS gather (``gather1_bwd_runs_kernel``: a warp-segmented scan of equal
+    indices, then one atomic per run) against float64: runs longer than a warp and across CTAs, one index for a
+    whole frame (a frame's hole pixels all map to one point), alternating keys, -1 and S inside runs (must not
+    write), Q not a multiple of 32; C = 65536 takes the generic kernel."""
+    B, Cc, S, Q = RUN_CASES[case]
+    gen = torch.Generator(device=cuda).manual_seed(len(case))
+    idx = torch.stack([runs(gen, Q, 600 if case.startswith(("runs", "out_of")) else 40, S, cuda) for _ in range(B)])
+    if case == "one_index_per_frame":
+        idx[0], idx[1] = 17, S - 1
+    if case == "alternating_keys":
+        idx[:, 0::2], idx[:, 1::2] = 5, 6
+        idx[1, 1::2] = 5 + S // 2
+    if case == "out_of_range_in_runs_i64":
+        idx = idx.long()
+        idx[:, 37::101], idx[:, 53::97] = -1, S
+    idx = idx.int() if idx.dtype != torch.int64 else idx
+    idx3 = idx.reshape(B, Q, 1)
+    f3 = torch.randn((B, Cc, S), generator=gen, device=cuda)
+    gout = torch.randn((B, Cc, Q), generator=gen, device=cuda)
+    res = {}
+    names = kernel_names(lambda: res.setdefault("g", ops._gather_max_bwd(f3, idx3, gout, LAYOUT_NCS)))
+    assert ("gather_max_bwd_kernel" if Cc > 65535 else "gather1_bwd_runs_kernel") in names, names
+    want, mag, cnt = want_gather_bwd(f3.double(), idx3, gout)
+    check_atomic_sum(res["g"], want, mag, cnt, case)
+
+
+# ------------------------------------------------------------------ forward against backward, for each forward kernel
+FWD_CASES = {"staged": (24, 3072, 768, 16, "ncs", "gather_max_ncs_staged_kernel"),
+             "staged_v4": (24, 3072, 12288, 1, "ncs", "gather1_ncs_staged_v4_kernel"),
+             "direct": (24, 76800, 3072, 12, "ncs", "gather_max_ncs_direct_kernel"),
+             "klane": (24, 76800, 1536, 16, "ncs", "gather_max_ncs_klane_kernel"),
+             "gather1_ncs_direct": (24, 307200, 12288, 1, "ncs", "gather1_ncs_direct_kernel"),
+             "nsc": (24, 3072, 768, 16, "nsc", "gather_max_nsc_kernel"),
+             "nsc_odd_channels": (7, 3072, 768, 16, "nsc", "gather_max_nsc_kernel")}
+
+
+def tie_features(gen, B, Cc, S, dev):
+    """Features full of exact ties: multiples of 0.5 through a ReLU (so exact zeros), every fourth channel
+    non-positive before it (its maximum is always a tie of zeros); half of the zeros -0.0; 0.75 % NaN (two payloads,
+    one with the sign bit set), 0.25 % each of +inf and -inf."""
+    f = torch.randint(-4, 5, (B, Cc, S), generator=gen, device=dev).float() * 0.5
+    f[:, 0::4] = -f[:, 0::4].abs()
+    f = torch.relu(f)
+    r = torch.rand((B, Cc, S), generator=gen, device=dev)
+    f = torch.where((f == 0) & (r < 0.5), -0.0, f)
+    nan2 = torch.tensor([-0.0], device=dev).view(torch.int32).bitwise_or(0x7fc00001).view(torch.float32)
+    f = torch.where(r > 0.995, float("nan"), torch.where(r > 0.9925, nan2, f))
+    return torch.where((r > 0.99) & (r <= 0.9925), float("inf"),
+                       torch.where((r > 0.9875) & (r <= 0.99), -float("inf"), f))
+
+
+def bits(t):
+    return t.contiguous().view(torch.int32)
+
+
+@pytest.mark.parametrize("case", list(FWD_CASES))
+def test_forward_is_the_feature_the_backward_picks(cuda, case):
+    """For each forward kernel, chosen by shape and asserted by name: the forward's output is bitwise the feature
+    at the arg-max to which both backwards (atomic and deterministic) send the gradient, on features with exact
+    ties, -0.0 next to +0.0, NaN and +-inf; and it is torch's ``gather(...).max(dim=3)`` on the GPU (NaN where
+    torch has NaN).  Gradients are small integers, so the backward's sums are exact and must equal the float64
+    scatter onto the arg-max bit for bit."""
+    Cc, S, Q, K, layout, kernel = FWD_CASES[case]
+    B = 2
+    assert lib.ffb6d_gather_kernel_name(B, Cc, S, Q, K, LAYOUT_NCS if layout == "ncs" else LAYOUT_NSC).decode() == kernel
+    gen = torch.Generator(device=cuda).manual_seed(Q + K)
+    f3 = tie_features(gen, B, Cc, S, cuda)
+    # neighbours of a query are nearby positions, as in the KNN maps: many share values
+    base = torch.randint(0, S - 64, (B, Q, 1), generator=gen, device=cuda)
+    idx = (base + torch.randint(0, 64, (B, Q, K), generator=gen, device=cuda)).int()
+    src = f3 if layout == "ncs" else f3.transpose(1, 2).contiguous().transpose(1, 2)
+    res = {}
+    names = kernel_names(lambda: res.setdefault("out", ops._gather_max(src, idx)))
+    assert kernel in names, names
+    out = res["out"]
+    vals, kb = rule_argmax(f3, idx)
+    picked = vals.gather(3, kb.unsqueeze(-1)).squeeze(-1)
+    same = bits(out) == bits(picked)
+    if not same.all():
+        z = (picked == 0) & (out == 0)
+        nn = picked.isnan() & out.isnan()
+        pytest.fail("%s: %d of %d outputs differ bitwise from the feature at the backward's arg-max: %d of them a "
+                    "zero of the other sign, %d a NaN of another payload, %d other" % (
+                        case, int((~same).sum()), same.numel(), int((~same & z).sum()), int((~same & nn).sum()),
+                        int((~same & ~z & ~nn).sum())))
+    want_t = torch.gather(f3, 2, idx.long().reshape(B, 1, Q * K).expand(B, Cc, Q * K)).reshape(B, Cc, Q, K).max(3).values
+    nan = want_t.isnan()
+    assert torch.equal(out.isnan(), nan)
+    assert torch.equal(bits(out)[~nan], bits(want_t)[~nan]), case + ": differs from torch's max"
+    # the backward sends each query's gradient to that same neighbour
+    gout = torch.randint(1, 9, (B, Cc, Q), generator=gen, device=cuda).float()
+    want, _, _ = want_gather_bwd(f3.double(), idx, gout)
+    for det in (False, True):
+        got = gather_grad(f3, idx, gout, layout, det)
+        assert torch.equal(got.double(), want), "%s: the %s backward sends gradient elsewhere" % (
+            case, "deterministic" if det else "atomic")
 
 
 # ------------------------------------------------------------------ weight gradient
