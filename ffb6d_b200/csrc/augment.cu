@@ -319,10 +319,12 @@ static const char *check_record(const double *r)
 
 using namespace ffb6d;
 
+// The 2-D filters put the row tiles in grid.y: H <= 65535 * TY (as ffb6d_fill_depth bounds it)
 #define AUG_CHECK_SIZE(tag)                                                                                         \
-    FFB6D_CHECK_ARG(B >= 0 && B < 65536 && H >= 32 && W >= 32 && H < (1 << 20) && W < (1 << 20) &&                  \
+    FFB6D_CHECK_ARG(B >= 0 && B < 65536 && H >= 32 && W >= 32 && H <= 65535ll * TY && W < (1 << 20) &&              \
                     H * W * 3 < (1ll << 31),                                                                        \
-                    tag ": bad size (B=%lld H=%lld W=%lld; H, W >= 32)", (long long)B, (long long)H, (long long)W)
+                    tag ": bad size (B=%lld H=%lld W=%lld; H, W >= 32, H <= %lld)", (long long)B, (long long)H,     \
+                    (long long)W, 65535ll * TY)
 
 extern "C" int ffb6d_rgb_add_noise(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, const double *plan_host,
                                    const double *plan_dev, uint64_t seed, const double *noise, uint8_t *out,

@@ -669,27 +669,37 @@ static int check_indices_sync(const void *idx, int idx_is_i64, long long n, long
 // ------------------------------------------------------------------ host-side launch logic
 static int max_smem_optin() { return device_info().max_smem_optin; }
 
+// Channels per CTA of the staged kernels for a gather with KT neighbours (0: any K without a K-lane kernel), or 0
+// when the rows are not staged: rows longer than half the shared memory (two CTAs per SM hide the staging latency),
+// few queries against long rows (Q*K gathered elements << S: staging whole rows would read far more than the ~5
+// sectors a query's K adjacent neighbours touch per row -> K-lane gather instead), or more channel chunks than
+// grid.y holds (65535; the direct and K-lane kernels take every C the entry point admits).
+static int staged_channels(int64_t B, int64_t C, int64_t S, int64_t Q, int KT)
+{
+    const size_t budget = (size_t)(max_smem_optin() - 1024) / 2;
+    const size_t row_bytes = (size_t)S * sizeof(float);
+    const bool sparse_queries = (KT == 8 || KT == 16 || KT == 32) && Q * 40 < S;
+    if (C < 1 || row_bytes > budget || sparse_queries) return 0;
+    const int64_t want = 4 * num_sms();   // CTAs to aim for
+    int CC = (int)(budget / row_bytes);
+    if (CC > C) CC = (int)C;
+    // the K indices of a query are re-read once per channel chunk: keep chunks wide when K
+    // is large (index bytes ~ K/CC of the output bytes), narrow when K == 1
+    const int cc_cap = (KT == 1) ? 8 : 32;
+    if (CC > cc_cap) CC = cc_cap;
+    if (KT != 1)
+        while (CC > 4 && B * ceil_div(C, CC) < want) CC = (CC + 1) / 2;
+    return ceil_div(C, CC) <= 65535 ? CC : 0;
+}
+
 template <typename IdxT, int KT>
 static int launch_ncs(const float *feat, const IdxT *idx, float *out, int64_t B, int64_t C,
                       int64_t S, int64_t Q, int K, cudaStream_t st)
 {
-    const int smem_cap = max_smem_optin() - 1024;
     const size_t row_bytes = (size_t)S * sizeof(float);
-    // rows that fit shared memory twice over (two CTAs per SM hide the staging latency)
-    const size_t budget = (size_t)smem_cap / 2;
     const int64_t want = 4 * num_sms();   // CTAs to aim for
-    // few queries against long rows (Q*K gathered elements << S): staging whole rows would read far
-    // more than the ~5 sectors a query's K adjacent neighbours touch per row -> K-lane gather instead
-    const bool sparse_queries = (KT == 8 || KT == 16 || KT == 32) && Q * 40 < S;
-    if (row_bytes <= budget && !sparse_queries) {
-        int CC = (int)(budget / row_bytes);
-        if (CC > C) CC = (int)C;
-        // the K indices of a query are re-read once per channel chunk: keep chunks wide when K
-        // is large (index bytes ~ K/CC of the output bytes), narrow when K == 1
-        const int cc_cap = (KT == 1) ? 8 : 32;
-        if (CC > cc_cap) CC = cc_cap;
-        if (KT != 1)
-            while (CC > 4 && B * ceil_div(C, CC) < want) CC = (CC + 1) / 2;
+    const int CC = staged_channels(B, C, S, Q, KT);
+    if (CC) {
         const int64_t ctas = B * ceil_div(C, CC);
         int64_t nq = ctas < want ? ceil_div(want, ctas) : 1;
         // every query chunk stages the rows again: keep a chunk at least 4 rows long
@@ -763,16 +773,13 @@ extern "C" {
 const char *ffb6d_gather_kernel_name(int64_t B, int64_t C, int64_t S, int64_t Q, int K, int layout)
 {
     // mirrors gather_max_fwd_t / launch_ncs (aligned pointers assumed)
-    (void)B;
-    (void)C;
     if (layout == FFB6D_LAYOUT_NSC) return "gather_max_nsc_kernel";
-    const size_t budget = (size_t)(max_smem_optin() - 1024) / 2;
-    const bool fits = (size_t)S * sizeof(float) <= budget;
-    if (K == 1) return fits ? ((Q % 4 == 0) ? "gather1_ncs_staged_v4_kernel" : "gather_max_ncs_staged_kernel")
-                            : "gather1_ncs_direct_kernel";
-    const bool sparse_queries = (K == 8 || K == 16 || K == 32) && Q * 40 < S;
-    if (fits && !sparse_queries) return "gather_max_ncs_staged_kernel";
-    if (K == 8 || K == 16 || K == 32) return "gather_max_ncs_klane_kernel";
+    const bool klane = K == 8 || K == 16 || K == 32;
+    const bool staged = staged_channels(B, C, S, Q, (K == 1 || klane) ? K : 0) != 0;
+    if (K == 1) return staged ? ((Q % 4 == 0) ? "gather1_ncs_staged_v4_kernel" : "gather_max_ncs_staged_kernel")
+                              : "gather1_ncs_direct_kernel";
+    if (staged) return "gather_max_ncs_staged_kernel";
+    if (klane) return "gather_max_ncs_klane_kernel";
     return "gather_max_ncs_direct_kernel";
 }
 
@@ -788,6 +795,9 @@ int ffb6d_gather_max_fwd(const float *feat, const void *idx, int idx_is_i64, int
     FFB6D_CHECK_ARG(S < (1ll << 31) && Q < (1ll << 31) && C < (1ll << 31) && B < 65536 &&
                         C <= 65535ll * 8,
                     "gather_max_fwd: size too large");
+    // the channels-last kernel takes 8 queries per block in grid.x (at most 2^31 - 1 blocks)
+    FFB6D_CHECK_ARG(layout != FFB6D_LAYOUT_NSC || B * Q <= 8ll * 0x7fffffff,
+                    "gather_max_fwd: B*Q=%lld too large for the channels-last layout", (long long)(B * Q));
     if (B == 0 || C == 0 || Q == 0) return FFB6D_OK;
     FFB6D_CHECK_ARG(S > 0, "gather_max_fwd: empty source with non-empty index");
     FFB6D_CHECK_ARG(feat && idx && out, "gather_max_fwd: null pointer");

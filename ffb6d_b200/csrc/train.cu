@@ -22,6 +22,8 @@
 namespace ffb6d {
 
 constexpr int BN_THREADS = 256;
+// The BatchNorm kernels walk a row with unsigned positions: P < 2^31, a chunk <= 2^31 and a stride <= 65536 keep
+// p0 + chunk and p + stride below 2^32, where an int overflows for P within one stride of 2^31.
 
 __device__ __forceinline__ double block_sum(double v, double *red)
 {
@@ -40,25 +42,25 @@ __device__ __forceinline__ double block_sum(double v, double *red)
 // The shift keeps the one-pass variance Q/n - (A/n)^2 free of cancellation when a channel's |mean| is
 // large next to its spread: the terms are O(std), not O(|mean|), and a constant channel sums to exactly 0.
 __global__ void __launch_bounds__(BN_THREADS)
-bn_stats_kernel(const float *__restrict__ z, int B, int C, int P, int chunk, int nsplit, double *__restrict__ partial)
+bn_stats_kernel(const float *__restrict__ z, int B, int C, int P, unsigned chunk, int nsplit, double *__restrict__ partial)
 {
     __shared__ double red[BN_THREADS / 32];
     const int c = blockIdx.y, s = blockIdx.x;
-    const int p0 = s * chunk, p1 = min(P, p0 + chunk);
+    const unsigned p0 = s * chunk, p1 = min((unsigned)P, p0 + chunk);
     const float k = __ldg(z + (size_t)c * P);
     float a = 0.f, q = 0.f;
     const bool vec = ((P & 3) == 0) && ((chunk & 3) == 0) && ((reinterpret_cast<uintptr_t>(z) & 15) == 0);
     for (int b = 0; b < B; ++b) {
         const float *row = z + ((size_t)b * C + c) * P;
         if (vec) {
-            for (int p = p0 + 4 * threadIdx.x; p < p1; p += 4 * BN_THREADS) {
+            for (unsigned p = p0 + 4 * threadIdx.x; p < p1; p += 4 * BN_THREADS) {
                 float4 v = __ldg(reinterpret_cast<const float4 *>(row + p));
                 v.x -= k; v.y -= k; v.z -= k; v.w -= k;
                 a += (v.x + v.y) + (v.z + v.w);
                 q += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
             }
         } else {
-            for (int p = p0 + threadIdx.x; p < p1; p += BN_THREADS) {
+            for (unsigned p = p0 + threadIdx.x; p < p1; p += BN_THREADS) {
                 const float v = __ldg(row + p) - k;
                 a += v;
                 q += v * v;
@@ -117,7 +119,7 @@ bn_apply_kernel(const float *__restrict__ z, const float4 *__restrict__ stats, i
     float *dst = y + row * P;
     const bool vec = ((P & 3) == 0) && ((reinterpret_cast<uintptr_t>(z) & 15) == 0) && ((reinterpret_cast<uintptr_t>(y) & 15) == 0);
     if (vec) {
-        for (int p = 4 * (blockIdx.y * BN_THREADS + threadIdx.x); p < P; p += 4 * BN_THREADS * gridDim.y) {
+        for (unsigned p = 4 * (blockIdx.y * BN_THREADS + threadIdx.x); p < (unsigned)P; p += 4 * BN_THREADS * gridDim.y) {
             float4 v = __ldg(reinterpret_cast<const float4 *>(src + p));
             v.x = act_fwd(__fmaf_rn(v.x - st.x, st.z, st.w), act, slope);
             v.y = act_fwd(__fmaf_rn(v.y - st.x, st.z, st.w), act, slope);
@@ -126,7 +128,7 @@ bn_apply_kernel(const float *__restrict__ z, const float4 *__restrict__ stats, i
             *reinterpret_cast<float4 *>(dst + p) = v;
         }
     } else {
-        for (int p = blockIdx.y * BN_THREADS + threadIdx.x; p < P; p += BN_THREADS * gridDim.y)
+        for (unsigned p = blockIdx.y * BN_THREADS + threadIdx.x; p < (unsigned)P; p += BN_THREADS * gridDim.y)
             dst[p] = act_fwd(__fmaf_rn(__ldg(src + p) - st.x, st.z, st.w), act, slope);
     }
 }
@@ -141,16 +143,16 @@ __device__ __forceinline__ float act_grad(float g, float ypre, int act, float sl
 // partial[c][s] = (sum g', sum g' * xhat) over all frames of chunk s
 __global__ void __launch_bounds__(BN_THREADS)
 bn_bwd_reduce_kernel(const float *__restrict__ z, const float *__restrict__ g, const float4 *__restrict__ stats, int B, int C,
-                     int P, int chunk, int nsplit, int act, float slope, double *__restrict__ partial)
+                     int P, unsigned chunk, int nsplit, int act, float slope, double *__restrict__ partial)
 {
     __shared__ double red[BN_THREADS / 32];
     const int c = blockIdx.y, s = blockIdx.x;
-    const int p0 = s * chunk, p1 = min(P, p0 + chunk);
+    const unsigned p0 = s * chunk, p1 = min((unsigned)P, p0 + chunk);
     const float4 st = stats[c];
     float a = 0.f, q = 0.f;
     for (int b = 0; b < B; ++b) {
         const float *zr = z + ((size_t)b * C + c) * P, *gr = g + ((size_t)b * C + c) * P;
-        for (int p = p0 + threadIdx.x; p < p1; p += BN_THREADS) {
+        for (unsigned p = p0 + threadIdx.x; p < p1; p += BN_THREADS) {
             const float d = __ldg(zr + p) - st.x;
             const float gp = act_grad(__ldg(gr + p), __fmaf_rn(d, st.z, st.w), act, slope);
             a += gp;
@@ -193,7 +195,7 @@ bn_bwd_apply_kernel(const float *__restrict__ z, const float *__restrict__ g, co
     const float mb = sm.x * inv_n, mg = sm.y * inv_n;
     const float *zr = z + row * P, *gr = g + row * P;
     float *dr = dz + row * P;
-    for (int p = blockIdx.y * BN_THREADS + threadIdx.x; p < P; p += BN_THREADS * gridDim.y) {
+    for (unsigned p = blockIdx.y * BN_THREADS + threadIdx.x; p < (unsigned)P; p += BN_THREADS * gridDim.y) {
         const float d = __ldg(zr + p) - st.x;
         const float gp = act_grad(__ldg(gr + p), __fmaf_rn(d, st.z, st.w), act, slope);
         dr[p] = st.z * (gp - mb - (d * st.y) * mg);
@@ -454,13 +456,13 @@ wgrad_small_det_kernel(const float *__restrict__ dz, const float *__restrict__ x
     wgrad_small_body<T, true>(dz, x1, C1, x2, C2, part, Co, P, B, slabs_per_cta);
 }
 
-static void split_plan(int64_t C, int64_t P, int &chunk, int &nsplit)
+static void split_plan(int64_t C, int64_t P, unsigned &chunk, int &nsplit)
 {
     // enough CTAs to fill the machine twice, chunks of whole 1024-element strides
     int64_t want = std::max<int64_t>(1, ceil_div(2 * (int64_t)num_sms(), C));
     int64_t ch = ceil_div(ceil_div(P, want), 1024) * 1024;
     if (ch < 1024) ch = 1024;
-    chunk = (int)ch;
+    chunk = (unsigned)ch;
     nsplit = (int)ceil_div(P, ch);
 }
 
@@ -520,7 +522,8 @@ extern "C" {
 size_t ffb6d_bn_workspace_bytes(int64_t C, int64_t P)
 {
     if (C < 1 || P < 1) return 0;
-    int chunk, nsplit;
+    unsigned chunk;
+    int nsplit;
     split_plan(C, P, chunk, nsplit);
     return align_up((size_t)C * nsplit * 2 * sizeof(double), 256) + align_up((size_t)C * sizeof(float2), 256);
 }
@@ -536,7 +539,8 @@ int ffb6d_bn_train_fwd(const float *z, int64_t B, int64_t C, int64_t P, const fl
     FFB6D_CHECK_ARG((reinterpret_cast<uintptr_t>(stats) & 15) == 0, "bn_train_fwd: stats must be 16-byte aligned");
     FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_train_fwd: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    int chunk, nsplit;
+    unsigned chunk;
+    int nsplit;
     split_plan(C, P, chunk, nsplit);
     double *partial = (double *)workspace;
     bn_stats_kernel<<<dim3((unsigned)nsplit, (unsigned)C), BN_THREADS, 0, st>>>(z, (int)B, (int)C, (int)P, chunk, nsplit, partial);
@@ -563,7 +567,8 @@ int ffb6d_bn_train_bwd(const float *z, const float *grad_y, const float *stats, 
     FFB6D_CHECK_ARG((reinterpret_cast<uintptr_t>(stats) & 15) == 0, "bn_train_bwd: stats must be 16-byte aligned");
     FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_train_bwd: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    int chunk, nsplit;
+    unsigned chunk;
+    int nsplit;
     split_plan(C, P, chunk, nsplit);
     double *partial = (double *)workspace;
     float2 *sums = (float2 *)((char *)workspace + align_up((size_t)C * nsplit * 2 * sizeof(double), 256));
@@ -593,7 +598,8 @@ int ffb6d_bn_sync_moments(const float *z, int64_t B, int64_t C, int64_t P, doubl
     FFB6D_CHECK_ARG(FFB6D_ALIGNED(moments, 8), "bn_sync_moments: moments must be 8-byte aligned");
     FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_sync_moments: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    int chunk, nsplit;
+    unsigned chunk;
+    int nsplit;
     split_plan(C, P, chunk, nsplit);
     double *partial = (double *)workspace;
     bn_stats_kernel<<<dim3((unsigned)nsplit, (unsigned)C), BN_THREADS, 0, st>>>(z, (int)B, (int)C, (int)P, chunk, nsplit, partial);
@@ -638,7 +644,8 @@ int ffb6d_bn_sync_bwd_sums(const float *z, const float *grad_y, const float *sta
     FFB6D_CHECK_ARG(FFB6D_ALIGNED(sums, 8), "bn_sync_bwd_sums: sums must be 8-byte aligned");
     FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_sync_bwd_sums: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    int chunk, nsplit;
+    unsigned chunk;
+    int nsplit;
     split_plan(C, P, chunk, nsplit);
     double *partial = (double *)workspace;
     bn_bwd_reduce_kernel<<<dim3((unsigned)nsplit, (unsigned)C), BN_THREADS, 0, st>>>(
@@ -663,7 +670,8 @@ int ffb6d_bn_sync_bwd(const float *z, const float *grad_y, const float *stats, i
                     "bn_sync_bwd: gathered and count must be 8-byte aligned");
     FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_bn_workspace_bytes(C, P), "bn_sync_bwd: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    int chunk, nsplit;
+    unsigned chunk;
+    int nsplit;
     split_plan(C, P, chunk, nsplit);
     float2 *sums = (float2 *)((char *)workspace + align_up((size_t)C * nsplit * 2 * sizeof(double), 256));
     bn_sync_bwd_combine_kernel<<<(unsigned)ceil_div(C, BN_THREADS), BN_THREADS, 0, st>>>(gathered, (int)W, (int)C, count,

@@ -164,6 +164,7 @@ int ffb6d_knn_host(const float *points, size_t npts, size_t dim,
  * (models/ffb6d.py:309-312).  Pure selection: results are bitwise equal to the
  * reference (NaN propagates like torch.max).
  *   feat [B,C,S] f32 in `layout`, idx [B,Q,K] -> out [B,C,Q] f32 in `layout`.
+ * B < 65536, C <= 65535*8, S, Q < 2^31; with FFB6D_LAYOUT_NSC also B*Q <= 8*(2^31 - 1).
  * Indices must lie in [0,S).  The forward kernels do not check them (an offender reads a stale or
  * foreign element where torch.gather raises a device assert); the backward kernels skip offenders.
  * Debugging aid: ffb6d_check_indices below, or FFB6D_CHECK_INDICES=1 in the environment, which runs
@@ -555,7 +556,7 @@ int ffb6d_grid_subsample_host(const float *points, size_t N,
  *   where back_labels <= 0 (YCB) or back_labels[...,0] < 255 (LineMOD).  labels [B,H,W] u8, back_labels
  *   [B,H,W,back_label_channels] u8 (1 or 3), dpt / back_dpt / dpt_out [B,H,W] u16.  Outputs may equal inputs.
  * ffb6d_aug_noise_field: out [B,H,W,3] f64 = the normals ffb6d_rgb_add_noise draws for (seed, frame, stage).
- * All three need H, W >= 32, check sizes and null pointers before any launch (FFB6D_ERR_INVALID), allocate nothing and
+ * All three need 0 <= B < 65536, 32 <= H <= 524280 (65535 tiles of 8 rows), 32 <= W < 2^20 and H*W*3 < 2^31, check sizes and null pointers before any launch (FFB6D_ERR_INVALID), allocate nothing and
  * do not synchronise the host (capturable in a CUDA graph); they are deterministic.
  */
 #define FFB6D_AUG_VERSION 1

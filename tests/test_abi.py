@@ -54,6 +54,11 @@ def test_argument_validation_needs_no_gpu():
     assert lib.ffb6d_gather_max_fwd(p, o, 1, 1, 1, 1, 1, 1, 7, p, None) == _lib.ERR_INVALID  # layout
     assert lib.ffb6d_gather_max_fwd(p, o, 1, 1, 1, 0, 1, 1, 0, p, None) == _lib.ERR_INVALID  # S == 0
     assert lib.ffb6d_gather_max_fwd(p, o, 1, 0, 1, 1, 1, 1, 0, p, None) == _lib.OK          # B == 0
+    # channels-last: 8 queries per block in grid.x, so B*Q <= 8 * (2^31 - 1); NCS has no such bound
+    q = (1 << 31) - 1
+    assert lib.ffb6d_gather_max_fwd(p, o, 1, 9, 1, 1, q, 1, 1, p, None) == _lib.ERR_INVALID
+    assert "too large for the channels-last layout" in _lib.last_error()
+    assert lib.ffb6d_gather_max_fwd(p, o, 1, 0, 1, 1, q, 1, 1, p, None) == _lib.OK          # B*Q == 0
     assert lib.ffb6d_gather_neighbour_fwd(None, o, 1, 1, 1, 1, 1, 1, p, None) == _lib.ERR_INVALID
     assert lib.ffb6d_knn_workspace_bytes(1, 0, 1, 1) == 0
 

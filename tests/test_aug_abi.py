@@ -29,9 +29,12 @@ def noise_call(plan=None, **kw):
 
 
 @pytest.mark.parametrize("kw", [dict(B=-1), dict(B=65536), dict(H=31), dict(W=31), dict(H=1 << 16, W=1 << 15),
-                                dict(H=1 << 40, W=1 << 40), dict(H=3 << 61, W=4)])
+                                dict(H=1 << 40, W=1 << 40), dict(H=3 << 61, W=4), dict(H=65535 * 8 + 1, W=32),
+                                dict(H=600000, W=32)])
 def test_bad_sizes(kw):
     assert noise_call(**kw) == _lib.ERR_INVALID and "bad size" in _lib.last_error()
+    if kw.get("H", H) > 65535 * 8 and kw.get("W", W) == 32:     # rows the filters' grid.y cannot hold
+        assert "H <= 524280" in _lib.last_error()
     assert _lib.lib.ffb6d_aug_noise_field(1, kw.get("B", B), kw.get("H", H), kw.get("W", W), 0, P, None) \
         == _lib.ERR_INVALID
 
