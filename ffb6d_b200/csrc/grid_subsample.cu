@@ -3,8 +3,9 @@
 // Replaces grid_subsampling() (GS/cpp_subsampling/grid_subsampling/grid_subsampling.cpp:5-106),
 // which walks the cloud once and accumulates per-voxel sums in an unordered_map.  The GPU
 // version keeps the reference's arithmetic bit for bit:
-//   1. min/max of the cloud (reduction)            -> origin, NX, NY exactly as :27-31
-//   2. voxel key per point, same fp32 expression   -> key = iX + NX*iY + NX*NY*iZ   (:53-56)
+//   1. min/max of the cloud (reduction) by min_point / max_point's rule  -> origin, NX, NY exactly as :27-31
+//   2. voxel key per point, same fp32 expression   -> key = iX + NX*iY + NX*NY*iZ   (:53-56), with
+//      `(size_t)` of a float converted as x86-64 code converts it (x86_size_t), mod 2^64
 //   3. STABLE radix sort of (key, point index)     -> each voxel's points contiguous and still in
 //                                                     input order (cub::DeviceRadixSort, the
 //                                                     toolkit's library sort: this op is not on
@@ -23,41 +24,62 @@
 
 namespace ffb6d {
 
+// `(size_t)f` as x86-64 code computes it, which is what the reference's `(size_t)floor(...)` gives
+// (grid_subsampling.cpp:30-31, 53-55): below 2^63 a signed cvttss2si, so an index of -1 wraps to 2^64 - 1;
+// from 2^63 up, cvttss2si(f - 2^63) with the top bit flipped.  cvttss2si returns 2^63 for NaN and for values
+// outside [-2^63, 2^63), so NaN and -inf give 2^63, +inf and values >= 2^64 give 0.  A C cast is undefined
+// there, and the GPU's conversion saturates instead (-1 to 0, +inf to 2^64 - 1).
+__host__ __device__ inline unsigned long long x86_size_t(float f)
+{
+    const float two63 = 9223372036854775808.f;
+    const unsigned long long top = 1ull << 63;
+    const bool high = f >= two63;
+    const float g = high ? f - two63 : f;
+    const unsigned long long s = (g >= -two63 && g < two63) ? (unsigned long long)(long long)g : top;
+    return high ? s ^ top : s;
+}
+
+// Rank of point i as a candidate limit: the smallest rank is min_point's choice (descending = false) or
+// max_point's (true).  Equal values (+0 and -0) rank by index, NaN ranks last.
+__device__ __forceinline__ unsigned long long gs_limit_rank(float v, bool descending, unsigned int i)
+{
+    if (v != v) return ~0ull;
+    unsigned int u = __float_as_uint(v == 0.f ? 0.f : v);
+    u ^= (u & 0x80000000u) ? 0xffffffffu : 0x80000000u;   // monotone in v
+    if (descending) u = ~u;
+    return ((unsigned long long)u << 32) | i;
+}
+
 __global__ void __launch_bounds__(1024)
 gs_minmax_kernel(const float *__restrict__ pts, size_t N, float *__restrict__ out6)
 {
-    // single CTA: N is a pre-processing sized cloud, the reduction is not the bottleneck
-    const float INF = __int_as_float(0x7f800000);
-    float mn[3] = {INF, INF, INF}, mx[3] = {-INF, -INF, -INF};
+    // min_point / max_point (cloud.cpp:27-67) start from point 0 and replace on a strict '<' / '>': a NaN at
+    // point 0 stays the limit, later NaNs are never taken, and of equal values the first in input order wins.
+    // Single CTA: N is a pre-processing sized cloud, the reduction is not the bottleneck.
+    unsigned long long best[6] = {~0ull, ~0ull, ~0ull, ~0ull, ~0ull, ~0ull};
     for (size_t i = threadIdx.x; i < N; i += blockDim.x) {
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
             const float v = pts[3 * i + a];
-            // the reference compares with '<' / '>' starting from point 0 (cloud.cpp:27-67)
-            mn[a] = v < mn[a] ? v : mn[a];
-            mx[a] = v > mx[a] ? v : mx[a];
+            best[a] = min(best[a], gs_limit_rank(v, false, (unsigned int)i));
+            best[3 + a] = min(best[3 + a], gs_limit_rank(v, true, (unsigned int)i));
         }
     }
-    __shared__ float red[6][32];
+    __shared__ unsigned long long red[6][32];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
+    for (int c = 0; c < 6; ++c) {
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-            mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
-        }
-        if (lane == 0) {
-            red[a][wid] = mn[a];
-            red[3 + a][wid] = mx[a];
-        }
+        for (int o = 16; o > 0; o >>= 1) best[c] = min(best[c], __shfl_xor_sync(0xffffffffu, best[c], o));
+        if (lane == 0) red[c][wid] = best[c];
     }
     __syncthreads();
     if (threadIdx.x < 6) {
-        float v = red[threadIdx.x][0];
-        for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
-            v = threadIdx.x < 3 ? fminf(v, red[threadIdx.x][w]) : fmaxf(v, red[threadIdx.x][w]);
-        out6[threadIdx.x] = v;
+        unsigned long long r = red[threadIdx.x][0];
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) r = min(r, red[threadIdx.x][w]);
+        const int a = threadIdx.x % 3;
+        const float p0 = pts[a];
+        out6[threadIdx.x] = p0 != p0 ? p0 : pts[3 * (r & 0xffffffffu) + a];
     }
 }
 
@@ -69,10 +91,10 @@ gs_key_kernel(const float *__restrict__ pts, size_t N, float ox, float oy, float
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
     // (size_t)floor((p.x - origin.x) / sampleDl), fp32, IEEE division      (:53-55)
-    const unsigned long long iX = (unsigned long long)floorf(__fdiv_rn(__fsub_rn(pts[3 * i + 0], ox), dl));
-    const unsigned long long iY = (unsigned long long)floorf(__fdiv_rn(__fsub_rn(pts[3 * i + 1], oy), dl));
-    const unsigned long long iZ = (unsigned long long)floorf(__fdiv_rn(__fsub_rn(pts[3 * i + 2], oz), dl));
-    keys[i] = iX + NX * iY + NX * NY * iZ;
+    const unsigned long long iX = x86_size_t(floorf(__fdiv_rn(__fsub_rn(pts[3 * i + 0], ox), dl)));
+    const unsigned long long iY = x86_size_t(floorf(__fdiv_rn(__fsub_rn(pts[3 * i + 1], oy), dl)));
+    const unsigned long long iZ = x86_size_t(floorf(__fdiv_rn(__fsub_rn(pts[3 * i + 2], oz), dl)));
+    keys[i] = iX + NX * iY + NX * NY * iZ;   // wraps mod 2^64 like the reference's size_t
     order[i] = (unsigned int)i;
 }
 
@@ -220,8 +242,8 @@ extern "C" int ffb6d_grid_subsample_host(const float *points, size_t N, const fl
         org[a] = f * sampleDl;
     }
     volatile float ex = (mm[3] - org[0]) / sampleDl, ey = (mm[4] - org[1]) / sampleDl;
-    const unsigned long long NX = (unsigned long long)floorf(ex) + 1;
-    const unsigned long long NY = (unsigned long long)floorf(ey) + 1;
+    const unsigned long long NX = x86_size_t(floorf(ex)) + 1;
+    const unsigned long long NY = x86_size_t(floorf(ey)) + 1;
 
     // 2. keys, 3. stable sort by key
     FFB6D_CUDA(d_keys.alloc(N * 8));
