@@ -91,6 +91,9 @@ def _load():
         "ffb6d_att_pool_bwd": (ci, [vp, i64, vp, i64, vp, vp, i64, i64, ci, vp, vp, vp, vp]),
         "ffb6d_lfa_att_pool_fused": (ci, [vp, vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i64, ci, i64, i64, fp, vp, vp]),
         "ffb6d_att_pool_fwd": (ci, [vp, i64, vp, i64, vp, i64, i64, ci, vp, vp]),
+        "ffb6d_lfa_train_fwd": (ci, [vp, vp, ci, vp, vp, i64, i64, ci, i64, vp, vp]),
+        "ffb6d_lfa_train_bwd_workspace_bytes": (sz, [i64, i64, ci, i64]),
+        "ffb6d_lfa_train_bwd": (ci, [vp, vp, ci, vp, vp, vp, i64, i64, ci, i64, vp, vp, vp, vp, sz, vp]),
         "ffb6d_relative_pos_encoding_cm_fwd": (ci, [vp, vp, ci, i64, i64, ci, vp, vp]),
         "ffb6d_backproject": (ci, [vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp, vp, vp]),
         "ffb6d_point_item": (ci, [vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp, vp,

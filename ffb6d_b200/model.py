@@ -40,14 +40,21 @@ def _head(in_c, out_c):
 
 
 class FFB6DFusionNet(nn.Module):
-    def __init__(self, n_classes=2, n_pts=12288, n_kps=8, in_c=9, d_out=(32, 64, 128, 256), restructured=False):
+    def __init__(self, n_classes=2, n_pts=12288, n_kps=8, in_c=9, d_out=(32, 64, 128, 256), restructured=False,
+                 fused_lfa=False):
         """``restructured``: run the pixel branch of every fusion as ``W1 . rgb + (W2 . p2r)[idx]``
         (:meth:`ffb6d_b200.modules.Conv2d.forward_interp`) instead of the reference's order of operations; the
         interpolated maps are never built.  A plain attribute: it can be switched on a built or loaded model, and
-        the state dict is the same either way."""
+        the state dict is the same either way.
+
+        ``fused_lfa``: when the encoder's ``Dilated_res_block`` s run under autograd or in training mode, the gather,
+        ``fc`` and softmax pooling of each attentive pooling whose shape the fused kernels cover (K = 16, d/2 in
+        {16, 32, 64}: encoder levels 0-2) run on them (:meth:`ffb6d_b200.modules.Building_block.forward`, DESIGN.md
+        §4.19).  A plain attribute like ``restructured``; off by default."""
         super().__init__()
         self.n_cls, self.n_pts, self.n_kps = n_classes, n_pts, n_kps
         self.restructured = bool(restructured)
+        self.fused_lfa = bool(fused_lfa)
         # RandLA branch (models/RandLA/RandLANet.py:12-38)
         self.rndla_pre_stages = RandLAConv1d(in_c, 8, kernel_size=1, bn=True)
         self.rndla_ds_stages = nn.ModuleList()
@@ -114,7 +121,8 @@ class FFB6DFusionNet(nn.Module):
         ds_emb, fused_rgb = [], []
         for i in range(4):
             rgb_emb0 = rgb_stage(i, rgb_emb)
-            f_enc = self.rndla_ds_stages[i](p_emb, inputs["cld_xyz%d" % i], inputs["cld_nei_idx%d" % i])
+            f_enc = self.rndla_ds_stages[i](p_emb, inputs["cld_xyz%d" % i], inputs["cld_nei_idx%d" % i],
+                                            fused_lfa=self.fused_lfa)
             p_emb0 = ops.random_sample(f_enc, inputs["cld_sub_idx%d" % i])
             if i == 0:
                 ds_emb.append(f_enc)
@@ -179,10 +187,12 @@ class FFB6D(FFB6DFusionNet):
       whose backwards are this package's kernels (DESIGN.md §4.18).  Their backwards add in a fixed order, so the
       whole network trains under ``torch.use_deterministic_algorithms(True)``, where torch's adaptive-average-pool
       and bilinear-upsampling backwards raise.  The trunk, the 3x3 convs, BatchNorms and PReLUs of ``PSPUpsample``
-      and the dropouts stay torch modules (the CUDA RNG is drawn as on the torch path).  Off by default."""
+      and the dropouts stay torch modules (the CUDA RNG is drawn as on the torch path).  Off by default.
+    * ``fused_lfa``: as :class:`FFB6DFusionNet`."""
 
-    def __init__(self, n_classes, n_pts=12288, n_kps=8, restructured=False, fused_image_head=False):
-        super().__init__(n_classes=n_classes, n_pts=n_pts, n_kps=n_kps, restructured=restructured)
+    def __init__(self, n_classes, n_pts=12288, n_kps=8, restructured=False, fused_image_head=False, fused_lfa=False):
+        super().__init__(n_classes=n_classes, n_pts=n_pts, n_kps=n_kps, restructured=restructured,
+                         fused_lfa=fused_lfa)
         self.cnn_pre_stages, self.cnn_ds_stages, self.cnn_up_stages = cnn.image_branch()
         self.fused_image_head = bool(fused_image_head)
 

@@ -509,6 +509,27 @@ class _AttPool(torch.autograd.Function):
         return gf1, gf2, gatt
 
 
+class _LfaAttPool(torch.autograd.Function):
+    """``sum_k x_k * softmax_k(W_fc . x_k)``, ``x_k = cat(feature[idx[n, k]], f_xyz[:, n, k])``: the gather, ``fc`` and
+    softmax pooling of an ``Att_pooling`` on the fused training kernels (:func:`ffb6d_b200.ops.lfa_train_fwd`).  Saves
+    only its inputs; the backward recomputes the gathered rows, the logits and the softmax."""
+
+    @staticmethod
+    def forward(ctx, feature, neigh_idx, f_xyz, w_fc):
+        out = ops.lfa_train_fwd(feature, neigh_idx, f_xyz, w_fc)
+        ctx.save_for_backward(feature, neigh_idx, f_xyz, w_fc)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gout):
+        feature, neigh_idx, f_xyz, w_fc = ctx.saved_tensors
+        gf, gx, gw = ops.lfa_train_bwd(feature, neigh_idx, f_xyz, w_fc, gout, need_feature=ctx.needs_input_grad[0])
+        if gf is not None:
+            gf = gf.reshape(feature.shape)
+        return gf, None, gx, gw
+
+
 def _gather_cm(feature, neigh_idx):
     """feature [B,C,N,1] -> neighbours channel-major [B,C,N,K]: ``gather_neighbour`` + ``permute(0,3,1,2)``
     (RandLANet.py:200-203) as one K = 1 gather (differentiable)."""
@@ -545,9 +566,21 @@ class Att_pooling(nn.Module):
             f_agg = ops.att_pool(feature_set, f2, att)
         return self.mlp(f_agg)
 
+    def forward_gathered(self, feature, neigh_idx, f_xyz):
+        """``forward(gather(feature, neigh_idx), f_xyz)`` with the gather, ``fc`` and the softmax pooling on the
+        fused training kernels (:class:`_LfaAttPool`): neither the gathered neighbours nor the logits are kept for
+        the backward.  ``feature [B,d/2,N,1]``, ``neigh_idx [B,N,16]``, ``f_xyz [B,d/2,N,16]``, d/2 in {16, 32, 64}."""
+        return self.mlp(_LfaAttPool.apply(feature, neigh_idx, f_xyz, self.fc.weight))
+
 
 class Building_block(nn.Module):
-    """models/RandLA/RandLANet.py:187-214 (local spatial encoding + two attentive poolings)."""
+    """models/RandLA/RandLANet.py:187-214 (local spatial encoding + two attentive poolings).
+
+    ``fused_lfa`` (a plain attribute, off by default; ``forward(..., fused_lfa=...)`` overrides it for one call): with
+    K = 16 and d/2 in {16, 32, 64}, each attentive pooling's gather, ``fc`` and softmax pooling run on the fused
+    training kernels (:meth:`Att_pooling.forward_gathered`), which keep neither the gathered neighbours nor the logits
+    for the backward.  ``mlp1``, ``mlp2`` and each pooling's ``mlp`` stay the same layers.  Other shapes take the
+    per-op path."""
 
     def __init__(self, d_out):
         super().__init__()
@@ -555,10 +588,19 @@ class Building_block(nn.Module):
         self.att_pooling_1 = Att_pooling(d_out, d_out // 2)
         self.mlp2 = RandLAConv2d(d_out // 2, d_out // 2, kernel_size=(1, 1), bn=True)
         self.att_pooling_2 = Att_pooling(d_out, d_out)
+        self.fused_lfa = False
 
-    def forward(self, xyz, feature, neigh_idx):
+    def _fusable(self, feature, neigh_idx):
+        d = self.att_pooling_1.fc.weight.shape[0]
+        return feature.dim() == 4 and feature.shape[1] * 2 == d and ops.lfa_fusable(feature.shape[1], neigh_idx.shape[2])
+
+    def forward(self, xyz, feature, neigh_idx, fused_lfa=None):
         f_xyz = ops.relative_pos_encoding(xyz, neigh_idx, channel_major=True)     # [B,10,N,K]
         f_xyz = self.mlp1(f_xyz)
+        if (self.fused_lfa if fused_lfa is None else fused_lfa) and self._fusable(feature, neigh_idx):
+            f_pc_agg = self.att_pooling_1.forward_gathered(feature, neigh_idx, f_xyz)
+            f_xyz = self.mlp2(f_xyz)
+            return self.att_pooling_2.forward_gathered(f_pc_agg, neigh_idx, f_xyz)
         f_pc_agg = self.att_pooling_1(_gather_cm(feature, neigh_idx), f_xyz)
         f_xyz = self.mlp2(f_xyz)
         return self.att_pooling_2(_gather_cm(f_pc_agg, neigh_idx), f_xyz)
@@ -577,12 +619,13 @@ class Dilated_res_block(nn.Module):
         self.mlp2 = RandLAConv2d(d_out, d_out * 2, kernel_size=(1, 1), bn=True, activation=None)
         self.shortcut = RandLAConv2d(d_in, d_out * 2, kernel_size=(1, 1), bn=True, activation=None)
 
-    def forward(self, feature, xyz, neigh_idx):
+    def forward(self, feature, xyz, neigh_idx, fused_lfa=None):
+        """``fused_lfa``: passed to :meth:`Building_block.forward` (None: ``self.lfa.fused_lfa``)."""
         if not self.training and not torch.is_grad_enabled():
             from . import randla
             return randla.dilated_res_block(self.state_dict(), "", feature, xyz, neigh_idx)   # fused residual GEMM
         f_pc = self.mlp1(feature)
-        f_pc = self.lfa(xyz, f_pc, neigh_idx)
+        f_pc = self.lfa(xyz, f_pc, neigh_idx, fused_lfa=fused_lfa)
         f_pc = self.mlp2(f_pc)
         shortcut = self.shortcut(feature)
         return F_.leaky_relu(f_pc + shortcut, negative_slope=0.2)

@@ -658,8 +658,79 @@ def lfa_att_pool_fused(xyz, neigh_idx, feature, mlp1, mlp2, fc_weight, mlp_out, 
 
 
 def lfa_fusable(d_half, k):
-    """True when :func:`lfa_att_pool_fused` covers this width / neighbour count."""
+    """True when :func:`lfa_att_pool_fused` (and the training kernels of :func:`lfa_train_fwd`) cover this width /
+    neighbour count."""
     return int(k) == 16 and int(d_half) in (16, 32, 64)
+
+
+def _lfa_train_args(feature, neigh_idx, f_xyz, w_fc):
+    """Shapes first (so that a mismatch reads as one on any device), then the device: dense float32 CUDA tensors
+    ``feature [B,Dh,N]``, ``idx [B,N,K]``, ``f_xyz [B,Dh,N,K]``, ``w_fc [2Dh,2Dh]``."""
+    if feature.dim() == 4 and feature.shape[3] == 1:
+        feature = feature.squeeze(3)
+    if feature.dim() != 3:
+        raise ValueError("feature must be [B,d/2,N,1] or [B,d/2,N], got %s" % (tuple(feature.shape),))
+    B, Dh, N = feature.shape
+    if neigh_idx.dim() != 3 or tuple(neigh_idx.shape[:2]) != (B, N):
+        raise ValueError("neigh_idx must be [B,N,K] = [%d,%d,K], got %s" % (B, N, tuple(neigh_idx.shape)))
+    K = neigh_idx.shape[2]
+    if tuple(f_xyz.shape) != (B, Dh, N, K):
+        raise ValueError("f_xyz must be [B,d/2,N,K] = %s, got %s" % ((B, Dh, N, K), tuple(f_xyz.shape)))
+    w = w_fc.reshape(w_fc.shape[0], -1)
+    if tuple(w.shape) != (2 * Dh, 2 * Dh):
+        raise ValueError("w_fc must be [d,d] = [%d,%d], got %s" % (2 * Dh, 2 * Dh, tuple(w_fc.shape)))
+    for t, name in ((feature, "feature"), (neigh_idx, "neigh_idx"), (f_xyz, "f_xyz"), (w_fc, "w_fc")):
+        _need_cuda(t, name)
+    for t, name in ((feature, "feature"), (f_xyz, "f_xyz"), (w_fc, "w_fc")):
+        if t.dtype != torch.float32:
+            raise TypeError("%s must be float32, got %s" % (name, t.dtype))
+    idx_c, i64 = _idx_arg(neigh_idx, "neigh_idx")
+    return feature.contiguous(), idx_c, i64, f_xyz.contiguous(), w.contiguous(), (B, N, K, Dh)
+
+
+def lfa_train_fwd(feature, neigh_idx, f_xyz, w_fc):
+    """The attentive pooling of a ``Building_block`` on its gathered neighbours, in training (``ffb6d_lfa_train_fwd``):
+    ``f_agg = sum_k x_k * softmax_k(w_fc . x_k)`` with ``x_k = cat(feature[:, idx[n, k]], f_xyz[:, n, k])``
+    (models/RandLA/RandLANet.py:200-212, 243-248), without materialising the gathered neighbours or the logits.
+
+    :param feature: ``[B,d/2,N,1]`` (or ``[B,d/2,N]``); :param neigh_idx: ``[B,N,16]`` int32 / int64
+    :param f_xyz: ``[B,d/2,N,16]``; :param w_fc: ``Att_pooling.fc.weight`` ``[d,d,1,1]`` (or ``[d,d]``)
+    :return: ``f_agg [B,d,N,1]``.  K = 16 and d/2 in {16, 32, 64} (:func:`lfa_fusable`); other shapes raise."""
+    f, idx_c, i64, fx, w, (B, N, K, Dh) = _lfa_train_args(feature, neigh_idx, f_xyz, w_fc)
+    out = torch.empty((B, 2 * Dh, N, 1), dtype=torch.float32, device=f.device)
+    with torch.cuda.device(f.device):
+        check(lib.ffb6d_lfa_train_fwd(f.data_ptr(), idx_c.data_ptr(), i64, fx.data_ptr(), w.data_ptr(), B, N, K, Dh,
+                                      out.data_ptr(), _stream(f.device)))
+    return out
+
+
+def lfa_train_bwd(feature, neigh_idx, f_xyz, w_fc, grad_agg, need_feature=True):
+    """Backward of :func:`lfa_train_fwd` (``ffb6d_lfa_train_bwd``), recomputing the gathered rows, the logits and the
+    softmax from the inputs.  Returns ``(grad_feature [B,d/2,N,1] or None, grad_f_xyz [B,d/2,N,16], grad_w_fc [d,d])``.
+
+    The feature half of the gradient comes out of the kernel per edge, ``[B,d/2,N*16]``, the gradient of the per-op
+    path's K = 1 neighbour gather, and is scattered onto the points by that gather's own backward
+    (:func:`_gather_max_bwd`): fp32 atomics by default, a segment sum under :func:`deterministic_backward`.  The edge
+    buffer lives only for this call.  ``grad_w_fc`` is summed without atomics in a fixed order in both modes."""
+    f, idx_c, i64, fx, w, (B, N, K, Dh) = _lfa_train_args(feature, neigh_idx, f_xyz, w_fc)
+    if tuple(grad_agg.shape) not in ((B, 2 * Dh, N, 1), (B, 2 * Dh, N)):
+        raise ValueError("grad_agg must be [B,d,N,1] = %s, got %s" % ((B, 2 * Dh, N, 1), tuple(grad_agg.shape)))
+    g = grad_agg.contiguous().float()
+    dev = f.device
+    edge = torch.empty((B, Dh, N * K), dtype=torch.float32, device=dev)
+    gx = torch.empty((B, Dh, N, K), dtype=torch.float32, device=dev)
+    gw = torch.empty((2 * Dh, 2 * Dh), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        nbytes = int(lib.ffb6d_lfa_train_bwd_workspace_bytes(B, N, K, Dh))
+        ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+        check(lib.ffb6d_lfa_train_bwd(f.data_ptr(), idx_c.data_ptr(), i64, fx.data_ptr(), w.data_ptr(), g.data_ptr(),
+                                      B, N, K, Dh, edge.data_ptr(), gx.data_ptr(), gw.data_ptr(), ws.data_ptr(), nbytes,
+                                      _stream(dev)))
+    del ws
+    gf = None
+    if need_feature:
+        gf = _gather_max_bwd(f, idx_c.reshape(B, N * K, 1), edge, LAYOUT_NCS).unsqueeze(3)
+    return gf, gx, gw.reshape(w_fc.shape)
 
 
 # --------------------------------------------------------------------------- depth -> point sets

@@ -412,6 +412,35 @@ int ffb6d_lfa_att_pool_fused(const float *xyz, const void *idx, int idx_is_i64, 
                              int64_t B, int64_t N, int K, int64_t Dh, int64_t Do, float negative_slope,
                              float *out, ffb6d_stream_t stream);
 
+/*
+ * The attentive pooling of a Building_block in training (models/RandLA/RandLANet.py:200-212, 243-248), with the
+ * position MLPs' output f_xyz given:
+ *   x_k   = cat(feature[b, :, idx[b,n,k]], f_xyz[b, :, n, k])          (d = 2 Dh channels)
+ *   f_agg = sum_k x_k * softmax_k(w_fc . x_k)
+ * A warp owns a point; nothing of size N*K is written by the forward.
+ *   feature [B,Dh,N]; idx [B,N,16] int32 / int64 (values in [0, N)); f_xyz [B,Dh,N,16]; w_fc [2Dh,2Dh];
+ *   Dh in {16, 32, 64}, K = 16; f_agg [B,2Dh,N].  All f32, dense.
+ * ffb6d_lfa_train_bwd recomputes x, the logits and the softmax s from the same inputs and, with g = grad_agg
+ * [B,2Dh,N], dlogit = s * g * (x - f_agg) and dx = g * s + w_fc^T . dlogit, writes
+ *   grad_edge  [B,Dh,N*16]  the feature half of dx, one row per edge (n, k): the gradient of the K = 1 gather
+ *                           feature[:, :, idx.reshape(B, N*16)]; the caller scatters it onto the points
+ *                           (ffb6d_gather_max_bwd or ffb6d_gather_max_bwd_det with K = 1, Q = N*16, S = N)
+ *   grad_f_xyz [B,Dh,N,16]  the f_xyz half of dx
+ *   grad_w_fc  [2Dh,2Dh]    sum dlogit . x^T, overwritten; without atomics: one partial per CTA in `workspace`,
+ *                           summed in CTA order in fp64 and rounded once, so bit-identical from run to run
+ * grad_edge and grad_f_xyz 16-byte aligned; workspace: ffb6d_lfa_train_bwd_workspace_bytes(B, N, K, Dh) bytes,
+ * 16-byte aligned, asked on the device that runs the call (the partial count follows its SM count; 0 for sizes the
+ * calls reject or when there is no device).  B < 65536, N < 2^31.  No allocation, no host synchronisation.
+ */
+int ffb6d_lfa_train_fwd(const float *feature, const void *idx, int idx_is_i64, const float *f_xyz,
+                        const float *w_fc, int64_t B, int64_t N, int K, int64_t Dh, float *f_agg,
+                        ffb6d_stream_t stream);
+size_t ffb6d_lfa_train_bwd_workspace_bytes(int64_t B, int64_t N, int K, int64_t Dh);
+int ffb6d_lfa_train_bwd(const float *feature, const void *idx, int idx_is_i64, const float *f_xyz,
+                        const float *w_fc, const float *grad_agg, int64_t B, int64_t N, int K, int64_t Dh,
+                        float *grad_edge, float *grad_f_xyz, float *grad_w_fc, void *workspace,
+                        size_t workspace_bytes, ffb6d_stream_t stream);
+
 /* ---- depth map -> searched point sets ------------------------------------- */
 /*
  * Back-projection of the depth image and extraction of the four point sets the fusion
