@@ -29,6 +29,8 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   and ``final`` at inference, and their adjoints (:func:`psp_bottleneck_bwd`, :func:`psp_pool_bwd`,
   :func:`log_softmax_bwd`, :func:`upsample_bilinear2d_bwd`) for deterministic training;
   ``ffb6d_b200.model.FFB6D`` is the whole network.
+* :class:`GraphedTrainStep` (:mod:`ffb6d_b200.graphed`) -- a whole training step of ``FFB6DFusionNet`` / ``FFB6D``
+  (forward, ``ffb6d_loss``, backward, optimizer update) captured in one CUDA graph and replayed per batch.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -50,10 +52,11 @@ _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
+_GRAPHED = ("GraphedTrainStep",)
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched
@@ -65,6 +68,8 @@ def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op t
         return getattr(importlib.import_module(".tables", __name__), name)
     if name in _ITEM:
         return getattr(importlib.import_module(".item", __name__), name)
+    if name in _GRAPHED:
+        return getattr(importlib.import_module(".graphed", __name__), name)
     if name == "DataProcessing":
         return importlib.import_module(".helper_tool", __name__).DataProcessing
     if name in _SUBMODULES:

@@ -57,6 +57,7 @@ def _load():
         "ffb6d_knn_host": (ci, [vp, sz, sz, vp, sz, sz, vp]),
         "ffb6d_gather_max_fwd": (ci, [vp, vp, ci, i64, i64, i64, i64, ci, ci, vp, vp]),
         "ffb6d_check_indices": (ci, [vp, ci, i64, i64, vp]),
+        "ffb6d_check_indices_enabled": (ci, []),
         "ffb6d_gather_kernel_name": (C.c_char_p, [i64, i64, i64, i64, ci, ci]),
         "ffb6d_gather_max_bwd": (ci, [vp, vp, ci, vp, i64, i64, i64, i64, ci, ci, vp, vp]),
         "ffb6d_gather_neighbour_fwd": (ci, [vp, vp, ci, i64, i64, i64, i64, ci, vp, vp]),

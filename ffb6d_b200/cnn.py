@@ -89,6 +89,19 @@ def _version(params):
     return tuple((p._version, p.data_ptr()) for p in params)
 
 
+def _cached_pack(module, params, pack):
+    """``pack()`` of the weights ``params``, reused while their versions and storage are unchanged.  While the current
+    stream is capturing a CUDA graph the pack is made afresh and not cached: it is then recorded into the graph, and
+    every replay packs the weights as they are then (a captured optimizer step changes them between replays without
+    the host seeing it)."""
+    if torch.cuda.is_current_stream_capturing():
+        return pack()
+    ver = _version(params)
+    if module._packed is None or module._packed[0] != ver:
+        module._packed = (ver, pack())
+    return module._packed[1]
+
+
 class PSPModule(nn.Module):
     """Pyramid pooling: per size s an ``AdaptiveAvgPool2d(s)`` + bias-free 1x1 conv, each upsampled back
     (``align_corners=False``), concatenated with the input, 1x1 ``bottleneck`` (with bias), ReLU."""
@@ -114,14 +127,12 @@ class PSPModule(nn.Module):
         from . import ops
         if tuple(tuple(st[0].output_size) for st in self.stages) != tuple((s, s) for s in PSP_SIZES):
             raise ValueError("forward_fused: the kernels pool at the sizes %s only" % (PSP_SIZES,))
-        ver = _version(self.parameters())
-        if self._packed is None or self._packed[0] != ver:
-            self._packed = (ver, ops.psp_pack([st[1].weight for st in self.stages], self.bottleneck.weight,
-                                              self.bottleneck.bias))
+        packed = _cached_pack(self, list(self.parameters()), lambda: ops.psp_pack(
+            [st[1].weight for st in self.stages], self.bottleneck.weight, self.bottleneck.bias))
         params = [st[1].weight for st in self.stages] + [self.bottleneck.weight, self.bottleneck.bias]
         if _needs_grad(feats, params):
-            return _PSPFused.apply(feats, self._packed[1], *params)
-        return ops.psp_bottleneck(feats, ops.psp_pool(feats), self._packed[1])
+            return _PSPFused.apply(feats, packed, *params)
+        return ops.psp_bottleneck(feats, ops.psp_pool(feats), packed)
 
 
 def _needs_grad(x, params):
@@ -213,12 +224,10 @@ class Final(nn.Sequential):
         output is the same either way."""
         from . import ops
         conv = self[0]
-        ver = _version((conv.weight, conv.bias))
-        if self._packed is None or self._packed[0] != ver:
-            self._packed = (ver, ops.fusion_mlp_pack(conv.weight.detach()))
+        packed = _cached_pack(self, (conv.weight, conv.bias), lambda: ops.fusion_mlp_pack(conv.weight.detach()))
         if _needs_grad(x, (conv.weight, conv.bias)):
-            return _FinalFused.apply(x, self._packed[1], conv.weight, conv.bias)
-        return ops.conv1x1_log_softmax(x, self._packed[1], conv.bias)
+            return _FinalFused.apply(x, packed, conv.weight, conv.bias)
+        return ops.conv1x1_log_softmax(x, packed, conv.bias)
 
 
 class _FinalFused(torch.autograd.Function):

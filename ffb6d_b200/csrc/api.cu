@@ -140,6 +140,7 @@ extern "C" {
 int ffb6d_version(void) { return 2; }
 const char *ffb6d_last_error(void) { return g_err; }
 uint64_t ffb6d_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
+int ffb6d_check_indices_enabled(void) { return env().check_indices ? 1 : 0; }
 
 int ffb6d_device_count(void)
 {

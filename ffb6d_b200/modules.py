@@ -55,7 +55,10 @@ _const_cache = {}
 def _ones_zeros(n, device):
     key = (n, device)
     if key not in _const_cache:
-        _const_cache[key] = (torch.ones(n, device=device), torch.zeros(n, device=device))
+        consts = (torch.ones(n, device=device), torch.zeros(n, device=device))
+        if torch.cuda.is_current_stream_capturing():
+            return consts     # filled only when the graph replays: not for eager callers to find
+        _const_cache[key] = consts
     return _const_cache[key]
 
 

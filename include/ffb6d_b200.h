@@ -176,6 +176,9 @@ int ffb6d_gather_max_fwd(const float *feat, const void *idx, int idx_is_i64,
 /* Validates `count` indices against [0,S): returns FFB6D_ERR_INVALID (with the number of offenders
  * in ffb6d_last_error) if any lies outside.  Blocking: synchronises `stream`; not capturable. */
 int ffb6d_check_indices(const void *idx, int idx_is_i64, int64_t count, int64_t S, ffb6d_stream_t stream);
+/* 1 if this process's library runs that check in front of every gather (FFB6D_CHECK_INDICES as it read the
+ * environment once, at its first use), else 0.  Such gathers synchronise and cannot be captured in a CUDA graph. */
+int ffb6d_check_indices_enabled(void);
 /* Name of the kernel ffb6d_gather_max_fwd launches for a shape (for profiling tools). */
 const char *ffb6d_gather_kernel_name(int64_t B, int64_t C, int64_t S, int64_t Q, int K, int layout);
 /*
