@@ -30,7 +30,8 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   :func:`log_softmax_bwd`, :func:`upsample_bilinear2d_bwd`) for deterministic training;
   ``ffb6d_b200.model.FFB6D`` is the whole network.
 * :class:`GraphedTrainStep` (:mod:`ffb6d_b200.graphed`) -- a whole training step of ``FFB6DFusionNet`` / ``FFB6D``
-  (forward, ``ffb6d_loss``, backward, optimizer update) captured in one CUDA graph and replayed per batch.
+  (forward, ``ffb6d_loss``, backward, optimizer update) captured in one CUDA graph and replayed per batch;
+  :class:`GraphedEvalStep` -- the eval forward and its ``ffb6d_loss`` the same way, for validation and testing.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -52,7 +53,7 @@ _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
-_GRAPHED = ("GraphedTrainStep",)
+_GRAPHED = ("GraphedTrainStep", "GraphedEvalStep")
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
                "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "_lib")
 

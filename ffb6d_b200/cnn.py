@@ -90,16 +90,10 @@ def _version(params):
 
 
 def _cached_pack(module, params, pack):
-    """``pack()`` of the weights ``params``, reused while their versions and storage are unchanged.  While the current
-    stream is capturing a CUDA graph the pack is made afresh and not cached: it is then recorded into the graph, and
-    every replay packs the weights as they are then (a captured optimizer step changes them between replays without
-    the host seeing it)."""
-    if torch.cuda.is_current_stream_capturing():
-        return pack()
-    ver = _version(params)
-    if module._packed is None or module._packed[0] != ver:
-        module._packed = (ver, pack())
-    return module._packed[1]
+    """``pack()`` of the weights ``params``, reused while their versions and storage are unchanged, and made afresh
+    while a CUDA graph is being captured (:func:`ffb6d_b200.modules.weight_cache`)."""
+    from .modules import weight_cache
+    return weight_cache(module, "_packed", _version(params), pack)
 
 
 class PSPModule(nn.Module):

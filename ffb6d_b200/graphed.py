@@ -1,5 +1,5 @@
-"""FFB6D's training step as one CUDA graph: forward, ``ffb6d_loss``, backward and the optimizer update, captured once
-and replayed per batch (DESIGN.md §4.20).
+"""FFB6D's training step and its eval step, each as one CUDA graph captured once and replayed per batch
+(DESIGN.md §4.20, §4.21).
 
     opt = torch.optim.Adam(model.parameters(), lr=torch.tensor(1e-4, device="cuda"), capturable=True)
     step = GraphedTrainStep(model, opt, example_item)
@@ -12,6 +12,13 @@ One replay is ``opt.zero_grad()``, ``loss, info = ffb6d_loss(model(item), item, 
 (the train/eval flags, the model's path switches, torch's deterministic and TF32 switches, BatchNorm momentum and
 eps, dropout rates, the optimizer's non-tensor hyperparameters, ``requires_grad`` and the storage of every parameter,
 buffer and gradient) is compared on the host before every replay; when any of it changed, the step captures again.
+
+    model.eval()
+    evaluate = GraphedEvalStep(model, example_item)
+    end_points, loss, info = evaluate(item)     # model(item) and ffb6d_loss under torch.no_grad(), replayed
+
+The eval step reads the weights on the device at every replay, so it follows optimizer steps, ``load_state_dict``
+and graphed training steps without capturing again.
 """
 import os
 
@@ -27,6 +34,9 @@ from .model import FFB6D, FFB6DFusionNet
 # Adam's (and AdamW's) state, each created as zeros by its first step: what the warm-up's own first step created is
 # zeroed after it (an optimizer whose fresh state is not zero -- NAdam's mu_product, ASGD's eta -- is rejected)
 _ADAM_STATE = frozenset(("step", "exp_avg", "exp_avg_sq", "max_exp_avg_sq"))
+
+# the item keys ffb6d_loss reads: an eval step whose example item carries them also captures the loss
+_LOSS_KEYS = ("labels", "kp_targ_ofst", "ctr_targ_ofst")
 
 
 def _check_indices_on():
@@ -74,7 +84,116 @@ def _state_tensors(optimizer):
     return [t for p in optimizer.state for t in optimizer.state[p].values() if isinstance(t, torch.Tensor)]
 
 
-class GraphedTrainStep:
+class _GraphedStep:
+    """What the train and eval steps share: the argument checks, the static input buffers and their copy-in, the
+    baked key of the model, the side-stream warm-up and the capture.  A subclass defines ``_check`` (what cannot be
+    captured), ``_step`` (the captured work), ``_capture`` and ``__call__``; ``_module_key`` / ``_extra_key`` add
+    what only it bakes in."""
+
+    _wrapper_hint = ""
+
+    def __init__(self, model, example_item, warmup):
+        name = type(self).__name__
+        if isinstance(model, (nn.parallel.DistributedDataParallel, nn.DataParallel)):
+            raise ValueError("%s: a (Distributed)DataParallel model cannot be captured; %s" % (name, self._wrapper_hint))
+        if not isinstance(model, FFB6DFusionNet):
+            raise ValueError("%s: model must be an FFB6DFusionNet or FFB6D, got %s" % (name, type(model).__name__))
+        if not isinstance(example_item, dict):
+            raise ValueError("%s: example_item must be a dict, got %s" % (name, type(example_item).__name__))
+        if not isinstance(model, FFB6D) and not isinstance(example_item.get("rgb_feats"), (list, tuple)):
+            raise ValueError("%s: an FFB6DFusionNet item needs 'rgb_feats', the list of image-branch maps" % name)
+        if int(warmup) < 1:
+            raise ValueError("%s: warmup must be at least 1, got %r" % (name, warmup))
+        self.model = model
+        self._read_modules()
+        self._check(True)
+        self._static = _static_copy(example_item)
+        self._inputs = _tensors(self._static)
+        self._graph = None
+        self._key = None
+        self.captures = 0
+        self._capture(int(warmup))
+
+    def _read_modules(self):
+        """The module tree as a list, walked by every call's key (which also holds each module's children, so a
+        swapped submodule changes the key and the next capture reads the tree again)."""
+        self._modules = list(self.model.modules())
+
+    def _refuse_index_check(self):
+        if _check_indices_on():
+            raise ValueError("%s: FFB6D_CHECK_INDICES is set; the index check synchronises the host and cannot be "
+                             "captured" % type(self).__name__)
+
+    def _module_key(self, m):
+        return ()
+
+    def _extra_key(self):
+        return ()
+
+    def _baked(self):
+        """Every host value the captured step depends on, as one comparable tuple (about 0.6 ms for FFB6D)."""
+        model = self.model
+        key = [torch.are_deterministic_algorithms_enabled(), torch.backends.cudnn.deterministic,
+               torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32,
+               bool(model.restructured), bool(model.fused_lfa), bool(getattr(model, "fused_image_head", False))]
+        for m in self._modules:
+            key += (m.training, tuple(map(id, m._modules.values())))
+            if isinstance(m, nn.modules.batchnorm._BatchNorm):
+                key.append(m.eps)
+            key += self._module_key(m)
+            for p in m._parameters.values():
+                if p is not None:
+                    key += (id(p), p.data_ptr())
+            for b in m._buffers.values():
+                if b is not None:
+                    key += (id(b), b.data_ptr())
+        key += self._extra_key()
+        return tuple(key)
+
+    def _warm_up(self, n):
+        """``n`` eager steps on a side stream, ordered after the current stream's work and before what follows it:
+        cuDNN plans, the package's workspaces and its constant caches exist before capture starts."""
+        dev = next(self.model.parameters()).device
+        side = torch.cuda.Stream(dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(n):
+                self._step()
+        torch.cuda.current_stream(dev).wait_stream(side)
+
+    def _record(self):
+        """Capture one ``_step`` into a new graph; returns its outputs, which every replay overwrites."""
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = self._step()
+        self._graph = graph
+        self.captures += 1
+        return out
+
+    def _copy_in(self, item):
+        name = type(self).__name__
+        if not isinstance(item, dict):
+            raise ValueError("%s: the item must be a dict, got %s" % (name, type(item).__name__))
+        pairs = []
+        for path, buf in self._inputs:
+            t = _lookup(item, path)
+            where = "item" + "".join("[%r]" % k for k in path)
+            if t is None:
+                raise ValueError("%s: %s is missing" % (name, where))
+            if not isinstance(t, torch.Tensor):
+                raise ValueError("%s: %s must be a tensor, got %s" % (name, where, type(t).__name__))
+            if t.shape != buf.shape or t.dtype != buf.dtype or t.device != buf.device:
+                raise ValueError("%s: %s is %s %s on %s; the step was captured for %s %s on %s (it does not capture "
+                                 "again for new shapes: build a new step)"
+                                 % (name, where, tuple(t.shape), t.dtype, t.device, tuple(buf.shape), buf.dtype,
+                                    buf.device))
+            pairs.append((buf, t))
+        for buf, t in pairs:
+            if t.data_ptr() != buf.data_ptr():
+                buf.copy_(t)
+
+
+class GraphedTrainStep(_GraphedStep):
     """A training step of ``model`` (an :class:`~ffb6d_b200.model.FFB6DFusionNet` or
     :class:`~ffb6d_b200.model.FFB6D` in training mode) with ``optimizer``, captured in a CUDA graph.
 
@@ -101,34 +220,17 @@ class GraphedTrainStep:
     when the library loaded (the index check synchronises); a model in eval mode.
     """
 
+    _wrapper_hint = "multi-rank capture is not supported, pass the module of a single-rank run"
+
     def __init__(self, model, optimizer, example_item, warmup=3):
-        if isinstance(model, (nn.parallel.DistributedDataParallel, nn.DataParallel)):
-            raise ValueError("GraphedTrainStep: a (Distributed)DataParallel model cannot be captured; multi-rank "
-                             "capture is not supported, pass the module of a single-rank run")
-        if not isinstance(model, FFB6DFusionNet):
-            raise ValueError("GraphedTrainStep: model must be an FFB6DFusionNet or FFB6D, got %s" % type(model).__name__)
-        if not isinstance(example_item, dict):
-            raise ValueError("GraphedTrainStep: example_item must be a dict, got %s" % type(example_item).__name__)
-        if not isinstance(model, FFB6D) and not isinstance(example_item.get("rgb_feats"), (list, tuple)):
-            raise ValueError("GraphedTrainStep: an FFB6DFusionNet item needs 'rgb_feats', the list of image-branch maps")
-        if int(warmup) < 1:
-            raise ValueError("GraphedTrainStep: warmup must be at least 1, got %r" % (warmup,))
-        self.model, self.optimizer = model, optimizer
-        self._read_modules()
-        self._check(True)
-        self._static = _static_copy(example_item)
-        self._inputs = _tensors(self._static)
-        self._graph = self._loss = self._info = None
-        self._key = None
+        self.optimizer = optimizer
+        self._loss = self._info = None
         self._written = []
-        self.captures = 0
-        self._capture(int(warmup))
+        super().__init__(model, example_item, warmup)
 
     # ------------------------------------------------------------------------------------------ host checks
     def _read_modules(self):
-        """The module tree as a list, walked by every call's key (which also holds each module's children, so a
-        swapped submodule changes the key and the next capture reads the tree again)."""
-        self._modules = list(self.model.modules())
+        super()._read_modules()
         self._sync = any(isinstance(m, nn.SyncBatchNorm) for m in self._modules)
 
     def _check(self, modules):
@@ -137,9 +239,7 @@ class GraphedTrainStep:
         model, opt = self.model, self.optimizer
         if not model.training:
             raise ValueError("GraphedTrainStep: the model is in eval mode; it captures training steps only")
-        if _check_indices_on():
-            raise ValueError("GraphedTrainStep: FFB6D_CHECK_INDICES is set; the index check synchronises the host "
-                             "and cannot be captured")
+        self._refuse_index_check()
         if not isinstance(opt, torch.optim.Adam):      # AdamW is an Adam
             raise ValueError("GraphedTrainStep: the optimizer must be torch.optim.Adam or AdamW, got %s (the warm-up "
                              "is undone by restoring Adam's zero initial state)" % type(opt).__name__)
@@ -160,28 +260,25 @@ class GraphedTrainStep:
                         raise ValueError("GraphedTrainStep: SyncBatchNorm %r synchronises over several ranks; "
                                          "multi-rank capture is not supported" % name)
 
-    def _baked(self):
-        """Every host value the captured step depends on, as one comparable tuple (about 0.6 ms for FFB6D)."""
-        model, opt = self.model, self.optimizer
-        key = [torch.are_deterministic_algorithms_enabled(), torch.backends.cudnn.deterministic,
-               torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32,
-               bool(model.restructured), bool(model.fused_lfa), bool(getattr(model, "fused_image_head", False))]
-        for m in self._modules:
-            key += (m.training, tuple(map(id, m._modules.values())))
-            if isinstance(m, nn.modules.batchnorm._BatchNorm):
-                if m.momentum is None:
-                    self._check(True)                  # raises, naming the layer
-                key += (m.momentum, m.eps)
-            elif isinstance(m, nn.modules.dropout._DropoutNd):
-                key.append(m.p)
-            for p in m._parameters.values():
-                if p is not None:
-                    g = p.grad
-                    key += (id(p), p.data_ptr(), p.requires_grad, id(g), g.data_ptr() if g is not None else 0)
-            for b in m._buffers.values():
-                if b is not None:
-                    key += (id(b), b.data_ptr())
-        for group in opt.param_groups:      # the optimizer reads the keys of its defaults (not e.g. initial_lr)
+    def _module_key(self, m):
+        """BatchNorm momentum, dropout rates, and ``requires_grad`` and the gradient storage of every parameter."""
+        key = []
+        if isinstance(m, nn.modules.batchnorm._BatchNorm):
+            if m.momentum is None:
+                self._check(True)                  # raises, naming the layer
+            key.append(m.momentum)
+        elif isinstance(m, nn.modules.dropout._DropoutNd):
+            key.append(m.p)
+        for p in m._parameters.values():
+            if p is not None:
+                g = p.grad
+                key += (p.requires_grad, id(g), g.data_ptr() if g is not None else 0)
+        return key
+
+    def _extra_key(self):
+        """The optimizer's hyperparameters (it reads the keys of its defaults, not e.g. initial_lr)."""
+        opt, key = self.optimizer, []
+        for group in opt.param_groups:
             key.append(tuple(id(p) for p in group["params"]))
             for k in sorted(opt.defaults):
                 v = group.get(k)
@@ -189,7 +286,7 @@ class GraphedTrainStep:
                     key += (k, id(v), v.data_ptr())
                 else:
                     key += (k, v)
-        return tuple(key)
+        return key
 
     # ------------------------------------------------------------------------------------------ capture
     def _step(self):
@@ -216,12 +313,7 @@ class GraphedTrainStep:
         saved = [t.detach().clone() for t in tracked]
         saved_state = {k: t.detach().clone() for k, t in before.items()}
         rng = torch.cuda.get_rng_state(dev)
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            for _ in range(warmup):
-                self._step()
-        torch.cuda.current_stream(dev).wait_stream(side)
+        self._warm_up(warmup)
         with torch.no_grad():
             for t, s in zip(tracked, saved):
                 t.copy_(s)
@@ -243,11 +335,7 @@ class GraphedTrainStep:
                              "zero; only Adam's own state can be restored after the warm-up" % (unknown,))
         del saved, saved_state
         opt.zero_grad(set_to_none=True)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            self._loss, self._info = self._step()
-        self._graph = graph
-        self.captures += 1
+        self._loss, self._info = self._record()
         # what a replay writes: its host version counters are advanced after each replay, as eager in-place
         # updates advance them, so version-keyed caches (the eval path's packed weights) see the new values
         self._written = (tracked + _state_tensors(opt) +
@@ -255,26 +343,6 @@ class GraphedTrainStep:
         self._key = self._baked()
 
     # ------------------------------------------------------------------------------------------ a step
-    def _copy_in(self, item):
-        if not isinstance(item, dict):
-            raise ValueError("GraphedTrainStep: the item must be a dict, got %s" % type(item).__name__)
-        pairs = []
-        for path, buf in self._inputs:
-            t = _lookup(item, path)
-            where = "item" + "".join("[%r]" % k for k in path)
-            if t is None:
-                raise ValueError("GraphedTrainStep: %s is missing" % where)
-            if not isinstance(t, torch.Tensor):
-                raise ValueError("GraphedTrainStep: %s must be a tensor, got %s" % (where, type(t).__name__))
-            if t.shape != buf.shape or t.dtype != buf.dtype or t.device != buf.device:
-                raise ValueError("GraphedTrainStep: %s is %s %s on %s; the step was captured for %s %s on %s (it "
-                                 "does not capture again for new shapes: build a new step)"
-                                 % (where, tuple(t.shape), t.dtype, t.device, tuple(buf.shape), buf.dtype, buf.device))
-            pairs.append((buf, t))
-        for buf, t in pairs:
-            if t.data_ptr() != buf.data_ptr():
-                buf.copy_(t)
-
     def __call__(self, item):
         self._check(self._sync)
         self._copy_in(item)
@@ -283,3 +351,73 @@ class GraphedTrainStep:
         self._graph.replay()
         increment_version(self._written)
         return self._loss, self._info
+
+
+class GraphedEvalStep(_GraphedStep):
+    """An eval step of ``model`` (an :class:`~ffb6d_b200.model.FFB6DFusionNet` or :class:`~ffb6d_b200.model.FFB6D`
+    in eval mode), captured in a CUDA graph: under ``torch.no_grad()``, ``model(item)`` (``model(item,
+    item["rgb_feats"])`` for :class:`FFB6DFusionNet`) and, when the example item carries ``labels``,
+    ``kp_targ_ofst`` and ``ctr_targ_ofst``, ``ffb6d_loss(end_points, item, valid=item.get("valid"))``, as
+    ``model_fn`` computes them with ``is_eval=True``.
+
+    :param example_item: as for :class:`GraphedTrainStep`; every CUDA tensor in it gets a static input buffer.
+    :param warmup: eager eval steps run on a side stream before the first capture.  Eval writes no parameter or
+      buffer, so nothing is restored after them.
+
+    Calling the step copies the item's tensors into the input buffers and replays the graph on the current stream.
+    It returns ``(end_points, loss, info)``: the network's outputs and :func:`ffb6d_b200.loss.ffb6d_loss`'s
+    ``(loss, info)``, or ``None, None`` without the loss keys.  They are the graph's tensors, which the next replay
+    overwrites (clone what you keep).
+
+    Every pack of weights or running statistics is made inside the graph, so each replay reads the parameters and
+    buffers as they are then: optimizer steps, ``load_state_dict``, new running statistics and
+    :class:`GraphedTrainStep` replays between calls need no new capture.  What capture bakes in is compared before
+    every replay (DESIGN.md §4.21): the module tree and every module's ``training``, ``restructured``,
+    ``fused_lfa``, ``fused_image_head``, torch's deterministic, cuDNN and TF32 switches, BatchNorm ``eps``, and the
+    identity and storage of every parameter and buffer; any change captures again (``captures`` counts).
+
+    Rejected with ``ValueError``: a model in training mode; a ``DistributedDataParallel`` / ``DataParallel`` wrapper
+    (pass its ``.module``); ``FFB6D_CHECK_INDICES`` set now or when the library loaded; an item whose keys, shapes,
+    dtypes or devices differ from the example's.  An ``nn.SyncBatchNorm`` over several ranks is accepted: in eval mode
+    it normalises with its running statistics and issues no collective, so each rank can evaluate through its own
+    step.
+    """
+
+    _wrapper_hint = "pass its .module (each rank evaluates through a step of its own)"
+
+    def __init__(self, model, example_item, warmup=3):
+        self._out = None
+        self._with_loss = isinstance(example_item, dict) and all(k in example_item for k in _LOSS_KEYS)
+        super().__init__(model, example_item, warmup)
+
+    def _check(self, modules=False):
+        """What cannot be captured at all: raise ``ValueError`` before any CUDA work."""
+        if self.model.training:
+            raise ValueError("GraphedEvalStep: the model is in training mode; call model.eval() first, it captures "
+                             "eval steps only")
+        self._refuse_index_check()
+
+    def _step(self):
+        item = self._static
+        with torch.no_grad():
+            out = self.model(item) if isinstance(self.model, FFB6D) else self.model(item, item["rgb_feats"])
+            loss = info = None
+            if self._with_loss:
+                loss, info = ffb6d_loss(out, item, valid=item.get("valid"))
+        return out, loss, info
+
+    def _capture(self, warmup):
+        self._graph = self._out = None     # release the previous graph's pool before the new one fills
+        self._read_modules()
+        self._check()
+        self._warm_up(warmup)
+        self._out = self._record()
+        self._key = self._baked()
+
+    def __call__(self, item):
+        self._check()
+        self._copy_in(item)
+        if self._baked() != self._key:
+            self._capture(1)
+        self._graph.replay()
+        return self._out

@@ -32,6 +32,7 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 import torch.nn.functional as F_
+from torch.autograd.graph import increment_version
 
 from . import dist as dist_, fusion, ops
 from ._lib import lib, check
@@ -60,6 +61,23 @@ def _ones_zeros(n, device):
             return consts     # filled only when the graph replays: not for eager callers to find
         _const_cache[key] = consts
     return _const_cache[key]
+
+
+def weight_cache(owner, attr, key, make):
+    """``make()``, a pack of weights (or running statistics) whose versions and storage ``key`` names, kept in
+    ``owner.<attr>`` as ``(key, pack)`` and reused while ``key`` is unchanged.
+
+    While the current stream is capturing a CUDA graph nothing is reused or stored: the pack is made afresh and so
+    recorded into the graph, and each replay packs the weights as they are then.  A reused pack would bake a pointer
+    to the cached tensor into the graph, which the next eager call after a weight update frees by replacing it; a
+    stored pack would be filled only when the graph replays, and eager callers would read it unfilled."""
+    if torch.cuda.is_current_stream_capturing():
+        return make()
+    hit = getattr(owner, attr)
+    if hit is None or hit[0] != key:
+        hit = (key, make())
+        setattr(owner, attr, hit)
+    return hit[1]
 
 
 def _gemm(x1, x2, w2d):
@@ -91,16 +109,21 @@ def _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, moment
             check(lib.ffb6d_bn_train_fwd(
                 z.data_ptr(), B, Co, P, gamma_p, beta_p, float(eps), float(momentum), rm_p, rv_p, int(act), float(slope),
                 stats.data_ptr(), y.data_ptr(), ws.data_ptr(), nbytes, ops._stream(z.device)))
-            return y, stats, None
-        group, world = sync
-        row = torch.empty(2 * Co + 1, dtype=torch.float64, device=z.device)
-        check(lib.ffb6d_bn_sync_moments(z.data_ptr(), B, Co, P, row.data_ptr(), ws.data_ptr(), nbytes,
-                                        ops._stream(z.device)))
-        rows = dist_.all_gather_rows(row, group, world)
-        count = torch.empty(1, dtype=torch.float64, device=z.device)
-        check(lib.ffb6d_bn_sync_fwd(
-            z.data_ptr(), B, Co, P, rows.data_ptr(), world, gamma_p, beta_p, float(eps), float(momentum), rm_p, rv_p,
-            int(act), float(slope), stats.data_ptr(), count.data_ptr(), y.data_ptr(), ops._stream(z.device)))
+            count = None
+        else:
+            group, world = sync
+            row = torch.empty(2 * Co + 1, dtype=torch.float64, device=z.device)
+            check(lib.ffb6d_bn_sync_moments(z.data_ptr(), B, Co, P, row.data_ptr(), ws.data_ptr(), nbytes,
+                                            ops._stream(z.device)))
+            rows = dist_.all_gather_rows(row, group, world)
+            count = torch.empty(1, dtype=torch.float64, device=z.device)
+            check(lib.ffb6d_bn_sync_fwd(
+                z.data_ptr(), B, Co, P, rows.data_ptr(), world, gamma_p, beta_p, float(eps), float(momentum), rm_p,
+                rv_p, int(act), float(slope), stats.data_ptr(), count.data_ptr(), y.data_ptr(), ops._stream(z.device)))
+    # the kernels updated the running statistics in place: advance their versions, as torch's in-place update does,
+    # so the eval path's version-keyed packs (weight_cache) fold the new statistics, also in a layer whose weights
+    # no optimizer step has touched
+    increment_version([t for t in (running_mean, running_var) if t is not None])
     return y, stats, count
 
 
@@ -295,7 +318,7 @@ class _ConvBase(nn.Module):
         if activation is not None:
             self.add_module(name + "activation", activation)
         self.act, self.slope = _act_code(activation)
-        self._packed = None      # (weight version, PackedWeight, scale, shift) of the eval path
+        self._packed = None      # (weight version, (PackedWeight, scale, shift)) of the eval path
         self._split = None       # ((weight version, C1), fusion.SplitFuse) of forward_interp's eval path
 
     @property
@@ -320,11 +343,8 @@ class _ConvBase(nn.Module):
         return scale, (conv.bias.detach().float() if conv.bias is not None else torch.zeros_like(scale))
 
     def _eval_pack(self):
-        ver = self._eval_version()
-        if self._packed is None or self._packed[0] != ver:
-            scale, shift = self._eval_affine()
-            self._packed = (ver, ops.fusion_mlp_pack(self._conv.weight.detach()), scale, shift)
-        return self._packed[1:]
+        return weight_cache(self, "_packed", self._eval_version(),
+                            lambda: (ops.fusion_mlp_pack(self._conv.weight.detach()),) + self._eval_affine())
 
     def _bn_sync(self):
         """``(process group, world size)`` when the training-mode BatchNorm normalises with the statistics of every
@@ -439,13 +459,10 @@ class Conv2d(_ConvBase):
             z = _InterpConvBnActTrain.apply(x1, p, idx, conv.weight, None, None, None, None, None, 0.0, 0.0, _ACT_NONE,
                                             0.0, False)
             return self._frozen_bn_act(z)
-        key = (self._eval_version(), C1)
-        if self._split is None or self._split[0] != key:
-            scale, shift = self._eval_affine()
-            self._split = (key, fusion.SplitFuse.from_weight(
-                conv.weight, scale, shift, C1, relu=(self.act == _ACT_RELU),
-                negative_slope=self.slope if self.act == _ACT_LEAKY else None))
-        return fusion.p2r_fuse(x1, p, idx, self._split[1])
+        split = weight_cache(self, "_split", (self._eval_version(), C1), lambda: fusion.SplitFuse.from_weight(
+            conv.weight, *self._eval_affine(), C1, relu=(self.act == _ACT_RELU),
+            negative_slope=self.slope if self.act == _ACT_LEAKY else None))
+        return fusion.p2r_fuse(x1, p, idx, split)
 
 
 class RandLAConv2d(_ConvBase):
@@ -555,11 +572,9 @@ class Att_pooling(nn.Module):
         w = self.fc.weight
         if torch.is_grad_enabled() and (w.requires_grad or f1.requires_grad or (f2 is not None and f2.requires_grad)):
             return _ConvBnActTrain.apply(f1, f2, w, None, None, None, None, None, 0.0, 0.0, _ACT_NONE, 0.0, False)
-        ver = (w._version, w.data_ptr())
-        if self._fc_pack is None or self._fc_pack[0] != ver:
-            self._fc_pack = (ver, ops.fusion_mlp_pack(w.detach()))
+        packed = weight_cache(self, "_fc_pack", (w._version, w.data_ptr()), lambda: ops.fusion_mlp_pack(w.detach()))
         one, zero = _ones_zeros(w.shape[0], f1.device)
-        return ops.fusion_mlp(f1, f2, self._fc_pack[1], one, zero, relu=False)
+        return ops.fusion_mlp(f1, f2, packed, one, zero, relu=False)
 
     def forward(self, feature_set, f2=None):
         att = self._att(feature_set, f2)
