@@ -32,6 +32,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
 * :class:`GraphedTrainStep` (:mod:`ffb6d_b200.graphed`) -- a whole training step of ``FFB6DFusionNet`` / ``FFB6D``
   (forward, ``ffb6d_loss``, backward, optimizer update) captured in one CUDA graph and replayed per batch;
   :class:`GraphedEvalStep` -- the eval forward and its ``ffb6d_loss`` the same way, for validation and testing.
+* :func:`farthest_point_sampling` -- ``fps_utils.farthest_point_sampling`` (utils/dataset_tools/fps/fps_utils.py:8-23)
+  on the GPU, batched over clouds; :mod:`ffb6d_b200.objinfo` -- the object tables of
+  utils/dataset_tools/gen_obj_info.py (box corners, radius, centre, keypoints) and their text files.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -48,16 +51,17 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "PackedWeight", "fold_batchnorm", "att_pool", "sample_valid_pixels", "check_indices", "mean_shift_fit", "best_fit_transform",
         "fill_missing", "segment_plan", "segment_sum", "point_item", "rgb_add_noise", "add_real_back",
         "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax",
-        "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d")
+        "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d",
+        "farthest_point_sampling")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
 _GRAPHED = ("GraphedTrainStep", "GraphedEvalStep")
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched

@@ -19,6 +19,10 @@ ERR_NO_DEVICE = -4
 LAYOUT_NCS = 0
 LAYOUT_NSC = 1
 MAX_K = 64
+FPS_MAX_CLUSTER = 8                              # FFB6D_FPS_MAX_* of include/ffb6d_b200.h
+FPS_MAX_POINTS = FPS_MAX_CLUSTER * 14336
+FPS_MAX_SAMPLES = FPS_MAX_POINTS
+FPS_MAX_CLOUDS = 65535
 
 
 class FFB6DError(RuntimeError):
@@ -122,6 +126,8 @@ def _load():
         "ffb6d_psp_pool_bwd": (ci, [vp, i64, i64, i64, i64, vp, vp]),
         "ffb6d_log_softmax_bwd": (ci, [vp, vp, i64, i64, i64, vp, vp]),
         "ffb6d_upsample_bilinear2d_bwd": (ci, [vp, i64, i64, i64, i64, i64, i64, vp, vp]),
+        "ffb6d_farthest_point_sampling_workspace_bytes": (sz, [i64, i64, i64]),
+        "ffb6d_farthest_point_sampling": (ci, [vp, vp, i64, i64, i64, vp, ci, vp, vp, sz, vp]),
         "ffb6d_grid_subsample_host": (ci, [vp, sz, vp, sz, vp, sz, fp, vp, vp, vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():

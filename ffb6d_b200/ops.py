@@ -992,6 +992,107 @@ def grid_sub_sampling(points, features=None, labels=None, grid_size=0.1, verbose
     return out[0] if len(out) == 1 else tuple(out)
 
 
+# --------------------------------------------------------------------------- farthest point sampling
+def _fps_host_ints(v, G, n, name):
+    """A host start / count argument: an int or G ints, as int32 [G]; None for a CUDA tensor (checked on the device)."""
+    if isinstance(v, torch.Tensor) and v.is_cuda:
+        return None
+    a = np.asarray(v.cpu() if isinstance(v, torch.Tensor) else v)
+    if a.dtype.kind not in "iu":
+        raise TypeError("%s must hold integers, got %s" % (name, a.dtype))
+    a = np.broadcast_to(a, (G,)) if a.ndim == 0 else a
+    if a.shape != (G,):
+        raise ValueError("%s must be an int or %d ints, got shape %s" % (name, G, a.shape))
+    if n is not None and (np.any(a < 0) or np.any(a >= n)):
+        raise ValueError("%s must lie in [0, %s), got %s" % (name, n, a))
+    return a.astype(np.int32)
+
+
+def farthest_point_sampling(pts, sn, init_center=False, start=None, return_index=False, n_points=None):
+    """Farthest point sampling on the GPU; mirrors ``fps_utils.farthest_point_sampling`` (utils/dataset_tools/fps/
+    fps_utils.py:8-23), whose selection it reproduces bit for bit (include/ffb6d_b200.h).
+
+    :param pts: numpy ``[P,3]`` (copied to the current CUDA device as float32, as the reference converts it), or a
+      float32 CUDA tensor ``[P,3]`` or ``[G,P,3]`` (G clouds in one launch)
+    :param sn: number of points to select, ``1 <= sn <= FFB6D_FPS_MAX_SAMPLES``; ``sn > P`` repeats index 0
+    :param init_center: start from the point farthest from the centre of the bounding box (deterministic)
+    :param start: without ``init_center``, the first index of each cloud: an int, ``G`` ints, or an int32 CUDA tensor
+      ``[G]`` (host values are range-checked here; a CUDA tensor's are checked by the kernel, which writes -1 into
+      the rows of clouds whose start is out of range).  ``None`` draws it uniformly from torch's CUDA generator,
+      where the reference uses ``rand()``
+    :param n_points: cloud ``g`` is its first ``n_points[g]`` points (int, ``G`` ints or int32 CUDA tensor);
+      ``None``: all ``P``
+    :return: ``pts[idxs]`` (``[sn,3]`` / ``[G,sn,3]``, numpy for numpy input), and with ``return_index`` also the
+      indices (int32)
+    """
+    as_numpy = not isinstance(pts, torch.Tensor)
+    if as_numpy:
+        x = np.ascontiguousarray(pts, np.float32)
+        if x.ndim != 2 or x.shape[1] != 3:
+            raise ValueError("pts must be [P,3], got shape %s" % (x.shape,))
+    else:
+        _need_cuda(pts, "pts")
+        if pts.dtype != torch.float32:
+            raise TypeError("pts must be float32, got %s" % pts.dtype)
+        if pts.dim() not in (2, 3) or pts.shape[-1] != 3:
+            raise ValueError("pts must be [P,3] or [G,P,3], got shape %s" % (tuple(pts.shape),))
+        x = pts
+    single = x.ndim == 2
+    G, P = (1, x.shape[0]) if single else x.shape[:2]
+    if isinstance(sn, bool) or not isinstance(sn, (int, np.integer)):
+        raise TypeError("sn must be an int, got %r" % (sn,))
+    sn = int(sn)
+    if not 1 <= sn <= _lib.FPS_MAX_SAMPLES:
+        raise ValueError("sn must lie in [1, %d], got %d" % (_lib.FPS_MAX_SAMPLES, sn))
+    if not (1 <= G <= _lib.FPS_MAX_CLOUDS and 1 <= P <= _lib.FPS_MAX_POINTS):
+        raise ValueError("need 1 <= G <= %d clouds of 1 <= P <= %d points, got G=%d, P=%d"
+                         % (_lib.FPS_MAX_CLOUDS, _lib.FPS_MAX_POINTS, G, P))
+    counts_h = st_h = None
+    n_hi = P
+    if n_points is not None:
+        counts_h = _fps_host_ints(n_points, G, None, "n_points")
+        if counts_h is None:
+            if n_points.dtype != torch.int32 or tuple(n_points.shape) != (G,):
+                raise ValueError("n_points must be an int32 CUDA tensor [%d]" % G)
+        elif np.any(counts_h < 1) or np.any(counts_h > P):
+            raise ValueError("n_points must lie in [1, %d], got %s" % (P, counts_h))
+        else:
+            n_hi = counts_h
+    if not init_center and start is not None:
+        st_h = _fps_host_ints(start, G, n_hi, "start")
+        if st_h is None and (start.dtype != torch.int32 or tuple(start.shape) != (G,)):
+            raise ValueError("start must be an int32 CUDA tensor [%d]" % G)
+
+    x = torch.from_numpy(x).to(torch.device("cuda", torch.cuda.current_device())) if as_numpy else x
+    x = (x[None] if single else x).contiguous()
+    dev = x.device
+    counts = None
+    if n_points is not None:
+        counts = torch.from_numpy(counts_h).to(dev) if counts_h is not None else n_points.to(dev).contiguous()
+    st = None
+    if not init_center:
+        if start is None:
+            n = counts.to(torch.float64) if counts is not None else torch.full((G,), float(P), dtype=torch.float64,
+                                                                                device=dev)
+            st = torch.minimum((torch.rand(G, dtype=torch.float64, device=dev) * n).floor(), n - 1).to(torch.int32)
+        else:
+            st = torch.from_numpy(st_h).to(dev) if st_h is not None else start.to(dev).contiguous()
+    idx = torch.empty((G, sn), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        nbytes = int(lib.ffb6d_farthest_point_sampling_workspace_bytes(G, P, sn))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes else None
+        check(lib.ffb6d_farthest_point_sampling(x.data_ptr(), counts.data_ptr() if counts is not None else None, G, P,
+                                                sn, st.data_ptr() if st is not None else None, int(bool(init_center)),
+                                                idx.data_ptr(), ws.data_ptr() if ws is not None else None, nbytes,
+                                                _stream(dev)))
+    sel = torch.gather(x, 1, idx.clamp(min=0).long()[..., None].expand(G, sn, 3))
+    if single:
+        sel, idx = sel[0], idx[0]
+    if as_numpy:
+        sel, idx = sel.cpu().numpy(), idx.cpu().numpy()
+    return (sel, idx) if return_index else sel
+
+
 def mean_shift_fit(votes, valid=None, bandwidth=0.05, max_iter=300, return_modes=False):
     """Gaussian mean shift of ``G`` independent vote sets in one persistent kernel: the batched form of
     ``MeanShiftTorch.fit`` (utils/meanshift_pytorch.py:33-57).

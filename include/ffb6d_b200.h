@@ -549,6 +549,33 @@ int ffb6d_mean_shift_fit(const float *votes, const unsigned char *valid, int64_t
  */
 int ffb6d_best_fit_transform(const float *A, const float *B, int64_t G, int64_t M, double *T, ffb6d_stream_t stream);
 
+/* ---- farthest point sampling (object keypoints) -------------------------- */
+/*
+ * Farthest point sampling of G clouds, replacing the reference's farthest_point_sampling /
+ * farthest_point_sampling_init_center (utils/dataset_tools/fps/src/farthest_point_sampling.cpp:166-204, called by
+ * fps/fps_utils.py:8-23 for the keypoints of utils/dataset_tools/gen_obj_info.py:86-117).  Bitwise the reference's
+ * selection: squared distances (p - q).(p - q) summed x, y, z in round-to-nearest fp32 without FMA; the arg-max
+ * takes the first index with a strictly greater min_dist from (index 0, 0.f), so when every remaining distance is 0
+ * (duplicate points, S > n) index 0 is selected again.
+ *   pts [G,P,3] f32; n_points_per_cloud [G] int32 (device) or NULL: cloud g is its first n_g points, 1 <= n_g <= P
+ *   (NULL: every cloud has P); start [G] int32 (device): the first index of each cloud (the reference draws it with
+ *   rand()), unread with init_center, which starts from the point farthest from the centre of the bounding box
+ *   -> idx_out [G,S] int32.  A cloud whose n_g or start lies out of range gets a row of -1.
+ * One thread-block cluster of ceil(P / 14336) CTAs per cloud keeps it in shared memory (DESIGN.md §4.22).
+ * 1 <= G <= FFB6D_FPS_MAX_CLOUDS, 1 <= P <= FFB6D_FPS_MAX_POINTS, 1 <= S <= FFB6D_FPS_MAX_SAMPLES; pointers 4-byte
+ * aligned.  The kernel needs no workspace: ffb6d_farthest_point_sampling_workspace_bytes returns 0 and ws may be
+ * NULL.  Sizes and pointers are checked before the launch (FFB6D_ERR_INVALID); one launch, no allocation, no host
+ * synchronisation (capturable in a CUDA graph); deterministic.
+ */
+#define FFB6D_FPS_MAX_CLUSTER 8
+#define FFB6D_FPS_MAX_POINTS (FFB6D_FPS_MAX_CLUSTER * 14336)
+#define FFB6D_FPS_MAX_SAMPLES FFB6D_FPS_MAX_POINTS
+#define FFB6D_FPS_MAX_CLOUDS 65535
+size_t ffb6d_farthest_point_sampling_workspace_bytes(int64_t G, int64_t P, int64_t S);
+int ffb6d_farthest_point_sampling(const float *pts, const int *n_points_per_cloud, int64_t G, int64_t P, int64_t S,
+                                  const int *start, int init_center, int *idx_out, void *ws, size_t ws_bytes,
+                                  ffb6d_stream_t stream);
+
 /* ---- grid subsampling --------------------------------------------------- */
 /*
  * Voxel-grid barycentre subsampling, replaces grid_subsampling()
