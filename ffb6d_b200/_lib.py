@@ -126,6 +126,10 @@ def _load():
         "ffb6d_psp_pool_bwd": (ci, [vp, i64, i64, i64, i64, vp, vp]),
         "ffb6d_log_softmax_bwd": (ci, [vp, vp, i64, i64, i64, vp, vp]),
         "ffb6d_upsample_bilinear2d_bwd": (ci, [vp, i64, i64, i64, i64, i64, i64, vp, vp]),
+        "ffb6d_upconv_taps_fwd": (ci, [vp, i64, i64, i64, i64, i64, i64, vp, vp, vp, vp, vp, vp]),
+        "ffb6d_upconv_taps_bwd": (ci, [vp, i64, i64, i64, i64, i64, i64, vp, vp]),
+        "ffb6d_prelu_fwd": (ci, [vp, i64, vp, vp, vp]),
+        "ffb6d_bn_prelu_bwd": (ci, [vp, vp, vp, i64, i64, i64, vp, vp, vp, vp]),
         "ffb6d_farthest_point_sampling_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_farthest_point_sampling": (ci, [vp, vp, i64, i64, i64, vp, ci, vp, vp, sz, vp]),
         "ffb6d_grid_subsample_host": (ci, [vp, sz, vp, sz, vp, sz, fp, vp, vp, vp, C.POINTER(sz)]),

@@ -20,6 +20,8 @@ differentiable: under autograd their backward is the adjoint kernels of DESIGN.m
 so follow ``torch.use_deterministic_algorithms(True)``, where torch's adaptive-average-pool and bilinear backwards
 raise.  :meth:`PSPUpsample.forward_fused` is the module with its x2 upsampling's backward on
 :func:`ffb6d_b200.ops.upsample_bilinear2d_bwd`.  ``FFB6D(fused_image_head=True)`` trains through all three.
+:meth:`PSPUpsample.forward_restructured` runs the whole stage (upsampling, 3x3 conv, BatchNorm, PReLU) on the kernels at
+the input's resolution, forward and backward (DESIGN.md §4.23); ``FFB6D(fused_upsample=True)`` takes it.
 """
 import math
 
@@ -191,6 +193,7 @@ class PSPUpsample(nn.Module):
         self.conv = nn.Sequential(nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True),
                                   nn.Conv2d(in_channels, out_channels, 3, padding=1),
                                   nn.BatchNorm2d(out_channels), nn.PReLU())
+        self._upconv_packed = None      # (weight version, ops.UpConvWeights) of forward_restructured
 
     def forward(self, x):
         return self.conv(x)
@@ -203,6 +206,121 @@ class PSPUpsample(nn.Module):
         if up.mode != "bilinear" or not up.align_corners or up.size is not None:
             raise ValueError("forward_fused: bilinear upsampling with align_corners=True by a scale factor only")
         return act(bn(conv(ops.upsample_bilinear2d(x, up.scale_factor))))
+
+    def forward_restructured(self, x):
+        """The same on this package's kernels at the input's resolution, without the upsampled map (DESIGN.md §4.23):
+        ``conv3x3(up(x)) + b = b + sum_t S_t(up(W_t x))``, the stacked GEMM ``[9 Co, Ci] . x`` and a tap epilogue
+        (:func:`ffb6d_b200.ops.upsample_conv3x3`), the weight stacked and packed once per weight version.
+
+        * training mode: :class:`_UpConvTrain`, batch-statistics BatchNorm (running statistics updated as
+          ``nn.BatchNorm2d`` does; synchronised over the ranks after ``convert_sync_batchnorm``), PReLU, and a
+          backward that adds in a fixed order;
+        * eval under autograd: the conv with that backward (:class:`_UpConv`), then the module's BatchNorm and PReLU;
+        * eval without autograd: one epilogue applies the folded BatchNorm and PReLU.
+
+        Raises ``ValueError`` unless the module is x2 bilinear upsampling with ``align_corners=True``, a 3x3 conv with
+        padding 1 and stride 1, and a PReLU with one weight."""
+        from . import modules, ops
+        up, conv, bn, act = self.conv
+        if (up.mode != "bilinear" or not up.align_corners or up.size is not None or
+                tuple(up.scale_factor if isinstance(up.scale_factor, tuple) else (up.scale_factor,) * 2) != (2.0, 2.0)):
+            raise ValueError("forward_restructured: x2 bilinear upsampling with align_corners=True only")
+        if (tuple(conv.kernel_size) != (3, 3) or tuple(conv.padding) != (1, 1) or tuple(conv.stride) != (1, 1) or
+                tuple(conv.dilation) != (1, 1) or conv.groups != 1 or conv.padding_mode != "zeros"):
+            raise ValueError("forward_restructured: a 3x3 conv with padding 1 and stride 1 only")
+        if not isinstance(act, nn.PReLU) or act.weight.numel() != 1:
+            raise ValueError("forward_restructured: nn.PReLU() with one weight only")
+        ops._f32_map(x, "x")
+        packed = modules.weight_cache(self, "_upconv_packed", _version([conv.weight]),
+                                      lambda: ops.upconv_pack(conv.weight))
+        if self.training:
+            B, _, Hi, Wi = x.shape
+            sync = modules.bn_sync(bn, True)
+            momentum = modules.bn_train_momentum(bn, (B, conv.out_channels, 2 * Hi, 2 * Wi), sync)
+            return _UpConvTrain.apply(x, packed, conv.weight, conv.bias, bn.weight, bn.bias, act.weight,
+                                      bn.running_mean, bn.running_var, bn.eps, momentum, sync)
+        if _needs_grad(x, list(self.parameters())):
+            return act(bn(_UpConv.apply(x, packed, conv.weight, conv.bias)))
+        scale, shift = ops.fold_batchnorm(bn)
+        return ops.upsample_conv3x3(x, packed, conv.bias, scale, shift, act.weight)
+
+
+def _upconv_bwd(ctx, dz, x, weight, packed):
+    """``(dx, dW, db)`` of ``z = conv3x3(up(x)) + b`` from ``dz``, per chunk of output channels: the tap adjoint
+    ``G = up^T(S_t^T dz)`` (:func:`ops.upconv_taps_bwd`), ``dW = sum_b G x^T`` (:func:`modules._wgrad`, ordered under
+    deterministic mode) unstacked to ``[Co, Ci, 3, 3]``, ``dx += W_stack^T G`` (the forward GEMM with K = 9 Cc), and
+    ``db`` the sum of ``dz`` (per-plane sums, then the frames in fp64)."""
+    from . import modules, ops
+    B, Ci, Hi, Wi = x.shape
+    w = weight.detach().float()
+    gx = gw = gb = None
+    gws = []
+    for co0, cc in packed.chunks:
+        g = ops.upconv_taps_bwd(dz, co0, cc)                         # [B, 9 cc, Hi, Wi]
+        if ctx.needs_input_grad[2]:
+            gws.append(modules._wgrad(g, x, None, B, 9 * cc, Hi * Wi).view(3, 3, cc, Ci).permute(2, 3, 0, 1))
+        if ctx.needs_input_grad[0]:
+            part = modules._gemm(g, None, ops.upconv_stack(w, co0, cc).t().contiguous())
+            gx = part if gx is None else gx.add_(part)
+        del g
+    if gws:
+        gw = torch.cat(gws, 0).contiguous()
+    if ctx.needs_input_grad[3]:
+        gb = dz.sum(dim=(2, 3)).double().sum(0).float()
+    return gx, gw, gb
+
+
+class _UpConv(torch.autograd.Function):
+    """``conv3x3(up(x)) + b`` of PSPUpsample on the kernels (:func:`ops.upsample_conv3x3`), with its backward
+    (:func:`_upconv_bwd`).  Saves ``x`` only."""
+
+    @staticmethod
+    def forward(ctx, x, packed, weight, bias):
+        from . import ops
+        x = x.contiguous()
+        ctx.packed = packed
+        ctx.save_for_backward(x, weight)
+        return ops.upsample_conv3x3(x, packed, bias)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad):
+        x, weight = ctx.saved_tensors
+        gx, gw, gb = _upconv_bwd(ctx, grad.contiguous(), x, weight, ctx.packed)
+        return gx, None, gw, gb
+
+
+class _UpConvTrain(torch.autograd.Function):
+    """PSPUpsample in training mode: ``z = conv3x3(up(x)) + b`` (:func:`ops.upsample_conv3x3`), BatchNorm with batch
+    statistics (:func:`modules._bn_act_fwd`, SyncBatchNorm included), PReLU (:func:`ops.prelu_`, in place on the
+    BatchNorm's output).  Saves ``x``, ``z`` and the BatchNorm's stats; the backward recomputes the PReLU's input
+    (:func:`ops.bn_prelu_bwd`), then :func:`modules._bn_act_bwd` and :func:`_upconv_bwd`."""
+
+    @staticmethod
+    def forward(ctx, x, packed, weight, bias, gamma, beta, alpha, running_mean, running_var, eps, momentum, sync):
+        from . import modules, ops
+        x = x.contiguous()
+        z = ops.upsample_conv3x3(x, packed, bias)
+        B, Co, Ho, Wo = z.shape
+        y, stats, count = modules._bn_act_fwd(z, B, Co, Ho * Wo, gamma, beta, running_mean, running_var, eps, momentum,
+                                              modules._ACT_NONE, 0.0, True, sync)
+        ops.prelu_(y, alpha)
+        ctx.packed, ctx.sync = packed, sync
+        ctx.save_for_backward(x, z, stats, count, weight, alpha)
+        return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad):
+        from . import modules, ops
+        x, z, stats, count, weight, alpha = ctx.saved_tensors
+        B, Co, Ho, Wo = z.shape
+        gu, galpha = ops.bn_prelu_bwd(z, grad.contiguous(), stats, alpha)
+        dz, ggamma, gbeta = modules._bn_act_bwd(z, gu, stats, B, Co, Ho * Wo, modules._ACT_NONE, 0.0, True, ctx.sync,
+                                                count)
+        del gu
+        gx, gw, gb = _upconv_bwd(ctx, dz, x, weight, ctx.packed)
+        return gx, None, gw, gb, ggamma, gbeta, galpha.reshape(alpha.shape), None, None, None, None, None
 
 
 class Final(nn.Sequential):

@@ -251,35 +251,6 @@ log_softmax_bwd_kernel(const float *__restrict__ gout, const float *__restrict__
 // (lambda_y * lambda_x) * grad in fp64 -- weight-0 taps included -- and rounds once.
 constexpr int UPB_THREADS = 256;
 
-struct AcAxis {
-    float scale;
-    int in, out;
-    __device__ __forceinline__ int i0(int dst) const
-    {
-        return min((int)__fmul_rn(scale, (float)dst), in - 1);
-    }
-    // the first dst whose i0 is >= t (out if none)
-    __device__ __forceinline__ int first_ge(int t) const
-    {
-        int d = (scale > 0.f) ? (int)fmin((double)t / (double)scale, (double)out) : (t <= 0 ? 0 : out);
-        d = max(0, min(d, out));
-        while (d > 0 && i0(d - 1) >= t) --d;
-        while (d < out && i0(d) < t) ++d;
-        return d;
-    }
-    // the weights with which dst taps v: i0(dst) == v contributes lambda0, i1(dst) == v lambda1
-    __device__ __forceinline__ void tap(int dst, int v, bool &h0, float &l0, bool &h1, float &l1) const
-    {
-        const float src = __fmul_rn(scale, (float)dst);
-        const int a = min((int)src, in - 1);
-        const int a1 = a + ((a < in - 1) ? 1 : 0);
-        l1 = __fsub_rn(src, (float)a);
-        l0 = __fsub_rn(1.f, l1);
-        h0 = (a == v);
-        h1 = (a1 == v);
-    }
-};
-
 __global__ void __launch_bounds__(UPB_THREADS)
 upsample_bilinear_ac_bwd_kernel(const float *__restrict__ gout, long long planes, int Hi, int Wi, int Ho, int Wo,
                                 float *__restrict__ gin)

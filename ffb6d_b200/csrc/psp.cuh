@@ -56,4 +56,48 @@ __device__ __forceinline__ PspTap psp_tap(int dst, int out_size, int in_size)
     return t;
 }
 
+// One axis of upsample_bilinear2d with align_corners=True (PSPUpsample's x2), in torch's float arithmetic: scale =
+// (float)(in - 1) / (out - 1) (0 when out == 1), src = scale * dst, i0 = (int)src, i1 = i0 + (i0 < in - 1),
+// lambda1 = src - i0, lambda0 = 1 - lambda1.  Shared by the upsampling's adjoint (psp.cu) and the restructured
+// upsample + 3x3 conv (upconv.cu), so that both read the taps torch's forward reads.
+struct AcAxis {
+    float scale;
+    int in, out;
+    __device__ __forceinline__ int i0(int dst) const
+    {
+        return min((int)__fmul_rn(scale, (float)dst), in - 1);
+    }
+    // the first dst whose i0 is >= t (out if none)
+    __device__ __forceinline__ int first_ge(int t) const
+    {
+        int d = (scale > 0.f) ? (int)fmin((double)t / (double)scale, (double)out) : (t <= 0 ? 0 : out);
+        d = max(0, min(d, out));
+        while (d > 0 && i0(d - 1) >= t) --d;
+        while (d < out && i0(d) < t) ++d;
+        return d;
+    }
+    // the two source coordinates of dst and their weights
+    __device__ __forceinline__ void taps(int dst, int &a0, int &a1, float &l0, float &l1) const
+    {
+        const float src = __fmul_rn(scale, (float)dst);
+        a0 = min((int)src, in - 1);
+        a1 = a0 + ((a0 < in - 1) ? 1 : 0);
+        l1 = __fsub_rn(src, (float)a0);
+        l0 = __fsub_rn(1.f, l1);
+    }
+    // the weights with which dst taps v: i0(dst) == v contributes lambda0, i1(dst) == v lambda1
+    __device__ __forceinline__ void tap(int dst, int v, bool &h0, float &l0, bool &h1, float &l1) const
+    {
+        int a, a1;
+        taps(dst, a, a1, l0, l1);
+        h0 = (a == v);
+        h1 = (a1 == v);
+    }
+};
+
+__device__ __forceinline__ AcAxis ac_axis(int in, int out)
+{
+    return AcAxis{(out > 1) ? (float)(in - 1) / (float)(out - 1) : 0.f, in, out};
+}
+
 }  // namespace ffb6d

@@ -135,7 +135,8 @@ class _GraphedStep:
         model = self.model
         key = [torch.are_deterministic_algorithms_enabled(), torch.backends.cudnn.deterministic,
                torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32,
-               bool(model.restructured), bool(model.fused_lfa), bool(getattr(model, "fused_image_head", False))]
+               bool(model.restructured), bool(model.fused_lfa), bool(getattr(model, "fused_image_head", False)),
+               bool(getattr(model, "fused_upsample", False))]
         for m in self._modules:
             key += (m.training, tuple(map(id, m._modules.values())))
             if isinstance(m, nn.modules.batchnorm._BatchNorm):
@@ -373,7 +374,7 @@ class GraphedEvalStep(_GraphedStep):
     buffers as they are then: optimizer steps, ``load_state_dict``, new running statistics and
     :class:`GraphedTrainStep` replays between calls need no new capture.  What capture bakes in is compared before
     every replay (DESIGN.md §4.21): the module tree and every module's ``training``, ``restructured``,
-    ``fused_lfa``, ``fused_image_head``, torch's deterministic, cuDNN and TF32 switches, BatchNorm ``eps``, and the
+    ``fused_lfa``, ``fused_image_head``, ``fused_upsample``, torch's deterministic, cuDNN and TF32 switches, BatchNorm ``eps``, and the
     identity and storage of every parameter and buffer; any change captures again (``captures`` counts).
 
     Rejected with ``ValueError``: a model in training mode; a ``DistributedDataParallel`` / ``DataParallel`` wrapper

@@ -179,8 +179,8 @@ class FFB6D(FFB6DFusionNet):
     * Training mode, or whenever autograd needs the image branch: its torch modules (cuDNN, batch statistics, active
       dropout), as the reference.
     * Eval mode without autograd: the PSP head (:meth:`ffb6d_b200.cnn.PSPModule.forward_fused`) and both uses of
-      ``final`` (:meth:`ffb6d_b200.cnn.Final.forward_fused`) run on this package's kernels; the trunk and the
-      ``PSPUpsample`` stages stay on cuDNN.
+      ``final`` (:meth:`ffb6d_b200.cnn.Final.forward_fused`) run on this package's kernels; the trunk and (unless
+      ``fused_upsample``) the ``PSPUpsample`` stages stay on cuDNN.
     * ``fused_image_head=True`` (a plain attribute like ``restructured``; it may be switched on a built or loaded
       model and does not change the state dict): whenever autograd needs the image branch, the PSP head, the x2
       upsampling of ``up_1`` / ``up_2`` / ``up_3`` and both uses of ``final`` run their ``forward_fused`` paths,
@@ -188,13 +188,19 @@ class FFB6D(FFB6DFusionNet):
       whole network trains under ``torch.use_deterministic_algorithms(True)``, where torch's adaptive-average-pool
       and bilinear-upsampling backwards raise.  The trunk, the 3x3 convs, BatchNorms and PReLUs of ``PSPUpsample``
       and the dropouts stay torch modules (the CUDA RNG is drawn as on the torch path).  Off by default.
+    * ``fused_upsample=True`` (a plain attribute like ``fused_image_head``, independent of it): ``up_1``, ``up_2`` and
+      ``up_3`` run :meth:`ffb6d_b200.cnn.PSPUpsample.forward_restructured` -- upsampling, 3x3 conv, BatchNorm and
+      PReLU on this package's kernels at the input's resolution (DESIGN.md §4.23) -- in training and in eval, with
+      or without autograd.  ``drop_2`` stays torch's.  Off by default.
     * ``fused_lfa``: as :class:`FFB6DFusionNet`."""
 
-    def __init__(self, n_classes, n_pts=12288, n_kps=8, restructured=False, fused_image_head=False, fused_lfa=False):
+    def __init__(self, n_classes, n_pts=12288, n_kps=8, restructured=False, fused_image_head=False, fused_lfa=False,
+                 fused_upsample=False):
         super().__init__(n_classes=n_classes, n_pts=n_pts, n_kps=n_kps, restructured=restructured,
                          fused_lfa=fused_lfa)
         self.cnn_pre_stages, self.cnn_ds_stages, self.cnn_up_stages = cnn.image_branch()
         self.fused_image_head = bool(fused_image_head)
+        self.fused_upsample = bool(fused_upsample)
 
     def _image_needs_grad(self, rgb):
         return torch.is_grad_enabled() and (rgb.requires_grad or any(
@@ -207,6 +213,12 @@ class FFB6D(FFB6DFusionNet):
         train_fused = self.fused_image_head and needs_grad
         final = self.cnn_up_stages[2][0]
         up = self.cnn_up_stages
+        fused_up = self.fused_upsample
+
+        def upsample(m, prev):
+            if fused_up:
+                return m.forward_restructured(prev)
+            return m.forward_fused(prev) if train_fused else m(prev)
 
         def stage(j, prev):
             if j == 0:
@@ -214,19 +226,17 @@ class FFB6D(FFB6DFusionNet):
             if train_fused and j == 3:
                 psp, drop_1 = self.cnn_ds_stages[3]
                 return drop_1(psp.forward_fused(prev))
-            if train_fused and j in (4, 5):
+            if (train_fused or fused_up) and j in (4, 5):
                 ups, drop_2 = up[j - 4]
-                return drop_2(ups.forward_fused(prev))
-            if train_fused and j == 6:
+                return drop_2(upsample(ups, prev))
+            if (train_fused or fused) and j == 6:
                 return final.forward_fused(prev)
-            if train_fused and j == 7:
-                return final.forward_fused(up[3][0].forward_fused(prev))
+            if (train_fused or fused) and j == 7:
+                return final.forward_fused(upsample(up[3][0], prev))             # up_3, then final
+            if fused_up and j == 7:
+                return final(upsample(up[3][0], prev))
             if fused and j == 3:
                 return self.cnn_ds_stages[3][0].forward_fused(prev)              # psp (+ drop_1, identity in eval)
-            if fused and j == 6:
-                return final.forward_fused(prev)
-            if fused and j == 7:
-                return final.forward_fused(self.cnn_up_stages[3][0](prev))      # up_3, then final
             return (self.cnn_ds_stages[j] if j < 4 else self.cnn_up_stages[j - 4])(prev)
 
         out = super().forward(inputs, rgb_stage_fn=stage)

@@ -281,6 +281,33 @@ class _InterpConvBnActTrain(torch.autograd.Function):
         return gx1, gp, None, gw, gbias, ggamma, gbeta, None, None, None, None, None, None, None, None
 
 
+def bn_sync(bn, training):
+    """``(process group, world size)`` when the training-mode BatchNorm ``bn`` normalises with the statistics of every
+    rank, decided as ``nn.SyncBatchNorm.forward`` does: the layer is training, its BatchNorm is an
+    ``nn.SyncBatchNorm``, torch.distributed is initialised, and the group (``process_group``, or WORLD) has more
+    than one rank.  None otherwise: the layer's own batch, today's kernels."""
+    if not (training and isinstance(bn, nn.SyncBatchNorm) and dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group if bn.process_group is not None else dist.group.WORLD
+    world = dist.get_world_size(group)
+    return (group, world) if world > 1 else None
+
+
+def bn_train_momentum(bn, shape, sync=None):
+    """Training-mode BatchNorm bookkeeping before a forward on an input of ``shape`` ``(B, C, ...)``, as
+    nn.BatchNorm2d does it: rejects one value per channel (unless synchronised over several ranks, as
+    nn.SyncBatchNorm), counts the batch, returns the momentum to update the running statistics with."""
+    if sync is None and shape[0] * math.prod(shape[2:]) == 1:     # as torch's BatchNorm in training
+        raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                         % (torch.Size((shape[0], bn.num_features) + tuple(shape[2:])),))
+    if bn.track_running_stats and bn.num_batches_tracked is not None:
+        bn.num_batches_tracked += 1
+    momentum = bn.momentum
+    if momentum is None:     # cumulative moving average, as nn.BatchNorm2d(momentum=None)
+        momentum = 1.0 / float(bn.num_batches_tracked) if bn.num_batches_tracked is not None else 0.0
+    return momentum
+
+
 class _BNWrap(nn.Sequential):
     """The reference's ``_BNBase``: a Sequential holding one BatchNorm2d named ``bn``."""
 
@@ -347,31 +374,10 @@ class _ConvBase(nn.Module):
                             lambda: (ops.fusion_mlp_pack(self._conv.weight.detach()),) + self._eval_affine())
 
     def _bn_sync(self):
-        """``(process group, world size)`` when the training-mode BatchNorm normalises with the statistics of every
-        rank, decided as ``nn.SyncBatchNorm.forward`` does: the layer is training, its BatchNorm is an
-        ``nn.SyncBatchNorm``, torch.distributed is initialised, and the group (``process_group``, or WORLD) has more
-        than one rank.  None otherwise: the layer's own batch, today's kernels."""
-        bn = self._bn
-        if not (self.training and isinstance(bn, nn.SyncBatchNorm) and dist.is_available() and dist.is_initialized()):
-            return None
-        group = bn.process_group if bn.process_group is not None else dist.group.WORLD
-        world = dist.get_world_size(group)
-        return (group, world) if world > 1 else None
+        return bn_sync(self._bn, self.training)
 
     def _train_momentum(self, x, sync=None):
-        """Training-mode BatchNorm bookkeeping before a forward, as nn.BatchNorm2d does it: rejects one value per
-        channel (unless synchronised over several ranks, as nn.SyncBatchNorm), counts the batch, returns the momentum
-        to update the running statistics with."""
-        bn = self._bn
-        if sync is None and x.shape[0] * math.prod(x.shape[2:]) == 1:     # as torch's BatchNorm in training
-            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
-                             % (torch.Size((x.shape[0], bn.num_features) + tuple(x.shape[2:])),))
-        if bn.track_running_stats and bn.num_batches_tracked is not None:
-            bn.num_batches_tracked += 1
-        momentum = bn.momentum
-        if momentum is None:     # cumulative moving average, as nn.BatchNorm2d(momentum=None)
-            momentum = 1.0 / float(bn.num_batches_tracked) if bn.num_batches_tracked is not None else 0.0
-        return momentum
+        return bn_train_momentum(self._bn, x.shape, sync)
 
     def _frozen_bn_act(self, z):
         """Eval-mode BatchNorm and the activation as differentiable elementwise torch ops."""

@@ -1631,3 +1631,138 @@ def upsample_bilinear2d(x, scale_factor=2):
     :func:`upsample_bilinear2d_bwd`.  :param x: ``[B,C,H,W]`` float32 CUDA."""
     _f32_map(x, "x")
     return _UpsampleBilinear2d.apply(x, scale_factor)
+
+
+# --------------------------------------------------------------------------- PSPUpsample at the input's resolution
+def upconv_chunk(Ci, Co):
+    """Output channels per chunk of :func:`upsample_conv3x3`: the chunk's tap table ``[B, 9 Cc, Hi, Wi]`` is at most
+    the upsampled input ``[B, Ci, 2 Hi, 2 Wi]`` the torch path forms (``9 Cc <= 4 Ci``; one channel when ``Ci < 3``)."""
+    return max(1, min(int(Co), 4 * int(Ci) // 9))
+
+
+class UpConvWeights:
+    """A 3x3 conv's weight ``[Co, Ci, 3, 3]`` stacked by tap and packed for :func:`upsample_conv3x3`, one
+    :class:`PackedWeight` per chunk of :func:`upconv_chunk` output channels: chunk ``(co0, Cc)`` holds ``[9 Cc, Ci]``
+    with row ``t Cc + j = W[co0 + j, :, ky, kx]``, ``t = 3 ky + kx``.  Build it once per weight version."""
+
+    def __init__(self, weight):
+        _need_cuda(weight, "weight")
+        if weight.dim() != 4 or tuple(weight.shape[2:]) != (3, 3):
+            raise ValueError("UpConvWeights: a [Co, Ci, 3, 3] weight expected, got %s" % (tuple(weight.shape),))
+        w = weight.detach().float()
+        self.Co, self.Ci = int(w.shape[0]), int(w.shape[1])
+        self.device = w.device
+        cc = upconv_chunk(self.Ci, self.Co)
+        self.chunks = [(co0, min(cc, self.Co - co0)) for co0 in range(0, self.Co, cc)]
+        self.packs = [PackedWeight(upconv_stack(w, co0, n)) for co0, n in self.chunks]
+
+
+def upconv_stack(weight, co0, cc):
+    """Rows ``t cc + j = weight[co0 + j, :, ky, kx]`` (``t = 3 ky + kx``) of a ``[Co, Ci, 3, 3]`` weight: ``[9 cc, Ci]``."""
+    return weight[co0:co0 + cc].permute(2, 3, 0, 1).reshape(9 * cc, weight.shape[1])
+
+
+def upconv_pack(weight):
+    """:class:`UpConvWeights` of a 3x3 conv's weight ``[Co, Ci, 3, 3]``."""
+    return UpConvWeights(weight)
+
+
+def _opt_f32(t, n, name, dev):
+    if t is None:
+        return None
+    _need_cuda(t, name)
+    t = t.detach().float().contiguous()
+    if t.numel() != n or t.device != dev:
+        raise ValueError("%s must have %d elements on %s" % (name, n, dev))
+    return t
+
+
+def upconv_taps_fwd(table, out, co0, bias=None, scale=None, shift=None, alpha=None):
+    """The epilogue of :func:`upsample_conv3x3` (``ffb6d_upconv_taps_fwd``, one launch): writes the chunk of output
+    channels ``co0 .. co0 + Cc - 1`` of ``out [B, Co, 2 Hi, 2 Wi]`` from its tap table ``table [B, 9 Cc, Hi, Wi]``:
+    ``act(affine(bias + sum of the nine shifted, upsampled planes))``; ``scale``/``shift`` ``[Co]`` the folded
+    BatchNorm, ``alpha [1]`` PReLU's weight (each optional).  Returns ``out``."""
+    t = _f32_map(table, "table")
+    o = _f32_map(out, "out")
+    if o.data_ptr() != out.data_ptr() or o.device != t.device:
+        raise ValueError("out must be contiguous and on the table's device (it is written in place)")
+    B, C9, Hi, Wi = t.shape
+    Co = o.shape[1]
+    if C9 % 9 or o.shape[0] != B or tuple(o.shape[2:]) != (2 * Hi, 2 * Wi):
+        raise ValueError("table [B, 9 Cc, Hi, Wi] and out [B, Co, 2 Hi, 2 Wi] expected, got %s and %s"
+                         % (tuple(t.shape), tuple(o.shape)))
+    if (scale is None) != (shift is None):
+        raise ValueError("scale and shift come together")
+    b, sc, sh = (_opt_f32(v, Co, n, t.device) for v, n in ((bias, "bias"), (scale, "scale"), (shift, "shift")))
+    a = _opt_f32(alpha, 1, "alpha", t.device)
+    ptr = lambda v: v.data_ptr() if v is not None else None
+    with torch.cuda.device(t.device):
+        check(lib.ffb6d_upconv_taps_fwd(t.data_ptr(), B, Co, int(co0), C9 // 9, Hi, Wi, ptr(b), ptr(sc), ptr(sh), ptr(a),
+                                        o.data_ptr(), _stream(t.device)))
+    return out
+
+
+def upconv_taps_bwd(grad_z, co0, cc):
+    """Adjoint of :func:`upconv_taps_fwd`'s tap sum (``ffb6d_upconv_taps_bwd``, one launch) for the chunk of ``cc``
+    output channels from ``co0``: ``grad_z [B, Co, Ho, Wo]`` (Ho, Wo even) -> ``[B, 9 cc, Ho / 2, Wo / 2]``."""
+    g = _f32_map(grad_z, "grad_z")
+    B, Co, Ho, Wo = g.shape
+    if Ho % 2 or Wo % 2:
+        raise ValueError("grad_z must be [B, Co, 2 Hi, 2 Wi], got %s" % (tuple(g.shape),))
+    gt = torch.empty((B, 9 * int(cc), Ho // 2, Wo // 2), dtype=torch.float32, device=g.device)
+    with torch.cuda.device(g.device):
+        check(lib.ffb6d_upconv_taps_bwd(g.data_ptr(), B, Co, int(co0), int(cc), Ho // 2, Wo // 2, gt.data_ptr(),
+                                        _stream(g.device)))
+    return gt
+
+
+def upsample_conv3x3(x, weights, bias=None, scale=None, shift=None, alpha=None, out=None):
+    """``conv3x3(upsample_x2(x, align_corners=True)) + bias``, padding 1, without the upsampled map: per chunk of
+    output channels the stacked GEMM at the input's resolution (``ffb6d_fusion_mlp_fwd_ex`` with the packed
+    :class:`UpConvWeights`) and its tap epilogue (:func:`upconv_taps_fwd`), optionally followed by the folded BatchNorm
+    ``scale``/``shift`` and PReLU ``alpha``.  :param x: ``[B, Ci, Hi, Wi]`` float32 CUDA.  :return: ``[B, Co, 2 Hi, 2 Wi]``"""
+    xc = _f32_map(x, "x")
+    B, Ci, Hi, Wi = xc.shape
+    if not isinstance(weights, UpConvWeights):
+        raise TypeError("weights must be ops.upconv_pack(conv.weight)")
+    if Ci != weights.Ci or weights.device != xc.device:
+        raise ValueError("the conv takes %d channels on %s, x has %d on %s" % (weights.Ci, weights.device, Ci, xc.device))
+    if out is None:
+        out = torch.empty((B, weights.Co, 2 * Hi, 2 * Wi), dtype=torch.float32, device=xc.device)
+    for (co0, cc), pk in zip(weights.chunks, weights.packs):
+        one, zero = torch.ones(9 * cc, device=xc.device), torch.zeros(9 * cc, device=xc.device)
+        table = fusion_mlp(xc, None, pk, one, zero, relu=False)          # [B, 9 cc, Hi, Wi]
+        upconv_taps_fwd(table, out, co0, bias, scale, shift, alpha)
+        del table
+    return out
+
+
+def prelu_(y, alpha):
+    """``nn.PReLU()`` with one weight, in place on ``y`` float32 CUDA (``ffb6d_prelu_fwd``); ``alpha [1]`` is read on
+    the device, so the call can be captured in a CUDA graph.  Returns ``y``."""
+    _need_cuda(y, "y")
+    if y.dtype != torch.float32 or not y.is_contiguous():
+        raise ValueError("y must be contiguous float32")
+    a = _opt_f32(alpha, 1, "alpha", y.device)
+    with torch.cuda.device(y.device):
+        check(lib.ffb6d_prelu_fwd(y.data_ptr(), y.numel(), a.data_ptr(), y.data_ptr(), _stream(y.device)))
+    return y
+
+
+def bn_prelu_bwd(z, grad_y, stats, alpha):
+    """Backward of ``PReLU(u)``, ``u`` the training BatchNorm's output of ``z [B, C, ...]`` with the forward's
+    ``stats [C, 4]`` (``ffb6d_bn_prelu_bwd``, one launch; ``u`` recomputed, not saved).  :return: ``(grad_u,
+    grad_alpha [1])``; grad_alpha is the fp64 row sums added in a fixed order."""
+    _need_cuda(z, "z")
+    if z.dtype != torch.float32 or z.dim() < 2 or not z.is_contiguous():
+        raise ValueError("z must be contiguous float32 [B, C, ...]")
+    B, Cn = z.shape[0], z.shape[1]
+    g = _f32(grad_y, "grad_y", z.shape)
+    st = _f32(stats, "stats", (Cn, 4))
+    a = _opt_f32(alpha, 1, "alpha", z.device)
+    gu = torch.empty_like(z)
+    part = torch.empty(B * Cn, dtype=torch.float64, device=z.device)
+    with torch.cuda.device(z.device):
+        check(lib.ffb6d_bn_prelu_bwd(z.data_ptr(), g.data_ptr(), st.data_ptr(), B, Cn, z.numel() // (B * Cn),
+                                     a.data_ptr(), gu.data_ptr(), part.data_ptr(), _stream(z.device)))
+    return gu, part.sum().float().reshape(1)

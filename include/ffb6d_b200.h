@@ -753,6 +753,37 @@ int ffb6d_log_softmax_bwd(const float *grad_out, const float *out, int64_t B, in
 int ffb6d_upsample_bilinear2d_bwd(const float *grad_out, int64_t B, int64_t C, int64_t Hi, int64_t Wi, int64_t Ho,
                                   int64_t Wo, float *grad_in, ffb6d_stream_t stream);
 
+/*
+ * PSPUpsample (x2 bilinear upsampling with align_corners=True, 3x3 conv with padding 1, BatchNorm, PReLU) at the
+ * input's resolution (DESIGN.md §4.23): conv3x3(up(x)) + b = b + sum_t S_t(up(W_t x)), W_t = W[:, :, ky, kx],
+ * t = 3 ky + kx, S_t the shift to tap t on the upsampled grid.  The stacked product T = [W_0; ..; W_8] x of a chunk
+ * of Cc output channels co0 .. co0 + Cc - 1 (row t Cc + j = W[co0 + j, :, ky, kx]) is ffb6d_fusion_mlp_fwd_ex with
+ * the packed stacked weight; T is [B, 9 Cc, Hi, Wi].  Ho = 2 Hi, Wo = 2 Wi.  The taps are torch's float taps (as
+ * ffb6d_upsample_bilinear2d_bwd), all four read even at weight 0.  Every call checks sizes (1 <= B, Co, Cc, Hi, Wi;
+ * 0 <= co0, co0 + Cc <= Co; Hi, Wi < 2^23; B Co, 9 B Cc < 2^31), null pointers and 4-byte alignment before any
+ * launch (FFB6D_ERR_INVALID); one launch each, no allocation, no host synchronisation, no atomics: every output
+ * element is written once, its sum taken in a fixed order.
+ *
+ * ffb6d_upconv_taps_fwd: out[b, co0 + j, y, x] = act(affine(bias[co] + sum_t sum_4 lambda T[b, t Cc + j, src])) into
+ *   out [B, Co, Ho, Wo] (the chunk's channels only).  bias may be NULL (0); scale and shift (folded eval BatchNorm,
+ *   v * scale + shift) both or neither; alpha (PReLU's one weight, read on the device) may be NULL (no activation).
+ * ffb6d_upconv_taps_bwd: the adjoint, grad_table [B, 9 Cc, Hi, Wi] = up^T(S_t^T grad_z[:, co0 + j]) from
+ *   grad_z [B, Co, Ho, Wo], sums in fp64.
+ * ffb6d_prelu_fwd: y = x > 0 ? x : alpha[0] x over n elements (x may be y).  n < 2^50.
+ * ffb6d_bn_prelu_bwd: the backward of PReLU(u), u the training BatchNorm's output, recomputed from z [B, C, P] and the
+ *   stats [C, 4] of ffb6d_bn_train_fwd / ffb6d_bn_sync_fwd (16-byte aligned) as those kernels compute it: grad_u =
+ *   u > 0 ? grad_y : alpha grad_y, and grad_alpha_part [B C] fp64 (8-byte aligned), each (frame, channel) row's sum of
+ *   u grad_y where u <= 0, added in a fixed order.  B C < 2^31.
+ */
+int ffb6d_upconv_taps_fwd(const float *table, int64_t B, int64_t Co, int64_t co0, int64_t Cc, int64_t Hi, int64_t Wi,
+                          const float *bias, const float *scale, const float *shift, const float *alpha, float *out,
+                          ffb6d_stream_t stream);
+int ffb6d_upconv_taps_bwd(const float *grad_z, int64_t B, int64_t Co, int64_t co0, int64_t Cc, int64_t Hi, int64_t Wi,
+                          float *grad_table, ffb6d_stream_t stream);
+int ffb6d_prelu_fwd(const float *x, int64_t n, const float *alpha, float *y, ffb6d_stream_t stream);
+int ffb6d_bn_prelu_bwd(const float *z, const float *grad_y, const float *stats, int64_t B, int64_t C, int64_t P,
+                       const float *alpha, float *grad_u, double *grad_alpha_part, ffb6d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
