@@ -8,6 +8,8 @@ it.  Build it with ``python -c "import __graft_entry__ as g; g.build()"`` or
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libffb6d_b200.so")
 
@@ -67,7 +69,6 @@ def _load():
         "ffb6d_gather_neighbour_fwd": (ci, [vp, vp, ci, i64, i64, i64, i64, ci, vp, vp]),
         "ffb6d_gather_neighbour_bwd": (ci, [vp, vp, ci, i64, i64, i64, i64, ci, vp, vp]),
         "ffb6d_relative_pos_encoding_fwd": (ci, [vp, vp, ci, i64, i64, ci, vp, vp]),
-        "ffb6d_fusion_mlp_fwd": (ci, [vp, i64, vp, i64, vp, vp, vp, i64, i64, i64, ci, fp, vp, vp]),
         "ffb6d_fusion_mlp_pack_bytes": (sz, [i64, i64]),
         "ffb6d_fusion_mlp_pack": (ci, [vp, i64, i64, vp, sz, vp]),
         "ffb6d_fusion_mlp_fwd_packed": (ci, [vp, i64, vp, i64, vp, vp, vp, i64, i64, i64, ci, fp, vp, vp]),
@@ -151,6 +152,30 @@ def last_error():
 def check(rc):
     if rc != OK:
         raise FFB6DError(rc, last_error())
+
+
+def stream(device):
+    """The current torch stream of ``device`` as the ``ffb6d_stream_t`` argument of an entry point."""
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+def launch(fn, device, *args):
+    """``fn(*args, stream(device))`` with ``device`` current: how every device entry point of the library is called
+    (each takes its stream last).  Raises :class:`FFB6DError` on a failed status.  The stream is fetched inline, not
+    through :func:`stream`: this runs once per launch, and an eager training step is host-bound."""
+    with torch.cuda.device(device):
+        check(fn(*args, torch.cuda.current_stream(device).cuda_stream))
+
+
+def ptr(t):
+    """The device pointer of ``t`` for an optional argument: None (NULL) for None."""
+    return None if t is None else t.data_ptr()
+
+
+def workspace(nbytes, device):
+    """Scratch for an entry point whose ``*_bytes`` query answered ``nbytes``: at least 16 bytes, so never NULL even
+    where the answer is 0, and enough for every entry point's minimum.  Pass the entry point ``nbytes`` itself."""
+    return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
 
 
 def launch_count():

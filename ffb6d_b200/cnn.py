@@ -230,7 +230,7 @@ class PSPUpsample(nn.Module):
             raise ValueError("forward_restructured: a 3x3 conv with padding 1 and stride 1 only")
         if not isinstance(act, nn.PReLU) or act.weight.numel() != 1:
             raise ValueError("forward_restructured: nn.PReLU() with one weight only")
-        ops._f32_map(x, "x")
+        ops._tensor(x, "x", shape=4)
         packed = modules.weight_cache(self, "_upconv_packed", _version([conv.weight]),
                                       lambda: ops.upconv_pack(conv.weight))
         if self.training:

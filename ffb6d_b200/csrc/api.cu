@@ -137,7 +137,7 @@ using namespace ffb6d;
 
 extern "C" {
 
-int ffb6d_version(void) { return 2; }
+int ffb6d_version(void) { return 3; }
 const char *ffb6d_last_error(void) { return g_err; }
 uint64_t ffb6d_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 int ffb6d_check_indices_enabled(void) { return env().check_indices ? 1 : 0; }

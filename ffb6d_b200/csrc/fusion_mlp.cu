@@ -787,34 +787,6 @@ extern "C" int ffb6d_fusion_mlp_fwd_packed(const float *x1, int64_t C1, const fl
                                    0, FFB6D_LAYOUT_NCS, out, stream);
 }
 
-extern "C" int ffb6d_fusion_mlp_fwd(const float *x1, int64_t C1, const float *x2, int64_t C2, const float *weight,
-                                    const float *scale, const float *shift, int64_t B, int64_t Co, int64_t P,
-                                    int act, float negative_slope, float *out, ffb6d_stream_t stream)
-{
-    const int rc = mlp_check(x1, C1, x2, C2, weight, scale, shift, B, Co, P, act, out);
-    if (rc != FFB6D_OK) return rc > 0 ? FFB6D_OK : rc;
-    // raw weights: split them into a stream-ordered scratch block first (callers that keep their
-    // weights should pack once with ffb6d_fusion_mlp_pack and call ffb6d_fusion_mlp_fwd_packed)
-    const size_t bytes = ffb6d_fusion_mlp_pack_bytes(Co, C1 + C2);
-    static std::atomic<unsigned long long> pool_set_mask{0};
-    const int dev_bit = current_device() & (kMaxDevices - 1);
-    if (!((pool_set_mask.load(std::memory_order_relaxed) >> dev_bit) & 1ull)) {   // keep freed scratch blocks in the stream-ordered pool instead of returning them to the OS
-        int dev = 0;
-        cudaMemPool_t pool;
-        unsigned long long keep = ~0ull;
-        if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess)
-            cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-        pool_set_mask.fetch_or(1ull << dev_bit, std::memory_order_relaxed);
-    }
-    void *scratch = nullptr;
-    FFB6D_CUDA(cudaMallocAsync(&scratch, bytes, (cudaStream_t)stream));
-    int r = ffb6d_fusion_mlp_pack(weight, Co, C1 + C2, scratch, bytes, stream);
-    if (r == FFB6D_OK)
-        r = ffb6d_fusion_mlp_fwd_packed(x1, C1, x2, C2, scratch, scale, shift, B, Co, P, act, negative_slope, out, stream);
-    cudaFreeAsync(scratch, (cudaStream_t)stream);
-    return r;
-}
-
 extern "C" int ffb6d_fusion_mlp_wgrad(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2,
                                       int64_t B, int64_t Co, int64_t P, float *grad_w, ffb6d_stream_t stream)
 {

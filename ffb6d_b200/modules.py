@@ -35,7 +35,7 @@ import torch.nn.functional as F_
 from torch.autograd.graph import increment_version
 
 from . import dist as dist_, fusion, ops
-from ._lib import lib, check
+from ._lib import lib, launch, ptr, workspace
 
 _ACT_NONE, _ACT_RELU, _ACT_LEAKY = 0, 1, 2
 
@@ -96,30 +96,25 @@ def _bn_act_fwd(z, B, Co, P, gamma, beta, running_mean, running_var, eps, moment
         if act == _ACT_RELU:
             return torch.relu(z), None, None
         return (F_.leaky_relu(z, slope) if act == _ACT_LEAKY else z), None, None
-    stats = torch.empty((Co, 4), dtype=torch.float32, device=z.device)
+    dev = z.device
+    stats = torch.empty((Co, 4), dtype=torch.float32, device=dev)
     y = torch.empty_like(z)
     nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=z.device)
-    gamma_p = gamma.data_ptr() if gamma is not None else None
-    beta_p = beta.data_ptr() if beta is not None else None
-    rm_p = running_mean.data_ptr() if running_mean is not None else None
-    rv_p = running_var.data_ptr() if running_var is not None else None
-    with torch.cuda.device(z.device):
-        if sync is None:
-            check(lib.ffb6d_bn_train_fwd(
-                z.data_ptr(), B, Co, P, gamma_p, beta_p, float(eps), float(momentum), rm_p, rv_p, int(act), float(slope),
-                stats.data_ptr(), y.data_ptr(), ws.data_ptr(), nbytes, ops._stream(z.device)))
-            count = None
-        else:
-            group, world = sync
-            row = torch.empty(2 * Co + 1, dtype=torch.float64, device=z.device)
-            check(lib.ffb6d_bn_sync_moments(z.data_ptr(), B, Co, P, row.data_ptr(), ws.data_ptr(), nbytes,
-                                            ops._stream(z.device)))
-            rows = dist_.all_gather_rows(row, group, world)
-            count = torch.empty(1, dtype=torch.float64, device=z.device)
-            check(lib.ffb6d_bn_sync_fwd(
-                z.data_ptr(), B, Co, P, rows.data_ptr(), world, gamma_p, beta_p, float(eps), float(momentum), rm_p,
-                rv_p, int(act), float(slope), stats.data_ptr(), count.data_ptr(), y.data_ptr(), ops._stream(z.device)))
+    ws = workspace(nbytes, dev)
+    if sync is None:
+        launch(lib.ffb6d_bn_train_fwd, dev, z.data_ptr(), B, Co, P, ptr(gamma), ptr(beta), float(eps), float(momentum),
+               ptr(running_mean), ptr(running_var), int(act), float(slope), stats.data_ptr(), y.data_ptr(),
+               ws.data_ptr(), nbytes)
+        count = None
+    else:
+        group, world = sync
+        row = torch.empty(2 * Co + 1, dtype=torch.float64, device=dev)
+        launch(lib.ffb6d_bn_sync_moments, dev, z.data_ptr(), B, Co, P, row.data_ptr(), ws.data_ptr(), nbytes)
+        rows = dist_.all_gather_rows(row, group, world)
+        count = torch.empty(1, dtype=torch.float64, device=dev)
+        launch(lib.ffb6d_bn_sync_fwd, dev, z.data_ptr(), B, Co, P, rows.data_ptr(), world, ptr(gamma), ptr(beta),
+               float(eps), float(momentum), ptr(running_mean), ptr(running_var), int(act), float(slope),
+               stats.data_ptr(), count.data_ptr(), y.data_ptr())
     # the kernels updated the running statistics in place: advance their versions, as torch's in-place update does,
     # so the eval path's version-keyed packs (weight_cache) fold the new statistics, also in a layer whose weights
     # no optimizer step has touched
@@ -132,32 +127,28 @@ def _bn_act_bwd(z, gy, stats, B, Co, P, act, slope, has_bn, sync=None, count=Non
     ``sync`` (and the forward's ``count``) dz uses the sums of every rank (``ffb6d_bn_sync_bwd_sums``, an all-gather,
     ``ffb6d_bn_sync_bwd``); dgamma / dbeta stay this rank's, for the gradient all-reduce of DDP to add."""
     dev = z.device
-    with torch.cuda.device(dev):
-        if has_bn:
-            dz = torch.empty_like(z)
-            ggamma = torch.empty(Co, dtype=torch.float32, device=dev)
-            gbeta = torch.empty(Co, dtype=torch.float32, device=dev)
-            nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            if sync is None:
-                check(lib.ffb6d_bn_train_bwd(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
-                                             ggamma.data_ptr(), gbeta.data_ptr(), dz.data_ptr(), ws.data_ptr(), nbytes,
-                                             ops._stream(dev)))
-                return dz, ggamma, gbeta
-            group, world = sync
-            row = torch.empty(2 * Co, dtype=torch.float64, device=dev)
-            check(lib.ffb6d_bn_sync_bwd_sums(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
-                                             row.data_ptr(), ggamma.data_ptr(), gbeta.data_ptr(), ws.data_ptr(), nbytes,
-                                             ops._stream(dev)))
-            rows = dist_.all_gather_rows(row, group, world)
-            check(lib.ffb6d_bn_sync_bwd(z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, rows.data_ptr(), world,
-                                        count.data_ptr(), act, slope, dz.data_ptr(), ws.data_ptr(), nbytes,
-                                        ops._stream(dev)))
+    if has_bn:
+        dz = torch.empty_like(z)
+        ggamma = torch.empty(Co, dtype=torch.float32, device=dev)
+        gbeta = torch.empty(Co, dtype=torch.float32, device=dev)
+        nbytes = int(lib.ffb6d_bn_workspace_bytes(Co, P))
+        ws = workspace(nbytes, dev)
+        if sync is None:
+            launch(lib.ffb6d_bn_train_bwd, dev, z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
+                   ggamma.data_ptr(), gbeta.data_ptr(), dz.data_ptr(), ws.data_ptr(), nbytes)
             return dz, ggamma, gbeta
-        if act != _ACT_NONE:
-            dz = torch.empty_like(z)
-            check(lib.ffb6d_act_bwd(z.data_ptr(), gy.data_ptr(), z.numel(), act, slope, dz.data_ptr(), ops._stream(dev)))
-            return dz, None, None
+        group, world = sync
+        row = torch.empty(2 * Co, dtype=torch.float64, device=dev)
+        launch(lib.ffb6d_bn_sync_bwd_sums, dev, z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, act, slope,
+               row.data_ptr(), ggamma.data_ptr(), gbeta.data_ptr(), ws.data_ptr(), nbytes)
+        rows = dist_.all_gather_rows(row, group, world)
+        launch(lib.ffb6d_bn_sync_bwd, dev, z.data_ptr(), gy.data_ptr(), stats.data_ptr(), B, Co, P, rows.data_ptr(),
+               world, count.data_ptr(), act, slope, dz.data_ptr(), ws.data_ptr(), nbytes)
+        return dz, ggamma, gbeta
+    if act != _ACT_NONE:
+        dz = torch.empty_like(z)
+        launch(lib.ffb6d_act_bwd, dev, z.data_ptr(), gy.data_ptr(), z.numel(), act, slope, dz.data_ptr())
+        return dz, None, None
     return gy, None, None
 
 
@@ -166,16 +157,13 @@ def _wgrad(dz, x1, x2, B, Co, P):
     :func:`ffb6d_b200.ops.deterministic_backward` ``ffb6d_fusion_mlp_wgrad_det``, the splits added in a fixed order)."""
     C1, C2 = x1.shape[1], (x2.shape[1] if x2 is not None else 0)
     gw = torch.empty((Co, C1 + C2), dtype=torch.float32, device=dz.device)
-    with torch.cuda.device(dz.device):
-        if ops.deterministic_backward(weight_grad=True):
-            nbytes = int(lib.ffb6d_fusion_mlp_wgrad_det_workspace_bytes(C1, C2, B, Co, P))
-            ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dz.device)
-            check(lib.ffb6d_fusion_mlp_wgrad_det(dz.data_ptr(), x1.data_ptr(), C1,
-                                                 x2.data_ptr() if x2 is not None else None, C2, B, Co, P, ws.data_ptr(),
-                                                 nbytes, gw.data_ptr(), ops._stream(dz.device)))
-            return gw
-        check(lib.ffb6d_fusion_mlp_wgrad(dz.data_ptr(), x1.data_ptr(), C1, x2.data_ptr() if x2 is not None else None,
-                                         C2, B, Co, P, gw.data_ptr(), ops._stream(dz.device)))
+    if ops.deterministic_backward(weight_grad=True):
+        nbytes = int(lib.ffb6d_fusion_mlp_wgrad_det_workspace_bytes(C1, C2, B, Co, P))
+        ws = workspace(nbytes, dz.device)
+        launch(lib.ffb6d_fusion_mlp_wgrad_det, dz.device, dz.data_ptr(), x1.data_ptr(), C1, ptr(x2), C2, B, Co, P,
+               ws.data_ptr(), nbytes, gw.data_ptr())
+        return gw
+    launch(lib.ffb6d_fusion_mlp_wgrad, dz.device, dz.data_ptr(), x1.data_ptr(), C1, ptr(x2), C2, B, Co, P, gw.data_ptr())
     return gw
 
 
@@ -528,10 +516,8 @@ class _AttPool(torch.autograd.Function):
         g = gout.contiguous()
         gf1, gatt = torch.empty_like(f1), torch.empty_like(att)
         gf2 = torch.empty_like(f2) if f2 is not None else None
-        with torch.cuda.device(f1.device):
-            check(lib.ffb6d_att_pool_bwd(f1.data_ptr(), C1, f2.data_ptr() if f2 is not None else None, C2, att.data_ptr(),
-                                         g.data_ptr(), B, N, K, gf1.data_ptr(), gf2.data_ptr() if gf2 is not None else None,
-                                         gatt.data_ptr(), ops._stream(f1.device)))
+        launch(lib.ffb6d_att_pool_bwd, f1.device, f1.data_ptr(), C1, ptr(f2), C2, att.data_ptr(), g.data_ptr(), B, N, K,
+               gf1.data_ptr(), ptr(gf2), gatt.data_ptr())
         return gf1, gf2, gatt
 
 

@@ -12,7 +12,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import lib, check, LAYOUT_NCS, LAYOUT_NSC
+from ._lib import lib, check, launch, ptr, workspace, LAYOUT_NCS, LAYOUT_NSC
+from ._lib import stream as _stream   # noqa: F401  (the stream argument for direct lib.* calls: tests and tools)
 
 import os as _os
 _DEBUG_GRID = bool(_os.environ.get("FFB6D_DEBUG_GRID"))   # keep KNN workspaces for tools/grid_debug.py
@@ -21,15 +22,27 @@ _I64 = (torch.int64,)
 _IDX = (torch.int32, torch.int64)
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def _need_cuda(t, name):
     if not isinstance(t, torch.Tensor):
         raise TypeError("%s must be a torch.Tensor, got %r" % (name, type(t)))
     if not t.is_cuda:
         raise RuntimeError("%s must be a CUDA tensor: ffb6d_b200 has no CPU path" % name)
+
+
+def _tensor(t, name, dtype=torch.float32, shape=None, device=None):
+    """``t`` as a kernel reads it: a CUDA tensor of ``dtype``, of ``shape`` (a tuple) or of that many dimensions (an
+    int) when given, on ``device`` when given; returned contiguous.  Raises ValueError otherwise (TypeError /
+    RuntimeError for a non-tensor / a CPU tensor)."""
+    _need_cuda(t, name)
+    if isinstance(shape, int):
+        bad_shape, want = t.dim() != shape, "with %d dims" % shape
+    else:
+        bad_shape, want = shape is not None and tuple(t.shape) != tuple(shape), tuple(shape or ())
+    if t.dtype != dtype or bad_shape:
+        raise ValueError("%s must be %s %s, got %s %s" % (name, dtype, want, t.dtype, tuple(t.shape)))
+    if device is not None and t.device != device:
+        raise ValueError("%s is on %s, expected %s" % (name, t.device, device))
+    return t.contiguous()
 
 
 def deterministic_backward(weight_grad=False):
@@ -101,14 +114,12 @@ def knn_search(support_pts, query_pts, k, out_dtype=None, algo=0):
     if dt not in _IDX:
         raise TypeError("out_dtype must be torch.int32 or torch.int64")
     out = torch.empty((B, Q, k), dtype=dt, device=sup.device)
-    with torch.cuda.device(sup.device):
-        ws_bytes = int(lib.ffb6d_knn_workspace_bytes(B, S, Q, k)) if algo != 1 else 0
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=sup.device) if ws_bytes else None
-        check(lib.ffb6d_knn_batch_algo(sup.data_ptr(), qry.data_ptr(), B, S, Q, k, out.data_ptr(),
-                                       int(dt == torch.int64), ws.data_ptr() if ws is not None else None,
-                                       ws_bytes, int(algo), _stream(sup.device)))
+    ws_bytes = int(lib.ffb6d_knn_workspace_bytes(B, S, Q, k)) if algo != 1 else 0
+    ws = workspace(ws_bytes, sup.device)
+    launch(lib.ffb6d_knn_batch_algo, sup.device, sup.data_ptr(), qry.data_ptr(), B, S, Q, k, out.data_ptr(),
+           int(dt == torch.int64), ws.data_ptr(), ws_bytes, int(algo))
     if _DEBUG_GRID:
-        _debug_ws.append((B, S, Q, k, ws))
+        _debug_ws.append((B, S, Q, k, ws if ws_bytes else None))
     return out
 
 
@@ -131,11 +142,10 @@ class KnnGrid:
         self.support = sup
         self.B, self.S = sup.shape[0], sup.shape[1]
         self.k_hint = int(k_hint)
-        with torch.cuda.device(sup.device):
-            self.nbytes = int(lib.ffb6d_knn_grid_bytes(self.B, self.S))
-            self.mem = torch.empty(self.nbytes, dtype=torch.uint8, device=sup.device)
-            check(lib.ffb6d_knn_grid_build(sup.data_ptr(), self.B, self.S, self.k_hint,
-                                           self.mem.data_ptr(), self.nbytes, _stream(sup.device)))
+        self.nbytes = int(lib.ffb6d_knn_grid_bytes(self.B, self.S))
+        self.mem = torch.empty(self.nbytes, dtype=torch.uint8, device=sup.device)
+        launch(lib.ffb6d_knn_grid_build, sup.device, sup.data_ptr(), self.B, self.S, self.k_hint, self.mem.data_ptr(),
+               self.nbytes)
 
     def query(self, query_pts, k, out_dtype=None, query_width=0):
         """``query_pts [B,Q,3]`` -> ``[B,Q,k]`` neighbour indices into the support (int32 unless
@@ -153,13 +163,11 @@ class KnnGrid:
             raise TypeError("out_dtype must be torch.int32 or torch.int64")
         dev = self.support.device
         out = torch.empty((self.B, Q, k), dtype=dt, device=dev)
-        with torch.cuda.device(dev):
-            sb = int(lib.ffb6d_knn_grid_query_bytes(self.B, Q))
-            scratch = torch.empty(max(sb, 1), dtype=torch.uint8, device=dev)
-            qw = int(query_width) if query_width and Q % int(query_width) == 0 else 0
-            check(lib.ffb6d_knn_grid_query_organized(self.support.data_ptr(), qry.data_ptr(), self.B, self.S, Q, k,
-                                                     out.data_ptr(), int(dt == torch.int64), self.mem.data_ptr(),
-                                                     self.nbytes, scratch.data_ptr(), sb, qw, _stream(dev)))
+        sb = int(lib.ffb6d_knn_grid_query_bytes(self.B, Q))
+        scratch = workspace(sb, dev)
+        qw = int(query_width) if query_width and Q % int(query_width) == 0 else 0
+        launch(lib.ffb6d_knn_grid_query_organized, dev, self.support.data_ptr(), qry.data_ptr(), self.B, self.S, Q, k,
+               out.data_ptr(), int(dt == torch.int64), self.mem.data_ptr(), self.nbytes, scratch.data_ptr(), sb, qw)
         return out
 
 
@@ -192,9 +200,8 @@ class _GatherMax(torch.autograd.Function):
             out = torch.empty((B, Cc, Q), dtype=torch.float32, device=f3.device)
         else:
             out = torch.empty((B, Q, Cc), dtype=torch.float32, device=f3.device).transpose(1, 2)
-        with torch.cuda.device(f3.device):
-            check(lib.ffb6d_gather_max_fwd(f3.data_ptr(), idx_c.data_ptr(), i64, B, Cc, S, Q, K,
-                                           layout, out.data_ptr(), _stream(f3.device)))
+        launch(lib.ffb6d_gather_max_fwd, f3.device, f3.data_ptr(), idx_c.data_ptr(), i64, B, Cc, S, Q, K, layout,
+               out.data_ptr())
         ctx.save_for_backward(f3, idx_c)
         ctx.layout = layout
         return out
@@ -222,10 +229,8 @@ def _gather_max_bwd(f3, idx_c, gout, layout):
             return segment_sum(g, None, S, plan=SegmentPlan(idx_c.reshape(B, Q), S))
         _gather_max_bwd_det(f3, idx_c, g, layout, gf)
         return gf
-    with torch.cuda.device(f3.device):
-        check(lib.ffb6d_gather_max_bwd(f3.data_ptr(), idx_c.data_ptr(),
-                                       int(idx_c.dtype == torch.int64), g.data_ptr(), B, Cc, S,
-                                       Q, K, layout, gf.data_ptr(), _stream(f3.device)))
+    launch(lib.ffb6d_gather_max_bwd, f3.device, f3.data_ptr(), idx_c.data_ptr(), int(idx_c.dtype == torch.int64),
+           g.data_ptr(), B, Cc, S, Q, K, layout, gf.data_ptr())
     return gf
 
 
@@ -240,13 +245,10 @@ def _gather_max_bwd_det(f3, idx_c, g, layout, gf):
     """``ffb6d_gather_max_bwd_det`` into ``gf`` (the backward of :class:`_GatherMax` without atomics)."""
     B, Cc, S = f3.shape
     Q, K = idx_c.shape[1], idx_c.shape[2]
-    dev = f3.device
-    with torch.cuda.device(dev):
-        nbytes = int(lib.ffb6d_gather_max_bwd_det_workspace_bytes(B, Cc, S, Q, K))
-        ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
-        check(lib.ffb6d_gather_max_bwd_det(f3.data_ptr(), idx_c.data_ptr(), int(idx_c.dtype == torch.int64),
-                                           g.data_ptr(), B, Cc, S, Q, K, layout, ws.data_ptr(), nbytes,
-                                           gf.data_ptr(), _stream(dev)))
+    nbytes = int(lib.ffb6d_gather_max_bwd_det_workspace_bytes(B, Cc, S, Q, K))
+    ws = workspace(nbytes, f3.device)
+    launch(lib.ffb6d_gather_max_bwd_det, f3.device, f3.data_ptr(), idx_c.data_ptr(), int(idx_c.dtype == torch.int64),
+           g.data_ptr(), B, Cc, S, Q, K, layout, ws.data_ptr(), nbytes, gf.data_ptr())
 
 
 def _gather_max(feature, idx3):
@@ -314,8 +316,7 @@ def check_indices(idx, S):
     every gather (debugging aid, synchronises)."""
     _need_cuda(idx, "idx")
     idx_c, i64 = _idx_arg(idx, "idx")
-    with torch.cuda.device(idx_c.device):
-        check(lib.ffb6d_check_indices(idx_c.data_ptr(), i64, idx_c.numel(), int(S), _stream(idx_c.device)))
+    launch(lib.ffb6d_check_indices, idx_c.device, idx_c.data_ptr(), i64, idx_c.numel(), int(S))
 
 
 # --------------------------------------------------------------------------- neighbour gather
@@ -327,9 +328,8 @@ class _GatherNeighbour(torch.autograd.Function):
         B, S, D = pc.shape
         N, K = idx_c.shape[1], idx_c.shape[2]
         out = torch.empty((B, N, K, D), dtype=torch.float32, device=pc.device)
-        with torch.cuda.device(pc.device):
-            check(lib.ffb6d_gather_neighbour_fwd(pc.data_ptr(), idx_c.data_ptr(), i64, B, S, D, N, K,
-                                                 out.data_ptr(), _stream(pc.device)))
+        launch(lib.ffb6d_gather_neighbour_fwd, pc.device, pc.data_ptr(), idx_c.data_ptr(), i64, B, S, D, N, K,
+               out.data_ptr())
         ctx.save_for_backward(idx_c)
         ctx.shape = (B, S, D)
         return out
@@ -342,18 +342,15 @@ class _GatherNeighbour(torch.autograd.Function):
         N, K = idx_c.shape[1], idx_c.shape[2]
         g = gout.contiguous()
         gpc = torch.empty((B, S, D), dtype=torch.float32, device=g.device)
+        i64 = int(idx_c.dtype == torch.int64)
         if deterministic_backward():
-            with torch.cuda.device(g.device):
-                nbytes = int(lib.ffb6d_gather_neighbour_bwd_det_workspace_bytes(B, S, N, K))
-                ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=g.device)
-                check(lib.ffb6d_gather_neighbour_bwd_det(g.data_ptr(), idx_c.data_ptr(), int(idx_c.dtype == torch.int64),
-                                                         B, S, D, N, K, ws.data_ptr(), nbytes, gpc.data_ptr(),
-                                                         _stream(g.device)))
+            nbytes = int(lib.ffb6d_gather_neighbour_bwd_det_workspace_bytes(B, S, N, K))
+            ws = workspace(nbytes, g.device)
+            launch(lib.ffb6d_gather_neighbour_bwd_det, g.device, g.data_ptr(), idx_c.data_ptr(), i64, B, S, D, N, K,
+                   ws.data_ptr(), nbytes, gpc.data_ptr())
             return gpc, None
-        with torch.cuda.device(g.device):
-            check(lib.ffb6d_gather_neighbour_bwd(g.data_ptr(), idx_c.data_ptr(),
-                                                 int(idx_c.dtype == torch.int64), B, S, D, N, K,
-                                                 gpc.data_ptr(), _stream(g.device)))
+        launch(lib.ffb6d_gather_neighbour_bwd, g.device, g.data_ptr(), idx_c.data_ptr(), i64, B, S, D, N, K,
+               gpc.data_ptr())
         return gpc, None
 
 
@@ -393,14 +390,11 @@ def relative_pos_encoding(xyz, neigh_idx, channel_major=False):
     K = idx_c.shape[2]
     if channel_major:    # [B,10,N,K]: what .permute((0,3,1,2)).contiguous() gives (RandLANet.py:197-198)
         out = torch.empty((B, 10, N, K), dtype=torch.float32, device=xyz.device)
-        with torch.cuda.device(xyz.device):
-            check(lib.ffb6d_relative_pos_encoding_cm_fwd(xyz.data_ptr(), idx_c.data_ptr(), i64, B, N, K,
-                                                         out.data_ptr(), _stream(xyz.device)))
-        return out
-    out = torch.empty((B, N, K, 10), dtype=torch.float32, device=xyz.device)
-    with torch.cuda.device(xyz.device):
-        check(lib.ffb6d_relative_pos_encoding_fwd(xyz.data_ptr(), idx_c.data_ptr(), i64, B, N, K,
-                                                  out.data_ptr(), _stream(xyz.device)))
+        fn = lib.ffb6d_relative_pos_encoding_cm_fwd
+    else:
+        out = torch.empty((B, N, K, 10), dtype=torch.float32, device=xyz.device)
+        fn = lib.ffb6d_relative_pos_encoding_fwd
+    launch(fn, xyz.device, xyz.data_ptr(), idx_c.data_ptr(), i64, B, N, K, out.data_ptr())
     return out
 
 
@@ -426,9 +420,7 @@ class PackedWeight:
         self.device = w.device
         nbytes = lib.ffb6d_fusion_mlp_pack_bytes(self.Co, self.Ci)
         self.data = torch.empty(nbytes, dtype=torch.uint8, device=w.device)
-        with torch.cuda.device(w.device):
-            check(lib.ffb6d_fusion_mlp_pack(w.data_ptr(), self.Co, self.Ci, self.data.data_ptr(), nbytes,
-                                            _stream(w.device)))
+        launch(lib.ffb6d_fusion_mlp_pack, w.device, w.data_ptr(), self.Co, self.Ci, self.data.data_ptr(), nbytes)
 
 
 def fusion_mlp_pack(weight):
@@ -499,13 +491,10 @@ def fusion_mlp(x1, x2, weight, scale, shift, relu=True, negative_slope=None, add
         out = torch.empty((B, P, Co), dtype=torch.float32, device=x1.device)
     else:
         out = torch.empty((B, Co) + tail, dtype=torch.float32, device=x1.device)
-    with torch.cuda.device(x1.device):
-        check(lib.ffb6d_fusion_mlp_fwd_ex(
-            x1c.data_ptr(), C1, x2c.data_ptr() if x2c is not None else None, C2, packed.data.data_ptr(),
-            sc.data_ptr(), sh.data_ptr(), B, Co, P, 2 if negative_slope is not None else int(bool(relu)),
-            float(negative_slope or 0.0), addc.data_ptr() if addc is not None else None,
-            idxc.data_ptr() if idxc is not None else None, i64, NA,
-            LAYOUT_NSC if out_channels_last else LAYOUT_NCS, out.data_ptr(), _stream(x1.device)))
+    launch(lib.ffb6d_fusion_mlp_fwd_ex, x1.device, x1c.data_ptr(), C1, ptr(x2c), C2, packed.data.data_ptr(),
+           sc.data_ptr(), sh.data_ptr(), B, Co, P, 2 if negative_slope is not None else int(bool(relu)),
+           float(negative_slope or 0.0), ptr(addc), ptr(idxc), i64, NA, LAYOUT_NSC if out_channels_last else LAYOUT_NCS,
+           out.data_ptr())
     return out
 
 
@@ -530,10 +519,9 @@ class SegmentPlan:
         self.nbytes = int(getattr(lib, self._bytes)(self.B, self.P, self.NA))
         if self.nbytes == 0:
             raise ValueError("no segment plan for B=%d, P=%d, n_segments=%d" % (self.B, self.P, self.NA))
-        self.data = torch.empty(self.nbytes, dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            check(getattr(lib, self._build)(idx_c.data_ptr(), i64, self.B, self.P, self.NA, self.data.data_ptr(),
-                                            self.nbytes, _stream(self.device)))
+        self.data = workspace(self.nbytes, self.device)
+        launch(getattr(lib, self._build), self.device, idx_c.data_ptr(), i64, self.B, self.P, self.NA,
+               self.data.data_ptr(), self.nbytes)
 
     def csr(self):
         """``(offsets [B, n_segments+1], entries [B, P])`` int32 views of the plan; entries past
@@ -590,9 +578,8 @@ def segment_sum(grad, idx, n_segments, plan=None):
     if plan.device != grad.device:
         raise ValueError("plan lives on %s, grad on %s" % (plan.device, grad.device))
     out = torch.empty((B, Cc, plan.NA), dtype=torch.float32, device=grad.device)
-    with torch.cuda.device(grad.device):
-        check(getattr(lib, plan._sum)(g.data_ptr(), plan.data.data_ptr(), plan.nbytes, B, Cc, plan.P, plan.NA,
-                                      out.data_ptr(), _stream(grad.device)))
+    launch(getattr(lib, plan._sum), grad.device, g.data_ptr(), plan.data.data_ptr(), plan.nbytes, B, Cc, plan.P, plan.NA,
+           out.data_ptr())
     return out
 
 
@@ -614,9 +601,7 @@ def att_pool(f1, f2, att):
     if tuple(a.shape) != (B, C1 + C2, N, K) or f1c.dtype != torch.float32 or a.dtype != torch.float32:
         raise ValueError("att must be float32 [B,C1+C2,N,K] matching f1/f2")
     out = torch.empty((B, C1 + C2, N, 1), dtype=torch.float32, device=f1.device)
-    with torch.cuda.device(f1.device):
-        check(lib.ffb6d_att_pool_fwd(f1c.data_ptr(), C1, f2c.data_ptr() if f2c is not None else None, C2,
-                                     a.data_ptr(), B, N, K, out.data_ptr(), _stream(f1.device)))
+    launch(lib.ffb6d_att_pool_fwd, f1.device, f1c.data_ptr(), C1, ptr(f2c), C2, a.data_ptr(), B, N, K, out.data_ptr())
     return out
 
 
@@ -648,12 +633,9 @@ def lfa_att_pool_fused(xyz, neigh_idx, feature, mlp1, mlp2, fc_weight, mlp_out, 
     if w1.shape != (Dh, 10) or wfc.shape != (2 * Dh, 2 * Dh) or wo.shape[1] != 2 * Dh or (w2 is not None and w2.shape != (Dh, Dh)):
         raise ValueError("layer shapes do not match d/2 = %d" % Dh)
     out = torch.empty((B, Do, N, 1), dtype=torch.float32, device=f.device)
-    with torch.cuda.device(f.device):
-        check(lib.ffb6d_lfa_att_pool_fused(
-            xyz.data_ptr(), idx_c.data_ptr(), i64, f.data_ptr(), w1.data_ptr(), s1.data_ptr(), t1.data_ptr(),
-            w2.data_ptr() if w2 is not None else None, s2.data_ptr() if w2 is not None else None,
-            t2.data_ptr() if w2 is not None else None, wfc.data_ptr(), wo.data_ptr(), so.data_ptr(), to.data_ptr(),
-            B, N, K, Dh, Do, float(negative_slope), out.data_ptr(), _stream(f.device)))
+    launch(lib.ffb6d_lfa_att_pool_fused, f.device, xyz.data_ptr(), idx_c.data_ptr(), i64, f.data_ptr(), w1.data_ptr(),
+           s1.data_ptr(), t1.data_ptr(), ptr(w2), ptr(s2), ptr(t2), wfc.data_ptr(), wo.data_ptr(), so.data_ptr(),
+           to.data_ptr(), B, N, K, Dh, Do, float(negative_slope), out.data_ptr())
     return out
 
 
@@ -698,9 +680,8 @@ def lfa_train_fwd(feature, neigh_idx, f_xyz, w_fc):
     :return: ``f_agg [B,d,N,1]``.  K = 16 and d/2 in {16, 32, 64} (:func:`lfa_fusable`); other shapes raise."""
     f, idx_c, i64, fx, w, (B, N, K, Dh) = _lfa_train_args(feature, neigh_idx, f_xyz, w_fc)
     out = torch.empty((B, 2 * Dh, N, 1), dtype=torch.float32, device=f.device)
-    with torch.cuda.device(f.device):
-        check(lib.ffb6d_lfa_train_fwd(f.data_ptr(), idx_c.data_ptr(), i64, fx.data_ptr(), w.data_ptr(), B, N, K, Dh,
-                                      out.data_ptr(), _stream(f.device)))
+    launch(lib.ffb6d_lfa_train_fwd, f.device, f.data_ptr(), idx_c.data_ptr(), i64, fx.data_ptr(), w.data_ptr(), B, N, K,
+           Dh, out.data_ptr())
     return out
 
 
@@ -720,12 +701,10 @@ def lfa_train_bwd(feature, neigh_idx, f_xyz, w_fc, grad_agg, need_feature=True):
     edge = torch.empty((B, Dh, N * K), dtype=torch.float32, device=dev)
     gx = torch.empty((B, Dh, N, K), dtype=torch.float32, device=dev)
     gw = torch.empty((2 * Dh, 2 * Dh), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        nbytes = int(lib.ffb6d_lfa_train_bwd_workspace_bytes(B, N, K, Dh))
-        ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
-        check(lib.ffb6d_lfa_train_bwd(f.data_ptr(), idx_c.data_ptr(), i64, fx.data_ptr(), w.data_ptr(), g.data_ptr(),
-                                      B, N, K, Dh, edge.data_ptr(), gx.data_ptr(), gw.data_ptr(), ws.data_ptr(), nbytes,
-                                      _stream(dev)))
+    nbytes = int(lib.ffb6d_lfa_train_bwd_workspace_bytes(B, N, K, Dh))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_lfa_train_bwd, dev, f.data_ptr(), idx_c.data_ptr(), i64, fx.data_ptr(), w.data_ptr(), g.data_ptr(),
+           B, N, K, Dh, edge.data_ptr(), gx.data_ptr(), gw.data_ptr(), ws.data_ptr(), nbytes)
     del ws
     gf = None
     if need_feature:
@@ -762,15 +741,9 @@ def _intrinsics_arg(K, B, dev):
             raise ValueError("device intrinsics must be float64 [4] or [B,4] = (fx, fy, cx, cy)")
         return K.contiguous(), int(K.dim() == 2)
     Kn = np.asarray(K, dtype=np.float64)
-    if Kn.shape == (3, 3):
-        intr = np.array([Kn[0, 0], Kn[1, 1], Kn[0, 2], Kn[1, 2]], np.float64)
-        per_frame = 0
-    elif Kn.shape == (B, 3, 3):
-        intr = np.stack([Kn[:, 0, 0], Kn[:, 1, 1], Kn[:, 0, 2], Kn[:, 1, 2]], 1).copy()
-        per_frame = 1
-    else:
+    if Kn.shape not in ((3, 3), (B, 3, 3)):
         raise ValueError("K must be [3,3] or [B,3,3], got %s" % (Kn.shape,))
-    return torch.from_numpy(intr).to(dev), per_frame
+    return intrinsics_to_device(Kn, dev), int(Kn.ndim == 3)
 
 
 def point_item(depth_m, K, choose, rgb, labels, nrm_map, obj_cls, obj_kps, obj_ctr):
@@ -830,12 +803,9 @@ def point_item(depth_m, K, choose, rgb, labels, nrm_map, obj_cls, obj_kps, obj_c
     ctr_targ_ofst = torch.empty((B, N, 3), dtype=torch.float32, device=dev)
     args = [t.contiguous() for t in (depth_m, rgb, labels, obj_cls, obj_kps, obj_ctr)]
     depth_c, rgb_c, labels_c, cls_c, kps_c, ctr_c = args
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_point_item(depth_c.data_ptr(), B, H, W, intr_d.data_ptr(), per_frame, ch.data_ptr(), N,
-                                   rgb_c.data_ptr(), labels_c.data_ptr(), nrm.data_ptr(), cls_c.data_ptr(),
-                                   kps_c.data_ptr(), ctr_c.data_ptr(), n_obj, n_kps, cld_rgb_nrm.data_ptr(),
-                                   labels_pt.data_ptr(), kp_targ_ofst.data_ptr(), ctr_targ_ofst.data_ptr(),
-                                   _stream(dev)))
+    launch(lib.ffb6d_point_item, dev, depth_c.data_ptr(), B, H, W, intr_d.data_ptr(), per_frame, ch.data_ptr(), N,
+           rgb_c.data_ptr(), labels_c.data_ptr(), nrm.data_ptr(), cls_c.data_ptr(), kps_c.data_ptr(), ctr_c.data_ptr(),
+           n_obj, n_kps, cld_rgb_nrm.data_ptr(), labels_pt.data_ptr(), kp_targ_ofst.data_ptr(), ctr_targ_ofst.data_ptr())
     return cld_rgb_nrm, labels_pt, kp_targ_ofst, ctr_targ_ofst
 
 
@@ -857,11 +827,10 @@ def sample_valid_pixels(depth, n_points, seed=0, min_depth=1e-8, return_count=Fa
     dev = depth.device
     choose = torch.empty((B, 1, int(n_points)), dtype=torch.int32, device=dev)
     count = torch.empty((B,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        nbytes = int(lib.ffb6d_sample_pixels_workspace_bytes(B, H, W))
-        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-        check(lib.ffb6d_sample_pixels(depth.data_ptr(), B, H, W, float(min_depth), int(n_points), int(seed) & (2 ** 64 - 1),
-                                      choose.data_ptr(), count.data_ptr(), ws.data_ptr(), nbytes, _stream(dev)))
+    nbytes = int(lib.ffb6d_sample_pixels_workspace_bytes(B, H, W))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_sample_pixels, dev, depth.data_ptr(), B, H, W, float(min_depth), int(n_points),
+           int(seed) & (2 ** 64 - 1), choose.data_ptr(), count.data_ptr(), ws.data_ptr(), nbytes)
     return (choose, count) if return_count else choose
 
 
@@ -907,11 +876,9 @@ def _fill_depth(dpt, cam_scale, scale_2_80m=1, fill_type='multiscale', extrapola
     B, H, W = (1,) + tuple(raw.shape) if raw.dim() == 2 else tuple(raw.shape)
     dev = raw.device
     outs = [torch.empty(raw.shape, dtype=torch.float32, device=dev) if want else None for want in (want_raw, want_m)]
-    with torch.cuda.device(dev):
-        nbytes = int(lib.ffb6d_fill_depth_workspace_bytes(B, H, W))
-        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-        check(lib.ffb6d_fill_depth(raw.data_ptr(), B, H, W, cs, *(o.data_ptr() if o is not None else None for o in outs),
-                                   ws.data_ptr(), nbytes, _stream(dev)))
+    nbytes = int(lib.ffb6d_fill_depth_workspace_bytes(B, H, W))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_fill_depth, dev, raw.data_ptr(), B, H, W, cs, ptr(outs[0]), ptr(outs[1]), ws.data_ptr(), nbytes)
     return tuple(outs)
 
 
@@ -934,10 +901,8 @@ def _backproject(depth, intr_d, per_frame, choose):
     N = ch.shape[1]
     cld = torch.empty((B, N, 3), dtype=torch.float32, device=dev)
     pyr = {s: torch.empty((B, (H // s) * (W // s), 3), dtype=torch.float32, device=dev) for s in (2, 4, 8)}
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_backproject(depth.data_ptr(), B, H, W, intr_d.data_ptr(), per_frame, ch.data_ptr(), N,
-                                    cld.data_ptr(), pyr[2].data_ptr(), pyr[4].data_ptr(), pyr[8].data_ptr(),
-                                    _stream(dev)))
+    launch(lib.ffb6d_backproject, dev, depth.data_ptr(), B, H, W, intr_d.data_ptr(), per_frame, ch.data_ptr(), N,
+           cld.data_ptr(), pyr[2].data_ptr(), pyr[4].data_ptr(), pyr[8].data_ptr())
     return cld, pyr
 
 
@@ -1078,13 +1043,10 @@ def farthest_point_sampling(pts, sn, init_center=False, start=None, return_index
         else:
             st = torch.from_numpy(st_h).to(dev) if st_h is not None else start.to(dev).contiguous()
     idx = torch.empty((G, sn), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        nbytes = int(lib.ffb6d_farthest_point_sampling_workspace_bytes(G, P, sn))
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes else None
-        check(lib.ffb6d_farthest_point_sampling(x.data_ptr(), counts.data_ptr() if counts is not None else None, G, P,
-                                                sn, st.data_ptr() if st is not None else None, int(bool(init_center)),
-                                                idx.data_ptr(), ws.data_ptr() if ws is not None else None, nbytes,
-                                                _stream(dev)))
+    nbytes = int(lib.ffb6d_farthest_point_sampling_workspace_bytes(G, P, sn))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_farthest_point_sampling, dev, x.data_ptr(), ptr(counts), G, P, sn, ptr(st), int(bool(init_center)),
+           idx.data_ptr(), ws.data_ptr(), nbytes)
     sel = torch.gather(x, 1, idx.clamp(min=0).long()[..., None].expand(G, sn, 3))
     if single:
         sel, idx = sel[0], idx[0]
@@ -1127,12 +1089,10 @@ def mean_shift_fit(votes, valid=None, bandwidth=0.05, max_iter=300, return_modes
     labels = torch.empty((G, N), dtype=torch.uint8, device=dev)
     iters = torch.empty((G,), dtype=torch.int32, device=dev)
     modes = torch.empty((G, N, 3), dtype=torch.float32, device=dev) if return_modes else None
-    with torch.cuda.device(dev):
-        nbytes = int(lib.ffb6d_mean_shift_workspace_bytes(G, N))
-        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-        check(lib.ffb6d_mean_shift_fit(votes.data_ptr(), vptr, stride, G, N, float(bandwidth), int(max_iter),
-                                       centres.data_ptr(), labels.data_ptr(), iters.data_ptr(),
-                                       modes.data_ptr() if modes is not None else None, ws.data_ptr(), nbytes, _stream(dev)))
+    nbytes = int(lib.ffb6d_mean_shift_workspace_bytes(G, N))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_mean_shift_fit, dev, votes.data_ptr(), vptr, stride, G, N, float(bandwidth), int(max_iter),
+           centres.data_ptr(), labels.data_ptr(), iters.data_ptr(), ptr(modes), ws.data_ptr(), nbytes)
     out = (centres, labels.bool(), iters)
     return out + (modes,) if return_modes else out
 
@@ -1152,16 +1112,8 @@ def best_fit_transform(A, B):
     B = B.to(torch.float32).contiguous()
     G, M, _ = A.shape
     T = torch.empty((G, 3, 4), dtype=torch.float64, device=A.device)
-    with torch.cuda.device(A.device):
-        check(lib.ffb6d_best_fit_transform(A.data_ptr(), B.data_ptr(), G, M, T.data_ptr(), _stream(A.device)))
+    launch(lib.ffb6d_best_fit_transform, A.device, A.data_ptr(), B.data_ptr(), G, M, T.data_ptr())
     return T[0] if single else T
-
-
-def _aug_image(t, name, shape=None, dtype=torch.uint8):
-    _need_cuda(t, name)
-    if t.dtype != dtype or (shape is not None and tuple(t.shape) != tuple(shape)):
-        raise ValueError("%s must be %s %s, got %s %s" % (name, dtype, shape, t.dtype, tuple(t.shape)))
-    return t.contiguous()
 
 
 def rgb_add_noise(rgb, plan, seed, noise=None):
@@ -1188,17 +1140,13 @@ def rgb_add_noise(rgb, plan, seed, noise=None):
         raise ValueError("seed must fit 64 bits, got %r" % (seed,))
     dev = rgb.device
     if noise is not None:
-        noise = _aug_image(noise, "noise", (2, B, H, W, 3), torch.float64)
-        if noise.device != dev:
-            raise ValueError("noise is on %s, rgb on %s" % (noise.device, dev))
+        noise = _tensor(noise, "noise", torch.float64, (2, B, H, W, 3), dev)
     src = rgb.contiguous()
     plan_d = torch.from_numpy(plan).to(dev)
     out = torch.empty_like(src)
     work = torch.empty_like(src)
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_rgb_add_noise(src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), int(seed),
-                                      None if noise is None else noise.data_ptr(), out.data_ptr(), work.data_ptr(),
-                                      _stream(dev)))
+    launch(lib.ffb6d_rgb_add_noise, dev, src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), int(seed),
+           ptr(noise), out.data_ptr(), work.data_ptr())
     return out
 
 
@@ -1222,19 +1170,16 @@ def add_real_back(rgb, labels, dpt, back_rgb, back_labels, back_dpt, apply_rgb=N
     if rgb.dtype != torch.uint8 or rgb.dim() != 4 or rgb.shape[3] != 3:
         raise ValueError("rgb must be uint8 [B,H,W,3], got %s %s" % (rgb.dtype, tuple(rgb.shape)))
     B, H, W, _ = rgb.shape
-    labels = _aug_image(labels, "labels", (B, H, W))
-    dpt = _aug_image(dpt, "dpt", (B, H, W), torch.uint16)
-    back_rgb = _aug_image(back_rgb, "back_rgb", (B, H, W, 3))
+    dev = rgb.device
+    labels = _tensor(labels, "labels", torch.uint8, (B, H, W), dev)
+    dpt = _tensor(dpt, "dpt", torch.uint16, (B, H, W), dev)
+    back_rgb = _tensor(back_rgb, "back_rgb", torch.uint8, (B, H, W, 3), dev)
     _need_cuda(back_labels, "back_labels")
     if back_labels.dim() == 3:
         back_labels = back_labels[..., None]
     ch = back_labels.shape[-1] if back_labels.dim() == 4 else 0
-    back_labels = _aug_image(back_labels, "back_labels", (B, H, W, ch if ch in (1, 3) else -1))
-    back_dpt = _aug_image(back_dpt, "back_dpt", (B, H, W), torch.uint16)
-    for t, name in ((labels, "labels"), (dpt, "dpt"), (back_rgb, "back_rgb"), (back_labels, "back_labels"),
-                    (back_dpt, "back_dpt")):
-        if t.device != rgb.device:
-            raise ValueError("%s is on %s, rgb on %s" % (name, t.device, rgb.device))
+    back_labels = _tensor(back_labels, "back_labels", torch.uint8, (B, H, W, ch if ch in (1, 3) else -1), dev)
+    back_dpt = _tensor(back_dpt, "back_dpt", torch.uint16, (B, H, W), dev)
     act = np.ones(B, bool) if active is None else np.asarray(active, bool).reshape(-1)
     if dataset == "ycb":
         col = np.ones(B, bool) if apply_rgb is None else np.asarray(apply_rgb, bool).reshape(-1)
@@ -1244,16 +1189,13 @@ def add_real_back(rgb, labels, dpt, back_rgb, back_labels, back_dpt, apply_rgb=N
         col = np.asarray(apply_rgb, bool).reshape(-1)
     if act.shape != (B,) or col.shape != (B,):
         raise ValueError("apply_rgb and active must have one entry per frame (%d)" % B)
-    dev = rgb.device
     mode = torch.from_numpy((act * (1 + 2 * col)).astype(np.uint8)).to(dev)
     src = rgb.contiguous()
     rgb_out = torch.empty_like(src)
     dpt_out = torch.empty_like(dpt)
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_add_real_back(src.data_ptr(), labels.data_ptr(), dpt.data_ptr(), back_rgb.data_ptr(),
-                                      back_labels.data_ptr(), ch, back_dpt.data_ptr(), mode.data_ptr(),
-                                      0 if dataset == "ycb" else 1, B, H, W, rgb_out.data_ptr(), dpt_out.data_ptr(),
-                                      _stream(dev)))
+    launch(lib.ffb6d_add_real_back, dev, src.data_ptr(), labels.data_ptr(), dpt.data_ptr(), back_rgb.data_ptr(),
+           back_labels.data_ptr(), ch, back_dpt.data_ptr(), mode.data_ptr(), 0 if dataset == "ycb" else 1, B, H, W,
+           rgb_out.data_ptr(), dpt_out.data_ptr())
     return rgb_out, dpt_out
 
 
@@ -1292,9 +1234,8 @@ def color_jitter(rgb, plan, active=None):
         return out
     plan_d = torch.from_numpy(plan).to(dev)
     work = torch.empty(B, dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_color_jitter(src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), act.data_ptr(),
-                                     out.data_ptr(), work.data_ptr(), _stream(dev)))
+    launch(lib.ffb6d_color_jitter, dev, src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), act.data_ptr(),
+           out.data_ptr(), work.data_ptr())
     return out
 
 
@@ -1303,20 +1244,18 @@ def aug_noise_field(seed, B, H, W, stage, device="cuda"):
     ``2*pass`` is ``gaussian_noise``'s, ``2*pass + 1`` YCB's ``normal(0, 7)``'s (``ffb6d_aug_noise_field``)."""
     out = torch.empty((B, H, W, 3), dtype=torch.float64, device=device)
     _need_cuda(out, "out")
-    with torch.cuda.device(out.device):
-        check(lib.ffb6d_aug_noise_field(int(seed), B, H, W, int(stage), out.data_ptr(), _stream(out.device)))
+    launch(lib.ffb6d_aug_noise_field, out.device, int(seed), B, H, W, int(stage), out.data_ptr())
     return out
 
 
 # --------------------------------------------------------------------------- training loss
 def _loss_labels(labels, B, N, dev):
     _need_cuda(labels, "labels")
-    if labels.dtype not in _IDX:
-        raise TypeError("labels must be int32 or int64, got %s" % labels.dtype)
-    if labels.numel() != B * N or labels.device != dev:
+    lab, i64 = _idx_arg(labels, "labels")
+    if lab.numel() != B * N or lab.device != dev:
         raise ValueError("labels must hold %d x %d values on %s, got %s on %s"
                          % (B, N, dev, tuple(labels.shape), labels.device))
-    return labels.reshape(B, N).contiguous(), int(labels.dtype == torch.int64)
+    return lab.view(B, N), i64
 
 
 def _loss_valid(valid, B, dev):
@@ -1334,14 +1273,7 @@ def _loss_workspace(B, N, n_kps, dev):
     nbytes = lib.ffb6d_loss_workspace_bytes(B, N, n_kps)
     if nbytes == 0:
         raise ValueError("loss: unsupported size B=%d N=%d n_kps=%d" % (B, N, n_kps))
-    return torch.empty(nbytes, dtype=torch.uint8, device=dev)
-
-
-def _f32(t, name, shape):
-    _need_cuda(t, name)
-    if t.dtype != torch.float32 or tuple(t.shape) != tuple(shape):
-        raise ValueError("%s must be float32 %s, got %s %s" % (name, tuple(shape), t.dtype, tuple(t.shape)))
-    return t.contiguous()
+    return workspace(nbytes, dev), nbytes
 
 
 def focal_loss_fwd(logits, labels, valid=None, gamma=0.0, alpha=None, size_average=True, layout=0):
@@ -1358,18 +1290,16 @@ def focal_loss_fwd(logits, labels, valid=None, gamma=0.0, alpha=None, size_avera
     lab, is64 = _loss_labels(labels, B, N, dev)
     v = _loss_valid(valid, B, dev)
     if alpha is not None:
-        alpha = _f32(alpha, "alpha", alpha.shape)
-        if alpha.dim() != 1 or alpha.numel() < C or alpha.device != dev:
+        alpha = _tensor(alpha, "alpha", shape=1, device=dev)
+        if alpha.numel() < C:
             raise ValueError("alpha must be a [>= C] float32 tensor on %s" % dev)
-    ws = _loss_workspace(B, N, 1, dev)
+    ws, nbytes = _loss_workspace(B, N, 1, dev)
     out = torch.empty(2, dtype=torch.float32, device=dev)
     count = torch.empty((), dtype=torch.int64, device=dev)
     lse = torch.empty((B, N), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_focal_loss_fwd(x.data_ptr(), layout, lab.data_ptr(), is64, None if v is None else v.data_ptr(),
-                                       B, C, N, float(gamma), None if alpha is None else alpha.data_ptr(),
-                                       int(bool(size_average)), out.data_ptr(), out.data_ptr() + 4, count.data_ptr(),
-                                       lse.data_ptr(), ws.data_ptr(), ws.numel(), _stream(dev)))
+    launch(lib.ffb6d_focal_loss_fwd, dev, x.data_ptr(), layout, lab.data_ptr(), is64, ptr(v), B, C, N, float(gamma),
+           ptr(alpha), int(bool(size_average)), out.data_ptr(), out.data_ptr() + 4, count.data_ptr(), lse.data_ptr(),
+           ws.data_ptr(), nbytes)
     return out[0], out[1], count, lse
 
 
@@ -1381,14 +1311,11 @@ def focal_loss_bwd(logits, labels, valid, gamma, alpha, size_average, lse, count
     dev = x.device
     lab, is64 = _loss_labels(labels, B, N, dev)
     v = _loss_valid(valid, B, dev)
-    lse = _f32(lse, "lse", (B, N))
+    lse = _tensor(lse, "lse", shape=(B, N))
     g = grad_loss.to(torch.float32).reshape(1).contiguous()
     grad = torch.empty_like(x)
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_focal_loss_bwd(x.data_ptr(), layout, lab.data_ptr(), is64, None if v is None else v.data_ptr(),
-                                       B, C, N, float(gamma), None if alpha is None else alpha.data_ptr(),
-                                       int(bool(size_average)), lse.data_ptr(), count.data_ptr(), g.data_ptr(),
-                                       grad.data_ptr(), _stream(dev)))
+    launch(lib.ffb6d_focal_loss_bwd, dev, x.data_ptr(), layout, lab.data_ptr(), is64, ptr(v), B, C, N, float(gamma),
+           ptr(alpha), int(bool(size_average)), lse.data_ptr(), count.data_ptr(), g.data_ptr(), grad.data_ptr())
     return grad
 
 
@@ -1411,13 +1338,11 @@ def of_l1_loss_fwd(pred, targ, labels, valid=None):
     p, t, lab, is64, v = _of_args(pred, targ, labels, valid)
     B, K, N, _ = p.shape
     dev = p.device
-    ws = _loss_workspace(B, N, K, dev)
+    ws, nbytes = _loss_workspace(B, N, K, dev)
     out = torch.empty((B, K), dtype=torch.float32, device=dev)
     count = torch.empty(B, dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_of_l1_loss_fwd(p.data_ptr(), t.data_ptr(), lab.data_ptr(), is64,
-                                       None if v is None else v.data_ptr(), B, K, N, out.data_ptr(), count.data_ptr(),
-                                       ws.data_ptr(), ws.numel(), _stream(dev)))
+    launch(lib.ffb6d_of_l1_loss_fwd, dev, p.data_ptr(), t.data_ptr(), lab.data_ptr(), is64, ptr(v), B, K, N,
+           out.data_ptr(), count.data_ptr(), ws.data_ptr(), nbytes)
     return out, count
 
 
@@ -1427,13 +1352,11 @@ def of_l1_loss_bwd(pred, targ, labels, valid, count, grad_out):
     p, t, lab, is64, v = _of_args(pred, targ, labels, valid)
     B, K, N, _ = p.shape
     dev = p.device
-    count = _f32(count, "count", (B,))
-    g = _f32(grad_out.to(torch.float32), "grad_out", (B, K))
+    count = _tensor(count, "count", shape=(B,))
+    g = _tensor(grad_out.to(torch.float32), "grad_out", shape=(B, K))
     grad = torch.empty_like(p)
-    with torch.cuda.device(dev):
-        check(lib.ffb6d_of_l1_loss_bwd(p.data_ptr(), t.data_ptr(), lab.data_ptr(), is64,
-                                       None if v is None else v.data_ptr(), B, K, N, count.data_ptr(), g.data_ptr(),
-                                       grad.data_ptr(), _stream(dev)))
+    launch(lib.ffb6d_of_l1_loss_bwd, dev, p.data_ptr(), t.data_ptr(), lab.data_ptr(), is64, ptr(v), B, K, N,
+           count.data_ptr(), g.data_ptr(), grad.data_ptr())
     return grad
 
 
@@ -1442,22 +1365,14 @@ PSP_SIZES = (1, 2, 3, 6)
 _PSP_BINS = sum(s * s for s in PSP_SIZES)     # 50
 
 
-def _f32_map(x, name):
-    _need_cuda(x, name)
-    if x.dtype != torch.float32 or x.dim() != 4:
-        raise ValueError("%s must be float32 [B,C,H,W], got %s %s" % (name, x.dtype, tuple(x.shape)))
-    return x.contiguous()
-
-
 def psp_pool(x):
     """``[AdaptiveAvgPool2d(s)(x) for s in (1, 2, 3, 6)]`` (the priors of PSPModule, models/cnn/pspnet.py:19-28) in
     one read of ``x [B,C,H,W]`` float32 CUDA (``ffb6d_psp_pool``).  :return: four ``[B,C,s,s]`` tensors, views of one
     buffer in the block order :func:`psp_bottleneck` reads."""
-    xc = _f32_map(x, "x")
+    xc = _tensor(x, "x", shape=4)
     B, C, H, W = xc.shape
     out = torch.empty(_PSP_BINS * B * C, dtype=torch.float32, device=xc.device)
-    with torch.cuda.device(xc.device):
-        check(lib.ffb6d_psp_pool(xc.data_ptr(), B, C, H, W, out.data_ptr(), _stream(xc.device)))
+    launch(lib.ffb6d_psp_pool, xc.device, xc.data_ptr(), B, C, H, W, out.data_ptr())
     views, off = [], 0
     for s in PSP_SIZES:
         views.append(out[off:off + B * C * s * s].view(B, C, s, s))
@@ -1499,25 +1414,23 @@ def psp_bottleneck(x, pooled, weights):
     are packed GEMMs on the 50 pooled columns (``ffb6d_fusion_mlp_fwd_ex``, channels-last into one table), the rest
     is ``ffb6d_psp_bottleneck_fwd``.  :param x: ``[B,C,H,W]`` float32 CUDA; :param pooled: :func:`psp_pool` of ``x``;
     :param weights: :class:`PSPWeights`.  :return: ``[B,Co,H,W]``"""
-    xc = _f32_map(x, "x")
+    xc = _tensor(x, "x", shape=4)
     B, C, H, W = xc.shape
     if C != weights.C or weights.device != xc.device:
         raise ValueError("psp weights take %d channels on %s, x has %d on %s" % (weights.C, weights.device, C, xc.device))
     Co = weights.Co
     table = torch.empty(_PSP_BINS * B * Co, dtype=torch.float32, device=xc.device)
     out = torch.empty((B, Co, H, W), dtype=torch.float32, device=xc.device)
-    st = _stream(xc.device)
-    with torch.cuda.device(xc.device):
-        off = 0
-        for s, p, pk in zip(PSP_SIZES, pooled, weights.stages):
-            if tuple(p.shape) != (B, C, s, s) or not p.is_contiguous() or p.dtype != torch.float32:
-                raise ValueError("pooled must be psp_pool(x)")
-            check(lib.ffb6d_fusion_mlp_fwd_ex(p.data_ptr(), C, None, 0, pk.data.data_ptr(), weights.one.data_ptr(),
-                                              weights.zero.data_ptr(), B, Co, s * s, 0, 0.0, None, None, 0, 0,
-                                              LAYOUT_NSC, table.data_ptr() + 4 * off * Co, st))
-            off += B * s * s
-        check(lib.ffb6d_psp_bottleneck_fwd(xc.data_ptr(), B, C, H, W, weights.feat.data.data_ptr(),
-                                           weights.bias.data_ptr(), Co, table.data_ptr(), out.data_ptr(), st))
+    off = 0
+    for s, p, pk in zip(PSP_SIZES, pooled, weights.stages):
+        if tuple(p.shape) != (B, C, s, s) or not p.is_contiguous() or p.dtype != torch.float32:
+            raise ValueError("pooled must be psp_pool(x)")
+        launch(lib.ffb6d_fusion_mlp_fwd_ex, xc.device, p.data_ptr(), C, None, 0, pk.data.data_ptr(),
+               weights.one.data_ptr(), weights.zero.data_ptr(), B, Co, s * s, 0, 0.0, None, None, 0, 0, LAYOUT_NSC,
+               table.data_ptr() + 4 * off * Co)
+        off += B * s * s
+    launch(lib.ffb6d_psp_bottleneck_fwd, xc.device, xc.data_ptr(), B, C, H, W, weights.feat.data.data_ptr(),
+           weights.bias.data_ptr(), Co, table.data_ptr(), out.data_ptr())
     return out
 
 
@@ -1525,7 +1438,7 @@ def conv1x1_log_softmax(x, weight, bias):
     """``log_softmax(conv1x1(x, weight, bias), dim=1)`` in one tensor-core kernel (``ffb6d_conv1x1_log_softmax_fwd``):
     PSPNet's ``final`` (models/cnn/pspnet.py:108-112).  :param x: ``[B,Ci,H,W]`` float32 CUDA; :param weight:
     ``[Co,Ci(,1,1)]`` or its :class:`PackedWeight`, Co <= 128; :param bias: ``[Co]``.  :return: ``[B,Co,H,W]``"""
-    xc = _f32_map(x, "x")
+    xc = _tensor(x, "x", shape=4)
     B, Ci, H, W = xc.shape
     packed = weight if isinstance(weight, PackedWeight) else PackedWeight(weight)
     if packed.Ci != Ci or packed.device != xc.device:
@@ -1534,9 +1447,8 @@ def conv1x1_log_softmax(x, weight, bias):
     if b.numel() != packed.Co or b.device != xc.device:
         raise ValueError("bias must have %d elements on %s" % (packed.Co, xc.device))
     out = torch.empty((B, packed.Co, H, W), dtype=torch.float32, device=xc.device)
-    with torch.cuda.device(xc.device):
-        check(lib.ffb6d_conv1x1_log_softmax_fwd(xc.data_ptr(), B, Ci, H * W, packed.data.data_ptr(), b.data_ptr(),
-                                                packed.Co, out.data_ptr(), _stream(xc.device)))
+    launch(lib.ffb6d_conv1x1_log_softmax_fwd, xc.device, xc.data_ptr(), B, Ci, H * W, packed.data.data_ptr(),
+           b.data_ptr(), packed.Co, out.data_ptr())
     return out
 
 
@@ -1547,17 +1459,14 @@ def psp_bottleneck_bwd(grad_out, out):
     the gradient of the bottleneck's pre-ReLU sum (torch's ReLU backward on ``out``), that of the prior table in the
     forward's layout (block ``s`` is ``[B, s*s, Co]``, in the order of :data:`PSP_SIZES`), and the per-frame sums of
     ``grad_z`` (the bias gradient is their sum over the frames)."""
-    o = _f32_map(out, "out")
+    o = _tensor(out, "out", shape=4)
     B, Co, H, W = o.shape
-    g = _f32(grad_out, "grad_out", o.shape)
-    if g.device != o.device:
-        raise ValueError("grad_out and out must be on the same device")
+    g = _tensor(grad_out, "grad_out", shape=o.shape, device=o.device)
     gz = torch.empty_like(o)
     table = torch.empty((_PSP_BINS * B, Co), dtype=torch.float32, device=o.device)
     gsum = torch.empty((B, Co), dtype=torch.float32, device=o.device)
-    with torch.cuda.device(o.device):
-        check(lib.ffb6d_psp_bottleneck_bwd(g.data_ptr(), o.data_ptr(), B, Co, H, W, gz.data_ptr(), table.data_ptr(),
-                                           gsum.data_ptr(), _stream(o.device)))
+    launch(lib.ffb6d_psp_bottleneck_bwd, o.device, g.data_ptr(), o.data_ptr(), B, Co, H, W, gz.data_ptr(),
+           table.data_ptr(), gsum.data_ptr())
     return gz, table, gsum
 
 
@@ -1565,21 +1474,21 @@ def psp_pool_bwd(grad_pooled, grad_x):
     """Adjoint of :func:`psp_pool` (``ffb6d_psp_pool_bwd``, one launch), accumulated: ``grad_x [B,C,H,W]`` float32 CUDA
     (contiguous; updated in place and returned) ``+= sum_s pool_s^T(grad_pooled[s])``.  :param grad_pooled: the four
     ``[B,C,s,s]`` gradients of :func:`psp_pool`'s outputs, or one flat buffer in its block order."""
-    gx = _f32_map(grad_x, "grad_x")
+    gx = _tensor(grad_x, "grad_x", shape=4)
     if gx.data_ptr() != grad_x.data_ptr():
         raise ValueError("grad_x must be contiguous (it is updated in place)")
     B, C, H, W = gx.shape
     if isinstance(grad_pooled, torch.Tensor):
-        gp = _f32(grad_pooled, "grad_pooled", (_PSP_BINS * B * C,))
+        gp = _tensor(grad_pooled, "grad_pooled", shape=(_PSP_BINS * B * C,))
     else:
-        parts = [_f32(p, "grad_pooled[%d]" % i, (B, C, s, s)) for i, (s, p) in enumerate(zip(PSP_SIZES, grad_pooled))]
+        parts = [_tensor(p, "grad_pooled[%d]" % i, shape=(B, C, s, s))
+                 for i, (s, p) in enumerate(zip(PSP_SIZES, grad_pooled))]
         if len(parts) != len(PSP_SIZES):
             raise ValueError("grad_pooled must hold %d tensors" % len(PSP_SIZES))
         gp = torch.cat([p.reshape(-1) for p in parts])
     if gp.device != gx.device:
         raise ValueError("grad_pooled and grad_x must be on the same device")
-    with torch.cuda.device(gx.device):
-        check(lib.ffb6d_psp_pool_bwd(gp.data_ptr(), B, C, H, W, gx.data_ptr(), _stream(gx.device)))
+    launch(lib.ffb6d_psp_pool_bwd, gx.device, gp.data_ptr(), B, C, H, W, gx.data_ptr())
     return grad_x
 
 
@@ -1590,26 +1499,21 @@ def log_softmax_bwd(grad_out, out):
     if out.dtype != torch.float32 or out.dim() < 2:
         raise ValueError("out must be float32 [B,C,...], got %s %s" % (out.dtype, tuple(out.shape)))
     o = out.contiguous()
-    g = _f32(grad_out, "grad_out", o.shape)
-    if g.device != o.device:
-        raise ValueError("grad_out and out must be on the same device")
+    g = _tensor(grad_out, "grad_out", shape=o.shape, device=o.device)
     B, C = o.shape[0], o.shape[1]
     gi = torch.empty_like(o)
-    with torch.cuda.device(o.device):
-        check(lib.ffb6d_log_softmax_bwd(g.data_ptr(), o.data_ptr(), B, C, o.numel() // (B * C), gi.data_ptr(),
-                                        _stream(o.device)))
+    launch(lib.ffb6d_log_softmax_bwd, o.device, g.data_ptr(), o.data_ptr(), B, C, o.numel() // (B * C), gi.data_ptr())
     return gi
 
 
 def upsample_bilinear2d_bwd(grad_out, input_size):
     """Backward of ``F.interpolate(x, mode="bilinear", align_corners=True)`` (``ffb6d_upsample_bilinear2d_bwd``, one
     launch): ``grad_out [B,C,Ho,Wo]`` float32 CUDA, ``input_size = (Hi, Wi)``.  :return: ``grad_in [B,C,Hi,Wi]``"""
-    g = _f32_map(grad_out, "grad_out")
+    g = _tensor(grad_out, "grad_out", shape=4)
     B, C, Ho, Wo = g.shape
     Hi, Wi = (int(v) for v in input_size)
     gi = torch.empty((B, C, Hi, Wi), dtype=torch.float32, device=g.device)
-    with torch.cuda.device(g.device):
-        check(lib.ffb6d_upsample_bilinear2d_bwd(g.data_ptr(), B, C, Hi, Wi, Ho, Wo, gi.data_ptr(), _stream(g.device)))
+    launch(lib.ffb6d_upsample_bilinear2d_bwd, g.device, g.data_ptr(), B, C, Hi, Wi, Ho, Wo, gi.data_ptr())
     return gi
 
 
@@ -1629,7 +1533,7 @@ def upsample_bilinear2d(x, scale_factor=2):
     """``F.interpolate(x, scale_factor=scale_factor, mode="bilinear", align_corners=True)`` (``nn.Upsample`` of
     PSPUpsample, models/cnn/pspnet.py:36-48) with a deterministic backward: the forward is torch's, the backward
     :func:`upsample_bilinear2d_bwd`.  :param x: ``[B,C,H,W]`` float32 CUDA."""
-    _f32_map(x, "x")
+    _tensor(x, "x", shape=4)
     return _UpsampleBilinear2d.apply(x, scale_factor)
 
 
@@ -1667,23 +1571,13 @@ def upconv_pack(weight):
     return UpConvWeights(weight)
 
 
-def _opt_f32(t, n, name, dev):
-    if t is None:
-        return None
-    _need_cuda(t, name)
-    t = t.detach().float().contiguous()
-    if t.numel() != n or t.device != dev:
-        raise ValueError("%s must have %d elements on %s" % (name, n, dev))
-    return t
-
-
 def upconv_taps_fwd(table, out, co0, bias=None, scale=None, shift=None, alpha=None):
     """The epilogue of :func:`upsample_conv3x3` (``ffb6d_upconv_taps_fwd``, one launch): writes the chunk of output
     channels ``co0 .. co0 + Cc - 1`` of ``out [B, Co, 2 Hi, 2 Wi]`` from its tap table ``table [B, 9 Cc, Hi, Wi]``:
     ``act(affine(bias + sum of the nine shifted, upsampled planes))``; ``scale``/``shift`` ``[Co]`` the folded
     BatchNorm, ``alpha [1]`` PReLU's weight (each optional).  Returns ``out``."""
-    t = _f32_map(table, "table")
-    o = _f32_map(out, "out")
+    t = _tensor(table, "table", shape=4)
+    o = _tensor(out, "out", shape=4)
     if o.data_ptr() != out.data_ptr() or o.device != t.device:
         raise ValueError("out must be contiguous and on the table's device (it is written in place)")
     B, C9, Hi, Wi = t.shape
@@ -1693,26 +1587,23 @@ def upconv_taps_fwd(table, out, co0, bias=None, scale=None, shift=None, alpha=No
                          % (tuple(t.shape), tuple(o.shape)))
     if (scale is None) != (shift is None):
         raise ValueError("scale and shift come together")
-    b, sc, sh = (_opt_f32(v, Co, n, t.device) for v, n in ((bias, "bias"), (scale, "scale"), (shift, "shift")))
-    a = _opt_f32(alpha, 1, "alpha", t.device)
-    ptr = lambda v: v.data_ptr() if v is not None else None
-    with torch.cuda.device(t.device):
-        check(lib.ffb6d_upconv_taps_fwd(t.data_ptr(), B, Co, int(co0), C9 // 9, Hi, Wi, ptr(b), ptr(sc), ptr(sh), ptr(a),
-                                        o.data_ptr(), _stream(t.device)))
+    b, sc, sh, a = (None if v is None else _tensor(v.detach().float().reshape(-1), name, shape=(n,), device=t.device)
+                    for v, name, n in ((bias, "bias", Co), (scale, "scale", Co), (shift, "shift", Co),
+                                       (alpha, "alpha", 1)))
+    launch(lib.ffb6d_upconv_taps_fwd, t.device, t.data_ptr(), B, Co, int(co0), C9 // 9, Hi, Wi, ptr(b), ptr(sc), ptr(sh),
+           ptr(a), o.data_ptr())
     return out
 
 
 def upconv_taps_bwd(grad_z, co0, cc):
     """Adjoint of :func:`upconv_taps_fwd`'s tap sum (``ffb6d_upconv_taps_bwd``, one launch) for the chunk of ``cc``
     output channels from ``co0``: ``grad_z [B, Co, Ho, Wo]`` (Ho, Wo even) -> ``[B, 9 cc, Ho / 2, Wo / 2]``."""
-    g = _f32_map(grad_z, "grad_z")
+    g = _tensor(grad_z, "grad_z", shape=4)
     B, Co, Ho, Wo = g.shape
     if Ho % 2 or Wo % 2:
         raise ValueError("grad_z must be [B, Co, 2 Hi, 2 Wi], got %s" % (tuple(g.shape),))
     gt = torch.empty((B, 9 * int(cc), Ho // 2, Wo // 2), dtype=torch.float32, device=g.device)
-    with torch.cuda.device(g.device):
-        check(lib.ffb6d_upconv_taps_bwd(g.data_ptr(), B, Co, int(co0), int(cc), Ho // 2, Wo // 2, gt.data_ptr(),
-                                        _stream(g.device)))
+    launch(lib.ffb6d_upconv_taps_bwd, g.device, g.data_ptr(), B, Co, int(co0), int(cc), Ho // 2, Wo // 2, gt.data_ptr())
     return gt
 
 
@@ -1721,7 +1612,7 @@ def upsample_conv3x3(x, weights, bias=None, scale=None, shift=None, alpha=None, 
     output channels the stacked GEMM at the input's resolution (``ffb6d_fusion_mlp_fwd_ex`` with the packed
     :class:`UpConvWeights`) and its tap epilogue (:func:`upconv_taps_fwd`), optionally followed by the folded BatchNorm
     ``scale``/``shift`` and PReLU ``alpha``.  :param x: ``[B, Ci, Hi, Wi]`` float32 CUDA.  :return: ``[B, Co, 2 Hi, 2 Wi]``"""
-    xc = _f32_map(x, "x")
+    xc = _tensor(x, "x", shape=4)
     B, Ci, Hi, Wi = xc.shape
     if not isinstance(weights, UpConvWeights):
         raise TypeError("weights must be ops.upconv_pack(conv.weight)")
@@ -1743,9 +1634,8 @@ def prelu_(y, alpha):
     _need_cuda(y, "y")
     if y.dtype != torch.float32 or not y.is_contiguous():
         raise ValueError("y must be contiguous float32")
-    a = _opt_f32(alpha, 1, "alpha", y.device)
-    with torch.cuda.device(y.device):
-        check(lib.ffb6d_prelu_fwd(y.data_ptr(), y.numel(), a.data_ptr(), y.data_ptr(), _stream(y.device)))
+    a = _tensor(alpha.detach().float().reshape(-1), "alpha", shape=(1,), device=y.device)
+    launch(lib.ffb6d_prelu_fwd, y.device, y.data_ptr(), y.numel(), a.data_ptr(), y.data_ptr())
     return y
 
 
@@ -1757,12 +1647,11 @@ def bn_prelu_bwd(z, grad_y, stats, alpha):
     if z.dtype != torch.float32 or z.dim() < 2 or not z.is_contiguous():
         raise ValueError("z must be contiguous float32 [B, C, ...]")
     B, Cn = z.shape[0], z.shape[1]
-    g = _f32(grad_y, "grad_y", z.shape)
-    st = _f32(stats, "stats", (Cn, 4))
-    a = _opt_f32(alpha, 1, "alpha", z.device)
+    g = _tensor(grad_y, "grad_y", shape=z.shape)
+    st = _tensor(stats, "stats", shape=(Cn, 4))
+    a = _tensor(alpha.detach().float().reshape(-1), "alpha", shape=(1,), device=z.device)
     gu = torch.empty_like(z)
     part = torch.empty(B * Cn, dtype=torch.float64, device=z.device)
-    with torch.cuda.device(z.device):
-        check(lib.ffb6d_bn_prelu_bwd(z.data_ptr(), g.data_ptr(), st.data_ptr(), B, Cn, z.numel() // (B * Cn),
-                                     a.data_ptr(), gu.data_ptr(), part.data_ptr(), _stream(z.device)))
+    launch(lib.ffb6d_bn_prelu_bwd, z.device, z.data_ptr(), g.data_ptr(), st.data_ptr(), B, Cn, z.numel() // (B * Cn),
+           a.data_ptr(), gu.data_ptr(), part.data_ptr())
     return gu, part.sum().float().reshape(1)

@@ -199,8 +199,7 @@ def build_ffb6d_indices_native(cld, pyramid, image_hw, k=K_NEIGH, index_dtype=to
     :param cld: ``[B, N0, 3]`` float32 CUDA; :param pyramid: ``{2: [B,HW/4,3], 4: ..., 8: ...}``
     :param image_hw: ``(H, W)`` of the full-resolution image"""
     import ctypes
-    from ._lib import lib, check
-    from .ops import _stream
+    from ._lib import lib, launch, workspace
     if cld.dim() != 3 or cld.shape[2] != 3 or not cld.is_cuda:
         raise ValueError("expected cld [B,N,3] on a CUDA device")
     cld = cld.contiguous().float()
@@ -216,11 +215,10 @@ def build_ffb6d_indices_native(cld, pyramid, image_hw, k=K_NEIGH, index_dtype=to
         inputs[key] = torch.empty((B, set_size(q, n0, H, W), kk), dtype=index_dtype, device=cld.device)
         ptrs[j] = inputs[key].data_ptr()
     nbytes = int(lib.ffb6d_build_indices_workspace_bytes(B, n0, H, W, int(k)))
-    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=cld.device)
-    with torch.cuda.device(cld.device):
-        check(lib.ffb6d_build_indices(cld.data_ptr(), img[2].data_ptr(), img[4].data_ptr(), img[8].data_ptr(), B, n0, H, W,
-                                      int(k), ctypes.cast(ptrs, ctypes.c_void_p), int(index_dtype == torch.int64),
-                                      ws.data_ptr(), nbytes, _stream(cld.device)))
+    ws = workspace(nbytes, cld.device)
+    launch(lib.ffb6d_build_indices, cld.device, cld.data_ptr(), img[2].data_ptr(), img[4].data_ptr(), img[8].data_ptr(),
+           B, n0, H, W, int(k), ctypes.cast(ptrs, ctypes.c_void_p), int(index_dtype == torch.int64), ws.data_ptr(),
+           nbytes)
     n = n0
     for i in range(N_DS_LAYERS):
         inputs["cld_xyz%d" % i] = cld if i == 0 else cld[:, :n, :].contiguous()

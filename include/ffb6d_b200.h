@@ -232,18 +232,12 @@ int ffb6d_relative_pos_encoding_cm_fwd(const float *xyz, const void *idx, int id
  * row-major, out [B,Co,P]; all f32, NCHW (point axis contiguous).
  * act: 0 none, 1 ReLU (the fusion layers), 2 LeakyReLU(negative_slope) (RandLA's pt_utils.Conv2d,
  * models/RandLA/pytorch_utils.py:163-197: conv -> BN(eps 1e-6) -> LeakyReLU(0.2)).
- */
-int ffb6d_fusion_mlp_fwd(const float *x1, int64_t C1, const float *x2, int64_t C2,
-                         const float *weight, const float *scale, const float *shift,
-                         int64_t B, int64_t Co, int64_t P, int act, float negative_slope,
-                         float *out, ffb6d_stream_t stream);
-
-/*
- * The same layer with the weights prepared once (inference: weights are constants).
- * ffb6d_fusion_mlp_pack splits weight [Co,Ci] into its TF32 hi/lo parts and lays them out as the
- * kernel's shared-memory tiles (`packed`: device, 16-byte aligned, ffb6d_fusion_mlp_pack_bytes(Co,
- * Ci) bytes); ffb6d_fusion_mlp_fwd_packed then streams those tiles with bulk-async (TMA) copies.
- * ffb6d_fusion_mlp_fwd = pack into a stream-ordered scratch block + fwd_packed.
+ *
+ * The weights are prepared once (inference: weights are constants), so the layer call allocates
+ * nothing.  ffb6d_fusion_mlp_pack splits weight [Co,Ci] into its TF32 hi/lo parts and lays them out
+ * as the kernel's shared-memory tiles (`packed`: device, 16-byte aligned,
+ * ffb6d_fusion_mlp_pack_bytes(Co, Ci) bytes); ffb6d_fusion_mlp_fwd_packed then streams those tiles
+ * with bulk-async (TMA) copies.
  */
 size_t ffb6d_fusion_mlp_pack_bytes(int64_t Co, int64_t Ci);
 int ffb6d_fusion_mlp_pack(const float *weight, int64_t Co, int64_t Ci, void *packed, size_t packed_bytes,
@@ -387,7 +381,7 @@ int ffb6d_fusion_mlp_wgrad_det(const float *grad_z, const float *x1, int64_t C1,
  * Attentive pooling core of RandLA's Att_pooling (models/RandLA/RandLANet.py:243-248):
  *   out[b,c,n] = sum_k f[b,c,n,k] * softmax_k(att[b,c,n,:])[k],   f = cat(f1, f2) along channels
  *   f1 [B,C1,N,K], f2 [B,C2,N,K] or NULL, att [B,C1+C2,N,K] -> out [B,C1+C2,N]   (f32, K <= 64)
- * (the scores `att` come from the layer's fc = 1x1 conv, i.e. ffb6d_fusion_mlp_fwd with act 0).
+ * (the scores `att` come from the layer's fc = 1x1 conv, i.e. ffb6d_fusion_mlp_fwd_ex with act 0).
  */
 int ffb6d_att_pool_fwd(const float *f1, int64_t C1, const float *f2, int64_t C2, const float *att,
                        int64_t B, int64_t N, int K, float *out, ffb6d_stream_t stream);

@@ -33,8 +33,8 @@ def test_header_symbols_exported():
     assert sorted(_lib.SYMBOLS) == syms
 
 
-def test_version_and_error_text():
-    assert _lib.lib.ffb6d_version() == 2
+def test_abi_version_and_error_text():
+    assert _lib.lib.ffb6d_version() == 3
     assert isinstance(_lib.last_error(), str)
 
 

@@ -112,9 +112,9 @@ LIMITS = {
         "1 <= B < 65536, 1 <= P, NA < 2^31, CSR bytes per frame < 2^31; ceil(C/32) <= 65535",
         "csr_* + segment_sum_kernel: test_segment_sum_at_limits"),
     # fusion_mlp.cu
-    "ffb6d_fusion_mlp_fwd / _packed / _ex": (
+    "ffb6d_fusion_mlp_fwd_ex / _fwd_packed": (
         "B < 65536, 1 <= Co <= 65535*128, P < 2^31, C1 + C2 < 2^31; NA < 2^31 with an addend",
-        "the wgmma layer: test_fusion_mlp_fwd_at_limits (Co = 65535*128; B*Co*P > 2^31)"),
+        "the wgmma layer: test_fusion_mlp_fwd_ex_at_limits (Co = 65535*128; B*Co*P > 2^31)"),
     "ffb6d_fusion_mlp_wgrad / _wgrad_det": (
         "B < 65536, Co <= 65535*128, C1 + C2 <= 65535*128, P < 2^31, B*P < 2^31", "not covered here"),
     "ffb6d_conv1x1_log_softmax_fwd": ("B < 65536, 1 <= Co <= 128, Ci, P < 2^31", "not covered here"),
@@ -188,7 +188,7 @@ def flat_samples(n, *extra):
     return torch.from_numpy(s[(s >= 0) & (s < n)])
 
 
-def test_limits_table_names_real_entry_points():
+def test_limits_table_names_exported_entry_points():
     for name in LIMITS:
         for sym in name.split(" / "):
             if "*" not in sym and sym.startswith("ffb6d_"):
@@ -755,7 +755,7 @@ def test_segment_sum_at_limits(cuda, B, C, P, NA):
 # ------------------------------------------------------------------ fusion layer
 @pytest.mark.parametrize("B,C1,Co,P", [(1, 1, 65535 * 128, 4), (1, 4, 128, (FLAT + 8192) // 128)],
                          ids=["widest_co", "out_past_2_31"])
-def test_fusion_mlp_fwd_at_limits(cuda, B, C1, Co, P):
+def test_fusion_mlp_fwd_ex_at_limits(cuda, B, C1, Co, P):
     n = B * Co * P
     need(n * 4 / GiB + 3.0)
     g = torch.Generator(device=cuda).manual_seed(Co + P)
@@ -764,8 +764,11 @@ def test_fusion_mlp_fwd_at_limits(cuda, B, C1, Co, P):
     scale = 1 + 0.1 * torch.randn(Co, generator=g, device=cuda)
     shift = 0.1 * torch.randn(Co, generator=g, device=cuda)
     out = sentinel(B, Co, P)
-    check(lib.ffb6d_fusion_mlp_fwd(x.data_ptr(), C1, None, 0, w.data_ptr(), scale.data_ptr(), shift.data_ptr(), B, Co,
-                                   P, 1, 0.0, out.data_ptr(), _stream(cuda)))
+    nb = int(lib.ffb6d_fusion_mlp_pack_bytes(Co, C1))
+    packed = torch.empty(nb, dtype=torch.uint8, device=cuda)
+    check(lib.ffb6d_fusion_mlp_pack(w.data_ptr(), Co, C1, packed.data_ptr(), nb, _stream(cuda)))
+    check(lib.ffb6d_fusion_mlp_fwd_ex(x.data_ptr(), C1, None, 0, packed.data_ptr(), scale.data_ptr(), shift.data_ptr(),
+                                      B, Co, P, 1, 0.0, None, None, 0, 0, LAYOUT_NCS, out.data_ptr(), _stream(cuda)))
     assert all_written(out)
     t = flat_samples(n, n - P + np.arange(64)).to(cuda)               # + the start of the last channel
     b, co, p = t // (Co * P), (t // P) % Co, t % P
