@@ -25,6 +25,11 @@ FPS_MAX_CLUSTER = 8                              # FFB6D_FPS_MAX_* of include/ff
 FPS_MAX_POINTS = FPS_MAX_CLUSTER * 14336
 FPS_MAX_SAMPLES = FPS_MAX_POINTS
 FPS_MAX_CLOUDS = 65535
+POSE_EVAL_GT_TILE = 512                          # FFB6D_POSE_EVAL_* of include/ffb6d_b200.h
+POSE_EVAL_PRED_TILE = 512
+POSE_EVAL_MAX_OBJECTS = 65535
+POSE_EVAL_MAX_POINTS = 1 << 20
+POSE_EVAL_MAX_MESHES = (1 << 31) - 2
 
 
 class FFB6DError(RuntimeError):
@@ -133,6 +138,8 @@ def _load():
         "ffb6d_bn_prelu_bwd": (ci, [vp, vp, vp, i64, i64, i64, vp, vp, vp, vp]),
         "ffb6d_farthest_point_sampling_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_farthest_point_sampling": (ci, [vp, vp, i64, i64, i64, vp, ci, vp, vp, sz, vp]),
+        "ffb6d_pose_add_adds_workspace_bytes": (sz, [i64, i64]),
+        "ffb6d_pose_add_adds": (ci, [vp, vp, i64, i64, vp, vp, vp, i64, vp, vp, vp, sz, vp]),
         "ffb6d_grid_subsample_host": (ci, [vp, sz, vp, sz, vp, sz, fp, vp, vp, vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():

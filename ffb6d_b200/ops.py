@@ -1055,6 +1055,46 @@ def farthest_point_sampling(pts, sn, init_center=False, start=None, return_index
     return (sel, idx) if return_index else sel
 
 
+def pose_add_adds(mesh_pts, mesh_off, obj_mesh, pred_RT, gt_RT, max_points):
+    """ADD and ADD-S of ``M`` predicted poses in one launch: ``Basic_Utils.cal_add_cuda`` / ``cal_adds_cuda``
+    (utils/basic_utils.py:651-669) for every object of a batch.
+
+    ``mesh_pts [P,3]`` float32: the meshes stacked; ``mesh_off [n_meshes+1]`` int32: mesh ``c`` is rows
+    ``mesh_off[c] .. mesh_off[c+1]``; ``obj_mesh [M]`` int32: each object's mesh; ``pred_RT``, ``gt_RT [M,3,4]``
+    float32; ``max_points``: a bound on the size of every mesh scored (it sets the grid, so no sync is needed).
+    All tensors on one CUDA device.  Returns ``(add [M], adds [M])`` float32 CUDA tensors.  An object whose pose or
+    points are not finite, or whose mesh index, offsets or size is out of range on the device, gets NaN (see
+    include/ffb6d_b200.h); capturable in a CUDA graph."""
+    pts = _tensor(mesh_pts, "mesh_pts", torch.float32, 2)
+    dev = pts.device
+    if pts.shape[1] != 3:
+        raise ValueError("mesh_pts must be [P,3], got %s" % (tuple(pts.shape),))
+    off = _tensor(mesh_off, "mesh_off", torch.int32, 1, dev)
+    om = _tensor(obj_mesh, "obj_mesh", torch.int32, 1, dev)
+    M = om.shape[0]
+    pr = _tensor(pred_RT, "pred_RT", torch.float32, (M, 3, 4), dev)
+    gt = _tensor(gt_RT, "gt_RT", torch.float32, (M, 3, 4), dev)
+    if isinstance(max_points, bool) or not isinstance(max_points, (int, np.integer)):
+        raise TypeError("max_points must be an int, got %r" % (max_points,))
+    if not 1 <= max_points <= _lib.POSE_EVAL_MAX_POINTS:
+        raise ValueError("max_points must lie in [1, %d], got %d" % (_lib.POSE_EVAL_MAX_POINTS, max_points))
+    if M > _lib.POSE_EVAL_MAX_OBJECTS:
+        raise ValueError("at most %d objects per call, got %d" % (_lib.POSE_EVAL_MAX_OBJECTS, M))
+    if off.shape[0] < 2 and M > 0:
+        raise ValueError("mesh_off must hold n_meshes + 1 >= 2 offsets, got %d" % off.shape[0])
+    if pts.shape[0] > 2 ** 31 - 1:
+        raise ValueError("mesh_pts has %d rows, more than int32 offsets address" % pts.shape[0])
+    add = torch.empty(M, dtype=torch.float32, device=dev)
+    adds = torch.empty(M, dtype=torch.float32, device=dev)
+    if M == 0:
+        return add, adds
+    nbytes = int(lib.ffb6d_pose_add_adds_workspace_bytes(M, int(max_points)))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_pose_add_adds, dev, pts.data_ptr(), off.data_ptr(), off.shape[0] - 1, int(max_points),
+           om.data_ptr(), pr.data_ptr(), gt.data_ptr(), M, add.data_ptr(), adds.data_ptr(), ws.data_ptr(), nbytes)
+    return add, adds
+
+
 def mean_shift_fit(votes, valid=None, bandwidth=0.05, max_iter=300, return_modes=False):
     """Gaussian mean shift of ``G`` independent vote sets in one persistent kernel: the batched form of
     ``MeanShiftTorch.fit`` (utils/meanshift_pytorch.py:33-57).

@@ -570,6 +570,39 @@ int ffb6d_farthest_point_sampling(const float *pts, const int *n_points_per_clou
                                   const int *start, int init_center, int *idx_out, void *ws, size_t ws_bytes,
                                   ffb6d_stream_t stream);
 
+/* ---- pose scoring (ADD / ADD-S) ------------------------------------------ */
+/*
+ * ADD and ADD-S of M predicted poses, replacing Basic_Utils.cal_add_cuda / cal_adds_cuda (utils/basic_utils.py:
+ * 651-669) as eval_metric / eval_metric_lm call them once per object (utils/pvn3d_eval_utils_kpls.py:162-195,
+ * 287-304).  For object m with mesh points x_i, the rows mesh_off[c] .. mesh_off[c+1] of mesh_pts, c = obj_mesh[m],
+ * and the poses P = pred_RT[m], G = gt_RT[m]:
+ *   add[m]  = mean_i |P x_i - G x_i|
+ *   adds[m] = mean_i min_j |P x_j - G x_i|
+ *   mesh_pts [sum of mesh sizes, 3] f32; mesh_off [n_meshes + 1] int32 with mesh_off[n_meshes] <= the rows of
+ *   mesh_pts; obj_mesh [M] int32; pred_RT, gt_RT [M,3,4] f32 row-major -> add, adds [M] f32.
+ * d = P x_j - G x_i is formed before |d|^2 (no |a|^2 + |b|^2 - 2 a.b), the min is taken over squared distances with
+ * NaN propagating like torch.min, and one sqrt follows; sums run in fp64 in a fixed order, rounded once to f32, so
+ * results are deterministic and pred_RT == gt_RT gives 0 exactly.  A non-finite value in an object's poses or
+ * points gives that object NaN.  So does, without a fault, an obj_mesh[m] outside [0, n_meshes), a negative or
+ * decreasing offset, or a mesh of 0 or more than max_points points; other objects are unaffected.
+ * max_points is the host's bound on every scored mesh's size: it sets the grid (ceil(max_points /
+ * FFB6D_POSE_EVAL_GT_TILE) x M CTAs, DESIGN.md §4.24) without a sync.
+ * 0 <= M <= FFB6D_POSE_EVAL_MAX_OBJECTS (M = 0 is a no-op), 1 <= max_points <= FFB6D_POSE_EVAL_MAX_POINTS,
+ * 1 <= n_meshes <= FFB6D_POSE_EVAL_MAX_MESHES when M > 0; pointers 4-byte aligned, the workspace 16-byte aligned.
+ * workspace: ffb6d_pose_add_adds_workspace_bytes(M, max_points) bytes (FFB6D_ERR_WORKSPACE if missing or smaller).
+ * Arguments are checked before any launch (FFB6D_ERR_INVALID); two launches, no allocation, no host
+ * synchronisation (capturable in a CUDA graph).
+ */
+#define FFB6D_POSE_EVAL_GT_TILE 512
+#define FFB6D_POSE_EVAL_PRED_TILE 512
+#define FFB6D_POSE_EVAL_MAX_OBJECTS 65535
+#define FFB6D_POSE_EVAL_MAX_POINTS 1048576
+#define FFB6D_POSE_EVAL_MAX_MESHES 2147483646
+size_t ffb6d_pose_add_adds_workspace_bytes(int64_t M, int64_t max_points);
+int ffb6d_pose_add_adds(const float *mesh_pts, const int32_t *mesh_off, int64_t n_meshes, int64_t max_points,
+                        const int32_t *obj_mesh, const float *pred_RT, const float *gt_RT, int64_t M, float *add,
+                        float *adds, void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+
 /* ---- grid subsampling --------------------------------------------------- */
 /*
  * Voxel-grid barycentre subsampling, replaces grid_subsampling()
