@@ -20,7 +20,7 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   (datasets/ycb/ycb_dataset.py:79-163, datasets/linemod/linemod_dataset.py:114-186) on the GPU; the scalar draws stay
   in the worker (:mod:`ffb6d_b200.augment`).  :func:`color_jitter` -- the datasets' ``trancolor``
   (torchvision ``ColorJitter``) on the GPU, from plans of :func:`ffb6d_b200.augment.draw_color_jitter`.
-* :mod:`ffb6d_b200.pose` -- ``MeanShiftTorch``, ``best_fit_transform``, ``cal_frame_poses(_lm)``
+* :mod:`ffb6d_b200.pose` -- ``MeanShiftTorch``, ``best_fit_transform``, ``cal_batch_poses``, ``cal_frame_poses(_lm)``
   (utils/meanshift_pytorch.py:27-57, utils/pvn3d_eval_utils_kpls.py:28-160, 220-284): keypoint voting on the GPU;
   ``cal_add_cuda``, ``cal_adds_cuda``, ``cal_auc``, ``eval_metric(_lm)`` and ``TorchEval`` (utils/basic_utils.py:34-46,
   642-669, utils/pvn3d_eval_utils_kpls.py:162-195, 287-304, 326-505): the ADD / ADD-S scoring of a whole batch in
@@ -55,7 +55,7 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "fill_missing", "segment_plan", "segment_sum", "point_item", "rgb_add_noise", "add_real_back",
         "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax",
         "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d",
-        "farthest_point_sampling", "pose_add_adds")
+        "farthest_point_sampling", "pose_add_adds", "vote_poses")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")

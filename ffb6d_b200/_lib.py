@@ -30,6 +30,11 @@ POSE_EVAL_PRED_TILE = 512
 POSE_EVAL_MAX_OBJECTS = 65535
 POSE_EVAL_MAX_POINTS = 1 << 20
 POSE_EVAL_MAX_MESHES = (1 << 31) - 2
+VOTE_MAX_POINTS = (1 << 24) - 1                  # FFB6D_VOTE_* of include/ffb6d_b200.h
+VOTE_MAX_CLASSES = 1024
+VOTE_MAX_KPS = 64
+VOTE_MAX_SETS = 1 << 24
+VOTE_MAX_SLOTS = (1 << 31) - 1
 
 
 class FFB6DError(RuntimeError):
@@ -116,6 +121,9 @@ def _load():
         "ffb6d_mean_shift_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_mean_shift_fit": (ci, [vp, vp, i64, i64, i64, fp, ci, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_best_fit_transform": (ci, [vp, vp, i64, i64, vp, vp]),
+        "ffb6d_vote_poses_workspace_bytes": (sz, [i64, i64, i64, i64]),
+        "ffb6d_vote_poses": (ci, [vp, vp, vp, vp, vp, vp, vp, i64, i64, i64, i64, ci, ci, fp, ci, vp, vp, vp, vp, vp,
+                                  sz, vp]),
         "ffb6d_rgb_add_noise": (ci, [vp, i64, i64, i64, vp, vp, C.c_uint64, vp, vp, vp, vp]),
         "ffb6d_add_real_back": (ci, [vp, vp, vp, vp, vp, ci, vp, vp, ci, i64, i64, i64, vp, vp, vp]),
         "ffb6d_aug_noise_field": (ci, [C.c_uint64, i64, i64, i64, ci, vp, vp]),

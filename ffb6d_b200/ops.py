@@ -1137,6 +1137,50 @@ def mean_shift_fit(votes, valid=None, bandwidth=0.05, max_iter=300, return_modes
     return out + (modes,) if return_modes else out
 
 
+def vote_poses(pcld, mask, ctr_of, kp_of, mesh_kps, has_mesh, refine_thr=None, use_ctr=True, ctr_filter=True,
+               bandwidth=0.04, max_iter=300):
+    """The poses of every object of ``B`` frames in one call (``ffb6d_vote_poses``): the batched form of
+    ``cal_frame_poses`` (utils/pvn3d_eval_utils_kpls.py:65-160), every vote set of a stage in one mean-shift launch.
+
+    :param pcld: ``[B,N,3]`` float32 CUDA; ``mask`` ``[B,N]`` int64 predicted class ids in ``[0, n_cls)``;
+      ``ctr_of`` ``[B,1,N,3]``, ``kp_of`` ``[B,n_kps,N,3]`` float32.
+    :param mesh_kps: ``[n_cls,R,3]`` float32 object-frame keypoints, ``R = n_kps + use_ctr`` (centre last);
+      ``has_mesh`` ``[n_cls]`` bool/uint8: the classes whose row is filled.
+    :param refine_thr: ``[n_cls]`` float32 distances of the centre-clustering refinement, or None for none.
+    :return: ``(present [B,n_cls] bool, count [B,n_cls] int32, kps [B,n_cls,R,3] float32, poses [B,n_cls,3,4]
+      float64)`` CUDA tensors (see include/ffb6d_b200.h for the rows without a fit and the NaN rows).  No host
+      synchronisation: capturable in a CUDA graph."""
+    p = _tensor(pcld, "pcld", torch.float32, 3)
+    dev = p.device
+    B, N, _ = p.shape
+    if p.shape[2] != 3:
+        raise ValueError("pcld must be [B,N,3], got %s" % (tuple(p.shape),))
+    m = _tensor(mask, "mask", torch.int64, (B, N), dev)
+    c = _tensor(ctr_of, "ctr_of", torch.float32, (B, 1, N, 3), dev)
+    k = _tensor(kp_of, "kp_of", torch.float32, 4, dev)
+    n_kps = k.shape[1]
+    if tuple(k.shape) != (B, n_kps, N, 3):
+        raise ValueError("kp_of must be [B,n_kps,N,3] = [%d,n_kps,%d,3], got %s" % (B, N, tuple(k.shape)))
+    mk = _tensor(mesh_kps, "mesh_kps", torch.float32, 3, dev)
+    n_cls, R = mk.shape[0], n_kps + int(bool(use_ctr))
+    if tuple(mk.shape) != (n_cls, R, 3):
+        raise ValueError("mesh_kps must be [n_cls,%d,3], got %s" % (R, tuple(mk.shape)))
+    hm = _tensor(has_mesh.to(torch.uint8) if torch.is_tensor(has_mesh) and has_mesh.dtype == torch.bool else has_mesh,
+                 "has_mesh", torch.uint8, (n_cls,), dev)
+    thr = None if refine_thr is None else _tensor(refine_thr, "refine_thr", torch.float32, (n_cls,), dev)
+    present = torch.empty((B, n_cls), dtype=torch.uint8, device=dev)
+    count = torch.empty((B, n_cls), dtype=torch.int32, device=dev)
+    kps = torch.empty((B, n_cls, R, 3), dtype=torch.float32, device=dev)
+    poses = torch.empty((B, n_cls, 3, 4), dtype=torch.float64, device=dev)
+    nbytes = int(lib.ffb6d_vote_poses_workspace_bytes(B, N, n_cls, n_kps))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_vote_poses, dev, p.data_ptr(), m.data_ptr(), c.data_ptr(), k.data_ptr(), mk.data_ptr(),
+           hm.data_ptr(), ptr(thr), B, N, n_cls, n_kps, int(bool(use_ctr)), int(bool(ctr_filter)), float(bandwidth),
+           int(max_iter), present.data_ptr(), count.data_ptr(), kps.data_ptr(), poses.data_ptr(), ws.data_ptr(),
+           nbytes)
+    return present.bool(), count, kps, poses
+
+
 def best_fit_transform(A, B):
     """Least-squares rigid transform of point sets ``A -> B`` (pvn3d_eval_utils_kpls.py:28-59), batched.
 

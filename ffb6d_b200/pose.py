@@ -5,7 +5,8 @@ Mirrors of the reference's evaluation helpers, same names and argument meaning:
 * :class:`MeanShiftTorch` -- ``utils/meanshift_pytorch.py:27-57`` (``fit``; ``fit_multi_clus`` is only used by
   that file's own ``__main__`` and is not provided);
 * :func:`best_fit_transform` -- ``utils/pvn3d_eval_utils_kpls.py:28-59`` (numpy in, numpy ``[3,4]`` out);
-* :func:`cal_frame_poses`, :func:`cal_frame_poses_lm` -- ``utils/pvn3d_eval_utils_kpls.py:65-160, 220-284``;
+* :func:`cal_frame_poses`, :func:`cal_frame_poses_lm` -- ``utils/pvn3d_eval_utils_kpls.py:65-160, 220-284``, B = 1
+  calls of :func:`cal_batch_poses`, which votes every object of a batch without a host sync;
 * :func:`cal_add_cuda`, :func:`cal_adds_cuda`, :func:`cal_auc`, :func:`VOCap` -- ``utils/basic_utils.py:34-46,
   642-669`` (``Basic_Utils`` methods there, functions here);
 * :func:`eval_metric`, :func:`eval_metric_lm`, :class:`TorchEval` -- ``utils/pvn3d_eval_utils_kpls.py:162-195,
@@ -14,8 +15,9 @@ Mirrors of the reference's evaluation helpers, same names and argument meaning:
 
 The reference reads mesh keypoints, mesh centres and object radii from dataset files through its module-level
 ``bs_utils`` / ``config``; here the caller passes them (``mesh_kps``, ``cls_radius``).  Everything numeric runs in
-:func:`ffb6d_b200.ops.mean_shift_fit` (one persistent kernel for all keypoints of an object instead of one
-N x N torch program per keypoint and a host sync per iteration) and :func:`ffb6d_b200.ops.best_fit_transform`.
+:func:`ffb6d_b200.ops.vote_poses` (all vote sets of a batch in one persistent mean-shift kernel per stage instead of
+one N x N torch program per keypoint and a host sync per iteration), :func:`ffb6d_b200.ops.mean_shift_fit` and
+:func:`ffb6d_b200.ops.best_fit_transform`.
 """
 import numpy as np
 import torch
@@ -54,69 +56,132 @@ def best_fit_transform(A, B):
     return ops.best_fit_transform(a, b).cpu().numpy()
 
 
-def _vote_object(pred_ctr, pred_kp, cls_msk, radius, use_ctr, use_ctr_clus_flter):
-    """Centre + keypoints of one object: the two clustering steps of pvn3d_eval_utils_kpls.py:122-137."""
-    ms = MeanShiftTorch(bandwidth=radius)
-    ctr, ctr_labels = ms.fit_batch(pred_ctr[None], cls_msk)
-    kp_msk = ctr_labels[0] if use_ctr_clus_flter else cls_msk       # `cls_voted_kps[:, ctr_labels, :]`
-    kps, _ = ms.fit_batch(pred_kp, kp_msk)
-    return torch.cat((kps, ctr), 0) if use_ctr else kps
+class VoteTable:
+    """The per-class inputs of :func:`cal_batch_poses`, resident on the GPU and indexed by class id ``0 .. n_cls-1``.
+
+    ``mesh_kps``: mapping ``cls_id -> [rows,3]`` object-frame keypoints, the centre last (what the reference loads
+    with ``bs_utils.get_kps`` / ``get_ctr``), every one with the same number of rows; ``cls_radius``: sequence
+    indexed by ``cls_id - 1`` (``config.ycb_r_lst``) or None.  Holds ``kps [n_cls,rows,3]`` float32 (zero for ids
+    without keypoints), ``has_mesh [n_cls]`` uint8 and ``refine_thr [n_cls]`` float32, the refinement distance
+    ``float32(float64(r) * 0.8)`` as the reference rounds it (None without ``cls_radius``)."""
+
+    def __init__(self, mesh_kps, n_cls, cls_radius=None, device=None):
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        arrs = {int(c): np.asarray(torch.as_tensor(v).detach().cpu(), np.float32) for c, v in mesh_kps.items()}
+        if any(c < 0 or c >= n_cls for c in arrs):
+            raise ValueError("mesh_kps ids must lie in [0, %d), got %s" % (n_cls, sorted(arrs)))
+        shapes = {a.shape for a in arrs.values()}
+        if len(shapes) > 1 or any(len(sh) != 2 or sh[1] != 3 for sh in shapes):
+            raise ValueError("mesh_kps must all be [rows,3] with one row count, got %s" % sorted(shapes))
+        rows = shapes.pop()[0] if shapes else 1
+        kps = np.zeros((n_cls, rows, 3), np.float32)
+        has = np.zeros(n_cls, np.uint8)
+        for c, a in arrs.items():
+            kps[c], has[c] = a, 1
+        self.n_cls = n_cls
+        self.kps = torch.as_tensor(kps, device=dev)
+        self.has_mesh = torch.as_tensor(has, device=dev)
+        self.refine_thr = None
+        if cls_radius is not None:
+            r = np.asarray(cls_radius, np.float64).reshape(-1)
+            if r.shape[0] < n_cls - 1:
+                raise ValueError("cls_radius needs n_cls - 1 = %d entries, got %d" % (n_cls - 1, r.shape[0]))
+            thr = np.zeros(n_cls, np.float32)
+            thr[1:] = (r[:n_cls - 1] * 0.8).astype(np.float32)
+            self.refine_thr = torch.as_tensor(thr, device=dev)
+        self.device = dev
+
+    def rows(self, R):
+        """``[n_cls,R,3]``: the first ``R`` keypoint rows of every class."""
+        if R > self.kps.shape[1]:
+            raise ValueError("mesh_kps have %d rows, %d needed" % (self.kps.shape[1], R))
+        return self.kps[:, :R].contiguous()
+
+
+def _vote(table, pclds, masks, ctr_ofs, kp_ofs, use_ctr, ctr_filter, refine):
+    n_kps = kp_ofs.shape[1]
+    return ops.vote_poses(pclds, masks.long(), ctr_ofs, kp_ofs, table.rows(n_kps + int(bool(use_ctr))),
+                          table.has_mesh, table.refine_thr if refine else None, use_ctr, ctr_filter, bandwidth=0.04,
+                          max_iter=300)
+
+
+def cal_batch_poses(pclds, masks, ctr_ofs, kp_ofs, use_ctr, n_cls, use_ctr_clus_flter, *, mesh_kps, cls_radius=None):
+    """:func:`cal_frame_poses` of a whole batch in one :func:`ffb6d_b200.ops.vote_poses` call, without a host
+    synchronisation: ``pclds [B,N,3]``, ``masks [B,N]``, ``ctr_ofs [B,1,N,3]``, ``kp_ofs [B,n_kps,N,3]`` as the
+    network's ``end_points`` hold them.  ``mesh_kps``: a :class:`VoteTable`, or the mapping one is built from with
+    ``n_cls`` and ``cls_radius``.  ``use_ctr_clus_flter`` turns on the centre-clustering refinement of the mask
+    (when there are radii) and the centre-label filter of the keypoint votes, as in the reference.
+
+    Returns ``(present [B,n_cls] bool, count [B,n_cls] int32, kps [B,n_cls,n_kps+use_ctr,3] float32,
+    poses [B,n_cls,3,4] float64)`` CUDA tensors: ``present`` the classes of the unrefined mask (the reference's
+    ``pred_cls_ids``), ``count`` their points after refinement; a class left without points has the identity pose
+    and zero keypoints, an absent class zeros, and a frame with a mask id outside ``[0, n_cls)`` NaN rows, as does a
+    present class without keypoints in ``mesh_kps``."""
+    table = mesh_kps if isinstance(mesh_kps, VoteTable) else VoteTable(mesh_kps, n_cls, cls_radius, pclds.device)
+    return _vote(table, pclds, masks, ctr_ofs, kp_ofs, use_ctr, use_ctr_clus_flter,
+                 use_ctr_clus_flter and table.refine_thr is not None)
+
+
+def _to_host(*ts):
+    """Numpy copies of the CUDA tensors ``ts``, through one device-to-host copy."""
+    flat = torch.cat([t.contiguous().reshape(-1).view(torch.uint8) for t in ts]).cpu().numpy()
+    out, o = [], 0
+    for t in ts:
+        dt = np.dtype(str(t.dtype).replace("torch.", "")) if t.dtype != torch.bool else np.dtype(np.bool_)
+        n = t.numel() * dt.itemsize
+        out.append(flat[o:o + n].view(dt).reshape(tuple(t.shape)))
+        o += n
+    return out
+
+
+def _frame_lists(present, count, kps, poses, has_mesh, n_kps):
+    """The reference's ``(pred_cls_ids, pred_pose_lst, pred_kps_lst)`` of one frame from its host rows."""
+    if np.isnan(poses[0]).any():
+        raise ValueError("the mask holds a class id outside [0, %d)" % present.shape[0])
+    ids = np.flatnonzero(present).astype(np.int64)
+    missing = [int(c) for c in ids if not has_mesh[c]]
+    if missing:
+        raise ValueError("no mesh keypoints for predicted class(es) %s" % missing)
+    pose_lst, kps_lst = [], []
+    for c in ids:
+        empty = count[c] == 0
+        pose_lst.append(np.identity(4)[:3, :] if empty else poses[c])
+        kps_lst.append(np.zeros((n_kps + 1, 3)) if empty else kps[c])
+    return ids, pose_lst, kps_lst
 
 
 def cal_frame_poses(pcld, mask, ctr_of, pred_kp_of, use_ctr, n_cls, use_ctr_clus_flter, gt_kps=None, gt_ctrs=None,
                     debug=False, kp_type="farthest", *, mesh_kps, cls_radius=None):
-    """YCB-style multi-object voting (pvn3d_eval_utils_kpls.py:65-160).
+    """YCB-style multi-object voting (pvn3d_eval_utils_kpls.py:65-160): :func:`cal_batch_poses` of one frame.
 
-    ``pcld [N,3]``, ``mask [N]`` predicted class ids, ``ctr_of [1,N,3]``, ``pred_kp_of [n_kps,N,3]`` (CUDA).
-    ``mesh_kps``: mapping ``cls_id -> [n_kps(+1),3]`` array of object-frame keypoints (the centre last when
-    ``use_ctr``), what the reference loads with ``bs_utils.get_kps`` / ``get_ctr``; ``cls_radius``: sequence
-    indexed by ``cls_id - 1`` (``config.ycb_r_lst``), needed for the centre-clustering mask filter.
-    Returns ``(pred_cls_ids, pred_pose_lst, pred_kps_lst)`` like the reference."""
-    n_kps, n_pts, _ = pred_kp_of.shape
-    pred_ctr = pcld - ctr_of[0]
-    pred_kp = pcld.view(1, n_pts, 3) - pred_kp_of
-    radius = 0.04
-    pred_cls_ids = np.unique(mask[mask > 0].contiguous().cpu().numpy())
-    if use_ctr_clus_flter and len(pred_cls_ids) > 0 and cls_radius is not None:
-        # refine the mask: a point takes the class of the nearest voted centre when it is close enough (:85-109)
-        ms = MeanShiftTorch(bandwidth=radius)
-        msks = torch.stack([mask == int(c) for c in pred_cls_ids])
-        ctrs, _ = ms.fit_batch(pred_ctr[None].expand(len(pred_cls_ids), n_pts, 3).contiguous(), msks)
-        min_dis, min_idx = torch.cdist(pred_ctr, ctrs).min(dim=1)
-        ids_t = torch.as_tensor(pred_cls_ids.astype(np.int64), device=mask.device)
-        closest = ids_t[min_idx].to(mask.dtype)
-        r = torch.as_tensor(np.asarray(cls_radius, np.float32), device=mask.device)[(ids_t - 1).clamp(min=0)][min_idx]
-        update = (mask > 0) & (min_dis < r * 0.8)
-        mask = torch.where(update, closest, mask)
-    pred_pose_lst, pred_kps_lst = [], []
-    for cls_id in pred_cls_ids:
-        if cls_id == 0:
-            break
-        cls_msk = mask == int(cls_id)
-        if int(cls_msk.sum()) < 1:
-            pred_pose_lst.append(np.identity(4)[:3, :])
-            pred_kps_lst.append(np.zeros((n_kps + 1, 3)))
-            continue
-        kpc = _vote_object(pred_ctr, pred_kp, cls_msk, radius, use_ctr, use_ctr_clus_flter)
-        mk = torch.as_tensor(np.asarray(mesh_kps[int(cls_id)], np.float32), device=kpc.device)
-        pred_pose_lst.append(ops.best_fit_transform(mk, kpc).cpu().numpy())
-        pred_kps_lst.append(kpc.cpu().numpy())
-    return pred_cls_ids, pred_pose_lst, pred_kps_lst
+    ``pcld [N,3]``, ``mask [N]`` predicted class ids in ``[0, n_cls)``, ``ctr_of [1,N,3]``, ``pred_kp_of
+    [n_kps,N,3]`` (CUDA).  ``mesh_kps``: mapping ``cls_id -> [n_kps(+1),3]`` array of object-frame keypoints (the
+    centre last when ``use_ctr``), what the reference loads with ``bs_utils.get_kps`` / ``get_ctr``; ``cls_radius``:
+    sequence indexed by ``cls_id - 1`` (``config.ycb_r_lst``), needed for the centre-clustering mask refinement.
+    Returns ``(pred_cls_ids, pred_pose_lst, pred_kps_lst)`` like the reference; raises ValueError for a mask id out
+    of range or a predicted class without keypoints."""
+    n_kps = pred_kp_of.shape[0]
+    table = VoteTable(mesh_kps, n_cls, cls_radius, pcld.device)
+    present, count, kps, poses = _vote(table, pcld[None], mask[None], ctr_of[None], pred_kp_of[None], use_ctr,
+                                       use_ctr_clus_flter, use_ctr_clus_flter and cls_radius is not None)
+    poses, kps, count, present, has = _to_host(poses[0], kps[0], count[0], present[0], table.has_mesh)
+    return _frame_lists(present, count, kps, poses, has, n_kps)
+
+
+def _lm_table(mesh_kps, device):
+    return VoteTable({1: mesh_kps}, 2, None, device)
 
 
 def cal_frame_poses_lm(pcld, mask, ctr_of, pred_kp_of, use_ctr, n_cls, use_ctr_clus_flter, obj_id, debug=False, *,
                        mesh_kps):
-    """LineMOD-style single-object voting (pvn3d_eval_utils_kpls.py:220-284): class 1 is the object.
+    """LineMOD-style single-object voting (pvn3d_eval_utils_kpls.py:220-284): class 1 is the object, every other id
+    background; a :func:`cal_batch_poses` of one frame with two classes and no refinement.
     ``mesh_kps [n_kps(+1),3]``: object-frame keypoints of ``obj_id`` (centre last when ``use_ctr``)."""
-    n_kps, n_pts, _ = pred_kp_of.shape
-    pred_ctr = pcld - ctr_of[0]
-    pred_kp = pcld.view(1, n_pts, 3) - pred_kp_of
-    cls_msk = mask == 1
-    if int(cls_msk.sum()) < 1:
-        return [np.identity(4)[:3, :]]
-    kpc = _vote_object(pred_ctr, pred_kp, cls_msk, 0.04, use_ctr, use_ctr_clus_flter)
-    mk = torch.as_tensor(np.asarray(mesh_kps, np.float32), device=kpc.device)
-    return [ops.best_fit_transform(mk, kpc).cpu().numpy()]
+    table = _lm_table(mesh_kps, pcld.device)
+    present, _, _, poses = _vote(table, pcld[None], (mask == 1)[None], ctr_of[None], pred_kp_of[None], use_ctr,
+                                 use_ctr_clus_flter, False)
+    poses, present = _to_host(poses[0, 1], present[0, 1])
+    return [poses if present else np.identity(4)[:3, :]]
 
 
 # ---------------------------------------------------------------------------------------------------- pose scoring
@@ -297,9 +362,9 @@ class TorchEval:
     ``cls_id -> [n_kps(+1),3]``, see :func:`cal_frame_poses`), ``cls_radius`` (``config.ycb_r_lst``) and
     ``sym_cls_ids`` (``config.ycb_sym_cls_ids`` or ``config_lm.lm_sym_cls_ids``).
 
-    :meth:`eval_pose_parallel` votes each frame with :func:`cal_frame_poses` / :func:`cal_frame_poses_lm` and then
-    scores every object of the batch in one :func:`ffb6d_b200.ops.pose_add_adds` launch; the lists grow frame by
-    frame, object by object, as the reference's ``executor.map`` makes them.  :meth:`cal_auc` and :meth:`cal_lm_add`
+    :meth:`eval_pose_parallel` votes the batch in one :func:`cal_batch_poses` call and scores every object of it in
+    one :func:`ffb6d_b200.ops.pose_add_adds` launch; the lists grow frame by frame, object by object, as the
+    reference's ``executor.map`` makes them.  :meth:`cal_auc` and :meth:`cal_lm_add`
     return the dict the reference pickles plus the averages it prints; they print nothing and write no file.
 
     One deliberate difference: the reference's ``cal_auc`` / ``cal_lm_add`` append to ``cls_add_s_dis[0]`` on every
@@ -309,8 +374,9 @@ class TorchEval:
     def __init__(self, mesh_pts, mesh_kps, cls_radius=None, sym_cls_ids=(), n_cls=22):
         self.n_cls = n_cls
         self.mesh_table = MeshTable(mesh_pts)
-        self.mesh_kps = mesh_kps
-        self.cls_radius = cls_radius
+        dev = self.mesh_table.device
+        self.vote_table = VoteTable({c: k for c, k in mesh_kps.items() if 0 <= int(c) < n_cls}, n_cls, cls_radius, dev)
+        self.lm_tables = {int(c): _lm_table(k, dev) for c, k in mesh_kps.items()}
         self.sym_cls_ids = list(sym_cls_ids)
         self.cls_add_dis = [[] for _ in range(n_cls)]
         self.cls_adds_dis = [[] for _ in range(n_cls)]
@@ -323,42 +389,49 @@ class TorchEval:
                            use_ctr=True, obj_id=0, kp_type="farthest", ds="ycb"):
         """Vote and score one batch (pvn3d_eval_utils_kpls.py:448-500), appending to the per-class lists.  ``rgbs``,
         ``gt_ctr_ofs``, ``labels``, ``cnt``, ``min_cnt`` and ``merge_clus`` are accepted and unread, as in the
-        reference."""
-        bs = pred_kp_ofs.shape[0]
-        masks = masks.long()
-        ids_h = _ids_column(cls_ids.reshape(-1, 1)).reshape(bs, -1)
-        cls, poses, where, per_frame = [], [], [], []
+        reference.  One :func:`cal_batch_poses` call votes the batch, each ground-truth object's predicted pose is
+        taken on the device, one :func:`ffb6d_b200.ops.pose_add_adds` launch scores every object, and one
+        device-to-host copy brings back what the lists need."""
+        bs, n_obj = RTs.shape[0], RTs.shape[1]
+        dev = self.mesh_table.device
+        gt = RTs.reshape(bs * n_obj, 3, 4).to(dev, torch.float32)
         if ds == "ycb":
-            gt_kps_h = gt_kps.detach().cpu().numpy()
+            n_kps = pred_kp_ofs.shape[1]
+            present, count, kps, poses = _vote(self.vote_table, pclds, masks, pred_ctr_ofs, pred_kp_ofs, use_ctr,
+                                               use_ctr_clus_flter,
+                                               use_ctr_clus_flter and self.vote_table.refine_thr is not None)
+            ids = torch.as_tensor(cls_ids).to(dev).reshape(bs, n_obj, -1)[:, :, 0].long()
+            ok = (ids >= 0) & (ids < self.n_cls)
+            pick = torch.where(ok, ids, 0)
+            pred = poses[torch.arange(bs, device=dev)[:, None], pick].float()     # absent classes: zero rows
+            pred = torch.where(ok[..., None, None], pred, 0.0).reshape(bs * n_obj, 3, 4)
+            om = ids.clamp(-1, 2 ** 31 - 1).int().reshape(-1)        # an id without a mesh scores NaN
+            add, adds = ops.pose_add_adds(self.mesh_table.pts, self.mesh_table.off, om,
+                                          pred.contiguous(), gt.contiguous(), self.mesh_table.max_points)
+            add, adds, poses, kps, count, present, ids_h, gt_kps_h, has = _to_host(
+                add, adds, poses, kps, count, present, ids, torch.as_tensor(gt_kps).to(dev), self.vote_table.has_mesh)
             for b in range(bs):
-                pred_cls_ids, pred_poses, pred_kpcs = cal_frame_poses(
-                    pclds[b], masks[b], pred_ctr_ofs[b], pred_kp_ofs[b], use_ctr, self.n_cls, use_ctr_clus_flter,
-                    gt_kps[b], gt_ctrs[b], kp_type=kp_type, mesh_kps=self.mesh_kps, cls_radius=self.cls_radius)
+                pred_cls_ids, pred_poses, pred_kpcs = _frame_lists(present[b], count[b], kps[b], poses[b], has, n_kps)
                 self.pred_id2pose_lst.append({cid: pose for cid, pose in zip(pred_cls_ids, pred_poses)})
-                c, p, e = _frame_objects(ids_h[b], pred_poses, pred_cls_ids, gt_kps_h[b], pred_kpcs)
-                per_frame.append((c, e))
-                cls += c
-                poses += p
-                where += [b * RTs.shape[1] + i for i in range(len(c))]
-        else:
-            for b in range(bs):
-                pose = cal_frame_poses_lm(pclds[b], masks[b], pred_ctr_ofs[b], pred_kp_ofs[b], use_ctr, self.n_cls,
-                                          use_ctr_clus_flter, obj_id, mesh_kps=self.mesh_kps[obj_id])[0]
-                per_frame.append(([int(obj_id)], None))
-                cls.append(int(obj_id))
-                poses.append(np.asarray(pose).astype(np.float32))
-                where.append(b * RTs.shape[1])
-        sel = torch.as_tensor(np.asarray(where, np.int64)).to(RTs.device)
-        add, adds = _score(self.mesh_table, cls, poses, RTs.reshape(-1, 3, 4)[sel])
-        k = 0
-        for c, errs in per_frame:
-            for j, cid in enumerate(c):
-                if errs is not None:
+                c, _, errs = _frame_objects(ids_h[b], pred_poses, pred_cls_ids, gt_kps_h[b], pred_kpcs)
+                for j, cid in enumerate(c):
                     self.pred_kp_errs[cid].append(errs[j])
-                for i in (cid, 0):
-                    self.cls_add_dis[i].append(add[k])
-                    self.cls_adds_dis[i].append(adds[k])
-                k += 1
+                    for i in (cid, 0):
+                        self.cls_add_dis[i].append(float(add[b * n_obj + j]))
+                        self.cls_adds_dis[i].append(float(adds[b * n_obj + j]))
+        else:
+            present, _, _, poses = _vote(self.lm_tables[int(obj_id)], pclds, masks == 1, pred_ctr_ofs, pred_kp_ofs,
+                                         use_ctr, use_ctr_clus_flter, False)
+            eye = torch.eye(3, 4, dtype=torch.float32, device=dev)
+            pred = torch.where(present[:, 1, None, None], poses[:, 1].float(), eye)      # no point: the identity
+            om = torch.full((bs,), int(obj_id), dtype=torch.int32, device=dev)
+            add, adds = ops.pose_add_adds(self.mesh_table.pts, self.mesh_table.off, om, pred.contiguous(),
+                                          gt.reshape(bs, n_obj, 3, 4)[:, 0].contiguous(), self.mesh_table.max_points)
+            add, adds = _to_host(add, adds)
+            for b in range(bs):
+                for i in (int(obj_id), 0):
+                    self.cls_add_dis[i].append(float(add[b]))
+                    self.cls_adds_dis[i].append(float(adds[b]))
 
     def _add_s_lists(self, cls_range):
         self.cls_add_s_dis = [[] for _ in range(self.n_cls)]

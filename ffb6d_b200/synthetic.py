@@ -244,6 +244,50 @@ def make_pose_frame(seed, n_kps=8):
     return dict(pcld=pcld, mask=mask, ctr_of=ctr_of, kp_of=kp_of, mesh=mesh, cls_radius=radius, poses=poses)
 
 
+def make_pose_batch(seed, B, n_points=12288, n_objects=5, n_cls=22, n_kps=8):
+    """A seeded batch of the network's per-point predictions at the size the test loop votes: ``B`` frames of
+    ``n_points`` points, each with ``n_objects`` objects of distinct classes drawn from ``1 .. n_cls-1`` (1 500 to
+    3 000 points each, fewer when they would leave under a tenth of the frame to the background) and background.  Object points vote their object's centre and keypoints with 4 mm noise, 5 %
+    of them far from everything; background points vote noise.  Returns ``pcld [B,N,3]``, ``mask [B,N]`` int64,
+    ``ctr_of [B,1,N,3]``, ``kp_of [B,n_kps,N,3]`` (float32), ``mesh {cls: [n_kps+1,3]}`` (centre last) for every
+    class and ``cls_radius`` (``n_cls - 1`` entries, indexed by ``cls - 1``)."""
+    rs = np.random.RandomState(seed)
+    mesh = {c: np.concatenate((rs.uniform(-0.08, 0.08, (n_kps, 3)), rs.uniform(-0.01, 0.01, (1, 3))))
+            for c in range(1, n_cls)}
+    cls_radius = list(rs.uniform(0.06, 0.14, n_cls - 1))
+    pcld = np.zeros((B, n_points, 3), np.float32)
+    mask = np.zeros((B, n_points), np.int64)
+    ctr_of = np.zeros((B, 1, n_points, 3), np.float32)
+    kp_of = np.zeros((B, n_kps, n_points, 3), np.float32)
+    for b in range(B):
+        cls = rs.choice(np.arange(1, n_cls), n_objects, replace=False)
+        sizes = rs.randint(1500, min(3000, int(0.9 * n_points) // n_objects) + 1, n_objects)
+        pts, lab, cv, kv = [], [], [], []
+        for k, (c, n) in enumerate(zip(cls, sizes)):
+            ang = 2 * np.pi * k / n_objects
+            T = np.concatenate((_rotation(rs), (np.array([0.35 * np.cos(ang), 0.25 * np.sin(ang), 1.0]) +
+                                                rs.uniform(-0.03, 0.03, 3))[:, None]), axis=1)
+            cam = mesh[c] @ T[:, :3].T + T[:, 3]
+            pts.append(cam[n_kps] + rs.normal(0, 0.03, (n, 3)))
+            lab.append(np.full(n, c))
+            v = cam[None] + rs.normal(0, 0.004, (n, n_kps + 1, 3))
+            bad = rs.rand(n) < 0.05
+            v[bad] = rs.uniform(-0.7, 0.7, (int(bad.sum()), n_kps + 1, 3)) + [0.0, 0.0, 1.0]
+            cv.append(v[:, n_kps])
+            kv.append(v[:, :n_kps].transpose(1, 0, 2))
+        nb = n_points - int(sizes.sum())
+        pts.append(rs.uniform(-0.5, 0.5, (nb, 3)) + [0.0, 0.0, 1.0])
+        lab.append(np.zeros(nb, np.int64))
+        cv.append(rs.uniform(-0.7, 0.7, (nb, 3)) + [0.0, 0.0, 1.0])
+        kv.append(rs.uniform(-0.7, 0.7, (n_kps, nb, 3)) + [0.0, 0.0, 1.0])
+        perm = rs.permutation(n_points)
+        p = np.concatenate(pts).astype(np.float32)[perm]
+        pcld[b], mask[b] = p, np.concatenate(lab)[perm]
+        ctr_of[b, 0] = p - np.concatenate(cv)[perm]
+        kp_of[b] = p[None] - np.concatenate(kv, axis=1)[:, perm]
+    return dict(pcld=pcld, mask=mask, ctr_of=ctr_of, kp_of=kp_of, mesh=mesh, cls_radius=cls_radius)
+
+
 def item_test_frames():
     """The frames of tests/golden/item_cases.npz by name, with the item shape each is sampled at:
     ``{name: (frame, dataset, n_points, n_objects)}``.  Two full 480x640 frames at 12288 points (YCB with 8

@@ -543,6 +543,48 @@ int ffb6d_mean_shift_fit(const float *votes, const unsigned char *valid, int64_t
  */
 int ffb6d_best_fit_transform(const float *A, const float *B, int64_t G, int64_t M, double *T, ffb6d_stream_t stream);
 
+/*
+ * The poses of every object of B frames, replacing cal_frame_poses (ffb6d/utils/pvn3d_eval_utils_kpls.py:65-160;
+ * LineMOD's cal_frame_poses_lm, :220-284, is the call with n_cls = 2 on the mask `mask == 1` and refine_thr = NULL).
+ *   pcld [B,N,3] f32; mask [B,N] int64 predicted class ids; ctr_of [B,1,N,3], kp_of [B,n_kps,N,3] f32 offsets;
+ *   mesh_kps [n_cls,R,3] f32 object-frame keypoints, R = n_kps + use_ctr, the centre last; has_mesh [n_cls] u8;
+ *   refine_thr [n_cls] f32 (class c's 0.8 x radius, rounded as float32(float64(r) * 0.8)) or NULL: no refinement
+ *   -> present [B,n_cls] u8: class c >= 1 has a point in the unrefined mask (the reference's pred_cls_ids);
+ *      count [B,n_cls] i32: the class's points after refinement;
+ *      kps [B,n_cls,R,3] f32: the voted keypoints, then the centre when use_ctr;
+ *      poses [B,n_cls,3,4] f64: the Kabsch fit of mesh_kps[c] onto kps[b,c] (ffb6d_best_fit_transform's kernel).
+ * Per frame, as the reference: with refine_thr, every present class's centre votes (pcld - ctr_of) are fitted, and
+ * an object point takes the class of the nearest of those centres (lowest class id on distance ties, distance
+ * |pred_ctr - ctr| formed as a difference) when it is below refine_thr of that class.  Then every class with points
+ * fits its centre votes (centre + inlier labels; with no label set the class's first point is kept, as the
+ * reference's `ctr_labels[0] = 1`) and its n_kps keypoint vote sets, over the labelled points when ctr_filter.
+ * Every vote set is compacted in ascending point order from pcld - of in fp32, so its centre and labels are
+ * bitwise those of ffb6d_mean_shift_fit on the same set: the same arithmetic, over a device-built set table.
+ * Rows without a fit: an absent class gets zeros; a present class left without points the identity pose and zero
+ * keypoints.  A mask id outside [0, n_cls) makes that frame's poses and keypoints NaN (present and count 0), and a
+ * present class with has_mesh 0 gets a NaN pose and keypoints, without a fault; other rows are unaffected.
+ * Three stages with refinement (two without), each one cooperative launch over every set of every frame
+ * (DESIGN.md §4.25); results are deterministic and do not depend on the other frames of the batch.
+ * 0 <= B (B = 0 is a no-op), 1 <= N <= FFB6D_VOTE_MAX_POINTS, 2 <= n_cls <= FFB6D_VOTE_MAX_CLASSES,
+ * 1 <= n_kps <= FFB6D_VOTE_MAX_KPS, B * n_cls * n_kps <= FFB6D_VOTE_MAX_SETS, n_kps * B * N <=
+ * FFB6D_VOTE_MAX_SLOTS (the int32 offsets of the packed points); use_ctr, ctr_filter in {0, 1}; bandwidth > 0
+ * finite, max_iter >= 0; pointers aligned to their element, the workspace to 256 bytes.
+ * workspace: ffb6d_vote_poses_workspace_bytes(B, N, n_cls, n_kps) bytes (FFB6D_ERR_WORKSPACE if missing or
+ * smaller).  Arguments are checked before any launch (FFB6D_ERR_INVALID); no allocation, no host synchronisation
+ * (capturable in a CUDA graph).
+ */
+#define FFB6D_VOTE_MAX_POINTS ((1 << 24) - 1)
+#define FFB6D_VOTE_MAX_CLASSES 1024
+#define FFB6D_VOTE_MAX_KPS 64
+#define FFB6D_VOTE_MAX_SETS (1 << 24)
+#define FFB6D_VOTE_MAX_SLOTS 2147483647
+size_t ffb6d_vote_poses_workspace_bytes(int64_t B, int64_t N, int64_t n_cls, int64_t n_kps);
+int ffb6d_vote_poses(const float *pcld, const int64_t *mask, const float *ctr_of, const float *kp_of,
+                     const float *mesh_kps, const unsigned char *has_mesh, const float *refine_thr, int64_t B,
+                     int64_t N, int64_t n_cls, int64_t n_kps, int use_ctr, int ctr_filter, float bandwidth, int max_iter,
+                     unsigned char *present, int *count, float *kps, double *poses, void *workspace,
+                     size_t workspace_bytes, ffb6d_stream_t stream);
+
 /* ---- farthest point sampling (object keypoints) -------------------------- */
 /*
  * Farthest point sampling of G clouds, replacing the reference's farthest_point_sampling /
