@@ -38,6 +38,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
 * :func:`farthest_point_sampling` -- ``fps_utils.farthest_point_sampling`` (utils/dataset_tools/fps/fps_utils.py:8-23)
   on the GPU, batched over clouds; :mod:`ffb6d_b200.objinfo` -- the object tables of
   utils/dataset_tools/gen_obj_info.py (box corners, radius, centre, keypoints) and their text files.
+* :mod:`ffb6d_b200.vis` -- ``Basic_Utils.project_p3d`` / ``draw_p2ds`` / ``get_label_color`` (utils/basic_utils.py:
+  268-295, 362-423) batched on the GPU, demo.py's ``cal_view_pred_pose`` for a whole batch and the trainers'
+  ``view_labels``.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -62,9 +65,9 @@ _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
 _GRAPHED = ("GraphedTrainStep", "GraphedEvalStep")
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched

@@ -35,6 +35,12 @@ VOTE_MAX_CLASSES = 1024
 VOTE_MAX_KPS = 64
 VOTE_MAX_SETS = 1 << 24
 VOTE_MAX_SLOTS = (1 << 31) - 1
+VIS_MAX_RADIUS = 64                              # FFB6D_VIS_* of include/ffb6d_b200.h
+VIS_MAX_SIDE = 16384
+VIS_MAX_SETS = 1 << 24
+VIS_MAX_ROWS = 1 << 24
+VIS_MAX_TABLE_ROWS = (1 << 31) - 1
+VIS_MAX_FRAMES = 65535
 
 
 class FFB6DError(RuntimeError):
@@ -148,6 +154,9 @@ def _load():
         "ffb6d_farthest_point_sampling": (ci, [vp, vp, i64, i64, i64, vp, ci, vp, vp, sz, vp]),
         "ffb6d_pose_add_adds_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_pose_add_adds": (ci, [vp, vp, i64, i64, vp, vp, vp, i64, vp, vp, vp, sz, vp]),
+        "ffb6d_project_p3d": (ci, [vp, ci, i64, vp, vp, vp, i64, i64, vp, vp, vp, ci, vp, vp]),
+        "ffb6d_draw_p2ds_workspace_bytes": (sz, [i64, i64, i64]),
+        "ffb6d_draw_p2ds": (ci, [vp, i64, i64, i64, vp, i64, i64, vp, vp, vp, vp, i64, vp, vp, ci, vp, sz, vp]),
         "ffb6d_grid_subsample_host": (ci, [vp, sz, vp, sz, vp, sz, fp, vp, vp, vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():

@@ -1095,6 +1095,120 @@ def pose_add_adds(mesh_pts, mesh_off, obj_mesh, pred_RT, gt_RT, max_points):
     return add, adds
 
 
+def _set_table(start, count, enable, dev):
+    st = _tensor(start, "start", torch.int32, 1, dev)
+    S = st.shape[0]
+    ct = _tensor(count, "count", torch.int32, (S,), dev)
+    en = None
+    if enable is not None:
+        en = _tensor(enable.to(torch.uint8) if torch.is_tensor(enable) and enable.dtype == torch.bool else enable,
+                     "enable", torch.uint8, (S,), dev)
+    if S > _lib.VIS_MAX_SETS:
+        raise ValueError("at most %d sets per call, got %d" % (_lib.VIS_MAX_SETS, S))
+    return st, ct, en, S
+
+
+def _max_rows(max_rows):
+    if isinstance(max_rows, bool) or not isinstance(max_rows, (int, np.integer)):
+        raise TypeError("max_rows must be an int, got %r" % (max_rows,))
+    if not 1 <= max_rows <= _lib.VIS_MAX_ROWS:
+        raise ValueError("max_rows must lie in [1, %d], got %d" % (_lib.VIS_MAX_ROWS, max_rows))
+    return int(max_rows)
+
+
+def project_p3d(pts, start, count, max_rows, K, cam_scale=1.0, pose=None, enable=None):
+    """``Basic_Utils.project_p3d`` (utils/basic_utils.py:268-277) of ``S`` point sets in one launch, bitwise numpy's
+    float64 arithmetic (include/ffb6d_b200.h, DESIGN.md §4.26).
+
+    :param pts: ``[n_rows,3]`` float32 or float64 CUDA, the point table; set ``s`` is rows ``start[s] ..
+      start[s] + count[s]`` (``start``, ``count`` ``[S]`` int32), drawn where ``enable[s]`` (``[S]`` bool/uint8, or
+      None for all).  A set whose rows leave the table or exceed ``max_rows`` is empty.
+    :param K: float64 ``[3,3]`` (every set) or ``[S,3,3]``; ``cam_scale``: a float or a float64 tensor ``[1]``
+      (``[S]`` with a per-set ``K``).  Without ``pose``, float32 points are scaled in float32 (numpy's casting of a
+      Python float).
+    :param pose: float64 ``[S,3,4]`` or None: the demo's ``np.dot(mesh, R.T) + t`` in float64 first.
+    :return: int32 ``[S,max_rows,2]``, ``(INT32_MIN, INT32_MIN)`` at padding rows.  Capturable in a CUDA graph."""
+    _need_cuda(pts, "pts")
+    p, dev = pts, pts.device
+    if p.dtype not in (torch.float32, torch.float64) or p.dim() != 2 or p.shape[1] != 3:
+        raise ValueError("pts must be float32 or float64 [n,3], got %s %s" % (p.dtype, tuple(p.shape)))
+    p = p.contiguous()
+    if p.shape[0] > _lib.VIS_MAX_TABLE_ROWS:
+        raise ValueError("pts has %d rows, more than int32 starts address" % p.shape[0])
+    st, ct, en, S = _set_table(start, count, enable, dev)
+    max_rows = _max_rows(max_rows)
+    k = _tensor(K, "K", torch.float64, K.dim() if torch.is_tensor(K) else 2, dev)
+    per_set = k.dim() == 3
+    if tuple(k.shape) != ((S, 3, 3) if per_set else (3, 3)):
+        raise ValueError("K must be float64 [3,3] or [S,3,3] = [%d,3,3], got %s" % (S, tuple(k.shape)))
+    if not torch.is_tensor(cam_scale):
+        cam_scale = torch.full((S if per_set else 1,), float(cam_scale), dtype=torch.float64, device=dev)
+    cs = _tensor(cam_scale, "cam_scale", torch.float64, (S if per_set else 1,), dev)
+    ps = None if pose is None else _tensor(pose, "pose", torch.float64, (S, 3, 4), dev)
+    out = torch.empty((S, max_rows, 2), dtype=torch.int32, device=dev)
+    if S == 0:
+        return out
+    launch(lib.ffb6d_project_p3d, dev, p.data_ptr(), int(p.dtype == torch.float64), p.shape[0], st.data_ptr(),
+           ct.data_ptr(), ptr(en), S, max_rows, ptr(ps), k.data_ptr(), cs.data_ptr(), int(per_set), out.data_ptr())
+    return out
+
+
+def draw_p2ds_workspace(img):
+    """The scratch :func:`draw_p2ds` needs for ``img [B,H,W,3]``: ``B H W`` 8-byte keys (19.7 MB at 8 x 480 x 640).
+    Pass it to every call on images of that size to keep them free of allocations."""
+    B, H, W = (int(v) for v in img.shape[:3])
+    return workspace(lib.ffb6d_draw_p2ds_workspace_bytes(B, H, W), img.device)
+
+
+def draw_p2ds(img, p2ds, frame, start, count, n_rows, radius, colors, enable=None, ws=None):
+    """``Basic_Utils.draw_p2ds`` (utils/basic_utils.py:283-295) of ``S`` sets in one call, in place: ``img [B,H,W,3]``
+    uint8 CUDA gets, for every row ``r < count[s]`` of every enabled set ``s``, the filled ``cv2.circle`` of radius
+    ``radius[s]`` at ``p2ds[s, r]`` clipped to ``[0,W] x [0,H]``, in frame ``frame[s]``; where circles overlap the last
+    in (set, row) order wins.
+
+    :param p2ds: int32 ``[S,max_rows,2]`` (what :func:`project_p3d` returns); ``frame``, ``radius`` ``[S]`` int32;
+      ``start``, ``count``, ``enable`` and ``n_rows`` the set table of :func:`project_p3d` (a set that is empty there
+      draws nothing); a frame out of ``[0,B)`` or a radius out of ``[0, 64]`` draws nothing.
+    :param colors: uint8 ``[S,3]`` (one colour per set) or ``[S,max_rows,3]`` (one per row).
+    :param ws: a :func:`draw_p2ds_workspace` of ``img``, or None to allocate one.
+    :return: ``img``.  No host synchronisation: capturable in a CUDA graph."""
+    im = _tensor(img, "img", torch.uint8, 4)
+    if im.data_ptr() != img.data_ptr():
+        raise ValueError("img must be contiguous: it is drawn in place")
+    dev = im.device
+    B, H, W, c3 = im.shape
+    if c3 != 3:
+        raise ValueError("img must be [B,H,W,3], got %s" % (tuple(im.shape),))
+    if not (1 <= H <= _lib.VIS_MAX_SIDE and 1 <= W <= _lib.VIS_MAX_SIDE) or B > _lib.VIS_MAX_FRAMES:
+        raise ValueError("img of %s: at most %d frames of 1 .. %d pixels a side" % (
+            tuple(im.shape), _lib.VIS_MAX_FRAMES, _lib.VIS_MAX_SIDE))
+    st, ct, en, S = _set_table(start, count, enable, dev)
+    pt = _tensor(p2ds, "p2ds", torch.int32, 3, dev)
+    max_rows = _max_rows(pt.shape[1])
+    if tuple(pt.shape) != (S, max_rows, 2):
+        raise ValueError("p2ds must be [S,max_rows,2] with S = %d, got %s" % (S, tuple(pt.shape)))
+    fr = _tensor(frame, "frame", torch.int32, (S,), dev)
+    rd = _tensor(radius, "radius", torch.int32, (S,), dev)
+    col = _tensor(colors, "colors", torch.uint8, colors.dim() if torch.is_tensor(colors) else 2, dev)
+    per_row = col.dim() == 3
+    if tuple(col.shape) != ((S, max_rows, 3) if per_row else (S, 3)):
+        raise ValueError("colors must be uint8 [S,3] or [S,max_rows,3], got %s" % (tuple(col.shape),))
+    if not 0 <= int(n_rows) <= _lib.VIS_MAX_TABLE_ROWS:
+        raise ValueError("n_rows must lie in [0, %d], got %d" % (_lib.VIS_MAX_TABLE_ROWS, int(n_rows)))
+    nbytes = int(lib.ffb6d_draw_p2ds_workspace_bytes(B, H, W))
+    if ws is None:
+        ws = workspace(nbytes, dev)
+    elif ws.device != dev or ws.numel() * ws.element_size() < nbytes:
+        raise ValueError("ws holds %d bytes on %s, %d needed on %s" % (ws.numel() * ws.element_size(), ws.device,
+                                                                      nbytes, dev))
+    if B == 0 or S == 0:
+        return img
+    launch(lib.ffb6d_draw_p2ds, dev, im.data_ptr(), B, H, W, pt.data_ptr(), S, max_rows, fr.data_ptr(), st.data_ptr(),
+           ct.data_ptr(), ptr(en), int(n_rows), rd.data_ptr(), col.data_ptr(), int(per_row), ws.data_ptr(),
+           ws.numel() * ws.element_size())
+    return img
+
+
 def mean_shift_fit(votes, valid=None, bandwidth=0.05, max_iter=300, return_modes=False):
     """Gaussian mean shift of ``G`` independent vote sets in one persistent kernel: the batched form of
     ``MeanShiftTorch.fit`` (utils/meanshift_pytorch.py:33-57).

@@ -191,15 +191,22 @@ class MeshTable:
     ``mesh_pts``: mapping ``cls_id -> [P,3]`` vertices in metres, what the reference's ``bs_utils.get_pointxyz(_cuda)``
     returns (YCB: ``models/<cls>/points.xyz``; LineMOD: the 2 000-vertex subsample the caller drew, the reference
     redraws it in every process).  Holds ``pts [sum P,3]`` float32, ``off [max id + 2]`` int32 (mesh ``c`` is rows
-    ``off[c] .. off[c+1]``; ids without a mesh are empty, and scoring one gives NaN) and ``max_points``."""
+    ``off[c] .. off[c+1]``; ids without a mesh are empty, and scoring one gives NaN) and ``max_points``.
 
-    def __init__(self, mesh_pts, device=None):
+    ``dtype=torch.float64`` keeps the vertices in float64, for drawing (:func:`ffb6d_b200.vis.draw_poses`): the demo
+    poses the meshes in float64, and rounding them to float32 would move points that lie near a half-pixel.  Scoring
+    (:func:`add_adds`) needs the float32 table."""
+
+    def __init__(self, mesh_pts, device=None, dtype=torch.float32):
+        if dtype not in (torch.float32, torch.float64):
+            raise ValueError("MeshTable dtype must be torch.float32 or torch.float64, got %s" % dtype)
+        np_dtype = np.float32 if dtype == torch.float32 else np.float64
         if not mesh_pts:
             raise ValueError("MeshTable needs at least one mesh")
         ids = sorted(int(c) for c in mesh_pts)
         if ids[0] < 0:
             raise ValueError("class ids must be >= 0, got %d" % ids[0])
-        arrs = {int(c): np.asarray(torch.as_tensor(v).detach().cpu(), np.float32) for c, v in mesh_pts.items()}
+        arrs = {int(c): np.asarray(torch.as_tensor(v).detach().cpu(), np_dtype) for c, v in mesh_pts.items()}
         sizes = np.zeros(ids[-1] + 1, np.int64)
         for c, a in arrs.items():
             if a.ndim != 2 or a.shape[1] != 3 or a.shape[0] < 1:
@@ -221,6 +228,8 @@ def add_adds(table, cls_ids, pred_RT, gt_RT):
     """ADD and ADD-S of ``M`` objects in one launch: object ``m`` is mesh ``cls_ids[m]`` of ``table`` under the
     poses ``pred_RT[m]``, ``gt_RT[m]`` (``[M,3,4]``, numpy or torch).  Returns ``(add [M], adds [M])`` float32
     CUDA tensors; see :func:`ffb6d_b200.ops.pose_add_adds`."""
+    if table.pts.dtype != torch.float32:
+        raise ValueError("add_adds scores a float32 MeshTable, got %s" % table.pts.dtype)
     dev = table.device
     ids = torch.as_tensor(np.asarray(cls_ids, np.int64) if not torch.is_tensor(cls_ids) else cls_ids)
     ids = ids.to(dev, torch.int32).reshape(-1)

@@ -645,6 +645,54 @@ int ffb6d_pose_add_adds(const float *mesh_pts, const int32_t *mesh_off, int64_t 
                         const int32_t *obj_mesh, const float *pred_RT, const float *gt_RT, int64_t M, float *add,
                         float *adds, void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
 
+/* ---- pose and label drawing ---------------------------------------------- */
+/*
+ * Projection and drawing of S point sets, replacing Basic_Utils.project_p3d and draw_p2ds (utils/basic_utils.py:
+ * 268-295) as demo.py's cal_view_pred_pose (demo.py:116-145) and the trainers' view_labels (train_ycb.py:189-204)
+ * call them once per object or frame (DESIGN.md §4.26).
+ * The set table: set s is the rows start[s] .. start[s] + count[s] of a point table of n_rows rows (start, count
+ * [S] int32, device), drawn only where enable[s] != 0 (enable [S] u8, or NULL: every set).  Outputs are padded to
+ * [S, max_rows, ...], row r of set s at s * max_rows + r.  A disabled set, and one with a negative start or count,
+ * count > max_rows or start + count > n_rows, is empty: it projects to padding and draws nothing, without a fault.
+ *
+ * ffb6d_project_p3d: pts [n_rows,3] f32 (pts_f64 = 0) or f64 (1); pose [S,3,4] f64 or NULL; K [3,3] f64 and
+ *   cam_scale [1] f64 shared (per_set = 0) or K [S,3,3] and cam_scale [S] (per_set = 1), all device
+ *   -> p2ds [S,max_rows,2] int32, (u, v) per row, (INT32_MIN, INT32_MIN) at padding.  Bitwise numpy's float64 code:
+ *   with a pose, y_j = fma(x2, R[j][2], fma(x1, R[j][1], x0 * R[j][0])) + t_j and y * cam_scale in f64; without,
+ *   x * cam_scale in the points' dtype (f32 points times (float)cam_scale, numpy's casting of a Python float), then
+ *   promoted; p_j = fma(z, K[j][2], fma(y, K[j][1], x * K[j][0])); p_2 < 1e-8 -> 1.0 (NaN stays); u = rint(p_0 /
+ *   p_2), v = rint(p_1 / p_2) (IEEE division, half to even); the int32 cast of x86's cvttsd2si: NaN and values
+ *   outside [-2^31, 2^31) give INT32_MIN.  One launch.
+ * ffb6d_draw_p2ds: draws into img [B,H,W,3] u8 (in place) the filled circle of cv2.circle(img, (x, y), radius[s],
+ *   colour, -1) (LINE_8, shift 0: OpenCV's integer midpoint circle, clipped to the image) at every row of every set,
+ *   x = clip(u, 0, W), y = clip(v, 0, H) (inclusive bounds, as the reference), in frame frame[s] (frame, radius [S]
+ *   int32, device).  colors [S,3] u8 (color_per_row = 0) or [S,max_rows,3] (1).  Where circles overlap within a
+ *   frame the last in (set, row) order wins; no other pixel is written.  A set whose frame lies outside [0, B) or
+ *   whose radius lies outside [0, FFB6D_VIS_MAX_RADIUS] draws nothing.  n_rows and start only decide, as above,
+ *   whether a set is empty.  A memset of the workspace and two launches (mark the winning key per pixel with
+ *   atomicMax, then paint); the result does not depend on scheduling.
+ *   workspace: ffb6d_draw_p2ds_workspace_bytes(B, H, W) = B H W 8 bytes, 8-byte aligned (FFB6D_ERR_WORKSPACE if
+ *   missing or smaller); the query returns 0 for sizes out of range.
+ * 0 <= S <= FFB6D_VIS_MAX_SETS (S = 0 is a no-op), 1 <= max_rows <= FFB6D_VIS_MAX_ROWS, 0 <= n_rows <=
+ * FFB6D_VIS_MAX_TABLE_ROWS, 0 <= B <= FFB6D_VIS_MAX_FRAMES (B = 0 is a no-op), 1 <= H, W <= FFB6D_VIS_MAX_SIDE;
+ * flags 0 or 1; pointers aligned to their element, p2ds to 8 bytes.  Arguments are checked before any launch
+ * (FFB6D_ERR_INVALID); no allocation, no host synchronisation (capturable in a CUDA graph).
+ */
+#define FFB6D_VIS_MAX_RADIUS 64
+#define FFB6D_VIS_MAX_SIDE 16384
+#define FFB6D_VIS_MAX_SETS (1 << 24)
+#define FFB6D_VIS_MAX_ROWS (1 << 24)
+#define FFB6D_VIS_MAX_TABLE_ROWS 2147483647
+#define FFB6D_VIS_MAX_FRAMES 65535
+int ffb6d_project_p3d(const void *pts, int pts_f64, int64_t n_rows, const int32_t *start, const int32_t *count,
+                      const unsigned char *enable, int64_t S, int64_t max_rows, const double *pose, const double *K,
+                      const double *cam_scale, int per_set, int32_t *p2ds, ffb6d_stream_t stream);
+size_t ffb6d_draw_p2ds_workspace_bytes(int64_t B, int64_t H, int64_t W);
+int ffb6d_draw_p2ds(unsigned char *img, int64_t B, int64_t H, int64_t W, const int32_t *p2ds, int64_t S,
+                    int64_t max_rows, const int32_t *frame, const int32_t *start, const int32_t *count,
+                    const unsigned char *enable, int64_t n_rows, const int32_t *radius, const unsigned char *colors,
+                    int color_per_row, void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+
 /* ---- grid subsampling --------------------------------------------------- */
 /*
  * Voxel-grid barycentre subsampling, replaces grid_subsampling()
