@@ -41,6 +41,10 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
 * :mod:`ffb6d_b200.vis` -- ``Basic_Utils.project_p3d`` / ``draw_p2ds`` / ``get_label_color`` (utils/basic_utils.py:
   268-295, 362-423) batched on the GPU, demo.py's ``cal_view_pred_pose`` for a whole batch and the trainers'
   ``view_labels``.
+* :func:`estimate_poses` (:mod:`ffb6d_b200.estimate`) -- decoded RGB-D frames in, object poses out: the inference
+  ``get_item`` (:func:`build_ffb6d_inputs`, no labels), the ``FFB6D`` eval forward and the voting, as the
+  reference's ``demo.py`` composes them; :class:`GraphedPoseStep` -- all of it captured in one CUDA graph and
+  replayed per batch.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -58,16 +62,17 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "fill_missing", "segment_plan", "segment_sum", "point_item", "rgb_add_noise", "add_real_back",
         "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax",
         "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d",
-        "farthest_point_sampling", "pose_add_adds", "vote_poses")
+        "farthest_point_sampling", "pose_add_adds", "vote_poses", "point_input")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
-             "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item")
+             "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item", "build_ffb6d_inputs")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
 _GRAPHED = ("GraphedTrainStep", "GraphedEvalStep")
+_ESTIMATE = ("estimate_poses", "GraphedPoseStep")
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "estimate", "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED + _ESTIMATE) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "estimate", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched
@@ -81,6 +86,8 @@ def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op t
         return getattr(importlib.import_module(".item", __name__), name)
     if name in _GRAPHED:
         return getattr(importlib.import_module(".graphed", __name__), name)
+    if name in _ESTIMATE:
+        return getattr(importlib.import_module(".estimate", __name__), name)
     if name == "DataProcessing":
         return importlib.import_module(".helper_tool", __name__).DataProcessing
     if name in _SUBMODULES:

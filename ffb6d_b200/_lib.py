@@ -120,6 +120,7 @@ def _load():
         "ffb6d_backproject": (ci, [vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp, vp, vp]),
         "ffb6d_point_item": (ci, [vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp, vp,
                                   vp]),
+        "ffb6d_point_input": (ci, [vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp, vp]),
         "ffb6d_sample_pixels_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_sample_pixels": (ci, [vp, i64, i64, i64, fp, i64, C.c_uint64, vp, vp, vp, sz, vp]),
         "ffb6d_fill_depth_workspace_bytes": (sz, [i64, i64, i64]),

@@ -1,5 +1,9 @@
 // point_item.cu -- the sampled points' network input and pose-training targets (sm_90a).
 //
+// Two entry points share one per-point feature routine (point_features): ffb6d_point_input writes the network
+// input cld_rgb_nrm alone (inference: no labels, no objects); ffb6d_point_item writes it together with the
+// point labels and the offset targets below.
+//
 // The half of the datasets' get_item that reads `choose` (datasets/ycb/ycb_dataset.py:237-247, 348-386 ==
 // datasets/linemod/linemod_dataset.py:284-293, 398-436): for point p of frame b at pixel px = choose[b,p]
 //   cld_rgb_nrm[b,:,p] = (xyz, rgb[px], nrm[px])         xyz = dpt_2_pcld's float64 point, rounded once
@@ -20,6 +24,41 @@
 namespace ffb6d {
 
 constexpr int ITEM_TILE = 64;
+constexpr int INPUT_TILE = 256;
+
+// cld_rgb_nrm[b,:,p] = (xyz, rgb[px], nrm[px]) of point p of frame b; returns the frame's flat pixel index of the
+// point in `pix` and the unrounded float64 point in `xyz` (what the offset targets are formed from)
+__device__ __forceinline__ void point_features(const float *__restrict__ depth, int H, int W,
+                                               const double *__restrict__ intr, int intr_per_frame,
+                                               const int *__restrict__ choose, int N, const uint8_t *__restrict__ rgb,
+                                               const float *__restrict__ nrm, float *__restrict__ cld_rgb_nrm, int b,
+                                               int p, size_t &pix, double xyz[3])
+{
+    const size_t HW = (size_t)H * W;
+    const int px = __ldg(choose + (size_t)b * N + p);
+    const double *k = intr + (intr_per_frame ? (size_t)b * 4 : 0);
+    backproject_px64(depth + b * HW, W, px / W, px % W, k[0], k[1], k[2], k[3], xyz);
+    pix = b * HW + px;
+    float *o = cld_rgb_nrm + (size_t)b * 9 * N + p;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        o[(size_t)c * N] = __double2float_rn(xyz[c]);
+        o[(size_t)(3 + c) * N] = (float)__ldg(rgb + pix * 3 + c);
+        o[(size_t)(6 + c) * N] = __ldg(nrm + pix * 3 + c);
+    }
+}
+
+__global__ void __launch_bounds__(INPUT_TILE)
+point_input_kernel(const float *__restrict__ depth, int H, int W, const double *__restrict__ intr, int intr_per_frame,
+                   const int *__restrict__ choose, int N, const uint8_t *__restrict__ rgb,
+                   const float *__restrict__ nrm, float *__restrict__ cld_rgb_nrm)
+{
+    const int b = blockIdx.y, p = blockIdx.x * INPUT_TILE + threadIdx.x;
+    if (p >= N) return;
+    size_t pix;
+    double xyz[3];
+    point_features(depth, H, W, intr, intr_per_frame, choose, N, rgb, nrm, cld_rgb_nrm, b, p, pix, xyz);
+}
 
 // shared floats of a tile's staged offsets: keypoint rows padded to an odd length (no bank conflicts), then centres
 static inline int item_row_len(int n_kps) { return (3 * n_kps) | 1; }
@@ -50,19 +89,9 @@ point_item_kernel(const float *__restrict__ depth, int H, int W, const double *_
     __syncthreads();
 
     if (p < N) {
-        const size_t HW = (size_t)H * W;
-        const int px = __ldg(choose + (size_t)b * N + p);
-        const double *k = intr + (intr_per_frame ? (size_t)b * 4 : 0);
+        size_t pix;
         double xyz[3];
-        backproject_px64(depth + b * HW, W, px / W, px % W, k[0], k[1], k[2], k[3], xyz);
-        const size_t pix = b * HW + px;
-        float *o = cld_rgb_nrm + (size_t)b * 9 * N + p;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            o[(size_t)c * N] = __double2float_rn(xyz[c]);
-            o[(size_t)(3 + c) * N] = (float)__ldg(rgb + pix * 3 + c);
-            o[(size_t)(6 + c) * N] = __ldg(nrm + pix * 3 + c);
-        }
+        point_features(depth, H, W, intr, intr_per_frame, choose, N, rgb, nrm, cld_rgb_nrm, b, p, pix, xyz);
         const int lab = __ldg(labels + pix);
         labels_pt[(size_t)b * N + p] = lab;
         const int s = slot_of[lab];
@@ -124,5 +153,26 @@ extern "C" int ffb6d_point_item(const float *depth_m, int64_t B, int64_t H, int6
         depth_m, (int)H, (int)W, intrinsics, intrinsics_per_frame, choose, (int)N, rgb, labels, nrm, obj_cls, obj_kps,
         obj_ctr, (int)n_obj, (int)n_kps, cld_rgb_nrm, labels_pt, kp_targ_ofst, ctr_targ_ofst);
     FFB6D_LAUNCH_OK("point_item_kernel");
+    return FFB6D_OK;
+}
+
+extern "C" int ffb6d_point_input(const float *depth_m, int64_t B, int64_t H, int64_t W, const double *intrinsics,
+                                 int intrinsics_per_frame, const int *choose, int64_t N, const uint8_t *rgb,
+                                 const float *nrm, float *cld_rgb_nrm, ffb6d_stream_t stream)
+{
+    FFB6D_CHECK_ARG(B >= 0 && B < 65536 && H >= 1 && W >= 1 && H * W < (1ll << 31) && N >= 0 && N < (1ll << 31),
+                    "point_input: bad size (B=%lld H=%lld W=%lld N=%lld)", (long long)B, (long long)H, (long long)W,
+                    (long long)N);
+    FFB6D_CHECK_ARG(intrinsics_per_frame == 0 || intrinsics_per_frame == 1,
+                    "point_input: intrinsics_per_frame must be 0 or 1");
+    if (B == 0 || N == 0) return FFB6D_OK;
+    FFB6D_CHECK_ARG(depth_m && intrinsics && choose && rgb && nrm && cld_rgb_nrm, "point_input: null pointer");
+    FFB6D_CHECK_ARG(aligned(intrinsics, 8) && aligned(depth_m, 4) && aligned(choose, 4) && aligned(nrm, 4) &&
+                    aligned(cld_rgb_nrm, 4), "point_input: misaligned pointer");
+    dim3 grid((unsigned)ceil_div(N, INPUT_TILE), (unsigned)B);
+    point_input_kernel<<<grid, INPUT_TILE, 0, (cudaStream_t)stream>>>(depth_m, (int)H, (int)W, intrinsics,
+                                                                      intrinsics_per_frame, choose, (int)N, rgb, nrm,
+                                                                      cld_rgb_nrm);
+    FFB6D_LAUNCH_OK("point_input_kernel");
     return FFB6D_OK;
 }

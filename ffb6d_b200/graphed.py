@@ -94,10 +94,7 @@ class _GraphedStep:
 
     def __init__(self, model, example_item, warmup):
         name = type(self).__name__
-        if isinstance(model, (nn.parallel.DistributedDataParallel, nn.DataParallel)):
-            raise ValueError("%s: a (Distributed)DataParallel model cannot be captured; %s" % (name, self._wrapper_hint))
-        if not isinstance(model, FFB6DFusionNet):
-            raise ValueError("%s: model must be an FFB6DFusionNet or FFB6D, got %s" % (name, type(model).__name__))
+        self._check_model(model)
         if not isinstance(example_item, dict):
             raise ValueError("%s: example_item must be a dict, got %s" % (name, type(example_item).__name__))
         if not isinstance(model, FFB6D) and not isinstance(example_item.get("rgb_feats"), (list, tuple)):
@@ -113,6 +110,13 @@ class _GraphedStep:
         self._key = None
         self.captures = 0
         self._capture(int(warmup))
+
+    def _check_model(self, model):
+        name = type(self).__name__
+        if isinstance(model, (nn.parallel.DistributedDataParallel, nn.DataParallel)):
+            raise ValueError("%s: a (Distributed)DataParallel model cannot be captured; %s" % (name, self._wrapper_hint))
+        if not isinstance(model, FFB6DFusionNet):
+            raise ValueError("%s: model must be an FFB6DFusionNet or FFB6D, got %s" % (name, type(model).__name__))
 
     def _read_modules(self):
         """The module tree as a list, walked by every call's key (which also holds each module's children, so a

@@ -763,22 +763,9 @@ def point_item(depth_m, K, choose, rgb, labels, nrm_map, obj_cls, obj_kps, obj_c
     """
     tensors = ((depth_m, "depth_m"), (choose, "choose"), (rgb, "rgb"), (labels, "labels"), (nrm_map, "nrm_map"),
                (obj_cls, "obj_cls"), (obj_kps, "obj_kps"), (obj_ctr, "obj_ctr"))
-    for t, name in tensors:
-        if not isinstance(t, torch.Tensor):
-            raise TypeError("%s must be a torch.Tensor, got %r" % (name, type(t)))
-    if depth_m.dim() != 3 or depth_m.dtype != torch.float32:
-        raise ValueError("depth_m must be float32 [B,H,W], got %s %s" % (depth_m.dtype, tuple(depth_m.shape)))
-    B, H, W = depth_m.shape
-    if choose.dtype not in _IDX:
-        raise ValueError("choose must be int32 or int64, got %s" % choose.dtype)
-    if not (choose.dim() == 2 or (choose.dim() == 3 and choose.shape[1] == 1)) or choose.shape[0] != B:
-        raise ValueError("choose must be [B,1,N] or [B,N], got %s" % (tuple(choose.shape),))
-    if rgb.dtype != torch.uint8 or tuple(rgb.shape) != (B, H, W, 3):
-        raise ValueError("rgb must be uint8 [B,H,W,3] = %s, got %s %s" % ((B, H, W, 3), rgb.dtype, tuple(rgb.shape)))
+    B, H, W = _point_input_checks(tensors, depth_m, choose, rgb, nrm_map)
     if labels.dtype != torch.uint8 or tuple(labels.shape) != (B, H, W):
         raise ValueError("labels must be uint8 [B,H,W], got %s %s" % (labels.dtype, tuple(labels.shape)))
-    if nrm_map.dtype not in (torch.float32, torch.float64) or tuple(nrm_map.shape) != (B, H, W, 3):
-        raise ValueError("nrm_map must be float32 or float64 [B,H,W,3], got %s %s" % (nrm_map.dtype, tuple(nrm_map.shape)))
     if obj_cls.dtype != torch.int32 or obj_cls.dim() != 2 or obj_cls.shape[0] != B:
         raise ValueError("obj_cls must be int32 [B,n_obj], got %s %s" % (obj_cls.dtype, tuple(obj_cls.shape)))
     n_obj = obj_cls.shape[1]
@@ -788,10 +775,7 @@ def point_item(depth_m, K, choose, rgb, labels, nrm_map, obj_cls, obj_kps, obj_c
     n_kps = obj_kps.shape[2]
     if obj_ctr.dtype != torch.float64 or tuple(obj_ctr.shape) != (B, n_obj, 3):
         raise ValueError("obj_ctr must be float64 [B,n_obj,3], got %s %s" % (obj_ctr.dtype, tuple(obj_ctr.shape)))
-    for t, name in tensors:
-        _need_cuda(t, name)
-        if t.device != depth_m.device:
-            raise ValueError("%s is on %s, depth_m on %s" % (name, t.device, depth_m.device))
+    _same_cuda_device(tensors, depth_m)
     dev = depth_m.device
     intr_d, per_frame = _intrinsics_arg(K, B, dev)
     ch = choose.reshape(B, -1).to(torch.int32).contiguous()
@@ -807,6 +791,53 @@ def point_item(depth_m, K, choose, rgb, labels, nrm_map, obj_cls, obj_kps, obj_c
            rgb_c.data_ptr(), labels_c.data_ptr(), nrm.data_ptr(), cls_c.data_ptr(), kps_c.data_ptr(), ctr_c.data_ptr(),
            n_obj, n_kps, cld_rgb_nrm.data_ptr(), labels_pt.data_ptr(), kp_targ_ofst.data_ptr(), ctr_targ_ofst.data_ptr())
     return cld_rgb_nrm, labels_pt, kp_targ_ofst, ctr_targ_ofst
+
+
+def _point_input_checks(tensors, depth_m, choose, rgb, nrm_map):
+    """The argument checks :func:`point_item` and :func:`point_input` share (types of all ``tensors``, then the
+    depth map, ``choose``, ``rgb`` and ``nrm_map``); returns ``(B, H, W)``."""
+    for t, name in tensors:
+        if not isinstance(t, torch.Tensor):
+            raise TypeError("%s must be a torch.Tensor, got %r" % (name, type(t)))
+    if depth_m.dim() != 3 or depth_m.dtype != torch.float32:
+        raise ValueError("depth_m must be float32 [B,H,W], got %s %s" % (depth_m.dtype, tuple(depth_m.shape)))
+    B, H, W = depth_m.shape
+    if choose.dtype not in _IDX:
+        raise ValueError("choose must be int32 or int64, got %s" % choose.dtype)
+    if not (choose.dim() == 2 or (choose.dim() == 3 and choose.shape[1] == 1)) or choose.shape[0] != B:
+        raise ValueError("choose must be [B,1,N] or [B,N], got %s" % (tuple(choose.shape),))
+    if rgb.dtype != torch.uint8 or tuple(rgb.shape) != (B, H, W, 3):
+        raise ValueError("rgb must be uint8 [B,H,W,3] = %s, got %s %s" % ((B, H, W, 3), rgb.dtype, tuple(rgb.shape)))
+    if nrm_map.dtype not in (torch.float32, torch.float64) or tuple(nrm_map.shape) != (B, H, W, 3):
+        raise ValueError("nrm_map must be float32 or float64 [B,H,W,3], got %s %s" % (nrm_map.dtype, tuple(nrm_map.shape)))
+    return B, H, W
+
+
+def _same_cuda_device(tensors, depth_m):
+    for t, name in tensors:
+        _need_cuda(t, name)
+        if t.device != depth_m.device:
+            raise ValueError("%s is on %s, depth_m on %s" % (name, t.device, depth_m.device))
+
+
+def point_input(depth_m, K, choose, rgb, nrm_map):
+    """The sampled points' network input on the GPU (``ffb6d_point_input``): ``cld_rgb_nrm [B,9,N]`` float32, the
+    point of each ``choose`` pixel, its colour and its normal, bitwise ``point_item(...)[0]`` for the same
+    arguments.  It needs no labels and no objects, so it serves frames whose pose is to be estimated.  Arguments
+    and checks as :func:`point_item`."""
+    tensors = ((depth_m, "depth_m"), (choose, "choose"), (rgb, "rgb"), (nrm_map, "nrm_map"))
+    B, H, W = _point_input_checks(tensors, depth_m, choose, rgb, nrm_map)
+    _same_cuda_device(tensors, depth_m)
+    dev = depth_m.device
+    intr_d, per_frame = _intrinsics_arg(K, B, dev)
+    ch = choose.reshape(B, -1).to(torch.int32).contiguous()
+    N = ch.shape[1]
+    nrm = nrm_map.to(torch.float32).contiguous()
+    cld_rgb_nrm = torch.empty((B, 9, N), dtype=torch.float32, device=dev)
+    depth_c, rgb_c = depth_m.contiguous(), rgb.contiguous()
+    launch(lib.ffb6d_point_input, dev, depth_c.data_ptr(), B, H, W, intr_d.data_ptr(), per_frame, ch.data_ptr(), N,
+           rgb_c.data_ptr(), nrm.data_ptr(), cld_rgb_nrm.data_ptr())
+    return cld_rgb_nrm
 
 
 def sample_valid_pixels(depth, n_points, seed=0, min_depth=1e-8, return_count=False):

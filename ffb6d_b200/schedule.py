@@ -271,6 +271,60 @@ MIN_VALID_PIXELS = 400
 _OBJECT_KEYS = ("RTs", "kp_3ds", "ctr_3ds", "cls_ids", "obj_cls", "obj_kps", "obj_ctr")
 
 
+def build_ffb6d_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed=0, fill=True, min_valid=MIN_VALID_PIXELS,
+                       k=K_NEIGH, index_dtype=torch.int32, streams=None):
+    """The inference half of the datasets' ``get_item`` for a batch on the GPU: every key ``FFB6D.forward`` reads,
+    from decoded frames that have no labels and no objects (what a deployed model sees).
+
+    The depth handling and the sampling are :func:`build_ffb6d_item`'s (``fill=True`` YCB, ``fill=False``
+    LineMOD), and :func:`ffb6d_b200.ops.point_input` builds ``cld_rgb_nrm``.  Every key returned here is bitwise
+    what :func:`build_ffb6d_item` returns under it for the same arguments.  No host synchronisation; with ``K``
+    given as device intrinsics (float64 ``[4]`` / ``[B,4]`` ``(fx, fy, cx, cy)`` CUDA) nothing is copied from the
+    host either, and the whole call can be captured in a CUDA graph.
+
+    :param dpt: ``[B,H,W]`` ``torch.uint16`` CUDA, the depth PNGs' raw values; :param cam_scale: raw units per metre
+    :param K: camera matrix as :func:`ffb6d_b200.ops.backproject` takes it
+    :param rgb: ``[B,H,W,3]`` uint8; :param nrm_map: ``[B,H,W,3]`` float32 / float64 normal map
+    :return: dict with ``rgb [B,3,H,W]`` uint8, ``cld_rgb_nrm [B,9,N]``, ``choose [B,1,N]``, ``dpt_map_m [B,H,W]``,
+      the tensors of :func:`build_ffb6d_indices` (``cld_xyz*`` and the index tensors) and ``valid [B]`` bool
+    """
+    return _build_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_valid, k, index_dtype, streams)[0]
+
+
+def _build_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_valid, k, index_dtype, streams,
+                  labels=None, obj=None):
+    """:func:`build_ffb6d_inputs`; with ``labels`` and ``obj`` (the device object tables) ``cld_rgb_nrm`` comes
+    from :func:`ffb6d_b200.ops.point_item` instead, and its targets are returned as well: ``(inputs,
+    (labels_pt, kp_targ_ofst, ctr_targ_ofst) or None)``."""
+    import numpy as np
+    from .ops import _fill_depth, _intrinsics_arg, sample_valid_pixels, point_input, point_item
+    if not isinstance(dpt, torch.Tensor) or dpt.dim() != 3 or dpt.dtype != torch.uint16:
+        raise ValueError("dpt must be a [B,H,W] torch.uint16 CUDA tensor")
+    dev = dpt.device
+    if fill:
+        filled, depth_m = _fill_depth(dpt, cam_scale)
+        choose, n_valid = sample_valid_pixels(filled, n_points, seed=seed, min_depth=MSK_DP_THRESHOLD,
+                                              return_count=True)
+    else:
+        # dpt_m = dpt_mm.astype(np.float32) / cam_scale; msk_dp = dpt_mm > 1e-6 is dpt_m > 0
+        cs = float(np.float32(cam_scale))
+        if not (cs > 0.0 and np.isfinite(cs)):
+            raise ValueError("cam_scale must be positive and finite, got %r" % (cam_scale,))
+        depth_m = dpt.to(torch.float32) / torch.full((), cs, dtype=torch.float32, device=dev)
+        choose, n_valid = sample_valid_pixels(depth_m, n_points, seed=seed, min_depth=0.0, return_count=True)
+    intr = _intrinsics_arg(K, dpt.shape[0], dev)[0]           # one copy of a host K, shared by both uses
+    item = build_ffb6d_indices_from_depth(depth_m, intr, choose, k=k, index_dtype=index_dtype, streams=streams)
+    targets = None
+    if labels is None:
+        cld_rgb_nrm = point_input(depth_m, intr, choose, rgb, nrm_map)
+    else:
+        cld_rgb_nrm, *targets = point_item(depth_m, intr, choose, rgb, labels, nrm_map, obj["obj_cls"],
+                                           obj["obj_kps"], obj["obj_ctr"])
+    item.update(rgb=rgb.permute(0, 3, 1, 2).contiguous(), cld_rgb_nrm=cld_rgb_nrm, choose=choose, dpt_map_m=depth_m,
+                valid=n_valid >= int(min_valid))
+    return item, targets
+
+
 def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points, seed=0, fill=True,
                      min_valid=MIN_VALID_PIXELS, k=K_NEIGH, index_dtype=torch.int32, streams=None):
     """The datasets' ``get_item`` for a batch on the GPU, from the decoded images to every ``item_dict`` key.
@@ -280,7 +334,8 @@ def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points,
     LineMOD (datasets/linemod/linemod_dataset.py:251-386): the raw ``dpt_mm`` as it is, with ``cam_scale`` 1000.
     Then :func:`ffb6d_b200.ops.point_item` builds ``cld_rgb_nrm``, ``labels`` and the offset targets of the
     sampled points.  The points are drawn by :func:`ffb6d_b200.ops.sample_valid_pixels` with ``seed``: the
-    reference's distribution, not numpy's random stream.
+    reference's distribution, not numpy's random stream.  This is :func:`build_ffb6d_inputs` plus the label and
+    target keys.
 
     :param dpt: ``[B,H,W]`` ``torch.uint16`` CUDA, the depth PNGs' raw values
     :param cam_scale: raw units per metre (YCB ``meta['factor_depth']``, LineMOD 1000), used as float32
@@ -297,29 +352,14 @@ def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points,
       and ``valid [B]`` bool
     """
     import numpy as np
-    from .ops import _fill_depth, sample_valid_pixels, point_item
     if not isinstance(dpt, torch.Tensor) or dpt.dim() != 3 or dpt.dtype != torch.uint16:
         raise ValueError("dpt must be a [B,H,W] torch.uint16 CUDA tensor")
     dev = dpt.device
-    if fill:
-        filled, depth_m = _fill_depth(dpt, cam_scale)
-        choose, n_valid = sample_valid_pixels(filled, n_points, seed=seed, min_depth=MSK_DP_THRESHOLD,
-                                              return_count=True)
-    else:
-        # dpt_m = dpt_mm.astype(np.float32) / cam_scale; msk_dp = dpt_mm > 1e-6 is dpt_m > 0
-        cs = float(np.float32(cam_scale))
-        if not (cs > 0.0 and np.isfinite(cs)):
-            raise ValueError("cam_scale must be positive and finite, got %r" % (cam_scale,))
-        depth_m = dpt.to(torch.float32) / torch.tensor(cs, dtype=torch.float32, device=dev)
-        choose, n_valid = sample_valid_pixels(depth_m, n_points, seed=seed, min_depth=0.0, return_count=True)
     if isinstance(objects, (list, tuple)):
         objects = {key: np.stack([np.asarray(o[key]) for o in objects]) for key in _OBJECT_KEYS}
     obj = {key: torch.as_tensor(objects[key]).to(dev) for key in _OBJECT_KEYS}
-    item = build_ffb6d_indices_from_depth(depth_m, K, choose, k=k, index_dtype=index_dtype, streams=streams)
-    cld_rgb_nrm, labels_pt, kp_targ_ofst, ctr_targ_ofst = point_item(
-        depth_m, K, choose, rgb, labels, nrm_map, obj["obj_cls"], obj["obj_kps"], obj["obj_ctr"])
-    item.update(rgb=rgb.permute(0, 3, 1, 2).contiguous(), cld_rgb_nrm=cld_rgb_nrm, choose=choose, labels=labels_pt,
-                rgb_labels=labels.to(torch.int32), dpt_map_m=depth_m, RTs=obj["RTs"], kp_targ_ofst=kp_targ_ofst,
-                ctr_targ_ofst=ctr_targ_ofst, cls_ids=obj["cls_ids"], ctr_3ds=obj["ctr_3ds"], kp_3ds=obj["kp_3ds"],
-                valid=n_valid >= int(min_valid))
+    item, (labels_pt, kp_targ_ofst, ctr_targ_ofst) = _build_inputs(
+        dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_valid, k, index_dtype, streams, labels, obj)
+    item.update(labels=labels_pt, rgb_labels=labels.to(torch.int32), RTs=obj["RTs"], kp_targ_ofst=kp_targ_ofst,
+                ctr_targ_ofst=ctr_targ_ofst, cls_ids=obj["cls_ids"], ctr_3ds=obj["ctr_3ds"], kp_3ds=obj["kp_3ds"])
     return item

@@ -8,7 +8,8 @@ Mirrors of the reference's helpers that have callers there, same names and argum
 * :func:`draw_p2ds` -- ``Basic_Utils.draw_p2ds`` (utils/basic_utils.py:283-295): ``cv2.circle(img, p, r, c, -1)``
   at every point, pixel for pixel;
 * :func:`cal_view_pred_pose` -- demo.py's ``cal_view_pred_pose`` (demo.py:85-151) for a whole batch, returning the
-  BGR images the demo writes; :func:`draw_poses` is its drawing step, sync-free and capturable in a CUDA graph;
+  BGR images the demo writes (the network and the vote are :func:`ffb6d_b200.estimate.forward_and_vote`, the steps
+  :func:`ffb6d_b200.estimate.estimate_poses` runs); :func:`draw_poses` is its drawing step, sync-free and capturable in a CUDA graph;
 * :func:`view_labels` -- the trainers' ``view_labels`` (train_ycb.py:189-204, train_lm.py:198-213), batched.
 
 Everything drawn runs in :func:`ffb6d_b200.ops.project_p3d` and :func:`ffb6d_b200.ops.draw_p2ds`: one launch
@@ -182,22 +183,17 @@ def cal_view_pred_pose(model, item, *, dataset, mesh_pts, mesh_kps, cls_radius=N
         raise ValueError("dataset must be 'ycb' or 'linemod', got %r" % (dataset,))
     if dataset == "linemod" and obj_id < 0:
         raise ValueError("LineMOD needs the object's obj_id")
+    from .estimate import forward_and_vote
     model.eval()
+    end_points, vt, (present, _, _, poses) = forward_and_vote(model, item, dataset, mesh_kps, cls_radius)
     with torch.no_grad():
-        end_points = model(item)
         segs = end_points["pred_rgbd_segs"]
         dev = segs.device
-        classes = torch.max(segs, 1)[1]
-        pcld = item["cld_rgb_nrm"][:, :3, :].permute(0, 2, 1).contiguous()
         table = mesh_pts if isinstance(mesh_pts, _pose.MeshTable) else _pose.MeshTable(mesh_pts, dev, torch.float64)
         images = _rgb_hwc(item["rgb"])
         ids = item["cls_ids"]
         if dataset == "ycb":
             n_cls = segs.shape[1]
-            vt = mesh_kps if isinstance(mesh_kps, _pose.VoteTable) else _pose.VoteTable(mesh_kps, n_cls, cls_radius,
-                                                                                         dev)
-            present, _, _, poses = _pose.cal_batch_poses(pcld, classes, end_points["pred_ctr_ofs"],
-                                                         end_points["pred_kp_ofs"], True, n_cls, True, mesh_kps=vt)
             bad = torch.stack((torch.isnan(poses[:, 0]).any(), (present & ~vt.has_mesh.bool()[None]).any()))
             bad_id, no_kps = bad.cpu().tolist()
             if bad_id:
@@ -207,11 +203,8 @@ def cal_view_pred_pose(model, item, *, dataset, mesh_pts, mesh_kps, cls_radius=N
             colors = [get_label_color(c, n_obj=22, mode=2) for c in range(n_cls)]
             images = images.flip(-1).contiguous()
             return draw_poses(images, table, ids, present, poses, K, colors)
-        lm = _pose._lm_table(mesh_kps, dev)
-        present, _, _, poses = _pose._vote(lm, pcld, classes == 1, end_points["pred_ctr_ofs"],
-                                           end_points["pred_kp_ofs"], True, False, False)
         eye = torch.eye(3, 4, dtype=torch.float64, device=dev)
-        B = pcld.shape[0]
+        B = segs.shape[0]
         pose1 = torch.where(present[:, 1, None, None], poses[:, 1], eye)
         lm_poses = torch.stack((eye.expand(B, 3, 4), pose1), 1).contiguous()
         lm_present = torch.zeros((B, 2), dtype=torch.bool, device=dev)

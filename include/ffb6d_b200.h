@@ -481,6 +481,18 @@ int ffb6d_point_item(const float *depth_m, int64_t B, int64_t H, int64_t W,
                      ffb6d_stream_t stream);
 
 /*
+ * The network-input half of ffb6d_point_item, for frames without labels or objects (inference):
+ *   cld_rgb_nrm [B,9,N] f32, bitwise what ffb6d_point_item writes for the same depth_m, intrinsics, choose, rgb
+ *   and nrm.  Arguments as there; the same size limits.  Sizes, null pointers and alignment are checked before any
+ *   launch (FFB6D_ERR_INVALID).  No allocation, no host synchronisation (capturable in a CUDA graph); deterministic.
+ */
+int ffb6d_point_input(const float *depth_m, int64_t B, int64_t H, int64_t W,
+                      const double *intrinsics, int intrinsics_per_frame,
+                      const int *choose, int64_t N,
+                      const uint8_t *rgb, const float *nrm,
+                      float *cld_rgb_nrm, ffb6d_stream_t stream);
+
+/*
  * Valid-pixel compaction + seeded point sampling on the device: replaces the reference's CPU recipe
  * (datasets/ycb/ycb_dataset.py:218-235: `nonzero()` of the depth mask, a random subset of N valid pixels --
  * or all of them repeated cyclically ('wrap') when fewer exist --, then a random permutation).
