@@ -34,7 +34,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   ``ffb6d_b200.model.FFB6D`` is the whole network.
 * :class:`GraphedTrainStep` (:mod:`ffb6d_b200.graphed`) -- a whole training step of ``FFB6DFusionNet`` / ``FFB6D``
   (forward, ``ffb6d_loss``, backward, optimizer update) captured in one CUDA graph and replayed per batch;
-  :class:`GraphedEvalStep` -- the eval forward and its ``ffb6d_loss`` the same way, for validation and testing.
+  :class:`GraphedEvalStep` -- the eval forward and its ``ffb6d_loss`` the same way, for validation and testing;
+  :class:`GraphedFrameTrainStep` -- :func:`build_ffb6d_train_item` (the training ``get_item`` with its augmentation,
+  from decoded frames) and the training step in one graph.
 * :func:`farthest_point_sampling` -- ``fps_utils.farthest_point_sampling`` (utils/dataset_tools/fps/fps_utils.py:8-23)
   on the GPU, batched over clouds; :mod:`ffb6d_b200.objinfo` -- the object tables of
   utils/dataset_tools/gen_obj_info.py (box corners, radius, centre, keypoints) and their text files.
@@ -62,12 +64,13 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "fill_missing", "segment_plan", "segment_sum", "point_item", "rgb_add_noise", "add_real_back",
         "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax",
         "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d",
-        "farthest_point_sampling", "pose_add_adds", "vote_poses", "point_input")
+        "farthest_point_sampling", "pose_add_adds", "vote_poses", "point_input", "rgb_noise_check_records",
+        "color_jitter_check_plans")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
-             "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item", "build_ffb6d_inputs")
+             "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item", "build_ffb6d_inputs", "build_ffb6d_train_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
-_GRAPHED = ("GraphedTrainStep", "GraphedEvalStep")
+_GRAPHED = ("GraphedTrainStep", "GraphedEvalStep", "GraphedFrameTrainStep")
 _ESTIMATE = ("estimate_poses", "GraphedPoseStep")
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
                "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "estimate", "_lib")

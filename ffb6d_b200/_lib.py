@@ -123,6 +123,7 @@ def _load():
         "ffb6d_point_input": (ci, [vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp, vp]),
         "ffb6d_sample_pixels_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_sample_pixels": (ci, [vp, i64, i64, i64, fp, i64, C.c_uint64, vp, vp, vp, sz, vp]),
+        "ffb6d_sample_pixels_dseed": (ci, [vp, i64, i64, i64, fp, i64, vp, vp, vp, vp, sz, vp]),
         "ffb6d_fill_depth_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_fill_depth": (ci, [vp, i64, i64, i64, fp, vp, vp, vp, sz, vp]),
         "ffb6d_mean_shift_workspace_bytes": (sz, [i64, i64]),
@@ -132,9 +133,12 @@ def _load():
         "ffb6d_vote_poses": (ci, [vp, vp, vp, vp, vp, vp, vp, i64, i64, i64, i64, ci, ci, fp, ci, vp, vp, vp, vp, vp,
                                   sz, vp]),
         "ffb6d_rgb_add_noise": (ci, [vp, i64, i64, i64, vp, vp, C.c_uint64, vp, vp, vp, vp]),
+        "ffb6d_rgb_add_noise_dseed": (ci, [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, vp]),
+        "ffb6d_rgb_noise_check_records": (ci, [vp, i64]),
         "ffb6d_add_real_back": (ci, [vp, vp, vp, vp, vp, ci, vp, vp, ci, i64, i64, i64, vp, vp, vp]),
         "ffb6d_aug_noise_field": (ci, [C.c_uint64, i64, i64, i64, ci, vp, vp]),
         "ffb6d_color_jitter": (ci, [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp]),
+        "ffb6d_color_jitter_check_plans": (ci, [vp, i64]),
         "ffb6d_loss_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_focal_loss_fwd": (ci, [vp, ci, vp, ci, vp, i64, i64, i64, fp, vp, ci, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_focal_loss_bwd": (ci, [vp, ci, vp, ci, vp, i64, i64, i64, fp, vp, ci, vp, vp, vp, vp, vp]),

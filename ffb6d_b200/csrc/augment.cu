@@ -242,12 +242,15 @@ __device__ __forceinline__ uint8_t add_clip_trunc(double x, double n)
 }
 
 // field (optional): [2,B,H,W,3] float64 normals to use instead of the generator's (stage 2*pass, 2*pass+1)
+// seed_dev (optional): the seed read on the device instead of the value (ffb6d_rgb_add_noise_dseed)
 __global__ void noise_kernel(const uint8_t *__restrict__ src, const double *__restrict__ plan, uint32_t n_el,
-                             uint64_t seed, const double *__restrict__ field, int B, uint8_t *__restrict__ dst)
+                             uint64_t seed, const uint64_t *__restrict__ seed_dev, const double *__restrict__ field,
+                             int B, uint8_t *__restrict__ dst)
 {
     const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     const int b = blockIdx.y;
     if (e >= n_el) return;
+    if (seed_dev) seed = __ldg((const unsigned long long *)seed_dev);
     const double *rec = plan + (size_t)b * FFB6D_AUG_REC_LEN;
     const size_t o = (size_t)b * n_el + e;
     uint8_t v = src[o];
@@ -315,6 +318,16 @@ static const char *check_record(const double *r)
     return nullptr;
 }
 
+// every frame's record, before any launch (ffb6d_rgb_add_noise, ffb6d_rgb_noise_check_records)
+static int check_records(const double *plan_host, int64_t B)
+{
+    for (int64_t b = 0; b < B; ++b) {
+        const char *bad = check_record(plan_host + b * FFB6D_AUG_REC_LEN);
+        FFB6D_CHECK_ARG(!bad, "rgb_add_noise: frame %lld: bad record (%s)", (long long)b, bad);
+    }
+    return FFB6D_OK;
+}
+
 }  // namespace ffb6d
 
 using namespace ffb6d;
@@ -326,20 +339,20 @@ using namespace ffb6d;
                     tag ": bad size (B=%lld H=%lld W=%lld; H, W >= 32, H <= %lld)", (long long)B, (long long)H,     \
                     (long long)W, 65535ll * TY)
 
-extern "C" int ffb6d_rgb_add_noise(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, const double *plan_host,
-                                   const double *plan_dev, uint64_t seed, const double *noise, uint8_t *out,
-                                   uint8_t *work, ffb6d_stream_t stream)
+// ffb6d_rgb_add_noise and ffb6d_rgb_add_noise_dseed: the seed by value, or (dseed) read from seed_dev on the device
+static int rgb_add_noise(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, const double *plan_host,
+                         const double *plan_dev, uint64_t seed, bool dseed, const uint64_t *seed_dev,
+                         const double *noise, uint8_t *out, uint8_t *work, ffb6d_stream_t stream)
 {
     AUG_CHECK_SIZE("rgb_add_noise");
     if (B == 0) return FFB6D_OK;
-    FFB6D_CHECK_ARG(rgb && plan_host && plan_dev && out && work, "rgb_add_noise: null pointer");
+    FFB6D_CHECK_ARG(rgb && plan_host && plan_dev && out && work && (seed_dev || !dseed), "rgb_add_noise: null pointer");
     FFB6D_CHECK_ARG(work != rgb && work != out, "rgb_add_noise: work must not alias rgb or out");
-    FFB6D_CHECK_ARG((uintptr_t)plan_host % 8 == 0 && (uintptr_t)plan_dev % 8 == 0 && (uintptr_t)noise % 8 == 0,
+    FFB6D_CHECK_ARG((uintptr_t)plan_host % 8 == 0 && (uintptr_t)plan_dev % 8 == 0 && (uintptr_t)noise % 8 == 0 &&
+                        (uintptr_t)seed_dev % 8 == 0,
                     "rgb_add_noise: misaligned pointer");
-    for (int64_t b = 0; b < B; ++b) {
-        const char *bad = check_record(plan_host + b * FFB6D_AUG_REC_LEN);
-        FFB6D_CHECK_ARG(!bad, "rgb_add_noise: frame %lld: bad record (%s)", (long long)b, bad);
-    }
+    const int rc = check_records(plan_host, B);
+    if (rc != FFB6D_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int HW = (int)(H * W);
     const dim3 pgrid((unsigned)ceil_div(HW, 256), (unsigned)B);
@@ -353,10 +366,33 @@ extern "C" int ffb6d_rgb_add_noise(const uint8_t *rgb, int64_t B, int64_t H, int
     gauss_kernel<<<tgrid, tblock, 0, st>>>(out, plan_dev, (int)H, (int)W, work);
     FFB6D_LAUNCH_OK("gauss_kernel");
     const uint32_t n_el = (uint32_t)(HW * 3);
-    noise_kernel<<<dim3((unsigned)ceil_div(n_el, 256), (unsigned)B), 256, 0, st>>>(work, plan_dev, n_el, seed, noise,
-                                                                                (int)B, out);
+    noise_kernel<<<dim3((unsigned)ceil_div(n_el, 256), (unsigned)B), 256, 0, st>>>(work, plan_dev, n_el, seed, seed_dev,
+                                                                                noise, (int)B, out);
     FFB6D_LAUNCH_OK("noise_kernel");
     return FFB6D_OK;
+}
+
+extern "C" int ffb6d_rgb_add_noise(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, const double *plan_host,
+                                   const double *plan_dev, uint64_t seed, const double *noise, uint8_t *out,
+                                   uint8_t *work, ffb6d_stream_t stream)
+{
+    return rgb_add_noise(rgb, B, H, W, plan_host, plan_dev, seed, false, nullptr, noise, out, work, stream);
+}
+
+extern "C" int ffb6d_rgb_add_noise_dseed(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, const double *plan_host,
+                                         const double *plan_dev, const uint64_t *seed_dev, const double *noise,
+                                         uint8_t *out, uint8_t *work, ffb6d_stream_t stream)
+{
+    return rgb_add_noise(rgb, B, H, W, plan_host, plan_dev, 0, true, seed_dev, noise, out, work, stream);
+}
+
+extern "C" int ffb6d_rgb_noise_check_records(const double *plan_host, int64_t B)
+{
+    FFB6D_CHECK_ARG(B >= 0 && B < 65536, "rgb_noise_check_records: bad size (B=%lld)", (long long)B);
+    if (B == 0) return FFB6D_OK;
+    FFB6D_CHECK_ARG(plan_host, "rgb_noise_check_records: null pointer");
+    FFB6D_CHECK_ARG((uintptr_t)plan_host % 8 == 0, "rgb_noise_check_records: misaligned pointer");
+    return check_records(plan_host, B);
 }
 
 extern "C" int ffb6d_add_real_back(const uint8_t *rgb, const uint8_t *labels, const uint16_t *dpt,

@@ -148,11 +148,12 @@ __device__ __forceinline__ unsigned permute_below(unsigned i, unsigned n, unsign
 
 __global__ void __launch_bounds__(256)
 sample_pixels_kernel(const int *__restrict__ list, const int *__restrict__ count, int HW, int N, unsigned long long seed,
-                     int *__restrict__ choose)
+                     const unsigned long long *__restrict__ seed_dev, int *__restrict__ choose)
 {
     const int b = blockIdx.y;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
+    if (seed_dev) seed = __ldg(seed_dev);             // the _dseed entry point: the seed is read at run time
     const int n = count[b];
     const unsigned key = mix32((unsigned)seed ^ mix32((unsigned)(seed >> 32) + 0x632be5abu * (unsigned)(b + 1)));
     int px = 0;
@@ -194,14 +195,16 @@ extern "C" size_t ffb6d_sample_pixels_workspace_bytes(int64_t B, int64_t H, int6
     return align_up((size_t)B * (size_t)H * (size_t)W * sizeof(int), 256) + align_up((size_t)B * sizeof(int), 256);
 }
 
-extern "C" int ffb6d_sample_pixels(const float *depth, int64_t B, int64_t H, int64_t W, float min_depth, int64_t N,
-                                   uint64_t seed, int *choose, int *valid_count, void *workspace, size_t workspace_bytes,
-                                   ffb6d_stream_t stream)
+// ffb6d_sample_pixels and ffb6d_sample_pixels_dseed: the seed by value, or (seed_dev not NULL) read on the device
+static int sample_pixels(const float *depth, int64_t B, int64_t H, int64_t W, float min_depth, int64_t N, uint64_t seed,
+                         bool dseed, const uint64_t *seed_dev, int *choose, int *valid_count, void *workspace,
+                         size_t workspace_bytes, ffb6d_stream_t stream)
 {
     FFB6D_CHECK_ARG(B >= 0 && H >= 1 && W >= 1 && N >= 0 && H * W < (1ll << 30) && N < (1ll << 30) && B < 65536,
                     "sample_pixels: bad size");
     if (B == 0 || N == 0) return FFB6D_OK;
-    FFB6D_CHECK_ARG(depth && choose && workspace, "sample_pixels: null pointer");
+    FFB6D_CHECK_ARG(depth && choose && workspace && (seed_dev || !dseed), "sample_pixels: null pointer");
+    FFB6D_CHECK_ARG((uintptr_t)seed_dev % 8 == 0, "sample_pixels: misaligned pointer");
     FFB6D_CHECK_ARG(workspace_bytes >= ffb6d_sample_pixels_workspace_bytes(B, H, W), "sample_pixels: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     const int HW = (int)(H * W);
@@ -209,8 +212,25 @@ extern "C" int ffb6d_sample_pixels(const float *depth, int64_t B, int64_t H, int
     int *count = (int *)((char *)workspace + align_up((size_t)B * HW * sizeof(int), 256));
     compact_valid_kernel<<<(unsigned)B, COMPACT_THREADS, 0, st>>>(depth, HW, min_depth, list, count);
     FFB6D_LAUNCH_OK("compact_valid_kernel");
-    sample_pixels_kernel<<<dim3((unsigned)ceil_div(N, 256), (unsigned)B), 256, 0, st>>>(list, count, HW, (int)N, seed, choose);
+    sample_pixels_kernel<<<dim3((unsigned)ceil_div(N, 256), (unsigned)B), 256, 0, st>>>(
+        list, count, HW, (int)N, seed, (const unsigned long long *)seed_dev, choose);
     FFB6D_LAUNCH_OK("sample_pixels_kernel");
     if (valid_count) FFB6D_CUDA(cudaMemcpyAsync(valid_count, count, (size_t)B * sizeof(int), cudaMemcpyDeviceToDevice, st));
     return FFB6D_OK;
+}
+
+extern "C" int ffb6d_sample_pixels(const float *depth, int64_t B, int64_t H, int64_t W, float min_depth, int64_t N,
+                                   uint64_t seed, int *choose, int *valid_count, void *workspace, size_t workspace_bytes,
+                                   ffb6d_stream_t stream)
+{
+    return sample_pixels(depth, B, H, W, min_depth, N, seed, false, nullptr, choose, valid_count, workspace, workspace_bytes,
+                         stream);
+}
+
+extern "C" int ffb6d_sample_pixels_dseed(const float *depth, int64_t B, int64_t H, int64_t W, float min_depth,
+                                         int64_t N, const uint64_t *seed_dev, int *choose, int *valid_count,
+                                         void *workspace, size_t workspace_bytes, ffb6d_stream_t stream)
+{
+    return sample_pixels(depth, B, H, W, min_depth, N, 0, true, seed_dev, choose, valid_count, workspace, workspace_bytes,
+                         stream);
 }

@@ -268,6 +268,16 @@ static const char *check_plan(const double *p)
     return nullptr;
 }
 
+// every frame's plan, before any launch (ffb6d_color_jitter, ffb6d_color_jitter_check_plans)
+static int check_plans(const double *plan_host, int64_t B)
+{
+    for (int64_t b = 0; b < B; ++b) {
+        const char *bad = check_plan(plan_host + b * FFB6D_JITTER_PLAN_LEN);
+        FFB6D_CHECK_ARG(!bad, "color_jitter: frame %lld: bad plan (%s)", (long long)b, bad);
+    }
+    return FFB6D_OK;
+}
+
 static bool overlaps(const void *a, size_t na, const void *b, size_t nb)
 {
     const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
@@ -293,10 +303,8 @@ extern "C" int ffb6d_color_jitter(const uint8_t *rgb, int64_t B, int64_t H, int6
                     "color_jitter: work must not alias rgb or out");
     FFB6D_CHECK_ARG(out == rgb || !overlaps(out, img_bytes, rgb, img_bytes),
                     "color_jitter: out must be rgb itself or not overlap it");
-    for (int64_t b = 0; b < B; ++b) {
-        const char *bad = check_plan(plan_host + b * FFB6D_JITTER_PLAN_LEN);
-        FFB6D_CHECK_ARG(!bad, "color_jitter: frame %lld: bad plan (%s)", (long long)b, bad);
-    }
+    const int rc = check_plans(plan_host, B);
+    if (rc != FFB6D_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int HW = (int)(H * W);
     const dim3 grid((unsigned)ceil_div(HW, JT * JPX), (unsigned)B);
@@ -307,4 +315,12 @@ extern "C" int ffb6d_color_jitter(const uint8_t *rgb, int64_t B, int64_t H, int6
     jitter_apply_kernel<<<grid, JT, 0, st>>>(rgb, plan_dev, active, HW, sums, out);
     FFB6D_LAUNCH_OK("jitter_apply_kernel");
     return FFB6D_OK;
+}
+
+extern "C" int ffb6d_color_jitter_check_plans(const double *plan_host, int64_t B)
+{
+    FFB6D_CHECK_ARG(B >= 1 && B < 65536, "color_jitter_check_plans: bad size (B=%lld)", (long long)B);
+    FFB6D_CHECK_ARG(plan_host, "color_jitter_check_plans: null pointer");
+    FFB6D_CHECK_ARG((uintptr_t)plan_host % 8 == 0, "color_jitter_check_plans: misaligned pointer");
+    return check_plans(plan_host, B);
 }

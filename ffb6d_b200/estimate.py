@@ -27,7 +27,7 @@ import torch
 from . import pose as _pose
 from .graphed import _GraphedStep
 from .model import FFB6D, FFB6DFusionNet
-from .ops import _intrinsics_arg
+from .ops import _frame_intrinsics, _intrinsics_arg
 from .schedule import build_ffb6d_inputs
 
 # the reference's config.n_sample_points (common.py:61)
@@ -81,11 +81,6 @@ def _check_model(model, name):
     if isinstance(model, FFB6DFusionNet) and not isinstance(model, FFB6D):
         raise ValueError("%s: an FFB6DFusionNet has no image branch; pose estimation from frames needs the whole "
                          "FFB6D" % name)
-
-
-def _frame_intrinsics(K):
-    """Per-frame camera matrices ``[B,3,3]`` float64 CUDA -> ``(fx, fy, cx, cy)`` ``[B,4]`` on the device."""
-    return torch.stack((K[:, 0, 0], K[:, 1, 1], K[:, 0, 2], K[:, 1, 2]), 1).contiguous()
 
 
 def vote_table(dataset, mesh_kps, n_cls, cls_radius=None, device=None):

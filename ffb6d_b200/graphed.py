@@ -19,16 +19,26 @@ buffer and gradient) is compared on the host before every replay; when any of it
 
 The eval step reads the weights on the device at every replay, so it follows optimizer steps, ``load_state_dict``
 and graphed training steps without capturing again.
+
+    step = GraphedFrameTrainStep(model, opt, example_batch, dataset="ycb", cam_scale=10000.0, K=K)
+    for it, batch in enumerate(loader):
+        loss, info = step(batch, seed=it)     # build_ffb6d_train_item and the training step, replayed
+
+:class:`GraphedFrameTrainStep` also captures the training ``get_item`` (DESIGN.md §4.28): the augmentation, the
+depth completion, the sampling, the 22 searches and the point arrays, from the collated batch's decoded frames.
 """
 import os
 
+import numpy as np
 import torch
 import torch.distributed as dist
 import torch.nn as nn
 from torch.autograd.graph import increment_version
 
+from . import ops
 from .loss import ffb6d_loss
 from .model import FFB6D, FFB6DFusionNet
+from .schedule import TRAIN_RECORD_KEYS, _train_item, check_train_batch
 
 
 # Adam's (and AdamW's) state, each created as zeros by its first step: what the warm-up's own first step created is
@@ -241,29 +251,30 @@ class GraphedTrainStep(_GraphedStep):
     def _check(self, modules):
         """What cannot be captured at all: raise ``ValueError`` before any CUDA work.  ``modules``: also walk the
         BatchNorms (momentum=None, SyncBatchNorm over several ranks)."""
-        model, opt = self.model, self.optimizer
+        model, opt, name = self.model, self.optimizer, type(self).__name__
         if not model.training:
-            raise ValueError("GraphedTrainStep: the model is in eval mode; it captures training steps only")
+            raise ValueError("%s: the model is in eval mode; it captures training steps only" % name)
         self._refuse_index_check()
         if not isinstance(opt, torch.optim.Adam):      # AdamW is an Adam
-            raise ValueError("GraphedTrainStep: the optimizer must be torch.optim.Adam or AdamW, got %s (the warm-up "
-                             "is undone by restoring Adam's zero initial state)" % type(opt).__name__)
+            raise ValueError("%s: the optimizer must be torch.optim.Adam or AdamW, got %s (the warm-up is undone by "
+                             "restoring Adam's zero initial state)" % (name, type(opt).__name__))
         for i, g in enumerate(opt.param_groups):
             if not g.get("capturable", False):
-                raise ValueError("GraphedTrainStep: optimizer param group %d needs capturable=True" % i)
+                raise ValueError("%s: optimizer param group %d needs capturable=True" % (name, i))
         if not modules:
             return
         multi_rank = dist.is_available() and dist.is_initialized()
         for name, m in model.named_modules():
             if isinstance(m, nn.modules.batchnorm._BatchNorm):
                 if m.momentum is None:
-                    raise ValueError("GraphedTrainStep: BatchNorm %r has momentum=None (a cumulative average read "
-                                     "from num_batches_tracked on the host); give it a float momentum" % name)
+                    raise ValueError("%s: BatchNorm %r has momentum=None (a cumulative average read from "
+                                     "num_batches_tracked on the host); give it a float momentum" % (type(self).__name__,
+                                                                                                     name))
                 if isinstance(m, nn.SyncBatchNorm) and multi_rank:
                     group = m.process_group if m.process_group is not None else dist.group.WORLD
                     if dist.get_world_size(group) > 1:
-                        raise ValueError("GraphedTrainStep: SyncBatchNorm %r synchronises over several ranks; "
-                                         "multi-rank capture is not supported" % name)
+                        raise ValueError("%s: SyncBatchNorm %r synchronises over several ranks; multi-rank capture "
+                                         "is not supported" % (type(self).__name__, name))
 
     def _module_key(self, m):
         """BatchNorm momentum, dropout rates, and ``requires_grad`` and the gradient storage of every parameter."""
@@ -295,7 +306,11 @@ class GraphedTrainStep(_GraphedStep):
 
     # ------------------------------------------------------------------------------------------ capture
     def _step(self):
-        opt, item = self.optimizer, self._static
+        return self._train(self._static)
+
+    def _train(self, item):
+        """One training step on ``item``: what a replay runs."""
+        opt = self.optimizer
         opt.zero_grad(set_to_none=True)
         out = self.model(item) if isinstance(self.model, FFB6D) else self.model(item, item["rgb_feats"])
         loss, info = ffb6d_loss(out, item, valid=item.get("valid"))
@@ -336,8 +351,8 @@ class GraphedTrainStep(_GraphedStep):
         if unknown:              # a subclass of Adam with state of its own: drop what the warm-up created, refuse
             for p in [p for p in opt.state if p not in had_state]:
                 del opt.state[p]
-            raise ValueError("GraphedTrainStep: the optimizer created state %s whose initial value is not known to be "
-                             "zero; only Adam's own state can be restored after the warm-up" % (unknown,))
+            raise ValueError("%s: the optimizer created state %s whose initial value is not known to be zero; only "
+                             "Adam's own state can be restored after the warm-up" % (type(self).__name__, unknown))
         del saved, saved_state
         opt.zero_grad(set_to_none=True)
         self._loss, self._info = self._record()
@@ -351,11 +366,151 @@ class GraphedTrainStep(_GraphedStep):
     def __call__(self, item):
         self._check(self._sync)
         self._copy_in(item)
+        return self._replay()
+
+    def _replay(self):
         if self._baked() != self._key:
             self._capture(1)
         self._graph.replay()
         increment_version(self._written)
         return self._loss, self._info
+
+
+class GraphedFrameTrainStep(GraphedTrainStep):
+    """:func:`ffb6d_b200.build_ffb6d_train_item` and a :class:`GraphedTrainStep` training step of an
+    :class:`~ffb6d_b200.model.FFB6D`, captured in one CUDA graph and replayed per batch: the colour jitter, both
+    ``rgb_add_noise`` passes, ``add_real_back``, the depth completion (YCB), the sampling, the 22 searches and the
+    point arrays, then ``zero_grad``, the forward, ``ffb6d_loss``, the backward and ``optimizer.step()``.
+
+    :param example_batch: a batch as :func:`~ffb6d_b200.build_ffb6d_train_item` takes it.  Its CUDA tensors (the
+      images, the background frames, the object tables, a per-frame ``K``) get static input buffers, as
+      :class:`GraphedTrainStep`'s item does; its host values (the worker's ``jitter``, ``jittered``, ``plans``,
+      ``augment``, ``apply_rgb``, and any other entry that is not a CUDA tensor) get device buffers that every call
+      fills through pinned staging memory.  Later batches must have the same keys, and each entry the same kind
+      (CUDA or host), shape and dtype.
+    :param warmup: eager steps before the first capture, undone as :class:`GraphedTrainStep` undoes them.
+
+    Baked in at construction: ``dataset``, ``cam_scale``, ``n_points`` and ``K`` (copied to the device once; with
+    ``batch['K']`` the per-frame matrices are inputs instead).  Everything else that capture bakes in, and every rule
+    that captures again, rejects or restores, is :class:`GraphedTrainStep`'s (DESIGN.md §4.20).
+
+    ``step(batch, seed)`` checks the batch's jitter plans and noise records on the host (a bad one raises
+    :class:`~ffb6d_b200._lib.FFB6DError` before anything is copied), copies the host values and ``seed`` (an int in
+    [0, 2^64), or a one-element int64 / uint64 CUDA tensor) through pinned buffers without synchronising the host,
+    copies the CUDA tensors into the input buffers on the current stream, and replays.  It returns ``(loss, info)``
+    of :func:`ffb6d_b200.loss.ffb6d_loss`: the graph's tensors, which the next replay overwrites.  The replay equals
+    ``build_ffb6d_train_item`` with that seed followed by an eager training step, bit for bit.
+
+    Rejected with ``ValueError``: what :class:`GraphedTrainStep` rejects; an :class:`FFB6DFusionNet` (its image maps
+    do not come from frames); a batch whose keys, or an entry's kind, shape, dtype or device, differ from the example.
+    """
+
+    _STAGING_SLOTS = 2
+
+    def __init__(self, model, optimizer, example_batch, *, dataset, cam_scale, K, n_points=12800, warmup=3):
+        name = type(self).__name__
+        self._check_model(model)
+        check_train_batch(example_batch, dataset, name)
+        self.dataset, self.cam_scale, self.n_points = dataset, cam_scale, int(n_points)
+        self._keys = set(example_batch)
+        dev = next(model.parameters()).device
+        device_part = {k: v for k, v in example_batch.items() if isinstance(v, torch.Tensor) and v.is_cuda}
+        host = self._host_values(example_batch, None)
+        B = example_batch["rgb"].shape[0]
+        self._intr = None if "K" in example_batch else ops._intrinsics_arg(K, B, dev)[0]
+        # the device buffers of the host values and of the seed, and the pinned slots they are copied from in turn
+        self._records = {k: torch.empty(t.shape, dtype=t.dtype, device=dev) for k, t in host.items()}
+        self._seed = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._pinned = [dict({k: torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for k, t in host.items()},
+                             _seed=torch.empty(1, dtype=torch.int64, pin_memory=True))
+                        for _ in range(self._STAGING_SLOTS)]
+        self._staged = [None] * self._STAGING_SLOTS
+        self._slot = 0
+        self._check_records(host)
+        self._stage(host, 0)
+        self._mirror = {k: host[k].numpy().copy() for k in ("jitter", "plans")}
+        super().__init__(model, optimizer, device_part, warmup)
+
+    def _check_model(self, model):
+        super()._check_model(model)
+        if not isinstance(model, FFB6D):
+            raise ValueError("%s: an FFB6DFusionNet has no image branch; training from frames needs the whole FFB6D"
+                             % type(self).__name__)
+
+    def _host_values(self, batch, want):
+        """Every entry of ``batch`` that is not a CUDA tensor, as a contiguous CPU tensor; with ``want`` (the example's
+        values) each must exist and match its shape and dtype."""
+        name, out = type(self).__name__, {}
+        for k, v in batch.items():
+            if isinstance(v, torch.Tensor) and v.is_cuda:
+                if want is not None and k in want:
+                    raise ValueError("%s: batch[%r] is a CUDA tensor; the step was captured with it on the host"
+                                     % (name, k))
+                continue
+            t = torch.as_tensor(v).contiguous()
+            if want is not None:
+                if k not in want:
+                    raise ValueError("%s: batch[%r] is on the host; the step was captured with it on the device"
+                                     % (name, k))
+                if t.shape != want[k].shape or t.dtype != want[k].dtype:
+                    raise ValueError("%s: batch[%r] is %s %s; the step was captured for %s %s"
+                                     % (name, k, tuple(t.shape), t.dtype, tuple(want[k].shape), want[k].dtype))
+            out[k] = t
+        missing = [k for k in TRAIN_RECORD_KEYS if k not in out]
+        if missing:
+            raise ValueError("%s: %s must be host values (the worker's draws), not CUDA tensors" % (name, missing))
+        return out
+
+    @staticmethod
+    def _check_records(host):
+        """The checks the jitter and noise entry points run on the host records, without a launch."""
+        ops.color_jitter_check_plans(host["jitter"].numpy())
+        plans = host["plans"].numpy()
+        for p in range(plans.shape[1]):
+            ops.rgb_noise_check_records(plans[:, p])
+
+    def _stage(self, host, seed):
+        """Copy the host values and the seed into their device buffers through the next pinned slot, on the current
+        stream.  The slot is written once the copies that last read it have run (an event, two calls back): the
+        host waits only when it is that far ahead of the stream."""
+        i = self._slot
+        self._slot = (i + 1) % self._STAGING_SLOTS
+        if self._staged[i] is not None:
+            self._staged[i].synchronize()
+        pin = self._pinned[i]
+        for k, t in host.items():
+            pin[k].copy_(t)
+            self._records[k].copy_(pin[k], non_blocking=True)
+        if isinstance(seed, torch.Tensor):
+            self._seed.copy_(seed.reshape(1).view(torch.int64))
+        else:
+            pin["_seed"][0] = seed - (1 << 64) if seed >= 1 << 63 else seed
+            self._seed.copy_(pin["_seed"], non_blocking=True)
+        self._staged[i] = torch.cuda.Event()
+        self._staged[i].record()
+
+    def _step(self):
+        batch = dict(self._static, **self._records)
+        item = _train_item(batch, self.dataset, self.cam_scale, self._intr, self.n_points, self._seed,
+                           records=self._mirror)
+        return self._train(item)
+
+    def __call__(self, batch, seed):
+        name = type(self).__name__
+        self._check(self._sync)
+        if not isinstance(batch, dict) or set(batch) != self._keys:
+            raise ValueError("%s: the batch holds keys %s; the step was captured for %s"
+                             % (name, sorted(map(str, batch)) if isinstance(batch, dict) else type(batch).__name__,
+                                sorted(map(str, self._keys))))
+        if isinstance(seed, torch.Tensor):
+            ops._device_seed(seed, self._seed.device)
+        elif isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
+            raise ValueError("%s: seed must be an int in [0, 2^64) or a one-element CUDA tensor, got %r" % (name, seed))
+        host = self._host_values(batch, self._records)
+        self._check_records(host)
+        self._copy_in({k: batch[k] for k in self._static})
+        self._stage(host, seed if isinstance(seed, torch.Tensor) else int(seed))
+        return self._replay()
 
 
 class GraphedEvalStep(_GraphedStep):

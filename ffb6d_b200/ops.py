@@ -746,6 +746,11 @@ def _intrinsics_arg(K, B, dev):
     return intrinsics_to_device(Kn, dev), int(Kn.ndim == 3)
 
 
+def _frame_intrinsics(K):
+    """Per-frame camera matrices ``[B,3,3]`` float64 CUDA -> ``(fx, fy, cx, cy)`` ``[B,4]`` on the device."""
+    return torch.stack((K[:, 0, 0], K[:, 1, 1], K[:, 0, 2], K[:, 1, 2]), 1).contiguous()
+
+
 def point_item(depth_m, K, choose, rgb, labels, nrm_map, obj_cls, obj_kps, obj_ctr):
     """The sampled points' input features and pose-training targets on the GPU (``ffb6d_point_item``): the half of
     the datasets' ``get_item`` that reads ``choose`` (datasets/ycb/ycb_dataset.py:237-247 and ``get_pose_gt_info``
@@ -840,6 +845,17 @@ def point_input(depth_m, K, choose, rgb, nrm_map):
     return cld_rgb_nrm
 
 
+def _device_seed(seed, dev):
+    """``seed`` when it is a one-element int64 / uint64 CUDA tensor on ``dev`` (read on the device by the ``_dseed``
+    entry points, so a captured call takes a new seed per replay; its 64 bits are the seed), None for a host int."""
+    if not isinstance(seed, torch.Tensor):
+        return None
+    if not seed.is_cuda or seed.device != dev or seed.dtype not in (torch.int64, torch.uint64) or seed.numel() != 1:
+        raise ValueError("a tensor seed must be one int64 / uint64 element on %s, got %s %s on %s"
+                         % (dev, seed.dtype, tuple(seed.shape), seed.device))
+    return seed.contiguous()
+
+
 def sample_valid_pixels(depth, n_points, seed=0, min_depth=1e-8, return_count=False):
     """The datasets' point sampling on the GPU (datasets/ycb/ycb_dataset.py:218-235): the valid pixels of each
     depth map (``depth > min_depth``) are compacted, ``n_points`` of them are drawn uniformly without replacement
@@ -847,7 +863,9 @@ def sample_valid_pixels(depth, n_points, seed=0, min_depth=1e-8, return_count=Fa
     random order.  Deterministic per ``seed``; the picks have the reference's distribution but do not replay
     numpy's random stream.
 
-    :param depth: ``[B,H,W]`` float32 CUDA; :return: ``choose [B,1,n_points]`` int32 flat pixel indices
+    :param depth: ``[B,H,W]`` float32 CUDA; :param seed: an int, or a one-element int64 / uint64 CUDA tensor read on
+      the device (the same picks as the int of the same 64 bits)
+    :return: ``choose [B,1,n_points]`` int32 flat pixel indices
       (what :func:`backproject` and the final ``choose`` gather take); with ``return_count`` also the number
       of valid pixels per frame ``[B]`` int32."""
     _need_cuda(depth, "depth")
@@ -860,8 +878,13 @@ def sample_valid_pixels(depth, n_points, seed=0, min_depth=1e-8, return_count=Fa
     count = torch.empty((B,), dtype=torch.int32, device=dev)
     nbytes = int(lib.ffb6d_sample_pixels_workspace_bytes(B, H, W))
     ws = workspace(nbytes, dev)
-    launch(lib.ffb6d_sample_pixels, dev, depth.data_ptr(), B, H, W, float(min_depth), int(n_points),
-           int(seed) & (2 ** 64 - 1), choose.data_ptr(), count.data_ptr(), ws.data_ptr(), nbytes)
+    seed_d = _device_seed(seed, dev)
+    if seed_d is None:
+        launch(lib.ffb6d_sample_pixels, dev, depth.data_ptr(), B, H, W, float(min_depth), int(n_points),
+               int(seed) & (2 ** 64 - 1), choose.data_ptr(), count.data_ptr(), ws.data_ptr(), nbytes)
+    else:
+        launch(lib.ffb6d_sample_pixels_dseed, dev, depth.data_ptr(), B, H, W, float(min_depth), int(n_points),
+               seed_d.data_ptr(), choose.data_ptr(), count.data_ptr(), ws.data_ptr(), nbytes)
     return (choose, count) if return_count else choose
 
 
@@ -1345,16 +1368,20 @@ def best_fit_transform(A, B):
     return T[0] if single else T
 
 
-def rgb_add_noise(rgb, plan, seed, noise=None):
+def rgb_add_noise(rgb, plan, seed, noise=None, plan_dev=None):
     """The datasets' ``rgb_add_noise`` (datasets/ycb/ycb_dataset.py:107-143, linemod_dataset.py:142-164) for a batch
     on the GPU (``ffb6d_rgb_add_noise``).
 
     :param rgb: ``[B,H,W,3]`` uint8 CUDA, H, W >= 32 (the channel roles are the reference's: it feeds RGB data to
       ``COLOR_BGR2HSV``)
     :param plan: ``[B, REC_LEN]`` float64 numpy records of :func:`ffb6d_b200.augment.draw_rgb_noise`
-    :param seed: key of the per-pixel normal draws (frame b of the batch, the record's pass); use one seed per batch
+    :param seed: key of the per-pixel normal draws (frame b of the batch, the record's pass); use one seed per batch.
+      An int, or a one-element int64 / uint64 CUDA tensor read on the device (the same draws as the int of the same
+      64 bits)
     :param noise: optional ``[2,B,H,W,3]`` float64 CUDA normals to use instead of the generator's (the first for
       ``gaussian_noise``, the second for YCB's ``normal(0, 7)``), e.g. to replay numpy's stream
+    :param plan_dev: optional ``[B, REC_LEN]`` float64 CUDA copy of ``plan`` for the kernels to read (``plan`` is
+      still what is checked); without it ``plan`` is copied to the device
     :return: ``[B,H,W,3]`` uint8
     """
     from . import augment as A
@@ -1365,18 +1392,37 @@ def rgb_add_noise(rgb, plan, seed, noise=None):
     plan = np.ascontiguousarray(plan, dtype=np.float64)
     if plan.shape != (B, A.REC_LEN):
         raise ValueError("plan must be float64 [B, %d] = [%d, %d], got %s" % (A.REC_LEN, B, A.REC_LEN, plan.shape))
-    if not (0 <= int(seed) < 1 << 64):
-        raise ValueError("seed must fit 64 bits, got %r" % (seed,))
     dev = rgb.device
+    seed_d = _device_seed(seed, dev)
+    if seed_d is None and not (0 <= int(seed) < 1 << 64):
+        raise ValueError("seed must fit 64 bits, got %r" % (seed,))
     if noise is not None:
         noise = _tensor(noise, "noise", torch.float64, (2, B, H, W, 3), dev)
     src = rgb.contiguous()
-    plan_d = torch.from_numpy(plan).to(dev)
+    if plan_dev is None:
+        plan_d = torch.from_numpy(plan).to(dev)
+    else:
+        plan_d = _tensor(plan_dev, "plan_dev", torch.float64, (B, A.REC_LEN), dev)
     out = torch.empty_like(src)
     work = torch.empty_like(src)
-    launch(lib.ffb6d_rgb_add_noise, dev, src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), int(seed),
-           ptr(noise), out.data_ptr(), work.data_ptr())
+    if seed_d is None:
+        launch(lib.ffb6d_rgb_add_noise, dev, src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), int(seed),
+               ptr(noise), out.data_ptr(), work.data_ptr())
+    else:
+        launch(lib.ffb6d_rgb_add_noise_dseed, dev, src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(),
+               seed_d.data_ptr(), ptr(noise), out.data_ptr(), work.data_ptr())
     return out
+
+
+def rgb_noise_check_records(plan):
+    """Check ``[B, REC_LEN]`` float64 host records as :func:`rgb_add_noise` checks them, without a launch
+    (``ffb6d_rgb_noise_check_records``): raises :class:`~ffb6d_b200._lib.FFB6DError` with its message for a bad
+    record."""
+    from . import augment as A
+    plan = np.ascontiguousarray(plan, dtype=np.float64)
+    if plan.ndim != 2 or plan.shape[1] != A.REC_LEN:
+        raise ValueError("plan must be float64 [B, %d], got %s" % (A.REC_LEN, plan.shape))
+    check(lib.ffb6d_rgb_noise_check_records(plan.ctypes.data, plan.shape[0]))
 
 
 def add_real_back(rgb, labels, dpt, back_rgb, back_labels, back_dpt, apply_rgb=None, dataset="ycb", active=None):
@@ -1389,7 +1435,8 @@ def add_real_back(rgb, labels, dpt, back_rgb, back_labels, back_dpt, apply_rgb=N
       frame's label image, YCB, or mask, LineMOD); :param back_dpt: ``[B,H,W]`` uint16
     :param apply_rgb: LineMOD: per-frame bools, the ``rand() < 0.6`` draw (YCB always composes the colour image)
     :param dataset: ``'ycb'`` or ``'linemod'``; :param active: per-frame bools, frames that go through
-      ``add_real_back`` at all (default: every frame); the others pass through unchanged
+      ``add_real_back`` at all (default: every frame); the others pass through unchanged.  When ``active`` and
+      ``apply_rgb`` are both ``[B]`` CUDA tensors, the flags are combined on the device (no host copy)
     :return: ``(rgb [B,H,W,3] uint8, dpt [B,H,W] uint16)``; the composed depth is uint16 and feeds
       :func:`fill_missing` as it is
     """
@@ -1409,16 +1456,23 @@ def add_real_back(rgb, labels, dpt, back_rgb, back_labels, back_dpt, apply_rgb=N
     ch = back_labels.shape[-1] if back_labels.dim() == 4 else 0
     back_labels = _tensor(back_labels, "back_labels", torch.uint8, (B, H, W, ch if ch in (1, 3) else -1), dev)
     back_dpt = _tensor(back_dpt, "back_dpt", torch.uint16, (B, H, W), dev)
-    act = np.ones(B, bool) if active is None else np.asarray(active, bool).reshape(-1)
-    if dataset == "ycb":
-        col = np.ones(B, bool) if apply_rgb is None else np.asarray(apply_rgb, bool).reshape(-1)
+    flags = (active, apply_rgb)
+    if all(isinstance(f, torch.Tensor) and f.is_cuda for f in flags):      # combined on the device: capturable
+        if any(tuple(f.shape) != (B,) or f.device != dev for f in flags):
+            raise ValueError("apply_rgb and active must have one entry per frame (%d) on %s" % (B, dev))
+        act, col = (f.to(torch.uint8) for f in flags)
+        mode = act * (1 + 2 * col)
     else:
-        if apply_rgb is None:
-            raise ValueError("LineMOD needs apply_rgb (the frame's rand() < 0.6 draw)")
-        col = np.asarray(apply_rgb, bool).reshape(-1)
-    if act.shape != (B,) or col.shape != (B,):
-        raise ValueError("apply_rgb and active must have one entry per frame (%d)" % B)
-    mode = torch.from_numpy((act * (1 + 2 * col)).astype(np.uint8)).to(dev)
+        act = np.ones(B, bool) if active is None else np.asarray(active, bool).reshape(-1)
+        if dataset == "ycb":
+            col = np.ones(B, bool) if apply_rgb is None else np.asarray(apply_rgb, bool).reshape(-1)
+        else:
+            if apply_rgb is None:
+                raise ValueError("LineMOD needs apply_rgb (the frame's rand() < 0.6 draw)")
+            col = np.asarray(apply_rgb, bool).reshape(-1)
+        if act.shape != (B,) or col.shape != (B,):
+            raise ValueError("apply_rgb and active must have one entry per frame (%d)" % B)
+        mode = torch.from_numpy((act * (1 + 2 * col)).astype(np.uint8)).to(dev)
     src = rgb.contiguous()
     rgb_out = torch.empty_like(src)
     dpt_out = torch.empty_like(dpt)
@@ -1428,7 +1482,7 @@ def add_real_back(rgb, labels, dpt, back_rgb, back_labels, back_dpt, apply_rgb=N
     return rgb_out, dpt_out
 
 
-def color_jitter(rgb, plan, active=None):
+def color_jitter(rgb, plan, active=None, plan_dev=None):
     """The datasets' ``trancolor`` (torchvision ``ColorJitter(0.2, 0.2, 0.2, 0.05)`` on the PIL image,
     datasets/ycb/ycb_dataset.py:190-193, linemod_dataset.py:220-223) for a batch on the GPU
     (``ffb6d_color_jitter``); bitwise what torchvision 0.26 with Pillow 12.2 computes.
@@ -1438,6 +1492,8 @@ def color_jitter(rgb, plan, active=None):
       frame's plan is validated, an inactive frame's too
     :param active: per-frame bools (a sequence, or a tensor), frames to jitter (default: every frame); the others,
       e.g. frames the dataset does not jitter, pass through unchanged
+    :param plan_dev: optional ``[B, JITTER_PLAN_LEN]`` float64 CUDA copy of ``plan`` for the kernels to read (``plan``
+      is still what is checked); without it ``plan`` is copied to the device
     :return: ``[B,H,W,3]`` uint8
     """
     from . import augment as A
@@ -1461,11 +1517,25 @@ def color_jitter(rgb, plan, active=None):
     out = torch.empty_like(src)
     if B * H * W == 0:
         return out
-    plan_d = torch.from_numpy(plan).to(dev)
+    if plan_dev is None:
+        plan_d = torch.from_numpy(plan).to(dev)
+    else:
+        plan_d = _tensor(plan_dev, "plan_dev", torch.float64, (B, A.JITTER_PLAN_LEN), dev)
     work = torch.empty(B, dtype=torch.int64, device=dev)
     launch(lib.ffb6d_color_jitter, dev, src.data_ptr(), B, H, W, plan.ctypes.data, plan_d.data_ptr(), act.data_ptr(),
            out.data_ptr(), work.data_ptr())
     return out
+
+
+def color_jitter_check_plans(plan):
+    """Check ``[B, JITTER_PLAN_LEN]`` float64 host plans as :func:`color_jitter` checks them, without a launch
+    (``ffb6d_color_jitter_check_plans``): raises :class:`~ffb6d_b200._lib.FFB6DError` with its message for a bad
+    plan."""
+    from . import augment as A
+    plan = np.ascontiguousarray(plan, dtype=np.float64)
+    if plan.ndim != 2 or plan.shape[1] != A.JITTER_PLAN_LEN:
+        raise ValueError("plan must be float64 [B, %d], got %s" % (A.JITTER_PLAN_LEN, plan.shape))
+    check(lib.ffb6d_color_jitter_check_plans(plan.ctypes.data, plan.shape[0]))
 
 
 def aug_noise_field(seed, B, H, W, stage, device="cuda"):

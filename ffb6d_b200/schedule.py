@@ -363,3 +363,69 @@ def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points,
     item.update(labels=labels_pt, rgb_labels=labels.to(torch.int32), RTs=obj["RTs"], kp_targ_ofst=kp_targ_ofst,
                 ctr_targ_ofst=ctr_targ_ofst, cls_ids=obj["cls_ids"], ctr_3ds=obj["ctr_3ds"], kp_3ds=obj["kp_3ds"])
     return item
+
+
+# the batch keys build_ffb6d_train_item reads (INTEGRATION.md, the worker / trainer split): the decoded images and the
+# background frames, the worker's augmentation draws (host values), and the object tables of pose_gt_objects
+TRAIN_IMAGE_KEYS = ("dpt", "rgb", "labels", "nrm_map", "back_rgb", "back_labels", "back_dpt")
+TRAIN_RECORD_KEYS = ("jitter", "jittered", "plans", "augment", "apply_rgb")
+TRAIN_BATCH_KEYS = TRAIN_IMAGE_KEYS + TRAIN_RECORD_KEYS + _OBJECT_KEYS
+
+
+def check_train_batch(batch, dataset, name):
+    """``ValueError`` unless ``dataset`` is known and ``batch`` is a dict holding every key of ``TRAIN_BATCH_KEYS``."""
+    if dataset not in ("ycb", "linemod"):
+        raise ValueError("%s: dataset must be 'ycb' or 'linemod', got %r" % (name, dataset))
+    if not isinstance(batch, dict):
+        raise ValueError("%s: the batch must be a dict, got %s" % (name, type(batch).__name__))
+    missing = [k for k in TRAIN_BATCH_KEYS if k not in batch]
+    if missing:
+        raise ValueError("%s: the batch lacks %s" % (name, missing))
+
+
+def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed):
+    """The training ``get_item`` of a collated batch on the GPU, in the reference's order: the colour jitter, the first
+    ``rgb_add_noise``, ``add_real_back``, the second ``rgb_add_noise``, :func:`build_ffb6d_item` (``fill=True`` for
+    YCB, ``False`` for LineMOD) and ``model_fn``'s ``rgb.float()``.  This is INTEGRATION.md's trainer composition in
+    one call.
+
+    :param batch: what the DataLoader collates from the worker's dict: CUDA tensors ``dpt``, ``rgb``, ``labels``,
+      ``nrm_map``, ``back_rgb``, ``back_labels``, ``back_dpt`` and the object tables of
+      :func:`ffb6d_b200.item.pose_gt_objects`; the worker's draws on the host: ``jitter [B,8]``, ``jittered [B]``,
+      ``plans [B,2,REC_LEN]``, ``augment [B]``, ``apply_rgb [B]``; optionally ``K [B,3,3]`` float64, one camera
+      matrix per frame (it replaces ``K``)
+    :param dataset: ``"ycb"`` or ``"linemod"``; :param cam_scale: raw depth units per metre
+    :param K: the camera matrix as :func:`build_ffb6d_item` takes it
+    :param seed: the key of the noise draws and of the point sampling: an int, or a one-element int64 / uint64 CUDA
+      tensor read on the device (the same bits as the int of the same 64 bits)
+    :return: the dict of :func:`build_ffb6d_item` with ``rgb`` as float32
+    """
+    check_train_batch(batch, dataset, "build_ffb6d_train_item")
+    return _train_item(batch, dataset, cam_scale, K, n_points, seed)
+
+
+def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None):
+    """:func:`build_ffb6d_train_item` on a checked batch.  ``records``: host copies of ``batch['jitter']`` and
+    ``batch['plans']`` when the batch holds those on the device (a graph's input buffers); the host copies are what
+    the entry points check, the device ones what the kernels read."""
+    import numpy as np
+    from .ops import _frame_intrinsics, add_real_back, color_jitter, rgb_add_noise
+    if records is None:
+        jitter, plans = np.asarray(batch["jitter"]), np.asarray(batch["plans"])
+        jitter_d = plans_d = None
+    else:
+        jitter, plans = records["jitter"], records["plans"]
+        jitter_d, plans_d = batch["jitter"], batch["plans"]
+    rgb = color_jitter(batch["rgb"], jitter, active=batch["jittered"], plan_dev=jitter_d)
+    rgb = rgb_add_noise(rgb, plans[:, 0], seed, plan_dev=None if plans_d is None else plans_d[:, 0])
+    rgb, dpt = add_real_back(rgb, batch["labels"], batch["dpt"], batch["back_rgb"], batch["back_labels"],
+                             batch["back_dpt"], batch["apply_rgb"], dataset, active=batch["augment"])
+    rgb = rgb_add_noise(rgb, plans[:, 1], seed, plan_dev=None if plans_d is None else plans_d[:, 1])
+    if "K" in batch:
+        K = batch["K"]
+        if isinstance(K, torch.Tensor) and K.is_cuda:
+            K = _frame_intrinsics(K)
+    item = build_ffb6d_item(dpt, cam_scale, K, rgb, batch["labels"], batch["nrm_map"], batch, n_points, seed=seed,
+                            fill=dataset == "ycb")
+    item["rgb"] = item["rgb"].float()
+    return item

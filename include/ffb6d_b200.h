@@ -505,6 +505,11 @@ size_t ffb6d_sample_pixels_workspace_bytes(int64_t B, int64_t H, int64_t W);
 int ffb6d_sample_pixels(const float *depth, int64_t B, int64_t H, int64_t W, float min_depth, int64_t N,
                         uint64_t seed, int *choose, int *valid_count, void *workspace, size_t workspace_bytes,
                         ffb6d_stream_t stream);
+/* ffb6d_sample_pixels with the seed read on the device from seed_dev (one uint64, 8-byte aligned), so that a
+ * captured CUDA graph takes a new seed per replay.  Same checks; for equal seed values, the same bits. */
+int ffb6d_sample_pixels_dseed(const float *depth, int64_t B, int64_t H, int64_t W, float min_depth, int64_t N,
+                              const uint64_t *seed_dev, int *choose, int *valid_count, void *workspace,
+                              size_t workspace_bytes, ffb6d_stream_t stream);
 
 /*
  * Depth completion of the raw sensor depth, replacing the CPU call
@@ -755,6 +760,15 @@ int ffb6d_grid_subsample_host(const float *points, size_t N,
 int ffb6d_rgb_add_noise(const uint8_t *rgb, int64_t B, int64_t H, int64_t W,
                         const double *plan_host, const double *plan_dev, uint64_t seed, const double *noise,
                         uint8_t *out, uint8_t *work, ffb6d_stream_t stream);
+/* ffb6d_rgb_add_noise with the seed read on the device from seed_dev (one uint64, 8-byte aligned): a captured
+ * CUDA graph takes a new seed per replay.  Same checks; for equal seed values, the same bits. */
+int ffb6d_rgb_add_noise_dseed(const uint8_t *rgb, int64_t B, int64_t H, int64_t W,
+                              const double *plan_host, const double *plan_dev, const uint64_t *seed_dev,
+                              const double *noise, uint8_t *out, uint8_t *work, ffb6d_stream_t stream);
+/* The record checks of ffb6d_rgb_add_noise alone, on the host, without a launch: plan_host [B,REC_LEN] f64,
+ * 0 <= B < 65536.  0 or FFB6D_ERR_INVALID with ffb6d_rgb_add_noise's ffb6d_last_error() text for a bad record.
+ * A caller that replays a captured call (whose records are copied to plan_dev) checks each batch with it. */
+int ffb6d_rgb_noise_check_records(const double *plan_host, int64_t B);
 int ffb6d_add_real_back(const uint8_t *rgb, const uint8_t *labels, const uint16_t *dpt,
                         const uint8_t *back_rgb, const uint8_t *back_labels, int back_label_channels,
                         const uint16_t *back_dpt, const uint8_t *mode, int dataset,
@@ -781,6 +795,9 @@ int ffb6d_aug_noise_field(uint64_t seed, int64_t B, int64_t H, int64_t W, int st
 int ffb6d_color_jitter(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, const double *plan_host,
                        const double *plan_dev, const uint8_t *active, uint8_t *out, int64_t *work,
                        ffb6d_stream_t stream);
+/* The plan checks of ffb6d_color_jitter alone, on the host, without a launch: plan_host [B,FFB6D_JITTER_PLAN_LEN]
+ * f64, 1 <= B < 65536.  0 or FFB6D_ERR_INVALID with ffb6d_color_jitter's ffb6d_last_error() text for a bad plan. */
+int ffb6d_color_jitter_check_plans(const double *plan_host, int64_t B);
 
 /*
  * FFB6D's training loss (models/loss.py:12-90, combined as train_ycb.py:237-253): FocalLoss and the offset L1 loss
