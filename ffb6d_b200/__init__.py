@@ -47,6 +47,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   ``get_item`` (:func:`build_ffb6d_inputs`, no labels), the ``FFB6D`` eval forward and the voting, as the
   reference's ``demo.py`` composes them; :class:`GraphedPoseStep` -- all of it captured in one CUDA graph and
   replayed per batch.
+* :class:`GraphedTestStep` (:mod:`ffb6d_b200.evaluate`) -- one batch of the reference's test (the eval ``get_item``,
+  the forward, the loss, the vote, ADD / ADD-S and a device record of every object) replayed from one CUDA graph,
+  and the AUC tables of the run computed on the GPU (:func:`eval_record`, :func:`eval_auc`).
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -65,17 +68,18 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax",
         "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d",
         "farthest_point_sampling", "pose_add_adds", "vote_poses", "point_input", "rgb_noise_check_records",
-        "color_jitter_check_plans")
+        "color_jitter_check_plans", "eval_record", "eval_auc")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item", "build_ffb6d_inputs", "build_ffb6d_train_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")
 _ITEM = ("pose_gt_objects",)
 _GRAPHED = ("GraphedTrainStep", "GraphedEvalStep", "GraphedFrameTrainStep")
 _ESTIMATE = ("estimate_poses", "GraphedPoseStep")
+_EVALUATE = ("GraphedTestStep",)
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "estimate", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "estimate", "evaluate", "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED + _ESTIMATE) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "estimate", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED + _ESTIMATE + _EVALUATE) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "estimate", "evaluate", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched
@@ -91,6 +95,8 @@ def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op t
         return getattr(importlib.import_module(".graphed", __name__), name)
     if name in _ESTIMATE:
         return getattr(importlib.import_module(".estimate", __name__), name)
+    if name in _EVALUATE:
+        return getattr(importlib.import_module(".evaluate", __name__), name)
     if name == "DataProcessing":
         return importlib.import_module(".helper_tool", __name__).DataProcessing
     if name in _SUBMODULES:

@@ -30,7 +30,9 @@ POSE_EVAL_PRED_TILE = 512
 POSE_EVAL_MAX_OBJECTS = 65535
 POSE_EVAL_MAX_POINTS = 1 << 20
 POSE_EVAL_MAX_MESHES = (1 << 31) - 2
-VOTE_MAX_POINTS = (1 << 24) - 1                  # FFB6D_VOTE_* of include/ffb6d_b200.h
+EVAL_ROW_WORDS = 20                              # FFB6D_EVAL_* of include/ffb6d_b200.h
+EVAL_MAX_ROWS = 1 << 24
+VOTE_MAX_POINTS =(1 << 24) - 1                  # FFB6D_VOTE_* of include/ffb6d_b200.h
 VOTE_MAX_CLASSES = 1024
 VOTE_MAX_KPS = 64
 VOTE_MAX_SETS = 1 << 24
@@ -159,7 +161,11 @@ def _load():
         "ffb6d_farthest_point_sampling": (ci, [vp, vp, i64, i64, i64, vp, ci, vp, vp, sz, vp]),
         "ffb6d_pose_add_adds_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_pose_add_adds": (ci, [vp, vp, i64, i64, vp, vp, vp, i64, vp, vp, vp, sz, vp]),
-        "ffb6d_project_p3d": (ci, [vp, ci, i64, vp, vp, vp, i64, i64, vp, vp, vp, ci, vp, vp]),
+        "ffb6d_eval_record": (ci, [vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i64, i64, i64, i64, i64, vp, i64, vp, vp,
+                                   vp, i64, vp]),
+        "ffb6d_eval_auc_workspace_bytes": (sz, [i64, i64]),
+        "ffb6d_eval_auc": (ci, [vp, vp, i64, i64, vp, C.c_double, vp, vp, vp, vp, sz, vp]),
+        "ffb6d_project_p3d":(ci, [vp, ci, i64, vp, vp, vp, i64, i64, vp, vp, vp, ci, vp, vp]),
         "ffb6d_draw_p2ds_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_draw_p2ds": (ci, [vp, i64, i64, i64, vp, i64, i64, vp, vp, vp, vp, i64, vp, vp, ci, vp, sz, vp]),
         "ffb6d_grid_subsample_host": (ci, [vp, sz, vp, sz, vp, sz, fp, vp, vp, vp, C.POINTER(sz)]),

@@ -1149,6 +1149,112 @@ def pose_add_adds(mesh_pts, mesh_off, obj_mesh, pred_RT, gt_RT, max_points):
     return add, adds
 
 
+def _u8(t, name, shape, dev):
+    if torch.is_tensor(t) and t.dtype == torch.bool:
+        t = t.view(torch.uint8)
+    return _tensor(t, name, torch.uint8, shape, dev)
+
+
+def _written(*ts):
+    for t in ts:
+        if not t.is_contiguous():
+            raise ValueError("the record table's tensors are written in place and must be contiguous")
+
+
+def eval_record(rows, state, cls_ids, present, pred_RT, add, adds, kps=None, gt_kps=None, valid=None, obj_id=0,
+                poses=None, frame_poses=None, frame_flags=None):
+    """One batch of a test run into the device record table (``ffb6d_eval_record``, see include/ffb6d_b200.h):
+    slot ``(b, j)`` becomes row ``state[0] + b * n_obj + j``, and ``state`` advances on the device.
+
+    :param rows: ``[capacity, EVAL_ROW_WORDS]`` int32; :param state: ``[4]`` int64 (rows used, frames, overflow)
+    :param cls_ids: ``[B, n_obj]`` int32 class ids (YCB; LineMOD reads only the shape)
+    :param present: ``[B, n_cls]`` bool / uint8 from the vote; :param pred_RT: the scored float32 poses, ``[B, n_obj,
+      3, 4]`` (YCB) or ``[B, 3, 4]`` (LineMOD); :param add, adds: their float32 scores, ``[B * n_obj]`` or ``[B]``
+    :param kps: ``[B, n_cls, n_kps + 1, 3]`` float32 vote keypoints, :param gt_kps: ``[B, n_obj, n_kps, 3]`` float32
+      (YCB)
+    :param valid: ``[B]`` bool, or None; :param obj_id: 0 for YCB, the LineMOD object's id otherwise
+    :param poses: ``[B, n_cls, 3, 4]`` float64, with ``frame_poses [F, n_cls, 3, 4]`` float64 and ``frame_flags
+      [F, n_cls]`` uint8: the optional frame table.
+    No host synchronisation; capturable in a CUDA graph."""
+    rw = _tensor(rows, "rows", torch.int32, 2)
+    dev = rw.device
+    if rw.shape[1] != _lib.EVAL_ROW_WORDS:
+        raise ValueError("rows must be [capacity, %d], got %s" % (_lib.EVAL_ROW_WORDS, tuple(rw.shape)))
+    st = _tensor(state, "state", torch.int64, (4,), dev)
+    _written(rows, state)
+    ids = _tensor(cls_ids, "cls_ids", torch.int32, 2, dev)
+    B, n_obj = ids.shape
+    pres = _u8(present, "present", 2, dev)
+    n_cls = pres.shape[1]
+    if pres.shape[0] != B:
+        raise ValueError("present must be [B=%d, n_cls], got %s" % (B, tuple(pres.shape)))
+    if isinstance(obj_id, bool) or not isinstance(obj_id, (int, np.integer)) or obj_id < 0:
+        raise ValueError("obj_id must be an int >= 0, got %r" % (obj_id,))
+    lm = obj_id > 0
+    pr = _tensor(pred_RT, "pred_RT", torch.float32, (B, 3, 4) if lm else (B, n_obj, 3, 4), dev)
+    a = _tensor(add, "add", torch.float32, (B if lm else B * n_obj,), dev)
+    s = _tensor(adds, "adds", torch.float32, (B if lm else B * n_obj,), dev)
+    k = g = None
+    R = n_kps = 0
+    if not lm:
+        if kps is None or gt_kps is None:
+            raise ValueError("a YCB record needs kps and gt_kps")
+        k = _tensor(kps, "kps", torch.float32, 4, dev)
+        g = _tensor(gt_kps, "gt_kps", torch.float32, 4, dev)
+        R, n_kps = k.shape[2], g.shape[2]
+        if tuple(k.shape) != (B, n_cls, R, 3) or tuple(g.shape) != (B, n_obj, n_kps, 3) or R != n_kps + 1:
+            raise ValueError("kps must be [B,n_cls,n_kps+1,3] and gt_kps [B,n_obj,n_kps,3] = [%d,%d,n_kps,3], got %s "
+                             "and %s" % (B, n_obj, tuple(k.shape), tuple(g.shape)))
+    v = None if valid is None else _u8(valid, "valid", (B,), dev)
+    fp = ff = ps = None
+    F_cap = 0
+    if frame_poses is not None or frame_flags is not None:
+        ff = _u8(frame_flags, "frame_flags", 2, dev)
+        F_cap = ff.shape[0]
+        fp = _tensor(frame_poses, "frame_poses", torch.float64, (F_cap, n_cls, 3, 4), dev)
+        ps = _tensor(poses, "poses", torch.float64, (B, n_cls, 3, 4), dev)
+        _written(frame_poses, frame_flags)
+        if ff.shape[1] != n_cls:
+            raise ValueError("frame_flags must be [F, n_cls=%d], got %s" % (n_cls, tuple(ff.shape)))
+    launch(lib.ffb6d_eval_record, dev, ptr(ids), ptr(v), pres.data_ptr(), ptr(k), ptr(ps), ptr(g), pr.data_ptr(),
+           a.data_ptr(), s.data_ptr(), B, n_obj, n_cls, R, n_kps, int(obj_id), rw.data_ptr(), rw.shape[0],
+           st.data_ptr(), ptr(fp), ptr(ff), F_cap)
+
+
+def eval_auc(rows, state, n_cls, sym=None, lm_thr=0.0, ws=None):
+    """The summary of a record table (``ffb6d_eval_auc``): ``(auc [3, n_cls], pct [2, n_cls], kp [2])`` float64
+    CUDA tensors -- the ADD, ADD-S and ADD(-S) AUCs per class in percent (class 0 over every object), the
+    percentages of ADD and ADD-S below ``lm_thr`` and the keypoint-error sum and count over the first ``state[0]``
+    rows.  ``sym``: ``[n_cls]`` bool / uint8 CUDA (ADD-S for ADD(-S)), or None.  ``ws``: a workspace of at least
+    :func:`eval_auc_workspace_bytes` bytes, or None to allocate one.  No host synchronisation."""
+    rw = _tensor(rows, "rows", torch.int32, 2)
+    dev = rw.device
+    if rw.shape[1] != _lib.EVAL_ROW_WORDS:
+        raise ValueError("rows must be [capacity, %d], got %s" % (_lib.EVAL_ROW_WORDS, tuple(rw.shape)))
+    st = _tensor(state, "state", torch.int64, (4,), dev)
+    n_cls = int(n_cls)
+    sy = None if sym is None else _u8(sym, "sym", (n_cls,), dev)
+    auc = torch.empty((3, n_cls), dtype=torch.float64, device=dev)
+    pct = torch.empty((2, n_cls), dtype=torch.float64, device=dev)
+    kp = torch.empty(2, dtype=torch.float64, device=dev)
+    nbytes = eval_auc_workspace_bytes(rw.shape[0], n_cls)
+    if ws is None:
+        ws = torch.empty(nbytes + 256, dtype=torch.uint8, device=dev)
+    off = -ws.data_ptr() % 256
+    launch(lib.ffb6d_eval_auc, dev, rw.data_ptr(), st.data_ptr(), rw.shape[0], n_cls, ptr(sy), float(lm_thr),
+           auc.data_ptr(), pct.data_ptr(), kp.data_ptr(), ws.data_ptr() + off, ws.numel() - off)
+    return auc, pct, kp
+
+
+def eval_auc_workspace_bytes(capacity, n_cls):
+    """Bytes :func:`eval_auc` needs for a table of ``capacity`` rows; raises ``ValueError`` outside the limits."""
+    nbytes = int(lib.ffb6d_eval_auc_workspace_bytes(int(capacity), int(n_cls)))
+    if nbytes == 0:
+        raise ValueError("eval_auc: need 1 <= capacity <= %d and 1 <= n_cls <= %d, got %d and %d"
+                         % (_lib.EVAL_MAX_ROWS, _lib.VOTE_MAX_CLASSES, capacity, n_cls))
+    return nbytes
+
+
 def _set_table(start, count, enable, dev):
     st = _tensor(start, "start", torch.int32, 1, dev)
     S = st.shape[0]

@@ -362,6 +362,70 @@ def eval_metric_lm(cls_ids, pred_pose_lst, RTs, mask, label, obj_id, *, mesh_tab
     return cls_add_dis, cls_adds_dis
 
 
+def _ycb_scores(mesh_table, vote_table, pclds, masks, ctr_ofs, kp_ofs, cls_ids, RTs, use_ctr, use_ctr_clus_flter):
+    """The device half of a YCB batch of :meth:`TorchEval.eval_pose_parallel`: the vote, each ground-truth object's
+    predicted pose (zero for a class the vote did not find) and its ADD / ADD-S.  Returns ``(votes, ids [B,n_obj]
+    int32, pred [B*n_obj,3,4] float32, add, adds)``; no host synchronisation."""
+    bs, n_obj = RTs.shape[0], RTs.shape[1]
+    dev = mesh_table.device
+    gt = RTs.reshape(bs * n_obj, 3, 4).to(dev, torch.float32)
+    votes = _vote(vote_table, pclds, masks, ctr_ofs, kp_ofs, use_ctr, use_ctr_clus_flter,
+                  use_ctr_clus_flter and vote_table.refine_thr is not None)
+    poses = votes[3]
+    ids = torch.as_tensor(cls_ids).to(dev).reshape(bs, n_obj, -1)[:, :, 0].long()
+    ok = (ids >= 0) & (ids < vote_table.n_cls)
+    pick = torch.where(ok, ids, 0)
+    pred = poses[torch.arange(bs, device=dev)[:, None], pick].float()     # absent classes: zero rows
+    pred = torch.where(ok[..., None, None], pred, 0.0).reshape(bs * n_obj, 3, 4).contiguous()
+    om = ids.clamp(-1, 2 ** 31 - 1).int()                      # an id without a mesh scores NaN
+    add, adds = ops.pose_add_adds(mesh_table.pts, mesh_table.off, om.reshape(-1), pred, gt.contiguous(),
+                                  mesh_table.max_points)
+    return votes, om, pred, add, adds
+
+
+def _ycb_record(rows, state, votes, ids, pred, add, adds, gt_kps, valid=None, frame_poses=None, frame_flags=None):
+    present, _, kps, poses = votes
+    bs, n_obj = ids.shape
+    gk = torch.as_tensor(gt_kps).to(kps.device, torch.float32)
+    ops.eval_record(rows, state, ids, present, pred.reshape(bs, n_obj, 3, 4), add, adds, kps=kps, gt_kps=gk,
+                    valid=valid, poses=poses if frame_poses is not None else None, frame_poses=frame_poses,
+                    frame_flags=frame_flags)
+
+
+def _lm_scores(mesh_table, lm_table, obj_id, pclds, masks, ctr_ofs, kp_ofs, RTs, use_ctr, use_ctr_clus_flter):
+    """The device half of a LineMOD batch: the two-class vote on ``masks == 1``, the object's predicted pose (the
+    identity where the vote found no point) and its ADD / ADD-S.  Returns ``(votes, pred [B,3,4], add, adds)``."""
+    bs, n_obj = RTs.shape[0], RTs.shape[1]
+    dev = mesh_table.device
+    gt = RTs.reshape(bs, n_obj, 3, 4)[:, 0].to(dev, torch.float32).contiguous()
+    votes = _vote(lm_table, pclds, masks == 1, ctr_ofs, kp_ofs, use_ctr, use_ctr_clus_flter, False)
+    present, poses = votes[0], votes[3]
+    eye = torch.eye(3, 4, dtype=torch.float32, device=dev)
+    pred = torch.where(present[:, 1, None, None], poses[:, 1].float(), eye).contiguous()
+    om = torch.full((bs,), obj_id, dtype=torch.int32, device=dev)
+    add, adds = ops.pose_add_adds(mesh_table.pts, mesh_table.off, om, pred, gt, mesh_table.max_points)
+    return votes, pred, add, adds
+
+
+def _lm_record(rows, state, votes, obj_id, n_obj, pred, add, adds, valid=None):
+    bs = pred.shape[0]
+    ids = torch.zeros((bs, n_obj), dtype=torch.int32, device=pred.device)      # read for its shape only
+    ops.eval_record(rows, state, ids, votes[0], pred, add, adds, valid=valid, obj_id=obj_id)
+
+
+def _append_rows(rows, cls_add_dis, cls_adds_dis, kp_errs=None):
+    """Append the host record rows ``rows [n, EVAL_ROW_WORDS]`` int32 to the per-class lists in row order: every
+    object to its class's list and to list 0, its keypoint error (with ``kp_errs``) to its class's."""
+    vals = rows.view(np.float32)
+    for r in np.flatnonzero(rows[:, 0] != -1):
+        cid = int(rows[r, 0])
+        if kp_errs is not None:
+            kp_errs[cid].append(float(vals[r, 5]))
+        for i in (cid, 0):
+            cls_add_dis[i].append(float(vals[r, 3]))
+            cls_adds_dis[i].append(float(vals[r, 4]))
+
+
 class TorchEval:
     """The reference's ``TorchEval`` (pvn3d_eval_utils_kpls.py:326-505): per-class ADD / ADD-S lists over a test run
     and their AUCs.
@@ -399,48 +463,30 @@ class TorchEval:
         """Vote and score one batch (pvn3d_eval_utils_kpls.py:448-500), appending to the per-class lists.  ``rgbs``,
         ``gt_ctr_ofs``, ``labels``, ``cnt``, ``min_cnt`` and ``merge_clus`` are accepted and unread, as in the
         reference.  One :func:`cal_batch_poses` call votes the batch, each ground-truth object's predicted pose is
-        taken on the device, one :func:`ffb6d_b200.ops.pose_add_adds` launch scores every object, and one
-        device-to-host copy brings back what the lists need."""
+        taken on the device, one :func:`ffb6d_b200.ops.pose_add_adds` launch scores every object, one
+        :func:`ffb6d_b200.ops.eval_record` launch lays the objects out as the lists take them (with their keypoint
+        errors), and one device-to-host copy brings back what the lists need."""
         bs, n_obj = RTs.shape[0], RTs.shape[1]
         dev = self.mesh_table.device
-        gt = RTs.reshape(bs * n_obj, 3, 4).to(dev, torch.float32)
+        rows = torch.empty((bs * n_obj, _lib.EVAL_ROW_WORDS), dtype=torch.int32, device=dev)
+        state = torch.zeros(4, dtype=torch.int64, device=dev)
         if ds == "ycb":
             n_kps = pred_kp_ofs.shape[1]
-            present, count, kps, poses = _vote(self.vote_table, pclds, masks, pred_ctr_ofs, pred_kp_ofs, use_ctr,
-                                               use_ctr_clus_flter,
-                                               use_ctr_clus_flter and self.vote_table.refine_thr is not None)
-            ids = torch.as_tensor(cls_ids).to(dev).reshape(bs, n_obj, -1)[:, :, 0].long()
-            ok = (ids >= 0) & (ids < self.n_cls)
-            pick = torch.where(ok, ids, 0)
-            pred = poses[torch.arange(bs, device=dev)[:, None], pick].float()     # absent classes: zero rows
-            pred = torch.where(ok[..., None, None], pred, 0.0).reshape(bs * n_obj, 3, 4)
-            om = ids.clamp(-1, 2 ** 31 - 1).int().reshape(-1)        # an id without a mesh scores NaN
-            add, adds = ops.pose_add_adds(self.mesh_table.pts, self.mesh_table.off, om,
-                                          pred.contiguous(), gt.contiguous(), self.mesh_table.max_points)
-            add, adds, poses, kps, count, present, ids_h, gt_kps_h, has = _to_host(
-                add, adds, poses, kps, count, present, ids, torch.as_tensor(gt_kps).to(dev), self.vote_table.has_mesh)
+            votes, ids, pred, add, adds = _ycb_scores(self.mesh_table, self.vote_table, pclds, masks, pred_ctr_ofs,
+                                                      pred_kp_ofs, cls_ids, RTs, use_ctr, use_ctr_clus_flter)
+            _ycb_record(rows, state, votes, ids, pred, add, adds, gt_kps)
+            present, count, kps, poses = votes
+            rows, poses, kps, count, present, has = _to_host(rows, poses, kps, count, present,
+                                                             self.vote_table.has_mesh)
             for b in range(bs):
-                pred_cls_ids, pred_poses, pred_kpcs = _frame_lists(present[b], count[b], kps[b], poses[b], has, n_kps)
+                pred_cls_ids, pred_poses, _ = _frame_lists(present[b], count[b], kps[b], poses[b], has, n_kps)
                 self.pred_id2pose_lst.append({cid: pose for cid, pose in zip(pred_cls_ids, pred_poses)})
-                c, _, errs = _frame_objects(ids_h[b], pred_poses, pred_cls_ids, gt_kps_h[b], pred_kpcs)
-                for j, cid in enumerate(c):
-                    self.pred_kp_errs[cid].append(errs[j])
-                    for i in (cid, 0):
-                        self.cls_add_dis[i].append(float(add[b * n_obj + j]))
-                        self.cls_adds_dis[i].append(float(adds[b * n_obj + j]))
         else:
-            present, _, _, poses = _vote(self.lm_tables[int(obj_id)], pclds, masks == 1, pred_ctr_ofs, pred_kp_ofs,
-                                         use_ctr, use_ctr_clus_flter, False)
-            eye = torch.eye(3, 4, dtype=torch.float32, device=dev)
-            pred = torch.where(present[:, 1, None, None], poses[:, 1].float(), eye)      # no point: the identity
-            om = torch.full((bs,), int(obj_id), dtype=torch.int32, device=dev)
-            add, adds = ops.pose_add_adds(self.mesh_table.pts, self.mesh_table.off, om, pred.contiguous(),
-                                          gt.reshape(bs, n_obj, 3, 4)[:, 0].contiguous(), self.mesh_table.max_points)
-            add, adds = _to_host(add, adds)
-            for b in range(bs):
-                for i in (int(obj_id), 0):
-                    self.cls_add_dis[i].append(float(add[b]))
-                    self.cls_adds_dis[i].append(float(adds[b]))
+            votes, pred, add, adds = _lm_scores(self.mesh_table, self.lm_tables[int(obj_id)], int(obj_id), pclds,
+                                                masks, pred_ctr_ofs, pred_kp_ofs, RTs, use_ctr, use_ctr_clus_flter)
+            _lm_record(rows, state, votes, int(obj_id), n_obj, pred, add, adds)
+            rows, = _to_host(rows)
+        _append_rows(rows, self.cls_add_dis, self.cls_adds_dis, self.pred_kp_errs if ds == "ycb" else None)
 
     def _add_s_lists(self, cls_range):
         self.cls_add_s_dis = [[] for _ in range(self.n_cls)]

@@ -662,6 +662,57 @@ int ffb6d_pose_add_adds(const float *mesh_pts, const int32_t *mesh_off, int64_t 
                         const int32_t *obj_mesh, const float *pred_RT, const float *gt_RT, int64_t M, float *add,
                         float *adds, void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
 
+/* ---- the test run's record and summary ------------------------------------ */
+/*
+ * The per-object lists of the reference's TorchEval (utils/pvn3d_eval_utils_kpls.py:326-505) as a device table, and
+ * its summary (cal_auc / cal_lm_add over Basic_Utils.cal_auc, utils/basic_utils.py:642-649), DESIGN.md §4.29.
+ *
+ * The table: rows [capacity, FFB6D_EVAL_ROW_WORDS] int32 and state [4] int64 (device, zeroed by the caller to start
+ * a run): state[0] the rows used, state[1] the frames recorded, state[2] the overflow flag.  A row's words:
+ *   0 class id (int32), or -1 for a skipped slot; 1 frame index (state[1] at the batch + b); 2 the class was
+ *   predicted (0 / 1); 3 ADD, 4 ADD-S, 5 keypoint error (float32 bits); 6..17 the scored predicted pose [3,4]
+ *   (float32 bits); 18, 19 zero.
+ *
+ * ffb6d_eval_record: one batch of B frames x n_obj object slots; slot (b, j) is written to row state[0] + b n_obj + j
+ * (the reference's list order, with no atomic in it), then state[0] += B n_obj and state[1] += B.  A slot is skipped
+ * when valid[b] == 0 (valid [B] u8, or NULL: every frame), and
+ *   YCB (obj_id = 0): from the frame's first zero cls_ids[b, j] on (cls_ids [B, n_obj] int32); the slot's class
+ *     c = cls_ids[b, j] is predicted when 0 <= c < n_cls and present[b, c] (present [B, n_cls] u8, the vote's); its
+ *     keypoint error is mean_k |gt_kps[b, j, k] - kps[b, c, k]| in f32 (kps [B, n_cls, R, 3] f32 with R >= n_kps + 1,
+ *     gt_kps [B, n_obj, n_kps, 3] f32; kps = 0 when c was not predicted); add, adds [B, n_obj] f32 and pred_RT
+ *     [B, n_obj, 3, 4] f32 are placed as given;
+ *   LineMOD (obj_id > 0): every slot but 0, which gets class obj_id, presence present[b, 1], add[b], adds[b],
+ *     pred_RT[b] and keypoint error 0; cls_ids, kps and gt_kps are unread (may be NULL).
+ * The frame table (optional; both or neither): frame_flags [frame_capacity, n_cls] u8 gets present[b, c] | 2 valid[b]
+ * and frame_poses [frame_capacity, n_cls, 3, 4] f64 the vote's poses [B, n_cls, 3, 4] at frame state[1] + b.
+ * If the batch does not fit (state[0] + B n_obj > capacity, or state[1] + B > frame_capacity with the frame table),
+ * nothing is written but state[2] = 1.  One launch (one CTA).
+ *
+ * ffb6d_eval_auc: over the rows r < min(state[0], capacity) whose class c lies in [1, n_cls):
+ *   auc [3, n_cls] f64: cal_auc of ADD, ADD-S and ADD(-S) (ADD-S where sym[c] != 0, sym [n_cls] u8 or NULL) per
+ *     class, class 0 over every counted row: distances > 0.1 are misses (exactly 0.1 counts), the accuracy is the f32
+ *     cumulative count over n, the area is VOCap's in f64, times 1000; no distance gives 0, a NaN distance NaN;
+ *   pct [2, n_cls] f64: the percentage of ADD, ADD-S < lm_thr per class (cal_lm_add; NaN for an empty class);
+ *   kp [2] f64: the sum of the rows' keypoint errors and their count (mean_kp_err).
+ * The distances are ordered with CUB's radix sort; every sum runs in fp64 in a fixed order (deterministic).
+ * workspace: ffb6d_eval_auc_workspace_bytes(capacity, n_cls) bytes, 256-byte aligned.  Four launches.
+ *
+ * Both: 1 <= capacity, frame_capacity <= FFB6D_EVAL_MAX_ROWS; 1 <= n_cls <= FFB6D_VOTE_MAX_CLASSES; B n_obj <=
+ * FFB6D_POSE_EVAL_MAX_OBJECTS; YCB 1 <= n_kps <= FFB6D_VOTE_MAX_KPS.  Arguments are checked before any launch
+ * (FFB6D_ERR_INVALID); no allocation, no host synchronisation (capturable in a CUDA graph).
+ */
+#define FFB6D_EVAL_ROW_WORDS 20
+#define FFB6D_EVAL_MAX_ROWS (1 << 24)
+int ffb6d_eval_record(const int32_t *cls_ids, const uint8_t *valid, const uint8_t *present, const float *kps,
+                      const double *poses, const float *gt_kps, const float *pred_RT, const float *add,
+                      const float *adds, int64_t B, int64_t n_obj, int64_t n_cls, int64_t R, int64_t n_kps,
+                      int64_t obj_id, int32_t *rows, int64_t capacity, int64_t *state, double *frame_poses,
+                      uint8_t *frame_flags, int64_t frame_capacity, ffb6d_stream_t stream);
+size_t ffb6d_eval_auc_workspace_bytes(int64_t capacity, int64_t n_cls);
+int ffb6d_eval_auc(const int32_t *rows, const int64_t *state, int64_t capacity, int64_t n_cls, const uint8_t *sym,
+                   double lm_thr, double *auc, double *pct, double *kp, void *workspace, size_t workspace_bytes,
+                   ffb6d_stream_t stream);
+
 /* ---- pose and label drawing ---------------------------------------------- */
 /*
  * Projection and drawing of S point sets, replacing Basic_Utils.project_p3d and draw_p2ds (utils/basic_utils.py:
