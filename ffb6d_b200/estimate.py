@@ -25,62 +25,14 @@ completed depth, see INTEGRATION.md).
 import torch
 
 from . import pose as _pose
-from .graphed import _GraphedStep
-from .model import FFB6D, FFB6DFusionNet
+from .graphed import _GraphedEvalBase, _check_image_branch
 from .ops import _frame_intrinsics, _intrinsics_arg
-from .schedule import build_ffb6d_inputs
+from .schedule import build_ffb6d_inputs, check_dataset, check_frame_batch
 
 # the reference's config.n_sample_points (common.py:61)
 N_SAMPLE_POINTS = 480 * 640 // 24
 
-# dataset -> depth completion of the raw depth (the datasets' get_item)
-_FILL = {"ycb": True, "linemod": False}
 _FRAME_KEYS = ("dpt", "rgb", "nrm_map")
-_OPTIONAL_KEYS = ("K",)
-
-
-def _dataset_fill(dataset):
-    if dataset not in _FILL:
-        raise ValueError("dataset must be 'ycb' or 'linemod', got %r" % (dataset,))
-    return _FILL[dataset]
-
-
-def _check_frames(frames, name):
-    """``ValueError`` unless ``frames`` is a dict of the expected CUDA tensors (checked before any CUDA work)."""
-    if not isinstance(frames, dict):
-        raise ValueError("%s: frames must be a dict, got %s" % (name, type(frames).__name__))
-    missing = [k for k in _FRAME_KEYS if k not in frames]
-    if missing:
-        raise ValueError("%s: frames lack %s (they need %s)" % (name, missing, list(_FRAME_KEYS)))
-    unknown = sorted(str(k) for k in frames if k not in _FRAME_KEYS + _OPTIONAL_KEYS)
-    if unknown:
-        raise ValueError("%s: unknown frame keys %s (known: %s)" % (name, unknown, list(_FRAME_KEYS + _OPTIONAL_KEYS)))
-    for k, t in frames.items():
-        if not isinstance(t, torch.Tensor):
-            raise ValueError("%s: frames[%r] must be a tensor, got %s" % (name, k, type(t).__name__))
-    dpt, rgb, nrm = frames["dpt"], frames["rgb"], frames["nrm_map"]
-    if dpt.dtype != torch.uint16 or dpt.dim() != 3:
-        raise ValueError("%s: frames['dpt'] must be uint16 [B,H,W], got %s %s" % (name, dpt.dtype, tuple(dpt.shape)))
-    B, H, W = dpt.shape
-    if rgb.dtype != torch.uint8 or tuple(rgb.shape) != (B, H, W, 3):
-        raise ValueError("%s: frames['rgb'] must be uint8 [B,H,W,3] = %s, got %s %s"
-                         % (name, (B, H, W, 3), rgb.dtype, tuple(rgb.shape)))
-    if nrm.dtype not in (torch.float32, torch.float64) or tuple(nrm.shape) != (B, H, W, 3):
-        raise ValueError("%s: frames['nrm_map'] must be float32 or float64 [B,H,W,3] = %s, got %s %s"
-                         % (name, (B, H, W, 3), nrm.dtype, tuple(nrm.shape)))
-    if "K" in frames and (frames["K"].dtype != torch.float64 or tuple(frames["K"].shape) != (B, 3, 3)):
-        raise ValueError("%s: frames['K'] must be float64 [B,3,3] = %s, got %s %s"
-                         % (name, (B, 3, 3), frames["K"].dtype, tuple(frames["K"].shape)))
-    for k, t in frames.items():
-        if not t.is_cuda or t.device != dpt.device:
-            raise ValueError("%s: frames[%r] is on %s; every frame tensor must be on one CUDA device (dpt: %s)"
-                             % (name, k, t.device, dpt.device))
-
-
-def _check_model(model, name):
-    if isinstance(model, FFB6DFusionNet) and not isinstance(model, FFB6D):
-        raise ValueError("%s: an FFB6DFusionNet has no image branch; pose estimation from frames needs the whole "
-                         "FFB6D" % name)
 
 
 def vote_table(dataset, mesh_kps, n_cls, cls_radius=None, device=None):
@@ -119,17 +71,14 @@ def forward_and_vote(model, item, dataset, mesh_kps, cls_radius=None):
 def _estimate(model, frames, dataset, cam_scale, intr, table, n_points, seed):
     """One estimate from checked frames, with device intrinsics ``intr`` and a device vote table."""
     item = build_ffb6d_inputs(frames["dpt"], cam_scale, intr, frames["rgb"], frames["nrm_map"], n_points, seed=seed,
-                              fill=_FILL[dataset])
+                              fill=dataset == "ycb")
     item["rgb"] = item["rgb"].to(torch.float32)             # model_fn's cast of the uint8 image
     _, _, (present, count, kps, poses) = forward_and_vote(model, item, dataset, table)
     return dict(present=present, count=count, kps=kps, poses=poses, valid=item["valid"])
 
 
-def _prepare(model, frames, dataset, K, mesh_kps, cls_radius, name):
-    """Checks, then the device intrinsics (None with per-frame ``frames['K']``) and the device vote table."""
-    _dataset_fill(dataset)
-    _check_model(model, name)
-    _check_frames(frames, name)
+def _prepare(model, frames, dataset, K, mesh_kps, cls_radius):
+    """The device intrinsics (None with per-frame ``frames['K']``) and the device vote table of checked frames."""
     dev = frames["dpt"].device
     intr = None if "K" in frames else _intrinsics_arg(K, frames["dpt"].shape[0], dev)[0]
     table = vote_table(dataset, mesh_kps, getattr(getattr(model, "module", model), "n_cls", None), cls_radius, dev)
@@ -159,14 +108,17 @@ def estimate_poses(model, frames, *, dataset, cam_scale, K, mesh_kps, cls_radius
 
     With ``K`` as device intrinsics (or ``frames['K']``) and ``mesh_kps`` a ``VoteTable``, the call makes no host
     synchronisation; a host ``K`` or a mapping is first copied to the device, which synchronises."""
-    intr, table = _prepare(model, frames, dataset, K, mesh_kps, cls_radius, "estimate_poses")
+    check_dataset(dataset, "estimate_poses")
+    _check_image_branch(model, "estimate_poses")
+    check_frame_batch(frames, "estimate_poses", _FRAME_KEYS)
+    intr, table = _prepare(model, frames, dataset, K, mesh_kps, cls_radius)
     model.eval()
     if intr is None:
         intr = _frame_intrinsics(frames["K"])
     return _estimate(model, frames, dataset, cam_scale, intr, table, n_points, seed)
 
 
-class GraphedPoseStep(_GraphedStep):
+class GraphedPoseStep(_GraphedEvalBase):
     """:func:`estimate_poses` captured in one CUDA graph and replayed per batch: the depth completion (YCB), the
     sampling, the 22 searches, the point features, the ``FFB6D`` eval forward, the argmax and the vote.
 
@@ -191,45 +143,21 @@ class GraphedPoseStep(_GraphedStep):
     frames whose keys, shapes, dtypes or devices differ from the example's.
     """
 
-    _wrapper_hint = "pass its .module"
+    _needs_image_branch = True
 
     def __init__(self, model, example_frames, *, dataset, cam_scale, K, mesh_kps, cls_radius=None,
                  n_points=N_SAMPLE_POINTS, seed=0, warmup=3):
+        name = type(self).__name__
+        check_dataset(dataset, name)
         self._check_model(model)
-        self._intr, self._table = _prepare(model, example_frames, dataset, K, mesh_kps, cls_radius,
-                                           type(self).__name__)
+        check_frame_batch(example_frames, name, _FRAME_KEYS)
+        self._intr, self._table = _prepare(model, example_frames, dataset, K, mesh_kps, cls_radius)
         self.dataset, self.cam_scale, self.n_points, self.seed = dataset, cam_scale, int(n_points), int(seed)
         self._keys = set(example_frames)
-        self._out = None
         super().__init__(model, example_frames, warmup)
-
-    def _check(self, modules=False):
-        """What cannot be captured at all: raise ``ValueError`` before any CUDA work."""
-        if self.model.training:
-            raise ValueError("GraphedPoseStep: the model is in training mode; call model.eval() first")
-        self._refuse_index_check()
 
     def _step(self):
         frames = self._static
         intr = _frame_intrinsics(frames["K"]) if "K" in frames else self._intr
         return _estimate(self.model, frames, self.dataset, self.cam_scale, intr, self._table, self.n_points,
                          self.seed)
-
-    def _capture(self, warmup):
-        self._graph = self._out = None     # release the previous graph's pool before the new one fills
-        self._read_modules()
-        self._check()
-        self._warm_up(warmup)
-        self._out = self._record()
-        self._key = self._baked()
-
-    def __call__(self, frames):
-        self._check()
-        if isinstance(frames, dict) and set(frames) != self._keys:
-            raise ValueError("GraphedPoseStep: the frames hold keys %s; the step was captured for %s"
-                             % (sorted(map(str, frames)), sorted(self._keys)))
-        self._copy_in(frames)
-        if self._baked() != self._key:
-            self._capture(1)
-        self._graph.replay()
-        return self._out

@@ -20,11 +20,10 @@ import torch
 from . import _lib, ops
 from . import pose as _pose
 from .estimate import N_SAMPLE_POINTS
-from .graphed import _GraphedStep
+from .graphed import _GraphedEvalBase
 from .loss import ffb6d_loss
-from .model import FFB6D
 from .ops import _frame_intrinsics, _intrinsics_arg
-from .schedule import _OBJECT_KEYS, build_ffb6d_item
+from .schedule import _OBJECT_KEYS, build_ffb6d_item, check_dataset, check_frame_batch
 
 _IMAGE_KEYS = ("dpt", "rgb", "labels", "nrm_map")
 _INFO_KEYS = ("loss_rgbd_seg", "loss_kp_of", "loss_ctr_of", "loss_all", "acc_rgbd")
@@ -32,32 +31,7 @@ _INFO_KEYS = ("loss_rgbd_seg", "loss_kp_of", "loss_ctr_of", "loss_all", "acc_rgb
 _LM_LIST_CLASSES = 22
 
 
-def _check_batch(batch, name):
-    """``ValueError`` unless ``batch`` is a dict of the test batch's CUDA tensors on one device."""
-    if not isinstance(batch, dict):
-        raise ValueError("%s: the batch must be a dict, got %s" % (name, type(batch).__name__))
-    missing = [k for k in _IMAGE_KEYS + _OBJECT_KEYS if k not in batch]
-    if missing:
-        raise ValueError("%s: the batch lacks %s" % (name, missing))
-    unknown = sorted(str(k) for k in batch if k not in _IMAGE_KEYS + _OBJECT_KEYS + ("K",))
-    if unknown:
-        raise ValueError("%s: unknown batch keys %s" % (name, unknown))
-    dev = batch["dpt"].device if isinstance(batch["dpt"], torch.Tensor) else None
-    for k, t in batch.items():
-        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != dev:
-            raise ValueError("%s: batch[%r] must be a CUDA tensor on the device of batch['dpt']" % (name, k))
-    dpt = batch["dpt"]
-    if dpt.dtype != torch.uint16 or dpt.dim() != 3:
-        raise ValueError("%s: batch['dpt'] must be uint16 [B,H,W], got %s %s" % (name, dpt.dtype, tuple(dpt.shape)))
-    B = dpt.shape[0]
-    if batch["RTs"].dim() != 4 or batch["RTs"].shape[0] != B:
-        raise ValueError("%s: batch['RTs'] must be [B,n_obj,3,4], got %s" % (name, tuple(batch["RTs"].shape)))
-    if "K" in batch and (batch["K"].dtype != torch.float64 or tuple(batch["K"].shape) != (B, 3, 3)):
-        raise ValueError("%s: batch['K'] must be float64 [B,3,3], got %s %s"
-                         % (name, batch["K"].dtype, tuple(batch["K"].shape)))
-
-
-class GraphedTestStep(_GraphedStep):
+class GraphedTestStep(_GraphedEvalBase):
     """One batch of the reference's test, captured in one CUDA graph and replayed per batch (see the module).
 
     :param model: an :class:`~ffb6d_b200.model.FFB6D` in eval mode
@@ -88,7 +62,7 @@ class GraphedTestStep(_GraphedStep):
     devices differ from the example's.
     """
 
-    _wrapper_hint = "pass its .module"
+    _needs_image_branch = True
 
     def __init__(self, model, example_batch, *, dataset, cam_scale, K, mesh_pts, mesh_kps, cls_radius=None,
                  sym_cls_ids=(), n_points=N_SAMPLE_POINTS, capacity, test_gt=False, obj_id=None, seed=0, warmup=3):
@@ -96,14 +70,13 @@ class GraphedTestStep(_GraphedStep):
         self._check_model(model)
         self.model = model
         self._check()
-        if dataset not in ("ycb", "linemod"):
-            raise ValueError("%s: dataset must be 'ycb' or 'linemod', got %r" % (name, dataset))
+        check_dataset(dataset, name)
         lm = dataset == "linemod"
         if lm and (isinstance(obj_id, bool) or not isinstance(obj_id, (int, np.integer)) or obj_id < 1):
             raise ValueError("%s: a LineMOD test needs obj_id, the object's class id >= 1, got %r" % (name, obj_id))
         if isinstance(capacity, bool) or not isinstance(capacity, (int, np.integer)) or capacity < 1:
             raise ValueError("%s: capacity must be an int >= 1 (frames), got %r" % (name, capacity))
-        _check_batch(example_batch, name)
+        check_frame_batch(example_batch, name, _IMAGE_KEYS + _OBJECT_KEYS)
         B, n_obj = example_batch["RTs"].shape[:2]
         if capacity * n_obj > _lib.EVAL_MAX_ROWS:
             raise ValueError("%s: capacity * n_obj = %d rows, at most %d" % (name, capacity * n_obj,
@@ -135,20 +108,7 @@ class GraphedTestStep(_GraphedStep):
             self._frame_flags = torch.zeros((self.capacity, self.n_cls), dtype=torch.uint8, device=dev)
         self._sums = torch.zeros(len(_INFO_KEYS) + 1, dtype=torch.float64, device=dev)
         self._one = torch.ones(1, dtype=torch.float64, device=dev)
-        self._out = None
         super().__init__(model, example_batch, warmup)
-
-    def _check_model(self, model):
-        super()._check_model(model)
-        if not isinstance(model, FFB6D):
-            raise ValueError("%s: an FFB6DFusionNet has no image branch; testing from frames needs the whole FFB6D"
-                             % type(self).__name__)
-
-    def _check(self, modules=False):
-        """What cannot be captured at all: raise ``ValueError`` before any CUDA work."""
-        if self.model.training:
-            raise ValueError("%s: the model is in training mode; call model.eval() first" % type(self).__name__)
-        self._refuse_index_check()
 
     # ------------------------------------------------------------------------------------------ capture
     def _step(self):
@@ -181,33 +141,15 @@ class GraphedTestStep(_GraphedStep):
                                  valid=item["valid"])
         return end_points, loss, info
 
-    def _capture(self, warmup):
-        """Warm up and capture; what the warm-up recorded is undone, so a capture in the middle of a run (after a
-        baked value changed) leaves the run's table and sums as they were."""
-        self._graph = self._out = None     # release the previous graph's pool before the new one fills
-        self._read_modules()
-        self._check()
+    def _warm_up(self, n):
+        """The warm-up with what it recorded undone, so a capture in the middle of a run (after a baked value
+        changed) leaves the run's table and sums as they were."""
         saved = (self._state.clone(), self._sums.clone())
-        self._warm_up(warmup)
+        super()._warm_up(n)
         self._state.copy_(saved[0])
         self._sums.copy_(saved[1])
-        self._out = self._record()
-        self._key = self._baked()
 
     # ------------------------------------------------------------------------------------------ a run
-    def __call__(self, batch):
-        self._check()
-        if not isinstance(batch, dict) or set(batch) != self._keys:
-            raise ValueError("%s: the batch holds keys %s; the step was captured for %s"
-                             % (type(self).__name__,
-                                sorted(map(str, batch)) if isinstance(batch, dict) else type(batch).__name__,
-                                sorted(map(str, self._keys))))
-        self._copy_in(batch)
-        if self._baked() != self._key:
-            self._capture(1)
-        self._graph.replay()
-        return self._out
-
     def reset(self):
         """Start a new test run: the table and the sums are emptied on the device, the graph is kept."""
         self._state.zero_()

@@ -94,17 +94,34 @@ def _state_tensors(optimizer):
     return [t for p in optimizer.state for t in optimizer.state[p].values() if isinstance(t, torch.Tensor)]
 
 
+def _check_image_branch(model, name):
+    """``ValueError`` for an :class:`FFB6DFusionNet` that is not a whole :class:`FFB6D`: work that starts from decoded
+    frames needs the image branch."""
+    if isinstance(model, FFB6DFusionNet) and not isinstance(model, FFB6D):
+        raise ValueError("%s: an FFB6DFusionNet has no image branch; working from decoded frames needs the whole FFB6D"
+                         % name)
+
+
+def _forward(model, item):
+    """``model(item)``; an :class:`FFB6DFusionNet` also takes the item's image-branch maps."""
+    return model(item) if isinstance(model, FFB6D) else model(item, item["rgb_feats"])
+
+
 class _GraphedStep:
-    """What the train and eval steps share: the argument checks, the static input buffers and their copy-in, the
-    baked key of the model, the side-stream warm-up and the capture.  A subclass defines ``_check`` (what cannot be
-    captured), ``_step`` (the captured work), ``_capture`` and ``__call__``; ``_module_key`` / ``_extra_key`` add
-    what only it bakes in."""
+    """What every graphed step shares: the argument checks, the static input buffers and their copy-in, the baked key
+    of the model, the side-stream warm-up, the capture and the replay.  A subclass defines ``_check`` (what cannot be
+    captured) and ``_step`` (the captured work); ``_module_key`` / ``_extra_key`` add what only it bakes in,
+    ``_warm_up`` what a warm-up must undo and ``_writes`` the tensors a replay writes in place.
+
+    Each subclass's constructor checks the model with :meth:`_check_model` first, before its own checks and any CUDA
+    work, and then calls this one."""
 
     _wrapper_hint = ""
+    _needs_image_branch = False      # the step starts from decoded frames: an FFB6DFusionNet is rejected
+    _keys = None                     # the keys of a flat batch, checked by every call (see _check_keys)
 
     def __init__(self, model, example_item, warmup):
         name = type(self).__name__
-        self._check_model(model)
         if not isinstance(example_item, dict):
             raise ValueError("%s: example_item must be a dict, got %s" % (name, type(example_item).__name__))
         if not isinstance(model, FFB6D) and not isinstance(example_item.get("rgb_feats"), (list, tuple)):
@@ -116,8 +133,8 @@ class _GraphedStep:
         self._check(True)
         self._static = _static_copy(example_item)
         self._inputs = _tensors(self._static)
-        self._graph = None
-        self._key = None
+        self._graph = self._out = self._key = None
+        self._written = []
         self.captures = 0
         self._capture(int(warmup))
 
@@ -127,6 +144,8 @@ class _GraphedStep:
             raise ValueError("%s: a (Distributed)DataParallel model cannot be captured; %s" % (name, self._wrapper_hint))
         if not isinstance(model, FFB6DFusionNet):
             raise ValueError("%s: model must be an FFB6DFusionNet or FFB6D, got %s" % (name, type(model).__name__))
+        if self._needs_image_branch:
+            _check_image_branch(model, name)
 
     def _read_modules(self):
         """The module tree as a list, walked by every call's key (which also holds each module's children, so a
@@ -185,6 +204,39 @@ class _GraphedStep:
         self.captures += 1
         return out
 
+    def _writes(self):
+        """The tensors a replay updates in place whose host version counters it advances (none for an eval step)."""
+        return []
+
+    def _capture(self, warmup):
+        """Warm up on a side stream (undoing what the warm-up changed, see ``_warm_up``), then capture one step."""
+        self._graph = self._out = None     # release the previous graph's pool before the new one fills
+        self._written = []
+        self._read_modules()
+        self._check(True)
+        self._warm_up(warmup)
+        self._out = self._record()
+        self._written = self._writes()
+        self._key = self._baked()
+
+    def _replay(self):
+        """Capture again if a baked value changed, then replay; returns the graph's outputs."""
+        if self._baked() != self._key:
+            self._capture(1)
+        self._graph.replay()
+        if self._written:
+            # as eager in-place updates advance them, so version-keyed caches (the eval path's packs) see new values
+            increment_version(self._written)
+        return self._out
+
+    def _check_keys(self, batch):
+        """A step built from a flat batch takes batches with the example's keys only."""
+        if self._keys is not None and (not isinstance(batch, dict) or set(batch) != self._keys):
+            raise ValueError("%s: the batch holds keys %s; the step was captured for %s"
+                             % (type(self).__name__,
+                                sorted(map(str, batch)) if isinstance(batch, dict) else type(batch).__name__,
+                                sorted(map(str, self._keys))))
+
     def _copy_in(self, item):
         name = type(self).__name__
         if not isinstance(item, dict):
@@ -238,9 +290,8 @@ class GraphedTrainStep(_GraphedStep):
     _wrapper_hint = "multi-rank capture is not supported, pass the module of a single-rank run"
 
     def __init__(self, model, optimizer, example_item, warmup=3):
+        self._check_model(model)
         self.optimizer = optimizer
-        self._loss = self._info = None
-        self._written = []
         super().__init__(model, example_item, warmup)
 
     # ------------------------------------------------------------------------------------------ host checks
@@ -312,19 +363,14 @@ class GraphedTrainStep(_GraphedStep):
         """One training step on ``item``: what a replay runs."""
         opt = self.optimizer
         opt.zero_grad(set_to_none=True)
-        out = self.model(item) if isinstance(self.model, FFB6D) else self.model(item, item["rgb_feats"])
-        loss, info = ffb6d_loss(out, item, valid=item.get("valid"))
+        loss, info = ffb6d_loss(_forward(self.model, item), item, valid=item.get("valid"))
         loss.backward()
         opt.step()
         return loss.detach(), info
 
-    def _capture(self, warmup):
-        """Warm up on a side stream, restore everything the warm-up changed, then capture one step."""
+    def _warm_up(self, n):
+        """The warm-up, then every parameter, buffer and optimizer state tensor and the CUDA generator restored."""
         model, opt = self.model, self.optimizer
-        self._graph = self._loss = self._info = None     # release the previous graph's pool before the new one fills
-        self._written = []
-        self._read_modules()
-        self._check(True)
         opt.zero_grad(set_to_none=True)
         dev = next(model.parameters()).device
         tracked = list(model.parameters()) + list(model.buffers())
@@ -333,7 +379,7 @@ class GraphedTrainStep(_GraphedStep):
         saved = [t.detach().clone() for t in tracked]
         saved_state = {k: t.detach().clone() for k, t in before.items()}
         rng = torch.cuda.get_rng_state(dev)
-        self._warm_up(warmup)
+        super()._warm_up(n)
         with torch.no_grad():
             for t, s in zip(tracked, saved):
                 t.copy_(s)
@@ -355,25 +401,17 @@ class GraphedTrainStep(_GraphedStep):
                              "Adam's own state can be restored after the warm-up" % (type(self).__name__, unknown))
         del saved, saved_state
         opt.zero_grad(set_to_none=True)
-        self._loss, self._info = self._record()
-        # what a replay writes: its host version counters are advanced after each replay, as eager in-place
-        # updates advance them, so version-keyed caches (the eval path's packed weights) see the new values
-        self._written = (tracked + _state_tensors(opt) +
-                         [p.grad for p in model.parameters() if p.grad is not None])
-        self._key = self._baked()
+
+    def _writes(self):
+        model = self.model
+        return (list(model.parameters()) + list(model.buffers()) + _state_tensors(self.optimizer) +
+                [p.grad for p in model.parameters() if p.grad is not None])
 
     # ------------------------------------------------------------------------------------------ a step
     def __call__(self, item):
         self._check(self._sync)
         self._copy_in(item)
         return self._replay()
-
-    def _replay(self):
-        if self._baked() != self._key:
-            self._capture(1)
-        self._graph.replay()
-        increment_version(self._written)
-        return self._loss, self._info
 
 
 class GraphedFrameTrainStep(GraphedTrainStep):
@@ -405,6 +443,7 @@ class GraphedFrameTrainStep(GraphedTrainStep):
     do not come from frames); a batch whose keys, or an entry's kind, shape, dtype or device, differ from the example.
     """
 
+    _needs_image_branch = True
     _STAGING_SLOTS = 2
 
     def __init__(self, model, optimizer, example_batch, *, dataset, cam_scale, K, n_points=12800, warmup=3):
@@ -429,13 +468,8 @@ class GraphedFrameTrainStep(GraphedTrainStep):
         self._check_records(host)
         self._stage(host, 0)
         self._mirror = {k: host[k].numpy().copy() for k in ("jitter", "plans")}
-        super().__init__(model, optimizer, device_part, warmup)
-
-    def _check_model(self, model):
-        super()._check_model(model)
-        if not isinstance(model, FFB6D):
-            raise ValueError("%s: an FFB6DFusionNet has no image branch; training from frames needs the whole FFB6D"
-                             % type(self).__name__)
+        self.optimizer = optimizer
+        _GraphedStep.__init__(self, model, device_part, warmup)     # GraphedTrainStep's, less the model check above
 
     def _host_values(self, batch, want):
         """Every entry of ``batch`` that is not a CUDA tensor, as a contiguous CPU tensor; with ``want`` (the example's
@@ -498,10 +532,7 @@ class GraphedFrameTrainStep(GraphedTrainStep):
     def __call__(self, batch, seed):
         name = type(self).__name__
         self._check(self._sync)
-        if not isinstance(batch, dict) or set(batch) != self._keys:
-            raise ValueError("%s: the batch holds keys %s; the step was captured for %s"
-                             % (name, sorted(map(str, batch)) if isinstance(batch, dict) else type(batch).__name__,
-                                sorted(map(str, self._keys))))
+        self._check_keys(batch)
         if isinstance(seed, torch.Tensor):
             ops._device_seed(seed, self._seed.device)
         elif isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
@@ -513,7 +544,28 @@ class GraphedFrameTrainStep(GraphedTrainStep):
         return self._replay()
 
 
-class GraphedEvalStep(_GraphedStep):
+class _GraphedEvalBase(_GraphedStep):
+    """An eval-mode step: the model in eval mode, nothing a replay writes outside its own outputs.  Calling it checks
+    the model, the batch's keys (when built from a flat batch) and the input buffers' shapes, copies the batch in and
+    replays."""
+
+    _wrapper_hint = "pass its .module"
+
+    def _check(self, modules=False):
+        """What cannot be captured at all: raise ``ValueError`` before any CUDA work."""
+        if self.model.training:
+            raise ValueError("%s: the model is in training mode; call model.eval() first, it captures eval steps only"
+                             % type(self).__name__)
+        self._refuse_index_check()
+
+    def __call__(self, batch):
+        self._check()
+        self._check_keys(batch)
+        self._copy_in(batch)
+        return self._replay()
+
+
+class GraphedEvalStep(_GraphedEvalBase):
     """An eval step of ``model`` (an :class:`~ffb6d_b200.model.FFB6DFusionNet` or :class:`~ffb6d_b200.model.FFB6D`
     in eval mode), captured in a CUDA graph: under ``torch.no_grad()``, ``model(item)`` (``model(item,
     item["rgb_feats"])`` for :class:`FFB6DFusionNet`) and, when the example item carries ``labels``,
@@ -546,38 +598,15 @@ class GraphedEvalStep(_GraphedStep):
     _wrapper_hint = "pass its .module (each rank evaluates through a step of its own)"
 
     def __init__(self, model, example_item, warmup=3):
-        self._out = None
+        self._check_model(model)
         self._with_loss = isinstance(example_item, dict) and all(k in example_item for k in _LOSS_KEYS)
         super().__init__(model, example_item, warmup)
-
-    def _check(self, modules=False):
-        """What cannot be captured at all: raise ``ValueError`` before any CUDA work."""
-        if self.model.training:
-            raise ValueError("GraphedEvalStep: the model is in training mode; call model.eval() first, it captures "
-                             "eval steps only")
-        self._refuse_index_check()
 
     def _step(self):
         item = self._static
         with torch.no_grad():
-            out = self.model(item) if isinstance(self.model, FFB6D) else self.model(item, item["rgb_feats"])
+            out = _forward(self.model, item)
             loss = info = None
             if self._with_loss:
                 loss, info = ffb6d_loss(out, item, valid=item.get("valid"))
         return out, loss, info
-
-    def _capture(self, warmup):
-        self._graph = self._out = None     # release the previous graph's pool before the new one fills
-        self._read_modules()
-        self._check()
-        self._warm_up(warmup)
-        self._out = self._record()
-        self._key = self._baked()
-
-    def __call__(self, item):
-        self._check()
-        self._copy_in(item)
-        if self._baked() != self._key:
-            self._capture(1)
-        self._graph.replay()
-        return self._out

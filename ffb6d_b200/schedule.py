@@ -271,6 +271,49 @@ MIN_VALID_PIXELS = 400
 _OBJECT_KEYS = ("RTs", "kp_3ds", "ctr_3ds", "cls_ids", "obj_cls", "obj_kps", "obj_ctr")
 
 
+def check_dataset(dataset, name):
+    """``ValueError`` unless ``dataset`` is ``"ycb"`` or ``"linemod"``."""
+    if dataset not in ("ycb", "linemod"):
+        raise ValueError("%s: dataset must be 'ycb' or 'linemod', got %r" % (name, dataset))
+
+
+def check_frame_batch(batch, name, keys):
+    """``ValueError`` unless ``batch`` is a dict of CUDA tensors on one device with exactly ``keys`` and optionally
+    ``K``: ``dpt`` uint16 ``[B,H,W]``, ``rgb`` uint8 ``[B,H,W,3]``, ``nrm_map`` float32 / float64 ``[B,H,W,3]``, ``K``
+    float64 ``[B,3,3]`` and, when ``keys`` hold it, ``RTs [B,n_obj,3,4]``.  Runs before any CUDA work."""
+    if not isinstance(batch, dict):
+        raise ValueError("%s: the batch must be a dict, got %s" % (name, type(batch).__name__))
+    missing = [k for k in keys if k not in batch]
+    if missing:
+        raise ValueError("%s: the batch lacks %s (it needs %s)" % (name, missing, list(keys)))
+    known = tuple(keys) + ("K",)
+    unknown = sorted(str(k) for k in batch if k not in known)
+    if unknown:
+        raise ValueError("%s: unknown batch keys %s (known: %s)" % (name, unknown, list(known)))
+    for k, t in batch.items():
+        if not isinstance(t, torch.Tensor):
+            raise ValueError("%s: batch[%r] must be a tensor, got %s" % (name, k, type(t).__name__))
+    dpt, rgb, nrm = batch["dpt"], batch["rgb"], batch["nrm_map"]
+    if dpt.dtype != torch.uint16 or dpt.dim() != 3:
+        raise ValueError("%s: batch['dpt'] must be uint16 [B,H,W], got %s %s" % (name, dpt.dtype, tuple(dpt.shape)))
+    B, H, W = dpt.shape
+    if rgb.dtype != torch.uint8 or tuple(rgb.shape) != (B, H, W, 3):
+        raise ValueError("%s: batch['rgb'] must be uint8 [B,H,W,3] = %s, got %s %s"
+                         % (name, (B, H, W, 3), rgb.dtype, tuple(rgb.shape)))
+    if nrm.dtype not in (torch.float32, torch.float64) or tuple(nrm.shape) != (B, H, W, 3):
+        raise ValueError("%s: batch['nrm_map'] must be float32 or float64 [B,H,W,3] = %s, got %s %s"
+                         % (name, (B, H, W, 3), nrm.dtype, tuple(nrm.shape)))
+    if "K" in batch and (batch["K"].dtype != torch.float64 or tuple(batch["K"].shape) != (B, 3, 3)):
+        raise ValueError("%s: batch['K'] must be float64 [B,3,3] = %s, got %s %s"
+                         % (name, (B, 3, 3), batch["K"].dtype, tuple(batch["K"].shape)))
+    if "RTs" in keys and (batch["RTs"].dim() != 4 or batch["RTs"].shape[0] != B):
+        raise ValueError("%s: batch['RTs'] must be [B,n_obj,3,4], got %s" % (name, tuple(batch["RTs"].shape)))
+    for k, t in batch.items():
+        if not t.is_cuda or t.device != dpt.device:
+            raise ValueError("%s: batch[%r] is on %s; every tensor must be a CUDA tensor on one CUDA device (dpt: %s)"
+                             % (name, k, t.device, dpt.device))
+
+
 def build_ffb6d_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed=0, fill=True, min_valid=MIN_VALID_PIXELS,
                        k=K_NEIGH, index_dtype=torch.int32, streams=None):
     """The inference half of the datasets' ``get_item`` for a batch on the GPU: every key ``FFB6D.forward`` reads,
@@ -374,8 +417,7 @@ TRAIN_BATCH_KEYS = TRAIN_IMAGE_KEYS + TRAIN_RECORD_KEYS + _OBJECT_KEYS
 
 def check_train_batch(batch, dataset, name):
     """``ValueError`` unless ``dataset`` is known and ``batch`` is a dict holding every key of ``TRAIN_BATCH_KEYS``."""
-    if dataset not in ("ycb", "linemod"):
-        raise ValueError("%s: dataset must be 'ycb' or 'linemod', got %r" % (name, dataset))
+    check_dataset(dataset, name)
     if not isinstance(batch, dict):
         raise ValueError("%s: the batch must be a dict, got %s" % (name, type(batch).__name__))
     missing = [k for k in TRAIN_BATCH_KEYS if k not in batch]

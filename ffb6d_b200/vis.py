@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from . import ops, pose as _pose
+from .schedule import check_dataset
 
 # get_label_color's two fixed tables (modes 0 and 1), one colour per class id 0 .. 21, in the order the reference
 # hands them to OpenCV (BGR)
@@ -179,8 +180,7 @@ def cal_view_pred_pose(model, item, *, dataset, mesh_pts, mesh_kps, cls_radius=N
     colour lands reversed, and always draws class 1, with the identity pose where it was not predicted.  Raises
     ValueError, as :func:`~ffb6d_b200.pose.cal_frame_poses`, for a mask id out of range or a predicted class
     without keypoints (YCB; its one host synchronisation)."""
-    if dataset not in ("ycb", "linemod"):
-        raise ValueError("dataset must be 'ycb' or 'linemod', got %r" % (dataset,))
+    check_dataset(dataset, "cal_view_pred_pose")
     if dataset == "linemod" and obj_id < 0:
         raise ValueError("LineMOD needs the object's obj_id")
     from .estimate import forward_and_vote

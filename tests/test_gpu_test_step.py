@@ -5,8 +5,8 @@ The record's rows against the numpy restatement (oracle/eval_record_oracle.py) a
 ``TorchEval.cal_auc`` / ``cal_lm_add`` on the same votes; the summary of a large hand-made table against the
 restatement; ``GraphedTestStep`` against the eager chain (``build_ffb6d_item``, the eval forward and loss,
 ``TorchEval.eval_pose_parallel``) over three seeded batches for YCB (one camera matrix per frame) and LineMOD, with a
-replay under the CUDA sync debug mode, ``reset()`` and a second run, and an overflowing batch; and the ``-test_gt``
-sanity check of the reference's README.  Frames are 120x160 with 4096 points."""
+replay under the CUDA sync debug mode, ``reset()`` and a second run, and an overflowing batch; a capture in the
+middle of a run; and the ``-test_gt`` sanity check of the reference's README.  Frames are 120x160 with 4096 points."""
 import numpy as np
 import pytest
 import torch
@@ -305,3 +305,24 @@ def test_test_gt_recovers_the_poses(cuda, dataset):
         assert len(r["add_dis_lst"][c]) > 0
         auc = r["add_s_auc_lst"][0 if dataset == "linemod" else c]
         assert auc >= 99.99, (c, auc, r["add_dis_lst"][c])
+
+
+@pytest.mark.parametrize("dataset", ["ycb", "linemod"])
+def test_capture_in_the_middle_of_a_run(cuda, dataset):
+    """A parameter re-pointed at an equal clone changes the baked key but no value: the next call captures again, and
+    its warm-up leaves the run's table and sums as they were, so the summary is that of a step that never captured
+    again."""
+    model = _model(dataset)
+    seq = [_test_batch(s, dataset) for s in (1, 2, 3)]
+    once = F.GraphedTestStep(model, seq[0], **_kw(dataset))
+    for batch in seq:
+        once(batch)
+    want = once.summary(DIAMETER)
+    step = F.GraphedTestStep(model, seq[0], **_kw(dataset))
+    step(seq[0])
+    step(seq[1])
+    p = next(model.parameters())
+    p.data = p.data.clone()
+    step(seq[2])
+    assert step.captures == 2 and once.captures == 1
+    assert repr(step.summary(DIAMETER)) == repr(want)
