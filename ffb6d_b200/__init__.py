@@ -50,6 +50,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
 * :class:`GraphedTestStep` (:mod:`ffb6d_b200.evaluate`) -- one batch of the reference's test (the eval ``get_item``,
   the forward, the loss, the vote, ADD / ADD-S and a device record of every object) replayed from one CUDA graph,
   and the AUC tables of the run computed on the GPU (:func:`eval_record`, :func:`eval_auc`).
+* :func:`depth_normal` -- surface normals of millimetre depth maps on the GPU (DESIGN.md §4.30), the opt-in stand-in
+  for the datasets' ``normalSpeed.depth_normal``; every item builder and graphed step from frames takes
+  ``normals="device"`` to compute them from the depth the reference uses.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -68,7 +71,7 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax",
         "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d",
         "farthest_point_sampling", "pose_add_adds", "vote_poses", "point_input", "rgb_noise_check_records",
-        "color_jitter_check_plans", "eval_record", "eval_auc")
+        "color_jitter_check_plans", "eval_record", "eval_auc", "depth_normal")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item", "build_ffb6d_inputs", "build_ffb6d_train_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")

@@ -43,6 +43,10 @@ VIS_MAX_SETS = 1 << 24
 VIS_MAX_ROWS = 1 << 24
 VIS_MAX_TABLE_ROWS = (1 << 31) - 1
 VIS_MAX_FRAMES = 65535
+NRM_MAX_KSIZE = 16                               # FFB6D_NRM_* of include/ffb6d_b200.h
+NRM_MAX_FRAMES = 65535
+NRM_MAX_HEIGHT = 65535 * 8 - 1
+NRM_MAX_FRAME_PIXELS = (1 << 31) - 1
 
 
 class FFB6DError(RuntimeError):
@@ -128,6 +132,8 @@ def _load():
         "ffb6d_sample_pixels_dseed": (ci, [vp, i64, i64, i64, fp, i64, vp, vp, vp, vp, sz, vp]),
         "ffb6d_fill_depth_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_fill_depth": (ci, [vp, i64, i64, i64, fp, vp, vp, vp, sz, vp]),
+        "ffb6d_depth_normal": (ci, [vp, i64, i64, i64, vp, ci, ci, ci, ci, ci, vp, vp]),
+        "ffb6d_depth_to_mm": (ci, [vp, i64, fp, vp, vp]),
         "ffb6d_mean_shift_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_mean_shift_fit": (ci, [vp, vp, i64, i64, i64, fp, ci, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_best_fit_transform": (ci, [vp, vp, i64, i64, vp, vp]),

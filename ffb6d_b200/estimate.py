@@ -19,8 +19,9 @@ labels (:func:`ffb6d_b200.schedule.build_ffb6d_inputs`), ``rgb`` cast to float32
 * ``"linemod"``: the raw depth (``fill=False``); the two-class vote on ``mask == 1`` without refinement, as
   ``cal_frame_poses_lm`` (``n_cls = 2``, the object at row 1).
 
-Normals stay an input (``nrm_map``): the reference computes them with the external ``normalSpeed`` (YCB from the
-completed depth, see INTEGRATION.md).
+Normals are an input (``nrm_map``) by default: the reference computes them with the external ``normalSpeed`` (YCB from
+the completed depth, see INTEGRATION.md).  With ``normals="device"`` the frames hold no ``nrm_map`` and the normals
+are computed on the device from that same depth (:func:`ffb6d_b200.ops.depth_normal`, DESIGN.md §4.30).
 """
 import torch
 
@@ -68,10 +69,10 @@ def forward_and_vote(model, item, dataset, mesh_kps, cls_radius=None):
     return end_points, table, votes
 
 
-def _estimate(model, frames, dataset, cam_scale, intr, table, n_points, seed):
+def _estimate(model, frames, dataset, cam_scale, intr, table, n_points, seed, normals):
     """One estimate from checked frames, with device intrinsics ``intr`` and a device vote table."""
-    item = build_ffb6d_inputs(frames["dpt"], cam_scale, intr, frames["rgb"], frames["nrm_map"], n_points, seed=seed,
-                              fill=dataset == "ycb")
+    item = build_ffb6d_inputs(frames["dpt"], cam_scale, intr, frames["rgb"], frames.get("nrm_map"), n_points, seed=seed,
+                              fill=dataset == "ycb", normals=normals)
     item["rgb"] = item["rgb"].to(torch.float32)             # model_fn's cast of the uint8 image
     _, _, (present, count, kps, poses) = forward_and_vote(model, item, dataset, table)
     return dict(present=present, count=count, kps=kps, poses=poses, valid=item["valid"])
@@ -86,7 +87,7 @@ def _prepare(model, frames, dataset, K, mesh_kps, cls_radius):
 
 
 def estimate_poses(model, frames, *, dataset, cam_scale, K, mesh_kps, cls_radius=None, n_points=N_SAMPLE_POINTS,
-                   seed=0):
+                   seed=0, normals="input"):
     """The object poses of a batch of decoded RGB-D frames, eager: the composition the module describes.
 
     :param model: an :class:`~ffb6d_b200.model.FFB6D`; it is switched to eval mode, as the reference's demo does
@@ -101,6 +102,8 @@ def estimate_poses(model, frames, *, dataset, cam_scale, K, mesh_kps, cls_radius
       keypoints (centre last), LineMOD the ``[n_kps+1,3]`` keypoints of the object
     :param cls_radius: YCB ``config.ycb_r_lst``, for the centre-clustering refinement (None: no refinement)
     :param n_points: points sampled per frame, the reference's 12800 by default; :param seed: the sampling seed
+    :param normals: ``"input"``: ``frames['nrm_map']`` is the normal map; ``"device"``: the frames hold no ``nrm_map``
+      and :func:`ffb6d_b200.build_ffb6d_inputs` computes it from the depth
     :return: dict of CUDA tensors ``present [B,n_cls]`` bool, ``count [B,n_cls]`` int32, ``kps [B,n_cls,n_kps+1,3]``
       float32, ``poses [B,n_cls,3,4]`` float64 (rows as :func:`~ffb6d_b200.pose.cal_batch_poses` gives them;
       LineMOD ``n_cls = 2``, the object at row 1) and ``valid [B]`` bool (False: fewer than 400 valid depth pixels,
@@ -110,12 +113,12 @@ def estimate_poses(model, frames, *, dataset, cam_scale, K, mesh_kps, cls_radius
     synchronisation; a host ``K`` or a mapping is first copied to the device, which synchronises."""
     check_dataset(dataset, "estimate_poses")
     _check_image_branch(model, "estimate_poses")
-    check_frame_batch(frames, "estimate_poses", _FRAME_KEYS)
+    check_frame_batch(frames, "estimate_poses", _FRAME_KEYS, normals)
     intr, table = _prepare(model, frames, dataset, K, mesh_kps, cls_radius)
     model.eval()
     if intr is None:
         intr = _frame_intrinsics(frames["K"])
-    return _estimate(model, frames, dataset, cam_scale, intr, table, n_points, seed)
+    return _estimate(model, frames, dataset, cam_scale, intr, table, n_points, seed, normals)
 
 
 class GraphedPoseStep(_GraphedEvalBase):
@@ -127,7 +130,7 @@ class GraphedPoseStep(_GraphedEvalBase):
       by the caller, or goes through :func:`estimate_poses`)
     :param warmup: eager estimates run on a side stream before the first capture
 
-    Baked in at construction: ``dataset``, ``cam_scale``, ``n_points``, ``seed`` (so the same frame gives the same
+    Baked in at construction: ``dataset``, ``cam_scale``, ``n_points``, ``normals``, ``seed`` (so the same frame gives the same
     points on every replay, as :func:`estimate_poses` with that seed does), ``K`` (copied to the device once; with
     ``frames['K']`` the per-frame matrices are inputs instead) and the vote table (built from ``mesh_kps`` and
     ``cls_radius`` once, or the given :class:`~ffb6d_b200.pose.VoteTable`).
@@ -146,13 +149,14 @@ class GraphedPoseStep(_GraphedEvalBase):
     _needs_image_branch = True
 
     def __init__(self, model, example_frames, *, dataset, cam_scale, K, mesh_kps, cls_radius=None,
-                 n_points=N_SAMPLE_POINTS, seed=0, warmup=3):
+                 n_points=N_SAMPLE_POINTS, seed=0, warmup=3, normals="input"):
         name = type(self).__name__
         check_dataset(dataset, name)
         self._check_model(model)
-        check_frame_batch(example_frames, name, _FRAME_KEYS)
+        check_frame_batch(example_frames, name, _FRAME_KEYS, normals)
         self._intr, self._table = _prepare(model, example_frames, dataset, K, mesh_kps, cls_radius)
         self.dataset, self.cam_scale, self.n_points, self.seed = dataset, cam_scale, int(n_points), int(seed)
+        self.normals = normals
         self._keys = set(example_frames)
         super().__init__(model, example_frames, warmup)
 
@@ -160,4 +164,4 @@ class GraphedPoseStep(_GraphedEvalBase):
         frames = self._static
         intr = _frame_intrinsics(frames["K"]) if "K" in frames else self._intr
         return _estimate(self.model, frames, self.dataset, self.cam_scale, intr, self._table, self.n_points,
-                         self.seed)
+                         self.seed, self.normals)

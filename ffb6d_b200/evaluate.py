@@ -50,6 +50,8 @@ class GraphedTestStep(_GraphedEvalBase):
       object rows
     :param test_gt: vote from the labels and target offsets instead of the predictions (``-test_gt``)
     :param obj_id: the LineMOD object's class id (``config.cls_id``)
+    :param normals: ``"input"``: the batch's ``nrm_map``; ``"device"``: the batch holds no ``nrm_map`` and the normals
+      are computed from the depth (:func:`ffb6d_b200.build_ffb6d_item`)
 
     ``step(batch)`` copies the batch into the input buffers and replays; it returns ``(end_points, loss, info)``,
     graph-owned device tensors that the next replay overwrites, and does not synchronise.  :meth:`summary`
@@ -65,7 +67,8 @@ class GraphedTestStep(_GraphedEvalBase):
     _needs_image_branch = True
 
     def __init__(self, model, example_batch, *, dataset, cam_scale, K, mesh_pts, mesh_kps, cls_radius=None,
-                 sym_cls_ids=(), n_points=N_SAMPLE_POINTS, capacity, test_gt=False, obj_id=None, seed=0, warmup=3):
+                 sym_cls_ids=(), n_points=N_SAMPLE_POINTS, capacity, test_gt=False, obj_id=None, seed=0, warmup=3,
+                 normals="input"):
         name = type(self).__name__
         self._check_model(model)
         self.model = model
@@ -76,7 +79,8 @@ class GraphedTestStep(_GraphedEvalBase):
             raise ValueError("%s: a LineMOD test needs obj_id, the object's class id >= 1, got %r" % (name, obj_id))
         if isinstance(capacity, bool) or not isinstance(capacity, (int, np.integer)) or capacity < 1:
             raise ValueError("%s: capacity must be an int >= 1 (frames), got %r" % (name, capacity))
-        check_frame_batch(example_batch, name, _IMAGE_KEYS + _OBJECT_KEYS)
+        check_frame_batch(example_batch, name, _IMAGE_KEYS + _OBJECT_KEYS, normals)
+        self.normals = normals
         B, n_obj = example_batch["RTs"].shape[:2]
         if capacity * n_obj > _lib.EVAL_MAX_ROWS:
             raise ValueError("%s: capacity * n_obj = %d rows, at most %d" % (name, capacity * n_obj,
@@ -114,8 +118,8 @@ class GraphedTestStep(_GraphedEvalBase):
     def _step(self):
         b = self._static
         intr = _frame_intrinsics(b["K"]) if "K" in b else self._intr
-        item = build_ffb6d_item(b["dpt"], self.cam_scale, intr, b["rgb"], b["labels"], b["nrm_map"], b,
-                                self.n_points, seed=self.seed, fill=self.dataset == "ycb")
+        item = build_ffb6d_item(b["dpt"], self.cam_scale, intr, b["rgb"], b["labels"], b.get("nrm_map"), b,
+                                self.n_points, seed=self.seed, fill=self.dataset == "ycb", normals=self.normals)
         item["rgb"] = item["rgb"].float()                     # model_fn's cast
         with torch.no_grad():
             end_points = self.model(item)

@@ -428,8 +428,9 @@ class GraphedFrameTrainStep(GraphedTrainStep):
       (CUDA or host), shape and dtype.
     :param warmup: eager steps before the first capture, undone as :class:`GraphedTrainStep` undoes them.
 
-    Baked in at construction: ``dataset``, ``cam_scale``, ``n_points`` and ``K`` (copied to the device once; with
-    ``batch['K']`` the per-frame matrices are inputs instead).  Everything else that capture bakes in, and every rule
+    Baked in at construction: ``dataset``, ``cam_scale``, ``n_points``, ``normals`` (as
+    :func:`~ffb6d_b200.build_ffb6d_train_item` takes it; with ``"device"`` batches hold no ``nrm_map``) and ``K``
+    (copied to the device once; with ``batch['K']`` the per-frame matrices are inputs instead).  Everything else that capture bakes in, and every rule
     that captures again, rejects or restores, is :class:`GraphedTrainStep`'s (DESIGN.md §4.20).
 
     ``step(batch, seed)`` checks the batch's jitter plans and noise records on the host (a bad one raises
@@ -446,11 +447,12 @@ class GraphedFrameTrainStep(GraphedTrainStep):
     _needs_image_branch = True
     _STAGING_SLOTS = 2
 
-    def __init__(self, model, optimizer, example_batch, *, dataset, cam_scale, K, n_points=12800, warmup=3):
+    def __init__(self, model, optimizer, example_batch, *, dataset, cam_scale, K, n_points=12800, warmup=3,
+                 normals="input"):
         name = type(self).__name__
         self._check_model(model)
-        check_train_batch(example_batch, dataset, name)
-        self.dataset, self.cam_scale, self.n_points = dataset, cam_scale, int(n_points)
+        check_train_batch(example_batch, dataset, name, normals)
+        self.dataset, self.cam_scale, self.n_points, self.normals = dataset, cam_scale, int(n_points), normals
         self._keys = set(example_batch)
         dev = next(model.parameters()).device
         device_part = {k: v for k, v in example_batch.items() if isinstance(v, torch.Tensor) and v.is_cuda}
@@ -526,7 +528,7 @@ class GraphedFrameTrainStep(GraphedTrainStep):
     def _step(self):
         batch = dict(self._static, **self._records)
         item = _train_item(batch, self.dataset, self.cam_scale, self._intr, self.n_points, self._seed,
-                           records=self._mirror)
+                           records=self._mirror, normals=self.normals)
         return self._train(item)
 
     def __call__(self, batch, seed):

@@ -936,6 +936,54 @@ def _fill_depth(dpt, cam_scale, scale_2_80m=1, fill_type='multiscale', extrapola
     return tuple(outs)
 
 
+def depth_normal(dpt_mm, K, k_size=5, distance_threshold=2000, difference_threshold=20, point_into_surface=False):
+    """Surface normals of millimetre depth maps on the GPU (``ffb6d_depth_normal``, DESIGN.md §4.30): the batched
+    ``normalSpeed.depth_normal(d, K[0][0], K[1][1], k_size, distance_threshold, difference_threshold,
+    point_into_surface)`` of the datasets (datasets/ycb/ycb_dataset.py:207-210), computed by a specified estimator: the
+    least-squares depth-gradient fit of OpenCV's LINEMOD with the camera's fx, fy.  Whether ``normalSpeed`` gives the
+    same values is not known; the reference's trained checkpoints were trained on ``normalSpeed``'s.
+
+    :param dpt_mm: ``[H,W]`` or ``[B,H,W]`` ``torch.uint16`` CUDA, depth in millimetres (0 = hole)
+    :param K: camera matrix as :func:`backproject` takes it (host ``[3,3]`` / ``[B,3,3]``, or device float64
+      ``(fx, fy, cx, cy)`` ``[4]`` / ``[B,4]``: no host copy, capturable); only fx and fy are read
+    :param k_size: the neighbour offset r in pixels; :param distance_threshold: depths at or beyond it (mm) get a zero
+      normal; :param difference_threshold: neighbours whose depth differs by this many mm or more are left out
+    :param point_into_surface: negate the normals (they face the camera by default)
+    :return: float32 ``[..., H, W, 3]``; ``(0, 0, 0)`` at holes, beyond ``distance_threshold`` and where the fit is
+      degenerate
+    """
+    _need_cuda(dpt_mm, "dpt_mm")
+    if dpt_mm.dtype != torch.uint16 or dpt_mm.dim() not in (2, 3):
+        raise ValueError("dpt_mm must be torch.uint16 [H,W] or [B,H,W], got %s %s" % (dpt_mm.dtype, tuple(dpt_mm.shape)))
+    for name, v in (("k_size", k_size), ("distance_threshold", distance_threshold),
+                    ("difference_threshold", difference_threshold)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise ValueError("%s must be an int, got %r" % (name, v))
+    d = dpt_mm.contiguous()
+    B, H, W = (1,) + tuple(d.shape) if d.dim() == 2 else tuple(d.shape)
+    dev = d.device
+    intr_d, per_frame = _intrinsics_arg(K, B, dev)
+    nrm = torch.empty(tuple(d.shape) + (3,), dtype=torch.float32, device=dev)
+    launch(lib.ffb6d_depth_normal, dev, d.data_ptr(), B, H, W, intr_d.data_ptr(), per_frame, int(k_size),
+           int(distance_threshold), int(difference_threshold), int(bool(point_into_surface)), nrm.data_ptr())
+    return nrm
+
+
+def depth_to_mm(depth, divisor=10.0):
+    """``(depth / divisor).astype(np.uint16)`` on the GPU (``ffb6d_depth_to_mm``): a float32 IEEE division, then a
+    truncation, as numpy computes it for in-range values (out of range, where numpy's cast is undefined, it saturates).
+    With ``divisor`` 10 this is the YCB dataset's millimetre map of the completed depth (ycb_dataset.py:207).
+
+    :param depth: float32 CUDA tensor of any shape; :return: ``torch.uint16`` of the same shape"""
+    _need_cuda(depth, "depth")
+    if depth.dtype != torch.float32:
+        raise ValueError("depth must be float32, got %s" % depth.dtype)
+    src = depth.contiguous()
+    out = torch.empty(src.shape, dtype=torch.uint16, device=src.device)
+    launch(lib.ffb6d_depth_to_mm, src.device, src.data_ptr(), src.numel(), float(np.float32(divisor)), out.data_ptr())
+    return out
+
+
 def intrinsics_to_device(K, device, batch=None):
     """Camera matrix ``[3,3]`` / ``[B,3,3]`` -> float64 ``[4]`` / ``[B,4]`` (fx, fy, cx, cy) on the device."""
     Kn = np.asarray(K, dtype=np.float64)

@@ -277,10 +277,42 @@ def check_dataset(dataset, name):
         raise ValueError("%s: dataset must be 'ycb' or 'linemod', got %r" % (name, dataset))
 
 
-def check_frame_batch(batch, name, keys):
+# where the normal map comes from: "input", the caller's nrm_map (normalSpeed's in the reference), or "device",
+# depth_normal of the depth the datasets take it from (DESIGN.md §4.30)
+NORMALS = ("input", "device")
+# normalSpeed.depth_normal's k_size, distance_threshold, difference_threshold and point_into_surface in both datasets
+# (ycb_dataset.py:208-210, linemod_dataset.py:252-254)
+NORMAL_ARGS = (5, 2000, 20, False)
+# YCB's millimetre map is (dpt_um / 10).astype(np.uint16) of the completed depth (ycb_dataset.py:207)
+YCB_MM_DIVISOR = 10.0
+
+
+def check_normals(normals, name, nrm_map=None):
+    """``ValueError`` unless ``normals`` is one of ``NORMALS``, and with ``"device"`` unless ``nrm_map`` is None."""
+    if not (isinstance(normals, str) and normals in NORMALS):
+        raise ValueError("%s: normals must be 'input' or 'device', got %r" % (name, normals))
+    if normals == "device" and nrm_map is not None:
+        raise ValueError("%s: nrm_map is given with normals='device'; pass None (the normals are computed from the "
+                         "depth)" % name)
+
+
+def _normal_keys(batch, name, keys, normals):
+    """``keys`` without ``nrm_map`` under ``normals="device"``, where a batch holding ``nrm_map`` is refused."""
+    check_normals(normals, name)
+    if normals == "input":
+        return tuple(keys)
+    if isinstance(batch, dict) and "nrm_map" in batch:
+        raise ValueError("%s: the batch holds nrm_map with normals='device'; leave it out (the normals are computed "
+                         "from the depth)" % name)
+    return tuple(k for k in keys if k != "nrm_map")
+
+
+def check_frame_batch(batch, name, keys, normals="input"):
     """``ValueError`` unless ``batch`` is a dict of CUDA tensors on one device with exactly ``keys`` and optionally
     ``K``: ``dpt`` uint16 ``[B,H,W]``, ``rgb`` uint8 ``[B,H,W,3]``, ``nrm_map`` float32 / float64 ``[B,H,W,3]``, ``K``
-    float64 ``[B,3,3]`` and, when ``keys`` hold it, ``RTs [B,n_obj,3,4]``.  Runs before any CUDA work."""
+    float64 ``[B,3,3]`` and, when ``keys`` hold it, ``RTs [B,n_obj,3,4]``.  With ``normals="device"`` the batch must not
+    hold ``nrm_map``.  Runs before any CUDA work."""
+    keys = _normal_keys(batch, name, keys, normals)
     if not isinstance(batch, dict):
         raise ValueError("%s: the batch must be a dict, got %s" % (name, type(batch).__name__))
     missing = [k for k in keys if k not in batch]
@@ -293,14 +325,15 @@ def check_frame_batch(batch, name, keys):
     for k, t in batch.items():
         if not isinstance(t, torch.Tensor):
             raise ValueError("%s: batch[%r] must be a tensor, got %s" % (name, k, type(t).__name__))
-    dpt, rgb, nrm = batch["dpt"], batch["rgb"], batch["nrm_map"]
+    dpt, rgb = batch["dpt"], batch["rgb"]
     if dpt.dtype != torch.uint16 or dpt.dim() != 3:
         raise ValueError("%s: batch['dpt'] must be uint16 [B,H,W], got %s %s" % (name, dpt.dtype, tuple(dpt.shape)))
     B, H, W = dpt.shape
     if rgb.dtype != torch.uint8 or tuple(rgb.shape) != (B, H, W, 3):
         raise ValueError("%s: batch['rgb'] must be uint8 [B,H,W,3] = %s, got %s %s"
                          % (name, (B, H, W, 3), rgb.dtype, tuple(rgb.shape)))
-    if nrm.dtype not in (torch.float32, torch.float64) or tuple(nrm.shape) != (B, H, W, 3):
+    nrm = batch.get("nrm_map")
+    if nrm is not None and (nrm.dtype not in (torch.float32, torch.float64) or tuple(nrm.shape) != (B, H, W, 3)):
         raise ValueError("%s: batch['nrm_map'] must be float32 or float64 [B,H,W,3] = %s, got %s %s"
                          % (name, (B, H, W, 3), nrm.dtype, tuple(nrm.shape)))
     if "K" in batch and (batch["K"].dtype != torch.float64 or tuple(batch["K"].shape) != (B, 3, 3)):
@@ -315,7 +348,7 @@ def check_frame_batch(batch, name, keys):
 
 
 def build_ffb6d_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed=0, fill=True, min_valid=MIN_VALID_PIXELS,
-                       k=K_NEIGH, index_dtype=torch.int32, streams=None):
+                       k=K_NEIGH, index_dtype=torch.int32, streams=None, normals="input"):
     """The inference half of the datasets' ``get_item`` for a batch on the GPU: every key ``FFB6D.forward`` reads,
     from decoded frames that have no labels and no objects (what a deployed model sees).
 
@@ -327,20 +360,27 @@ def build_ffb6d_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed=0, fill=T
 
     :param dpt: ``[B,H,W]`` ``torch.uint16`` CUDA, the depth PNGs' raw values; :param cam_scale: raw units per metre
     :param K: camera matrix as :func:`ffb6d_b200.ops.backproject` takes it
-    :param rgb: ``[B,H,W,3]`` uint8; :param nrm_map: ``[B,H,W,3]`` float32 / float64 normal map
+    :param rgb: ``[B,H,W,3]`` uint8; :param nrm_map: ``[B,H,W,3]`` float32 / float64 normal map, or None with
+      ``normals="device"``
+    :param normals: ``"input"``: ``nrm_map`` is the normal map; ``"device"``: it is computed from the depth by
+      :func:`ffb6d_b200.ops.depth_normal` with the datasets' ``normalSpeed`` arguments, from the completed depth's
+      millimetre map (YCB, :func:`ffb6d_b200.ops.depth_to_mm`) or the raw depth (LineMOD)
     :return: dict with ``rgb [B,3,H,W]`` uint8, ``cld_rgb_nrm [B,9,N]``, ``choose [B,1,N]``, ``dpt_map_m [B,H,W]``,
       the tensors of :func:`build_ffb6d_indices` (``cld_xyz*`` and the index tensors) and ``valid [B]`` bool
     """
-    return _build_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_valid, k, index_dtype, streams)[0]
+    check_normals(normals, "build_ffb6d_inputs", nrm_map)
+    return _build_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_valid, k, index_dtype, streams,
+                         normals=normals)[0]
 
 
 def _build_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_valid, k, index_dtype, streams,
-                  labels=None, obj=None):
+                  labels=None, obj=None, normals="input"):
     """:func:`build_ffb6d_inputs`; with ``labels`` and ``obj`` (the device object tables) ``cld_rgb_nrm`` comes
     from :func:`ffb6d_b200.ops.point_item` instead, and its targets are returned as well: ``(inputs,
     (labels_pt, kp_targ_ofst, ctr_targ_ofst) or None)``."""
     import numpy as np
-    from .ops import _fill_depth, _intrinsics_arg, sample_valid_pixels, point_input, point_item
+    from .ops import (_fill_depth, _intrinsics_arg, sample_valid_pixels, point_input, point_item, depth_normal,
+                      depth_to_mm)
     if not isinstance(dpt, torch.Tensor) or dpt.dim() != 3 or dpt.dtype != torch.uint16:
         raise ValueError("dpt must be a [B,H,W] torch.uint16 CUDA tensor")
     dev = dpt.device
@@ -355,7 +395,10 @@ def _build_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_val
             raise ValueError("cam_scale must be positive and finite, got %r" % (cam_scale,))
         depth_m = dpt.to(torch.float32) / torch.full((), cs, dtype=torch.float32, device=dev)
         choose, n_valid = sample_valid_pixels(depth_m, n_points, seed=seed, min_depth=0.0, return_count=True)
-    intr = _intrinsics_arg(K, dpt.shape[0], dev)[0]           # one copy of a host K, shared by both uses
+    intr = _intrinsics_arg(K, dpt.shape[0], dev)[0]           # one copy of a host K, shared by every use
+    if normals == "device":
+        # the depth the datasets give normalSpeed: YCB the completed depth (after add_real_back), LineMOD dpt_mm
+        nrm_map = depth_normal(depth_to_mm(filled, YCB_MM_DIVISOR) if fill else dpt, intr, *NORMAL_ARGS)
     item = build_ffb6d_indices_from_depth(depth_m, intr, choose, k=k, index_dtype=index_dtype, streams=streams)
     targets = None
     if labels is None:
@@ -369,7 +412,7 @@ def _build_inputs(dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_val
 
 
 def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points, seed=0, fill=True,
-                     min_valid=MIN_VALID_PIXELS, k=K_NEIGH, index_dtype=torch.int32, streams=None):
+                     min_valid=MIN_VALID_PIXELS, k=K_NEIGH, index_dtype=torch.int32, streams=None, normals="input"):
     """The datasets' ``get_item`` for a batch on the GPU, from the decoded images to every ``item_dict`` key.
 
     ``fill=True`` is YCB (datasets/ycb/ycb_dataset.py:204-336): depth completion of the raw depth, ``msk_dp``,
@@ -384,7 +427,8 @@ def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points,
     :param cam_scale: raw units per metre (YCB ``meta['factor_depth']``, LineMOD 1000), used as float32
     :param K: camera matrix as :func:`ffb6d_b200.ops.backproject` takes it
     :param rgb: ``[B,H,W,3]`` uint8; :param labels: ``[B,H,W]`` uint8 label image
-    :param nrm_map: ``[B,H,W,3]`` float32 / float64 normal map (computed by the caller, see INTEGRATION.md)
+    :param nrm_map: ``[B,H,W,3]`` float32 / float64 normal map (computed by the caller, see INTEGRATION.md), or None
+      with ``normals="device"``
     :param objects: the per-object arrays of :func:`ffb6d_b200.item.pose_gt_objects`, as a dict of ``[B,...]``
       arrays or tensors (what a DataLoader collates) or a list of B per-frame dicts
     :param min_valid: frames with fewer valid depth pixels are flagged ``valid = False``: the reference returns
@@ -393,8 +437,10 @@ def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points,
       ``labels [B,N]``, ``rgb_labels [B,H,W]`` int32, ``dpt_map_m [B,H,W]``, ``RTs``, ``kp_targ_ofst [B,N,n_kps,3]``,
       ``ctr_targ_ofst [B,N,3]``, ``cls_ids``, ``ctr_3ds``, ``kp_3ds``, the tensors of :func:`build_ffb6d_indices`,
       and ``valid [B]`` bool
+    :param normals: ``"input"`` or ``"device"``, as for :func:`build_ffb6d_inputs`
     """
     import numpy as np
+    check_normals(normals, "build_ffb6d_item", nrm_map)
     if not isinstance(dpt, torch.Tensor) or dpt.dim() != 3 or dpt.dtype != torch.uint16:
         raise ValueError("dpt must be a [B,H,W] torch.uint16 CUDA tensor")
     dev = dpt.device
@@ -402,7 +448,8 @@ def build_ffb6d_item(dpt, cam_scale, K, rgb, labels, nrm_map, objects, n_points,
         objects = {key: np.stack([np.asarray(o[key]) for o in objects]) for key in _OBJECT_KEYS}
     obj = {key: torch.as_tensor(objects[key]).to(dev) for key in _OBJECT_KEYS}
     item, (labels_pt, kp_targ_ofst, ctr_targ_ofst) = _build_inputs(
-        dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_valid, k, index_dtype, streams, labels, obj)
+        dpt, cam_scale, K, rgb, nrm_map, n_points, seed, fill, min_valid, k, index_dtype, streams, labels, obj,
+        normals)
     item.update(labels=labels_pt, rgb_labels=labels.to(torch.int32), RTs=obj["RTs"], kp_targ_ofst=kp_targ_ofst,
                 ctr_targ_ofst=ctr_targ_ofst, cls_ids=obj["cls_ids"], ctr_3ds=obj["ctr_3ds"], kp_3ds=obj["kp_3ds"])
     return item
@@ -415,17 +462,19 @@ TRAIN_RECORD_KEYS = ("jitter", "jittered", "plans", "augment", "apply_rgb")
 TRAIN_BATCH_KEYS = TRAIN_IMAGE_KEYS + TRAIN_RECORD_KEYS + _OBJECT_KEYS
 
 
-def check_train_batch(batch, dataset, name):
-    """``ValueError`` unless ``dataset`` is known and ``batch`` is a dict holding every key of ``TRAIN_BATCH_KEYS``."""
+def check_train_batch(batch, dataset, name, normals="input"):
+    """``ValueError`` unless ``dataset`` is known and ``batch`` is a dict holding every key of ``TRAIN_BATCH_KEYS``
+    (without ``nrm_map``, which it must not hold, under ``normals="device"``)."""
     check_dataset(dataset, name)
+    keys = _normal_keys(batch, name, TRAIN_BATCH_KEYS, normals)
     if not isinstance(batch, dict):
         raise ValueError("%s: the batch must be a dict, got %s" % (name, type(batch).__name__))
-    missing = [k for k in TRAIN_BATCH_KEYS if k not in batch]
+    missing = [k for k in keys if k not in batch]
     if missing:
         raise ValueError("%s: the batch lacks %s" % (name, missing))
 
 
-def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed):
+def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed, normals="input"):
     """The training ``get_item`` of a collated batch on the GPU, in the reference's order: the colour jitter, the first
     ``rgb_add_noise``, ``add_real_back``, the second ``rgb_add_noise``, :func:`build_ffb6d_item` (``fill=True`` for
     YCB, ``False`` for LineMOD) and ``model_fn``'s ``rgb.float()``.  This is INTEGRATION.md's trainer composition in
@@ -440,13 +489,15 @@ def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed):
     :param K: the camera matrix as :func:`build_ffb6d_item` takes it
     :param seed: the key of the noise draws and of the point sampling: an int, or a one-element int64 / uint64 CUDA
       tensor read on the device (the same bits as the int of the same 64 bits)
+    :param normals: ``"input"``: the batch's ``nrm_map``; ``"device"``: the batch holds no ``nrm_map`` and the normals
+      are computed from the composed depth (YCB: completed too), in the reference's order (:func:`build_ffb6d_item`)
     :return: the dict of :func:`build_ffb6d_item` with ``rgb`` as float32
     """
-    check_train_batch(batch, dataset, "build_ffb6d_train_item")
-    return _train_item(batch, dataset, cam_scale, K, n_points, seed)
+    check_train_batch(batch, dataset, "build_ffb6d_train_item", normals)
+    return _train_item(batch, dataset, cam_scale, K, n_points, seed, normals=normals)
 
 
-def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None):
+def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None, normals="input"):
     """:func:`build_ffb6d_train_item` on a checked batch.  ``records``: host copies of ``batch['jitter']`` and
     ``batch['plans']`` when the batch holds those on the device (a graph's input buffers); the host copies are what
     the entry points check, the device ones what the kernels read."""
@@ -467,7 +518,7 @@ def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None):
         K = batch["K"]
         if isinstance(K, torch.Tensor) and K.is_cuda:
             K = _frame_intrinsics(K)
-    item = build_ffb6d_item(dpt, cam_scale, K, rgb, batch["labels"], batch["nrm_map"], batch, n_points, seed=seed,
-                            fill=dataset == "ycb")
+    item = build_ffb6d_item(dpt, cam_scale, K, rgb, batch["labels"], batch.get("nrm_map"), batch, n_points, seed=seed,
+                            fill=dataset == "ycb", normals=normals)
     item["rgb"] = item["rgb"].float()
     return item

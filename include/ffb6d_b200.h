@@ -531,6 +531,41 @@ int ffb6d_fill_depth(const uint16_t *depth_raw, int64_t B, int64_t H, int64_t W,
                      float *filled_raw, float *depth_m, void *workspace, size_t workspace_bytes,
                      ffb6d_stream_t stream);
 
+/*
+ * Surface normals of a millimetre depth map (DESIGN.md §4.30): the least-squares depth-gradient fit of OpenCV's
+ * LINEMOD (`accumBilateral`) with the camera's fx, fy, not quantised.  An opt-in stand-in for the datasets'
+ * `normalSpeed.depth_normal(dpt_mm, fx, fy, k_size, distance_threshold, difference_threshold, point_into_surface)`
+ * (datasets/ycb/ycb_dataset.py:207-210); whether that package computes the same is not known.  For pixel (y, x) with
+ * d = depth_mm[b,y,x] and r = k_size:
+ *   d == 0 or d >= distance_threshold -> (0, 0, 0).  Otherwise over the 8 offsets (dx, dy) in {-r, 0, r}^2 \ {(0,0)}
+ *   inside the image, delta = D[y+dy,x+dx] - d; where |delta| < difference_threshold, in int64:
+ *   A0 += dx dx, A1 += dx dy, A2 += dy dy, b0 += dx delta, b1 += dy delta.  det = A0 A2 - A1^2, ddx = A2 b0 - A1 b1,
+ *   ddy = A0 b1 - A1 b0; det == 0 -> (0, 0, 0).  In float64 without contraction: nx = fx ddx, ny = fy ddy,
+ *   nz = -(double)(det d), s = sqrt((nx nx + ny ny) + nz nz); nrm = (nx/s, ny/s, nz/s), each rounded once to float32,
+ *   negated when point_into_surface is 1.
+ *   depth_mm [B,H,W] uint16; intrinsics (fx, fy, cx, cy) float64 on the device, [4] (intrinsics_per_frame = 0) or
+ *   [B,4] (only fx, fy are read); nrm [B,H,W,3] float32.
+ * 0 <= B <= FFB6D_NRM_MAX_FRAMES (B = 0 is a no-op), 1 <= H <= FFB6D_NRM_MAX_HEIGHT, 1 <= W, H W <=
+ * FFB6D_NRM_MAX_FRAME_PIXELS; 1 <= k_size <= FFB6D_NRM_MAX_KSIZE; 1 <= distance_threshold <= 65536;
+ * 1 <= difference_threshold <= 65535; intrinsics_per_frame, point_into_surface in {0, 1}; depth_mm 2-byte, intrinsics
+ * 8-byte, nrm 4-byte aligned.  Checked before any launch (FFB6D_ERR_INVALID).  One launch, no allocation, no host
+ * synchronisation (capturable in a CUDA graph); deterministic.
+ *
+ * ffb6d_depth_to_mm: depth_mm[i] = (uint16)trunc(depth[i] / divisor) over n floats, the division a float32 IEEE one:
+ * the YCB dataset's `(dpt_um / 10).astype(np.uint16)` of the completed depth (ycb_dataset.py:207) with divisor 10.
+ * Quotients outside [0, 65535] and NaN saturate (0 or 65535).  0 <= n <= FFB6D_NRM_MAX_FRAMES FFB6D_NRM_MAX_FRAME_PIXELS
+ * (n = 0 is a no-op); 0 < divisor < inf; depth 4-byte, depth_mm 2-byte aligned.
+ */
+#define FFB6D_NRM_MAX_KSIZE 16
+#define FFB6D_NRM_MAX_FRAMES 65535
+#define FFB6D_NRM_MAX_HEIGHT (65535 * 8 - 1)
+#define FFB6D_NRM_MAX_FRAME_PIXELS 2147483647ll
+int ffb6d_depth_normal(const uint16_t *depth_mm, int64_t B, int64_t H, int64_t W,
+                       const double *intrinsics, int intrinsics_per_frame,
+                       int k_size, int distance_threshold, int difference_threshold, int point_into_surface,
+                       float *nrm, ffb6d_stream_t stream);
+int ffb6d_depth_to_mm(const float *depth, int64_t n, float divisor, uint16_t *depth_mm, ffb6d_stream_t stream);
+
 /* ---- keypoint voting and pose fitting (the step after the network) -------- */
 /*
  * Gaussian mean shift of G independent vote sets, replacing MeanShiftTorch.fit
