@@ -51,20 +51,32 @@ constexpr int MLP_SMEM = NST * STAGE_BYTES + 64;      // stages + mbarriers: 192
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // round-to-nearest (ties away) to TF32's 10-bit mantissa with two full-rate integer ops; identical to
-// cvt.rna.tf32.f32 for finite inputs (that conversion runs on the quarter-rate conversion pipe)
+// cvt.rna.tf32.f32 for finite inputs below (2 - 2^-11) * 2^127 in magnitude (that conversion runs on the quarter-rate
+// conversion pipe).  Above, in the bit patterns 0x7F7FF000 .. 0x7F7FFFFF of either sign, the rounding carries into the
+// exponent and gives +-inf.
 __device__ __forceinline__ float to_tf32(float x)
 {
     return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
 
-// x = hi + lo.  For a NaN the integer add of to_tf32 can carry the high mantissa bits out of the exponent and wrap
-// it to +-0 (0x7FFFFFFF, the NaN the GPU's own arithmetic produces, among them), and x - hi is NaN for every
-// non-finite x, whose to_tf32 wraps too: an upstream NaN would vanish from the layer.  hi = fma(x - hi, 0, hi)
-// restores it (one FMA-pipe op; hi itself for finite x), so a NaN input comes out NaN, and so does +-inf
-// (inf - inf).
+// to_tf32 with the top band truncated instead, so that a finite x has a finite tf32: the sum is clamped to 0x7F7FFFFF
+// as an int32 (the positive band) and to 0xFF7FFFFF as a uint32 (the negative band); each clamp leaves the other sign
+// alone, and below the band neither fires.  ptxas fuses the add and the int32 clamp into one VIADDMNMX, so this costs
+// one integer op more than to_tf32.
+__device__ __forceinline__ float to_tf32_finite(float x)
+{
+    const uint32_t r = __float_as_uint(x) + 0x1000u;
+    return __uint_as_float(min((uint32_t)min((int)r, 0x7F7FFFFF), 0xFF7FFFFFu) & 0xFFFFE000u);
+}
+
+// x = hi + lo, to 2^-22 |x| + 2^-137 for every finite x (oracle/tf32_oracle.py restates it bit for bit).  Only hi needs
+// the truncated band: |x - hi| <= 2^-10 |x| never reaches it.  For a non-finite x, to_tf32_finite gives a finite value
+// or +-0 (for NaNs near 0x7FFFFFFF, the NaN the GPU's own arithmetic produces, the integer add wraps), and x - hi is
+// NaN or +-inf: an upstream NaN would vanish from the layer.  hi = fma(x - hi, 0, hi) restores it (one FMA-pipe op;
+// hi itself for finite x), so a NaN input comes out NaN, and so does +-inf.
 __device__ __forceinline__ void split1(float x, float &hi, float &lo)
 {
-    const float h = to_tf32(x), d = x - h;
+    const float h = to_tf32_finite(x), d = x - h;
     lo = to_tf32(d);
     hi = __fmaf_rn(d, 0.f, h);
 }
