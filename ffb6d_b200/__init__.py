@@ -53,6 +53,10 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
 * :func:`depth_normal` -- surface normals of millimetre depth maps on the GPU (DESIGN.md §4.30), the opt-in stand-in
   for the datasets' ``normalSpeed.depth_normal``; every item builder and graphed step from frames takes
   ``normals="device"`` to compute them from the depth the reference uses.
+* :func:`render_rgbd` (:mod:`ffb6d_b200.render`) -- synthetic RGB-D frames of vertex-coloured meshes on the GPU, a
+  z-buffer rasteriser (DESIGN.md §4.31) standing in for LineMOD's pre-rendered ``render`` pickles;
+  :func:`build_ffb6d_train_item` and :class:`GraphedFrameTrainStep` take ``meshes=`` a
+  :class:`~ffb6d_b200.render.RenderMeshTable` to render flagged frames of a batch.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -79,10 +83,12 @@ _ITEM = ("pose_gt_objects",)
 _GRAPHED = ("GraphedTrainStep", "GraphedEvalStep", "GraphedFrameTrainStep")
 _ESTIMATE = ("estimate_poses", "GraphedPoseStep")
 _EVALUATE = ("GraphedTestStep",)
+_RENDER = ("render_rgbd",)
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
-               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "estimate", "evaluate", "_lib")
+               "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "estimate", "evaluate", "render",
+               "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED + _ESTIMATE + _EVALUATE) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "estimate", "evaluate", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED + _ESTIMATE + _EVALUATE + _RENDER) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "estimate", "evaluate", "render", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched
@@ -100,6 +106,8 @@ def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op t
         return getattr(importlib.import_module(".estimate", __name__), name)
     if name in _EVALUATE:
         return getattr(importlib.import_module(".evaluate", __name__), name)
+    if name in _RENDER:
+        return getattr(importlib.import_module(".render", __name__), name)
     if name == "DataProcessing":
         return importlib.import_module(".helper_tool", __name__).DataProcessing
     if name in _SUBMODULES:

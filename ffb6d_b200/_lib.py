@@ -47,6 +47,14 @@ NRM_MAX_KSIZE = 16                               # FFB6D_NRM_* of include/ffb6d_
 NRM_MAX_FRAMES = 65535
 NRM_MAX_HEIGHT = 65535 * 8 - 1
 NRM_MAX_FRAME_PIXELS = (1 << 31) - 1
+RND_MAX_FRAMES = 65535                           # FFB6D_RND_* of include/ffb6d_b200.h
+RND_MAX_FRAME_PIXELS = (1 << 31) - 1
+RND_MAX_SLOTS = 4096
+RND_MAX_MESH_VERTS = (1 << 31) - 1
+RND_MAX_FRAME_FACES = 1 << 32
+RND_GUARD_BAND = 1 << 14
+RND_BIG_FACE_PIXELS = 256
+RND_QUEUE_CAP = 1 << 20
 
 
 class FFB6DError(RuntimeError):
@@ -134,6 +142,9 @@ def _load():
         "ffb6d_fill_depth": (ci, [vp, i64, i64, i64, fp, vp, vp, vp, sz, vp]),
         "ffb6d_depth_normal": (ci, [vp, i64, i64, i64, vp, ci, ci, ci, ci, ci, vp, vp]),
         "ffb6d_depth_to_mm": (ci, [vp, i64, fp, vp, vp]),
+        "ffb6d_render_workspace_bytes": (sz, [i64, i64, i64, i64, i64, i64]),
+        "ffb6d_render_rgbd": (ci, [vp, vp, vp, vp, vp, i64, i64, i64, vp, vp, vp, i64, i64, vp, ci, i64, i64,
+                                   C.c_double, vp, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_mean_shift_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_mean_shift_fit": (ci, [vp, vp, i64, i64, i64, fp, ci, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_best_fit_transform": (ci, [vp, vp, i64, i64, vp, vp]),

@@ -462,19 +462,62 @@ TRAIN_RECORD_KEYS = ("jitter", "jittered", "plans", "augment", "apply_rgb")
 TRAIN_BATCH_KEYS = TRAIN_IMAGE_KEYS + TRAIN_RECORD_KEYS + _OBJECT_KEYS
 
 
-def check_train_batch(batch, dataset, name, normals="input"):
+def check_train_batch(batch, dataset, name, normals="input", meshes=None):
     """``ValueError`` unless ``dataset`` is known and ``batch`` is a dict holding every key of ``TRAIN_BATCH_KEYS``
-    (without ``nrm_map``, which it must not hold, under ``normals="device"``)."""
+    (without ``nrm_map``, which it must not hold, under ``normals="device"``), and with ``meshes`` the render keys
+    (:func:`check_render_batch`)."""
     check_dataset(dataset, name)
     keys = _normal_keys(batch, name, TRAIN_BATCH_KEYS, normals)
     if not isinstance(batch, dict):
         raise ValueError("%s: the batch must be a dict, got %s" % (name, type(batch).__name__))
+    check_render_batch(batch, dataset, name, meshes, normals)
     missing = [k for k in keys if k not in batch]
     if missing:
         raise ValueError("%s: the batch lacks %s" % (name, missing))
 
 
-def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed, normals="input"):
+def check_render_batch(batch, dataset, name, meshes, normals):
+    """The render keys of a training batch (``ffb6d_b200.render.RENDER_KEYS``), checked on the host before any CUDA
+    work: with ``meshes`` (a :class:`~ffb6d_b200.render.RenderMeshTable`, LineMOD only, with ``normals="device"``)
+    the batch holds all four, ``rendered [B]`` bool, ``render_mesh [B,M]`` int32, ``render_RTs [B,M,3,4]`` float32
+    and ``render_label [B,M]`` uint8, host values or CUDA tensors, and host mesh indices lie in ``[-1,
+    len(meshes))``; without it, none.
+
+    ``meshes`` with ``normals="input"`` is refused: the reference takes a render's normals from the render's own
+    ``dpt_mm`` (linemod_dataset.py:251-254), which exists only on the device here, so no normal map the worker sends
+    can belong to a rendered frame."""
+    import numpy as np
+    from .render import RENDER_KEYS, RenderMeshTable, check_mesh_indices
+    held = [k for k in RENDER_KEYS if k in batch]
+    if meshes is None:
+        if held:
+            raise ValueError("%s: the batch holds the render keys %s but no meshes were given (pass meshes=, a "
+                             "RenderMeshTable)" % (name, held))
+        return
+    if dataset == "ycb":
+        raise ValueError("%s: meshes= renders LineMOD frames; YCB ships its synthetic frames and its meshes are "
+                         "textured" % name)
+    if not isinstance(meshes, RenderMeshTable):
+        raise ValueError("%s: meshes must be a RenderMeshTable, got %s" % (name, type(meshes).__name__))
+    if normals != "device":
+        raise ValueError("%s: meshes= needs normals='device': a rendered frame's normals come from its own depth, "
+                         "which exists only on the device, so a normal map from the batch cannot belong to it" % name)
+    missing = [k for k in RENDER_KEYS if k not in batch]
+    if missing:
+        raise ValueError("%s: meshes were given but the batch lacks the render keys %s" % (name, missing))
+    B = batch["dpt"].shape[0] if hasattr(batch.get("dpt"), "shape") else None
+    M = tuple(batch["render_mesh"].shape)[1:2] if hasattr(batch["render_mesh"], "shape") else ()
+    want = {"rendered": (torch.bool, (B,)), "render_mesh": (torch.int32, (B,) + M),
+            "render_RTs": (torch.float32, (B,) + M + (3, 4)), "render_label": (torch.uint8, (B,) + M)}
+    for k, (dtype, shape) in want.items():
+        t = batch[k] if isinstance(batch[k], torch.Tensor) else torch.as_tensor(np.asarray(batch[k]))
+        if t.dtype != dtype or tuple(t.shape) != shape or len(M) != 1:
+            raise ValueError("%s: batch[%r] must be %s %s, got %s %s" % (name, k, dtype, shape, t.dtype,
+                                                                       tuple(t.shape)))
+    check_mesh_indices(meshes, batch["render_mesh"], name)
+
+
+def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed, normals="input", meshes=None):
     """The training ``get_item`` of a collated batch on the GPU, in the reference's order: the colour jitter, the first
     ``rgb_add_noise``, ``add_real_back``, the second ``rgb_add_noise``, :func:`build_ffb6d_item` (``fill=True`` for
     YCB, ``False`` for LineMOD) and ``model_fn``'s ``rgb.float()``.  This is INTEGRATION.md's trainer composition in
@@ -491,18 +534,44 @@ def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed, norm
       tensor read on the device (the same bits as the int of the same 64 bits)
     :param normals: ``"input"``: the batch's ``nrm_map``; ``"device"``: the batch holds no ``nrm_map`` and the normals
       are computed from the composed depth (YCB: completed too), in the reference's order (:func:`build_ffb6d_item`)
+    :param meshes: LineMOD only, with ``normals="device"``: a :class:`~ffb6d_b200.render.RenderMeshTable`.  The batch
+      then also holds the render keys (``rendered [B]`` bool, ``render_mesh [B,M]`` int32, ``render_RTs [B,M,3,4]``
+      float32, ``render_label [B,M]`` uint8, host draws or CUDA tensors), and the flagged frames' ``dpt`` / ``rgb`` /
+      ``labels`` are replaced by :func:`~ffb6d_b200.render.render_rgbd` frames (``dpt_mm``) before the colour jitter,
+      as the reference loads a render pickle before ``get_item``'s augmentation.  Every frame's normals are then
+      computed from its composed depth, the rendered frames' from the render's.  The renders go into copies; the
+      batch's tensors are not written
     :return: the dict of :func:`build_ffb6d_item` with ``rgb`` as float32
     """
-    check_train_batch(batch, dataset, "build_ffb6d_train_item", normals)
-    return _train_item(batch, dataset, cam_scale, K, n_points, seed, normals=normals)
+    check_train_batch(batch, dataset, "build_ffb6d_train_item", normals, meshes)
+    return _train_item(batch, dataset, cam_scale, K, n_points, seed, normals=normals, meshes=meshes)
 
 
-def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None, normals="input"):
+def _render_frames(batch, meshes, K, in_place):
+    """The batch with its flagged frames' ``dpt`` / ``rgb`` / ``labels`` rendered (``dpt_mm``): into the batch's own
+    tensors with ``in_place`` (a graph's input buffers), else into copies."""
+    from .render import render_rgbd
+    out = tuple(batch[k] if in_place else batch[k].clone(memory_format=torch.contiguous_format)
+                for k in ("dpt", "rgb", "labels"))
+    B, H, W = out[0].shape
+    render_rgbd(meshes, batch["render_mesh"], batch["render_RTs"], batch["render_label"], K, H, W,
+                active=batch["rendered"], out=out)
+    return dict(batch, dpt=out[0], rgb=out[1], labels=out[2])
+
+
+def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None, normals="input", meshes=None,
+                in_place=False):
     """:func:`build_ffb6d_train_item` on a checked batch.  ``records``: host copies of ``batch['jitter']`` and
     ``batch['plans']`` when the batch holds those on the device (a graph's input buffers); the host copies are what
-    the entry points check, the device ones what the kernels read."""
+    the entry points check, the device ones what the kernels read.  ``in_place``: render into the batch's tensors."""
     import numpy as np
     from .ops import _frame_intrinsics, add_real_back, color_jitter, rgb_add_noise
+    if "K" in batch:
+        K = batch["K"]
+        if isinstance(K, torch.Tensor) and K.is_cuda:
+            K = _frame_intrinsics(K)
+    if meshes is not None:
+        batch = _render_frames(batch, meshes, K, in_place)
     if records is None:
         jitter, plans = np.asarray(batch["jitter"]), np.asarray(batch["plans"])
         jitter_d = plans_d = None
@@ -514,10 +583,6 @@ def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None, norm
     rgb, dpt = add_real_back(rgb, batch["labels"], batch["dpt"], batch["back_rgb"], batch["back_labels"],
                              batch["back_dpt"], batch["apply_rgb"], dataset, active=batch["augment"])
     rgb = rgb_add_noise(rgb, plans[:, 1], seed, plan_dev=None if plans_d is None else plans_d[:, 1])
-    if "K" in batch:
-        K = batch["K"]
-        if isinstance(K, torch.Tensor) and K.is_cuda:
-            K = _frame_intrinsics(K)
     item = build_ffb6d_item(dpt, cam_scale, K, rgb, batch["labels"], batch.get("nrm_map"), batch, n_points, seed=seed,
                             fill=dataset == "ycb", normals=normals)
     item["rgb"] = item["rgb"].float()

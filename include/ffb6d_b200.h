@@ -566,6 +566,56 @@ int ffb6d_depth_normal(const uint16_t *depth_mm, int64_t B, int64_t H, int64_t W
                        float *nrm, ffb6d_stream_t stream);
 int ffb6d_depth_to_mm(const float *depth, int64_t n, float divisor, uint16_t *depth_mm, ffb6d_stream_t stream);
 
+/*
+ * Synthetic RGB-D frames of vertex-coloured meshes (DESIGN.md §4.31): a z-buffer rasteriser, the GPU stand-in for
+ * the LineMOD `render` pickles (datasets/linemod/linemod_dataset.py:202-212).  Per frame b and slot s < M:
+ *   m = mesh_idx[b,s] (-1: empty slot; any value outside [0, n_meshes) draws nothing), RT = RTs[b,s] (float32 [3,4],
+ *   object to camera, metres), label[b,s] (uint8).
+ * Vertex stage, float64 without contraction: X = ((r0 x + r1 y) + r2 z) + t per row; the vertex is culled when
+ *   !(Z >= z_near) or Z is not finite (only non-finite poses or vertices make it so); u = fx (X/Z) + cx,
+ *   v = fy (Y/Z) + cy; culled when !(|u| <= 2^14 && |v| <= 2^14) (guard band); U = rint(256 u), V = rint(256 v) as
+ *   integers (1/256 pixel, ties to even).  A face with a culled vertex is not drawn (culled, not clipped).
+ * Coverage: pixel (col i, row j) samples P = (256 i, 256 j).  With E(a, b, P) = (b.x - a.x)(P.y - a.y) -
+ *   (b.y - a.y)(P.x - a.x): w0 = E(V1, V2, P), w1 = E(V2, V0, P), w2 = E(V0, V1, P), A = E(V0, V1, V2) (exact
+ *   integers).  A == 0: not drawn.  A < 0: A and every w negated (both windings draw).  P is covered when every
+ *   w_k > 0, or w_k == 0 on an owned edge: with (dx, dy) = sign(A) (b - a) of the edge's E(a, b, .), owned is
+ *   dy < 0 || (dy == 0 && dx > 0) (the top-left rule: of two faces sharing an edge exactly one draws it).
+ * Depth and colour, float64 without contraction: p_k = w_k (1/Z_k), S = (p0 + p1) + p2, depth = fl32(A / S);
+ *   colour channel c = clamp(floor((((p0 c0 + p1 c1) + p2 c2) / S) + 0.5), 0, 255) of the vertices' (r, g, b).
+ * Visibility: the least key (bits(depth) << 32) | (s max_faces + f) of a pixel wins: the nearest depth, ties to the
+ *   lower (slot, face).  Empty pixels are 0 in every output.
+ * Mesh table: xyz [V_total,3] float32 metres, vrgb [V_total,3] uint8, faces [F_total,3] int32 (mesh-local vertex
+ *   indices, checked by the caller: 0 <= index < the mesh's vertex count), vert_off / face_off [n_meshes + 1] int64
+ *   (mesh k owns rows [off[k], off[k+1])); max_verts / max_faces: the largest vertex / face count of a mesh.
+ * intrinsics (fx, fy, cx, cy) float64 on the device, [4] (intrinsics_per_frame = 0) or [B,4]; active [B] uint8 or
+ *   NULL (every frame): an inactive frame's outputs are not written.  Exactly one of depth [B,H,W] float32 metres and
+ *   depth_mm [B,H,W] uint16 = min(trunc(fl32(depth * 1000.0f)), 65535) (LineMOD's `dpt_mm`) is non-NULL; rgb
+ *   [B,H,W,3] uint8, labels [B,H,W] uint8.
+ * 0 <= B <= FFB6D_RND_MAX_FRAMES (B = 0 is a no-op), 1 <= H, W, H W <= FFB6D_RND_MAX_FRAME_PIXELS,
+ * 1 <= M <= FFB6D_RND_MAX_SLOTS, 1 <= n_meshes, 1 <= max_verts <= FFB6D_RND_MAX_MESH_VERTS, 1 <= max_faces,
+ * M max_faces <= FFB6D_RND_MAX_FRAME_FACES (the key's 32-bit index), B M max_faces < 2^62; 0.001 <= z_near < inf;
+ * intrinsics_per_frame in {0, 1}; every pointer aligned to its element, workspace to 16 bytes.  Checked before any
+ * launch (FFB6D_ERR_INVALID; FFB6D_ERR_WORKSPACE below ffb6d_render_workspace_bytes).  Launch shapes depend on the
+ * arguments only: one memset and four launches, no allocation, no host synchronisation (capturable in a CUDA graph).
+ * Deterministic: the result does not depend on the order of the atomics.  ffb6d_render_workspace_bytes returns 0
+ * for sizes the entry point refuses.
+ */
+#define FFB6D_RND_MAX_FRAMES 65535
+#define FFB6D_RND_MAX_FRAME_PIXELS 2147483647ll
+#define FFB6D_RND_MAX_SLOTS 4096
+#define FFB6D_RND_MAX_MESH_VERTS 2147483647ll
+#define FFB6D_RND_MAX_FRAME_FACES 4294967296ll
+#define FFB6D_RND_GUARD_BAND 16384
+#define FFB6D_RND_BIG_FACE_PIXELS 256
+#define FFB6D_RND_QUEUE_CAP (1 << 20)
+size_t ffb6d_render_workspace_bytes(int64_t B, int64_t M, int64_t H, int64_t W, int64_t max_verts, int64_t max_faces);
+int ffb6d_render_rgbd(const float *xyz, const uint8_t *vrgb, const int32_t *faces, const int64_t *vert_off,
+                      const int64_t *face_off, int64_t n_meshes, int64_t max_verts, int64_t max_faces,
+                      const int32_t *mesh_idx, const float *RTs, const uint8_t *label, int64_t B, int64_t M,
+                      const double *intrinsics, int intrinsics_per_frame, int64_t H, int64_t W, double z_near,
+                      const uint8_t *active, float *depth, uint16_t *depth_mm, uint8_t *rgb, uint8_t *labels,
+                      void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+
 /* ---- keypoint voting and pose fitting (the step after the network) -------- */
 /*
  * Gaussian mean shift of G independent vote sets, replacing MeanShiftTorch.fit
