@@ -57,6 +57,8 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   z-buffer rasteriser (DESIGN.md §4.31) standing in for LineMOD's pre-rendered ``render`` pickles;
   :func:`build_ffb6d_train_item` and :class:`GraphedFrameTrainStep` take ``meshes=`` a
   :class:`~ffb6d_b200.render.RenderMeshTable` to render flagged frames of a batch.
+* :func:`orb_detect` / :func:`orb_lift` -- ORB keypoints of ``cv2.ORB_create()``'s defaults on the GPU and their
+  lift onto the mesh (DESIGN.md §4.32), the stages behind :func:`ffb6d_b200.objinfo.textured_kp3ds`.
 * :mod:`ffb6d_b200.modules` -- ``nn.Module`` twins of the fusion ``Conv2d`` and of RandLA's
   ``Att_pooling`` / ``Building_block`` / ``Dilated_res_block`` (reference parameter names).
 
@@ -75,7 +77,7 @@ _OPS = ("knn_search", "random_sample", "nearest_interpolation", "gather_neighbou
         "aug_noise_field", "color_jitter", "psp_pool", "psp_pack", "psp_bottleneck", "conv1x1_log_softmax",
         "psp_bottleneck_bwd", "psp_pool_bwd", "log_softmax_bwd", "upsample_bilinear2d_bwd", "upsample_bilinear2d",
         "farthest_point_sampling", "pose_add_adds", "vote_poses", "point_input", "rgb_noise_check_records",
-        "color_jitter_check_plans", "eval_record", "eval_auc", "depth_normal")
+        "color_jitter_check_plans", "eval_record", "eval_auc", "depth_normal", "orb_detect", "orb_lift")
 _SCHEDULE = ("build_ffb6d_indices", "build_ffb6d_indices_from_depth", "build_ffb6d_indices_native",
              "build_ffb6d_indices_from_raw_depth", "build_ffb6d_item", "build_ffb6d_inputs", "build_ffb6d_train_item")
 _TABLES = ("knn_schedule", "gather_schedule", "fusion_mlp_schedule")

@@ -55,6 +55,11 @@ RND_MAX_FRAME_FACES = 1 << 32
 RND_GUARD_BAND = 1 << 14
 RND_BIG_FACE_PIXELS = 256
 RND_QUEUE_CAP = 1 << 20
+ORB_MAX_FRAMES = 65535                           # FFB6D_ORB_* of include/ffb6d_b200.h
+ORB_MIN_SIDE = 2
+ORB_MAX_SIDE = 8192
+ORB_LEVELS = 8
+ORB_MAX_OBJECTS = 65535
 
 
 class FFB6DError(RuntimeError):
@@ -145,6 +150,10 @@ def _load():
         "ffb6d_render_workspace_bytes": (sz, [i64, i64, i64, i64, i64, i64]),
         "ffb6d_render_rgbd": (ci, [vp, vp, vp, vp, vp, i64, i64, i64, vp, vp, vp, i64, i64, vp, ci, i64, i64,
                                    C.c_double, vp, vp, vp, vp, vp, vp, sz, vp]),
+        "ffb6d_orb_capacity": (i64, [i64, i64]),
+        "ffb6d_orb_workspace_bytes": (sz, [i64, i64, i64]),
+        "ffb6d_orb_detect": (ci, [vp, i64, i64, i64, vp, vp, vp, vp, i64, vp, sz, vp]),
+        "ffb6d_orb_lift": (ci, [vp, vp, i64, vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp]),
         "ffb6d_mean_shift_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_mean_shift_fit": (ci, [vp, vp, i64, i64, i64, fp, ci, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_best_fit_transform": (ci, [vp, vp, i64, i64, vp, vp]),

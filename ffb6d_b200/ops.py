@@ -969,6 +969,85 @@ def depth_normal(dpt_mm, K, k_size=5, distance_threshold=2000, difference_thresh
     return nrm
 
 
+def orb_detect(rgb):
+    """ORB keypoints of ``cv2.ORB_create()``'s defaults on the GPU (``ffb6d_orb_detect``, DESIGN.md §4.32): what
+    ``ORB_create().detect`` returns for each frame's BGR image, bit for bit as a set (pinned through
+    oracle/orb_oracle.py), in level then raster order.
+
+    :param rgb: ``[B,H,W,3]`` (or ``[H,W,3]``) uint8 CUDA, RGB as :func:`ffb6d_b200.render.render_rgbd` returns it;
+      ``2 <= H, W <= 8192``
+    :return: ``(count [B] int32, pt [B,cap,2] float32 (x, y), octave [B,cap] int32, response [B,cap] float32)`` on
+      the device (no synchronisation); frame b's keypoints are its first ``count[b]`` rows (later rows hold
+      scratch).  ``cap`` (``ffb6d_orb_capacity``) bounds what the detector can keep, so nothing is ever clipped.
+    """
+    if not isinstance(rgb, torch.Tensor) or rgb.dtype != torch.uint8:
+        raise ValueError("orb_detect: rgb must be a uint8 tensor, got %s" % getattr(rgb, "dtype", type(rgb).__name__))
+    _need_cuda(rgb, "rgb")
+    if rgb.dim() not in (3, 4) or rgb.shape[-1] != 3:
+        raise ValueError("orb_detect: rgb must be [B,H,W,3] or [H,W,3], got %s" % (tuple(rgb.shape),))
+    x = rgb.contiguous() if rgb.dim() == 4 else rgb.contiguous()[None]
+    B, H, W = (int(n) for n in x.shape[:3])
+    if not (_lib.ORB_MIN_SIDE <= H <= _lib.ORB_MAX_SIDE and _lib.ORB_MIN_SIDE <= W <= _lib.ORB_MAX_SIDE):
+        raise ValueError("orb_detect: H and W must lie in [%d, %d], got %dx%d"
+                         % (_lib.ORB_MIN_SIDE, _lib.ORB_MAX_SIDE, H, W))
+    if B > _lib.ORB_MAX_FRAMES:
+        raise ValueError("orb_detect: at most %d frames, got %d" % (_lib.ORB_MAX_FRAMES, B))
+    cap = int(lib.ffb6d_orb_capacity(H, W))
+    dev = x.device
+    count = torch.zeros(B, dtype=torch.int32, device=dev)
+    pt = torch.zeros((B, cap, 2), dtype=torch.float32, device=dev)
+    octave = torch.zeros((B, cap), dtype=torch.int32, device=dev)
+    response = torch.zeros((B, cap), dtype=torch.float32, device=dev)
+    nbytes = int(lib.ffb6d_orb_workspace_bytes(B, H, W))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_orb_detect, dev, x.data_ptr(), B, H, W, count.data_ptr(), pt.data_ptr(), octave.data_ptr(),
+           response.data_ptr(), cap, ws.data_ptr(), nbytes)
+    return count, pt, octave, response
+
+
+def orb_lift(count, pt, depth, K, RTs, views):
+    """Lift the keypoints of :func:`orb_detect` into the object frame as the reference's textured keypoint tool does
+    (``ffb6d_orb_lift``; rgbd_rnder_sift_kp3ds.py:138-155): the depth at ``(int(pt.y), int(pt.x))`` back-projected,
+    points with a non-finite x or ``z <= 1e-8`` dropped, then ``(p - t) . R``.
+
+    :param count, pt: as :func:`orb_detect` returns them for ``B = n_obj * views`` renders, object o's views being
+      frames ``o * views ... o * views + views - 1``
+    :param depth: ``[B,H,W]`` float32 CUDA metres (0 where nothing is drawn)
+    :param K: camera as :func:`backproject` takes it; :param RTs: ``[B,3,4]`` or ``[B,4,4]`` object-to-camera poses
+      (host arrays or CUDA tensors, taken as float64)
+    :return: ``(cloud [n_obj, views * cap, 3] float32, n_points [n_obj] int32)`` on the device: each object's points,
+      views in order, ready for ``farthest_point_sampling(cloud, n, n_points=n_points)``.
+    """
+    for t, name in ((count, "count"), (pt, "pt"), (depth, "depth")):
+        _need_cuda(t, name)
+    if count.dtype != torch.int32 or pt.dtype != torch.float32 or depth.dtype != torch.float32:
+        raise ValueError("orb_lift: count must be int32, pt and depth float32")
+    if depth.dim() != 3 or count.dim() != 1 or pt.dim() != 3 or pt.shape[-1] != 2:
+        raise ValueError("orb_lift: need count [B], pt [B,cap,2] and depth [B,H,W]")
+    B, H, W = (int(n) for n in depth.shape)
+    cap = int(lib.ffb6d_orb_capacity(H, W))
+    if tuple(count.shape) != (B,) or tuple(pt.shape) != (B, cap, 2):
+        raise ValueError("orb_lift: count must be [%d] and pt [%d,%d,2] for %dx%d frames, got %s and %s"
+                         % (B, B, cap, H, W, tuple(count.shape), tuple(pt.shape)))
+    if isinstance(views, bool) or not isinstance(views, (int, np.integer)) or views < 1 or B % views:
+        raise ValueError("orb_lift: views must be a positive int dividing B=%d, got %r" % (B, views))
+    views = int(views)
+    if B // views > _lib.ORB_MAX_OBJECTS or views * cap >= 1 << 31:
+        raise ValueError("orb_lift: %d objects of %d views exceed the limits" % (B // views, views))
+    dev = depth.device
+    rt = RTs if isinstance(RTs, torch.Tensor) else torch.from_numpy(np.asarray(RTs, np.float64))
+    if rt.dim() != 3 or rt.shape[0] != B or tuple(rt.shape[1:]) not in ((3, 4), (4, 4)):
+        raise ValueError("orb_lift: RTs must be [B,3,4] or [B,4,4], got %s" % (tuple(rt.shape),))
+    rt = rt[:, :3, :].to(device=dev, dtype=torch.float64).contiguous()
+    intr, per_frame = _intrinsics_arg(K, B, dev)
+    cloud = torch.zeros((B // views, views * cap, 3), dtype=torch.float32, device=dev)
+    n_points = torch.zeros(B // views, dtype=torch.int32, device=dev)
+    launch(lib.ffb6d_orb_lift, dev, count.contiguous().data_ptr(), pt.contiguous().data_ptr(), cap,
+           depth.contiguous().data_ptr(), B, H, W, intr.data_ptr(), per_frame, rt.data_ptr(), views,
+           cloud.data_ptr(), n_points.data_ptr())
+    return cloud, n_points
+
+
 def depth_to_mm(depth, divisor=10.0):
     """``(depth / divisor).astype(np.uint16)`` on the GPU (``ffb6d_depth_to_mm``): a float32 IEEE division, then a
     truncation, as numpy computes it for in-range values (out of range, where numpy's cast is undefined, it saturates).

@@ -616,6 +616,47 @@ int ffb6d_render_rgbd(const float *xyz, const uint8_t *vrgb, const int32_t *face
                       const uint8_t *active, float *depth, uint16_t *depth_mm, uint8_t *rgb, uint8_t *labels,
                       void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
 
+/*
+ * ORB keypoints of cv2.ORB_create()'s defaults (DESIGN.md §4.32; oracle/orb_oracle.py restates every step), the 2D
+ * stage of the reference's textured keypoint tool (utils/dataset_tools/rgbd_rnder_sift_kp3ds.py:138-166).
+ * ffb6d_orb_detect: rgb [B,H,W,3] uint8 -> per frame b, count[b] keypoints in pt [B,cap,2] float32 (x, y image
+ *   coordinates), octave [B,cap] int32 and response [B,cap] float32 (Harris), level then raster order; entries past
+ *   count[b] hold scratch (candidates of the Harris cut); pt, octave and response may be NULL when cap = 0.
+ *   cap = ffb6d_orb_capacity(H, W) = sum over the 8 levels of ceil(w_l' / 2) ceil(h_l' / 2), w_l' = max(w_l - 62, 0)
+ *   (the border-filtered level): strict 3x3 non-maximum suppression keeps at most one point per 2x2 block, so the
+ *   output can never overflow, however many points the tie-inclusive cuts keep.
+ *   Grey (3735 B + 19235 G + 9798 R + 2^14) >> 15; level l of size cvRound(W (1 / s_l)) x cvRound(H (1 / s_l)),
+ *   s_l = float32(pow(double(1.2f), l)), is INTER_LINEAR_EXACT of level l-1; FAST-9/16 at threshold 20 with strict
+ *   3x3 non-maximum suppression; 31 <= x < w_l - 31, 31 <= y < h_l - 31; every point whose FAST score is >= the
+ *   (2 n_l)-th best; Harris (7x7, k = 0.04, integer sums, float32 rounded per operation); every point whose response
+ *   is >= the n_l-th best, n_l = nfeaturesPerLevel of 500 features; pt = float32(x_l) s_l.
+ *   2 <= H, W <= FFB6D_ORB_MAX_SIDE, 0 <= B <= FFB6D_ORB_MAX_FRAMES (B = 0 is a no-op), cap as above.
+ * ffb6d_orb_lift: the keypoints of B = n_obj views renders (object o's views are frames o views ... o views + views
+ *   - 1) lifted into the object frame as the tool does: pixel (u, v) = (int(pt.x), int(pt.y)), z = depth[b, v, u]
+ *   (float32 metres), x = ((u - cx) z) / fx, y = ((v - cy) z) / fy in float64 without contraction; kept when x is
+ *   finite and z > 1e-8 (and the pixel lies in the frame); q = p - t, out_j = (q0 R0j + q1 R1j) + q2 R2j with the
+ *   view's RTs [B,3,4] float64 (object to camera), rounded once to float32.  cloud [n_obj, views cap, 3] float32
+ *   holds each object's points, views in order, keypoints in order; n_points [n_obj] int32 their number (entries past
+ *   it are not written).  intrinsics (fx, fy, cx, cy) float64, [4] or [B,4].  1 <= views, B = n_obj views,
+ *   n_obj <= FFB6D_ORB_MAX_OBJECTS, views cap < 2^31.
+ * Arguments are checked before any launch (FFB6D_ERR_INVALID; FFB6D_ERR_WORKSPACE below
+ * ffb6d_orb_workspace_bytes, which like ffb6d_orb_capacity returns 0 for sizes the entry point refuses).  Launch
+ * shapes depend on the arguments only and neither entry point synchronises: both can be captured in a CUDA graph.
+ * Deterministic: no atomic decides an output position.
+ */
+#define FFB6D_ORB_MAX_FRAMES 65535
+#define FFB6D_ORB_MIN_SIDE 2
+#define FFB6D_ORB_MAX_SIDE 8192
+#define FFB6D_ORB_LEVELS 8
+#define FFB6D_ORB_MAX_OBJECTS 65535
+int64_t ffb6d_orb_capacity(int64_t H, int64_t W);
+size_t ffb6d_orb_workspace_bytes(int64_t B, int64_t H, int64_t W);
+int ffb6d_orb_detect(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, int32_t *count, float *pt, int32_t *octave,
+                     float *response, int64_t cap, void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
+int ffb6d_orb_lift(const int32_t *count, const float *pt, int64_t cap, const float *depth, int64_t B, int64_t H,
+                   int64_t W, const double *intrinsics, int intrinsics_per_frame, const double *RTs, int64_t views,
+                   float *cloud, int32_t *n_points, ffb6d_stream_t stream);
+
 /* ---- keypoint voting and pose fitting (the step after the network) -------- */
 /*
  * Gaussian mean shift of G independent vote sets, replacing MeanShiftTorch.fit
