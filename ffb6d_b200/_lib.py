@@ -60,6 +60,12 @@ ORB_MIN_SIDE = 2
 ORB_MAX_SIDE = 8192
 ORB_LEVELS = 8
 ORB_MAX_OBJECTS = 65535
+SIFT_MAX_FRAMES = 65535                          # FFB6D_SIFT_* of include/ffb6d_b200.h
+SIFT_MIN_SIDE = 4
+SIFT_MAX_SIDE = 2048
+SIFT_MAX_CAP = 1 << 26
+SIFT_CHUNK = 16
+SIFT_MAX_COPIES = 18
 
 
 class FFB6DError(RuntimeError):
@@ -154,6 +160,10 @@ def _load():
         "ffb6d_orb_workspace_bytes": (sz, [i64, i64, i64]),
         "ffb6d_orb_detect": (ci, [vp, i64, i64, i64, vp, vp, vp, vp, i64, vp, sz, vp]),
         "ffb6d_orb_lift": (ci, [vp, vp, i64, vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp]),
+        "ffb6d_sift_capacity": (i64, [i64, i64]),
+        "ffb6d_sift_workspace_bytes": (sz, [i64, i64, i64]),
+        "ffb6d_sift_detect": (ci, [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, i64, vp, sz, vp]),
+        "ffb6d_sift_lift": (ci, [vp, vp, i64, vp, i64, i64, i64, vp, ci, vp, i64, vp, vp, vp]),
         "ffb6d_mean_shift_workspace_bytes": (sz, [i64, i64]),
         "ffb6d_mean_shift_fit": (ci, [vp, vp, i64, i64, i64, fp, ci, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_best_fit_transform": (ci, [vp, vp, i64, i64, vp, vp]),

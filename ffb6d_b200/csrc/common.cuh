@@ -89,6 +89,12 @@ int64_t wgrad_small_splits(int64_t B, int64_t P);
 int wgrad_small_det_launch(const float *grad_z, const float *x1, int64_t C1, const float *x2, int64_t C2, int64_t B,
                            int64_t Co, int64_t P, float *part, cudaStream_t st);
 
+// orb.cu: the lift of keypoints into the object frame behind ffb6d_orb_lift and ffb6d_sift_lift (arguments checked
+// by the entry points; frame b's first min(count[b], cap) points are lifted)
+int keypoint_lift_launch(const int32_t *count, const float *pt, int64_t cap, const float *depth, int64_t B, int64_t H,
+                         int64_t W, const double *intrinsics, int intrinsics_per_frame, const double *RTs,
+                         int64_t views, float *cloud, int32_t *n_points, cudaStream_t st);
+
 // Debugging switches, read ONCE per process (never in a launch path; results never depend on them).
 struct Env {
     bool check_indices;     // FFB6D_CHECK_INDICES=1: validate gather indices (synchronises; debugging aid)

@@ -409,7 +409,7 @@ __global__ void __launch_bounds__(kThreads) lift_kernel(LiftArgs a)
     int64_t m = 0;
     for (int64_t v = 0; v < a.views; ++v) {
         const int64_t b = obj * a.views + v;
-        const int n = a.count[b];
+        const int n = (int)min((int64_t)a.count[b], a.cap);     // a SIFT count past cap: only cap rows hold points
         const float *pt = a.pt + b * a.cap * 2;
         const float *dep = a.depth + b * (int64_t)a.H * a.W;
         const double *k = a.intr + (a.intr_per_frame ? b * 4 : 0);
@@ -543,6 +543,15 @@ extern "C" int ffb6d_orb_lift(const int32_t *count, const float *pt, int64_t cap
     FFB6D_CHECK_ARG(count && pt && depth && intrinsics && RTs && cloud && n_points, "orb_lift: null pointer");
     FFB6D_CHECK_ARG(aligned(count, 4) && aligned(pt, 4) && aligned(depth, 4) && aligned(intrinsics, 8) &&
                     aligned(RTs, 8) && aligned(cloud, 4) && aligned(n_points, 4), "orb_lift: misaligned pointer");
+    return keypoint_lift_launch(count, pt, cap, depth, B, H, W, intrinsics, intrinsics_per_frame, RTs, views, cloud,
+                                n_points, (cudaStream_t)stream);
+}
+
+// the lift of ffb6d_orb_lift and ffb6d_sift_lift, arguments checked by the caller
+int ffb6d::keypoint_lift_launch(const int32_t *count, const float *pt, int64_t cap, const float *depth, int64_t B,
+                                int64_t H, int64_t W, const double *intrinsics, int intrinsics_per_frame,
+                                const double *RTs, int64_t views, float *cloud, int32_t *n_points, cudaStream_t st)
+{
     LiftArgs a;
     a.count = count;
     a.pt = pt;
@@ -556,7 +565,7 @@ extern "C" int ffb6d_orb_lift(const int32_t *count, const float *pt, int64_t cap
     a.views = views;
     a.cloud = cloud;
     a.n_points = n_points;
-    lift_kernel<<<(unsigned)(B / views), kThreads, 0, (cudaStream_t)stream>>>(a);
+    lift_kernel<<<(unsigned)(B / views), kThreads, 0, st>>>(a);
     FFB6D_LAUNCH_OK("orb_lift_kernel");
     return FFB6D_OK;
 }

@@ -10,7 +10,8 @@ Mesh files are not read here: the caller passes the vertex array ``[N,3]`` (what
 returns, already divided by ``scale2m``).  The tool's textured keypoints -- ORB corners of renders from a sphere of
 views, lifted onto the mesh and reduced by farthest point sampling (rgbd_rnder_sift_kp3ds.py:138-166,
 gen_obj_info.py:119-126), the table the datasets read with ``use_orbfps`` -- run on the GPU through
-:func:`textured_kp3ds` (DESIGN.md §4.32).  Plain numpy; only :func:`gen_obj_info` and :func:`textured_kp3ds` load
+:func:`textured_kp3ds` (DESIGN.md §4.32); the tool's ``--extractor SIFT`` (the paper's SIFT-FPS keypoints) through
+``textured_kp3ds(..., extractor="SIFT")`` (§4.33).  Plain numpy; only :func:`gen_obj_info` and :func:`textured_kp3ds` load
 the CUDA library.
 """
 import math
@@ -98,22 +99,27 @@ def sphere_poses(radius, n_longitude=3, n_latitude=3):
     return np.stack([o2c_pose(camera_pose(p)) for p in camera_positions(n_longitude, n_latitude, sph_r)])
 
 
-def textured_kp3ds(table, mesh, K=TOOL_K, H=TOOL_H, W=TOOL_W, n_longitude=3, n_latitude=3, radius=None):
+def textured_kp3ds(table, mesh, K=TOOL_K, H=TOOL_H, W=TOOL_W, n_longitude=3, n_latitude=3, radius=None,
+                   extractor="ORB"):
     """The tool's ``extract_textured_kp3ds`` on the GPU for one or more meshes of a
     :class:`~ffb6d_b200.render.RenderMeshTable`: each object rendered from its sphere of views (``render_rgbd``),
-    ORB keypoints of every render (``orb_detect``) and their lift into the object frame (``orb_lift``).
+    ORB keypoints of every render (``orb_detect``) and their lift into the object frame (``orb_lift``); with
+    ``extractor="SIFT"`` the tool's SIFT branch, ``sift_detect`` and ``sift_lift``.
 
     :param mesh: an index into ``table``, or a list of them (one object each)
     :param K, H, W: the camera and frame size (the tool's defaults); :param n_longitude, n_latitude: the views
     :param radius: each object's box radius (:func:`get_r`), or None to compute it from the table's vertices
+    :param extractor: ``"ORB"`` or ``"SIFT"``, the tool's ``--extractor``
     :return: ``(cloud [n_obj, V cap, 3] float32, n_points [n_obj] int32, short [n_obj, V] bool)`` on the device, V =
       n_longitude n_latitude: each object's pooled points, views in order.  A view with fewer than 500 drawn pixels
       contributes no points and is flagged in ``short`` (the tool stops with an error there).
     """
     import torch
     from . import _lib
-    from .ops import orb_detect, orb_lift
+    from .ops import orb_detect, orb_lift, sift_detect, sift_lift
     from .render import RenderMeshTable, render_rgbd
+    if extractor not in ("ORB", "SIFT"):
+        raise ValueError("textured_kp3ds: extractor must be 'ORB' or 'SIFT', got %r" % (extractor,))
     if not isinstance(table, RenderMeshTable):
         raise ValueError("textured_kp3ds: table must be a RenderMeshTable, got %s" % type(table).__name__)
     objs = [int(m) for m in (mesh if isinstance(mesh, (list, tuple, np.ndarray)) else [mesh])]
@@ -125,9 +131,9 @@ def textured_kp3ds(table, mesh, K=TOOL_K, H=TOOL_H, W=TOOL_W, n_longitude=3, n_l
         raise ValueError("textured_kp3ds: %d objects of %d views exceed the render limit of %d frames"
                          % (len(objs), V, min(_lib.RND_MAX_FRAMES, _lib.ORB_MAX_FRAMES)))
     H, W = int(H), int(W)
-    if not (_lib.ORB_MIN_SIDE <= H <= _lib.ORB_MAX_SIDE and _lib.ORB_MIN_SIDE <= W <= _lib.ORB_MAX_SIDE):
-        raise ValueError("textured_kp3ds: H and W must lie in [%d, %d], got %dx%d"
-                         % (_lib.ORB_MIN_SIDE, _lib.ORB_MAX_SIDE, H, W))
+    lo, hi = (_lib.ORB_MIN_SIDE, _lib.ORB_MAX_SIDE) if extractor == "ORB" else (_lib.SIFT_MIN_SIDE, _lib.SIFT_MAX_SIDE)
+    if not (lo <= H <= hi and lo <= W <= hi):
+        raise ValueError("textured_kp3ds: H and W must lie in [%d, %d], got %dx%d" % (lo, hi, H, W))
     if radius is None:
         off = np.concatenate([[0], np.cumsum(table.n_verts)])
         xyz = table.xyz.cpu().numpy()
@@ -140,15 +146,16 @@ def textured_kp3ds(table, mesh, K=TOOL_K, H=TOOL_H, W=TOOL_W, n_longitude=3, n_l
     mesh_idx = np.repeat(np.asarray(objs, np.int32), V)[:, None]
     depth, rgb, _ = render_rgbd(table, mesh_idx, RT[:, None, :3, :].astype(np.float32), np.ones((B, 1), np.uint8),
                                 K, H, W)
-    count, pt, _, _ = orb_detect(rgb)
+    detect, lift = (orb_detect, orb_lift) if extractor == "ORB" else (sift_detect, sift_lift)
+    count, pt = detect(rgb)[:2]
     short = torch.count_nonzero(depth > 1e-8, dim=(1, 2)) < MIN_RENDER_PIXELS
     count = torch.where(short, torch.zeros_like(count), count)
-    cloud, n_points = orb_lift(count, pt, depth, K, RT, V)
+    cloud, n_points = lift(count, pt, depth, K, RT, V)
     return cloud, n_points, short.view(len(objs), V)
 
 
 def gen_obj_info(points, n_keypoint=8, init_center=False, start=None, *, mesh=None, K=TOOL_K, H=TOOL_H, W=TOOL_W,
-                 n_longitude=3, n_latitude=3, textured_start=None):
+                 n_longitude=3, n_latitude=3, textured_start=None, extractor="ORB"):
     """The tables ``gen_one_mesh_info`` computes for one object's vertices ``points [N,3]``.
 
     :param n_keypoint: number of farthest-point keypoints (the tool's ``--n_keypoint``, 8 in the reference's configs)
@@ -158,28 +165,35 @@ def gen_obj_info(points, n_keypoint=8, init_center=False, start=None, *, mesh=No
       ``points``): then the tool's textured keypoints are computed too (:func:`textured_kp3ds` with ``K``, ``H``,
       ``W``, ``n_longitude``, ``n_latitude``), and their farthest point sampling starts at ``textured_start`` (None:
       random, as the tool's)
+    :param extractor: the textured keypoints' detector, ``"ORB"`` or ``"SIFT"`` (the tool's ``--extractor``)
     :return: dict ``corners [8,3]``, ``radius``, ``center [3]`` and ``fps [n_keypoint,3]`` (float32 vertices).
       ``fps`` is what ``pose_gt_objects(kps=...)`` and ``cal_frame_poses(mesh_kps=...)`` take as an object's keypoints.
       With ``mesh`` also ``textured_fps [n_keypoint,3]`` (float32; what ``use_orbfps`` reads) and ``short_views``
-      (indices of views with fewer than 500 drawn pixels, which contributed no points).
+      (indices of views with fewer than 500 drawn pixels, which contributed no points).  With
+      ``extractor="SIFT"`` also ``extractor`` (``"SIFT"``), which :func:`write_obj_info` names the file by.
     """
     from ._lib import FPS_MAX_POINTS
     from .ops import farthest_point_sampling
     points = np.asarray(points)
     if points.ndim != 2 or points.shape[1] != 3 or points.shape[0] < 1:
         raise ValueError("points must be [N,3] with N >= 1, got shape %s" % (points.shape,))
+    if extractor not in ("ORB", "SIFT"):
+        raise ValueError("gen_obj_info: extractor must be 'ORB' or 'SIFT', got %r" % (extractor,))
     c3ds = get_3D_bbox(points)
     info = dict(corners=c3ds, radius=get_r(c3ds), center=get_centers_3d(c3ds),
                 fps=farthest_point_sampling(points, n_keypoint, init_center=init_center, start=start))
     if mesh is None:
         return info
-    cloud, n_points, short = textured_kp3ds(mesh, 0, K, H, W, n_longitude, n_latitude, radius=info["radius"])
+    cloud, n_points, short = textured_kp3ds(mesh, 0, K, H, W, n_longitude, n_latitude, radius=info["radius"],
+                                            extractor=extractor)
     n = int(n_points[0])
     if not 1 <= n <= FPS_MAX_POINTS:
         raise ValueError("gen_obj_info: %d textured keypoints; farthest point sampling takes 1 to %d" % (n, FPS_MAX_POINTS))
     info["textured_fps"] = farthest_point_sampling(cloud[0, :n].contiguous(), n_keypoint,
                                                    start=textured_start).cpu().numpy()
     info["short_views"] = np.nonzero(short[0].cpu().numpy())[0]
+    if extractor != "ORB":
+        info["extractor"] = extractor
     return info
 
 
@@ -188,7 +202,8 @@ def write_obj_info(info, sv_fd, obj_name):
     ``<obj>_radius.txt``, ``<obj>_center.txt`` and ``<obj>_fps.txt`` under ``sv_fd``, one point per line.  They load
     back with ``np.loadtxt(path, dtype=np.float32)``, as ``Basic_Utils.get_kps`` / ``get_ctr`` read them.  When
     ``info`` has ``textured_fps``, ``<obj>_ORB_fps.txt`` too (gen_obj_info.py:122-126), which the datasets read as
-    ``<obj>_8_kps.txt`` with ``use_orbfps``.
+    ``<obj>_8_kps.txt`` with ``use_orbfps`` -- ``<obj>_SIFT_fps.txt`` when ``info["extractor"]`` is ``"SIFT"``, the
+    tool's name for its SIFT branch.
     :return: dict of the paths written."""
     os.makedirs(sv_fd, exist_ok=True)
     paths = {k: os.path.join(sv_fd, "%s_%s.txt" % (obj_name, k)) for k in ("corners", "radius", "center", "fps")}
@@ -204,8 +219,9 @@ def write_obj_info(info, sv_fd, obj_name):
         for p3d in info["fps"]:
             print(p3d[0], p3d[1], p3d[2], file=of)
     if "textured_fps" in info:
-        paths["ORB_fps"] = os.path.join(sv_fd, "%s_ORB_fps.txt" % obj_name)
-        with open(paths["ORB_fps"], 'w') as of:
+        key = "%s_fps" % info.get("extractor", "ORB")
+        paths[key] = os.path.join(sv_fd, "%s_%s.txt" % (obj_name, key))
+        with open(paths[key], 'w') as of:
             for p3d in info["textured_fps"]:
                 print(p3d[0], p3d[1], p3d[2], file=of)
     return paths

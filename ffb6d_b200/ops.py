@@ -1048,6 +1048,96 @@ def orb_lift(count, pt, depth, K, RTs, views):
     return cloud, n_points
 
 
+def sift_detect(rgb, cap=None, check=True):
+    """SIFT keypoints of ``cv2.SIFT_create()``'s defaults on the GPU (``ffb6d_sift_detect``, DESIGN.md §4.33): what
+    ``SIFT_create().detect`` returns for each frame's BGR image, bitwise oracle/sift_oracle.py's, in canonical order
+    (octave, DoG layer, raster order, orientation peaks in histogram order).  Keypoints only, no descriptors.
+
+    :param rgb: ``[B,H,W,3]`` (or ``[H,W,3]``) uint8 CUDA, RGB as :func:`ffb6d_b200.render.render_rgbd` returns it;
+      ``4 <= H, W <= 2048``
+    :param cap: rows per frame of the outputs (None: ``ffb6d_sift_capacity(H, W)``, ``max(H W / 16, 256)``)
+    :param check: read the counts back once and, when a frame's keypoints did not fit, run again with a cap that
+      fits.  Pass False where nothing may synchronise (CUDA-graph capture); ``count[b] > cap`` then marks a frame
+      that did not fit, and a call with ``cap >= count[b]`` fits it.
+    :return: ``(count [B] int32, pt [B,cap,2] float32 (x, y), octave [B,cap] int32 (OpenCV's packing), size
+      [B,cap] float32, angle [B,cap] float32 degrees)`` on the device; frame b's keypoints are its first
+      ``count[b]`` rows.
+    """
+    if not isinstance(rgb, torch.Tensor) or rgb.dtype != torch.uint8:
+        raise ValueError("sift_detect: rgb must be a uint8 tensor, got %s" % getattr(rgb, "dtype", type(rgb).__name__))
+    _need_cuda(rgb, "rgb")
+    if rgb.dim() not in (3, 4) or rgb.shape[-1] != 3:
+        raise ValueError("sift_detect: rgb must be [B,H,W,3] or [H,W,3], got %s" % (tuple(rgb.shape),))
+    x = rgb.contiguous() if rgb.dim() == 4 else rgb.contiguous()[None]
+    B, H, W = (int(n) for n in x.shape[:3])
+    if not (_lib.SIFT_MIN_SIDE <= H <= _lib.SIFT_MAX_SIDE and _lib.SIFT_MIN_SIDE <= W <= _lib.SIFT_MAX_SIDE):
+        raise ValueError("sift_detect: H and W must lie in [%d, %d], got %dx%d"
+                         % (_lib.SIFT_MIN_SIDE, _lib.SIFT_MAX_SIDE, H, W))
+    if B > _lib.SIFT_MAX_FRAMES:
+        raise ValueError("sift_detect: at most %d frames, got %d" % (_lib.SIFT_MAX_FRAMES, B))
+    if cap is None:
+        cap = int(lib.ffb6d_sift_capacity(H, W))
+    if isinstance(cap, bool) or not isinstance(cap, (int, np.integer)) or not 0 <= cap <= _lib.SIFT_MAX_CAP:
+        raise ValueError("sift_detect: cap must be an int in [0, %d], got %r" % (_lib.SIFT_MAX_CAP, cap))
+    cap = int(cap)
+    dev = x.device
+    count = torch.zeros(B, dtype=torch.int32, device=dev)
+    pt = torch.zeros((B, cap, 2), dtype=torch.float32, device=dev)
+    octave = torch.zeros((B, cap), dtype=torch.int32, device=dev)
+    size = torch.zeros((B, cap), dtype=torch.float32, device=dev)
+    angle = torch.zeros((B, cap), dtype=torch.float32, device=dev)
+    response = torch.zeros((B, cap), dtype=torch.float32, device=dev)
+    nbytes = int(lib.ffb6d_sift_workspace_bytes(B, H, W))
+    ws = workspace(nbytes, dev)
+    launch(lib.ffb6d_sift_detect, dev, x.data_ptr(), B, H, W, count.data_ptr(), pt.data_ptr(), octave.data_ptr(),
+           size.data_ptr(), angle.data_ptr(), response.data_ptr(), cap, ws.data_ptr(), nbytes)
+    if check and B:
+        need = int(count.max())
+        if need > cap:
+            if need > _lib.SIFT_MAX_CAP:
+                raise ValueError("sift_detect: a frame has %d keypoints, more than the limit of %d"
+                                 % (need, _lib.SIFT_MAX_CAP))
+            return sift_detect(x, need, check=True)
+    return count, pt, octave, size, angle
+
+
+def sift_lift(count, pt, depth, K, RTs, views):
+    """Lift the keypoints of :func:`sift_detect` into the object frame (``ffb6d_sift_lift``): the lift of
+    :func:`orb_lift`, for any ``cap``; frame b's first ``min(count[b], cap)`` keypoints are lifted.  Arguments and
+    result as :func:`orb_lift`'s."""
+    for t, name in ((count, "count"), (pt, "pt"), (depth, "depth")):
+        _need_cuda(t, name)
+    if count.dtype != torch.int32 or pt.dtype != torch.float32 or depth.dtype != torch.float32:
+        raise ValueError("sift_lift: count must be int32, pt and depth float32")
+    if depth.dim() != 3 or count.dim() != 1 or pt.dim() != 3 or pt.shape[-1] != 2:
+        raise ValueError("sift_lift: need count [B], pt [B,cap,2] and depth [B,H,W]")
+    B, H, W = (int(n) for n in depth.shape)
+    cap = int(pt.shape[1])
+    if tuple(count.shape) != (B,) or pt.shape[0] != B or cap > _lib.SIFT_MAX_CAP:
+        raise ValueError("sift_lift: count must be [%d] and pt [%d,cap,2], cap <= %d, got %s and %s"
+                         % (B, B, _lib.SIFT_MAX_CAP, tuple(count.shape), tuple(pt.shape)))
+    if not (_lib.SIFT_MIN_SIDE <= H <= _lib.SIFT_MAX_SIDE and _lib.SIFT_MIN_SIDE <= W <= _lib.SIFT_MAX_SIDE):
+        raise ValueError("sift_lift: H and W must lie in [%d, %d], got %dx%d"
+                         % (_lib.SIFT_MIN_SIDE, _lib.SIFT_MAX_SIDE, H, W))
+    if isinstance(views, bool) or not isinstance(views, (int, np.integer)) or views < 1 or B % views:
+        raise ValueError("sift_lift: views must be a positive int dividing B=%d, got %r" % (B, views))
+    views = int(views)
+    if views * cap >= 1 << 31:
+        raise ValueError("sift_lift: %d views of %d rows exceed the limits" % (views, cap))
+    dev = depth.device
+    rt = RTs if isinstance(RTs, torch.Tensor) else torch.from_numpy(np.asarray(RTs, np.float64))
+    if rt.dim() != 3 or rt.shape[0] != B or tuple(rt.shape[1:]) not in ((3, 4), (4, 4)):
+        raise ValueError("sift_lift: RTs must be [B,3,4] or [B,4,4], got %s" % (tuple(rt.shape),))
+    rt = rt[:, :3, :].to(device=dev, dtype=torch.float64).contiguous()
+    intr, per_frame = _intrinsics_arg(K, B, dev)
+    cloud = torch.zeros((B // views, views * cap, 3), dtype=torch.float32, device=dev)
+    n_points = torch.zeros(B // views, dtype=torch.int32, device=dev)
+    launch(lib.ffb6d_sift_lift, dev, count.contiguous().data_ptr(), pt.contiguous().data_ptr(), cap,
+           depth.contiguous().data_ptr(), B, H, W, intr.data_ptr(), per_frame, rt.data_ptr(), views,
+           cloud.data_ptr(), n_points.data_ptr())
+    return cloud, n_points
+
+
 def depth_to_mm(depth, divisor=10.0):
     """``(depth / divisor).astype(np.uint16)`` on the GPU (``ffb6d_depth_to_mm``): a float32 IEEE division, then a
     truncation, as numpy computes it for in-range values (out of range, where numpy's cast is undefined, it saturates).

@@ -657,6 +657,48 @@ int ffb6d_orb_lift(const int32_t *count, const float *pt, int64_t cap, const flo
                    int64_t W, const double *intrinsics, int intrinsics_per_frame, const double *RTs, int64_t views,
                    float *cloud, int32_t *n_points, ffb6d_stream_t stream);
 
+/*
+ * SIFT keypoints of cv2.SIFT_create()'s defaults (DESIGN.md §4.33; oracle/sift_oracle.py restates every step), the 2D
+ * stage of the reference's textured keypoint tool with --extractor SIFT.  Keypoints only, no descriptors.
+ * ffb6d_sift_detect: rgb [B,H,W,3] uint8 -> per frame b, count[b] keypoints in pt [B,cap,2] float32 (x, y image
+ *   coordinates), octave [B,cap] int32 (OpenCV's packing: octave - 1 in the low byte, layer << 8, the quantised
+ *   scale offset << 16), size, angle (degrees) and response [B,cap] float32, in canonical order: octave, DoG layer
+ *   where the extremum was found, raster order, then orientation peaks in histogram order.
+ *   Grey (3735 B + 19235 G + 9798 R + 2^14) >> 15 as float32, upscaled 2x (INTER_LINEAR, exact); cvRound(log2(min(2H,
+ *   2W)) - 2) + 1 octaves of 6 Gaussian layers (getGaussianKernel taps, ks = cvRound(8 sigma + 1) | 1, reflect-101,
+ *   OpenCV's fma order per column path) and 5 DoG layers; extrema |v| > 1 and >= (<=) their 26 neighbours at least 5
+ *   pixels from an edge; adjustLocalExtrema (5 steps, Cramer's rule, contrast 0.04, edge 10); calcOrientationHist (36
+ *   bins, strict peaks >= 0.8 max, at most 18 per extremum); duplicates of equal (pt, size, angle) removed.
+ *   cap is the caller's: any 0 <= cap <= FFB6D_SIFT_MAX_CAP (ffb6d_sift_capacity(H, W) = max(H W / 16, 256) is a
+ *   default).  Nothing is clipped silently: when a frame's keypoints do not fit, count[b] > cap is the number found
+ *   before duplicates were removed, the rows hold the first cap of them undeduplicated, and a call with cap >=
+ *   count[b] fits.  pt, octave, size, angle and response may be NULL when cap = 0.
+ *   FFB6D_SIFT_MIN_SIDE <= H, W <= FFB6D_SIFT_MAX_SIDE, 0 <= B <= FFB6D_SIFT_MAX_FRAMES (B = 0 is a no-op).
+ *   Frames run in chunks of FFB6D_SIFT_CHUNK: ffb6d_sift_workspace_bytes(B, H, W) = min(B, FFB6D_SIFT_CHUNK) times a
+ *   per-frame size (6 + 5 + 1 layers of 2H x 2W floats, two 3 (2H)(2W) int candidate arrays and the row counts),
+ *   whatever B is beyond the chunk.
+ * ffb6d_sift_lift: ffb6d_orb_lift's lift for these keypoints: any cap as above, frame b's first min(count[b], cap)
+ *   points (the caller makes sure count[b] <= cap); B / views <= FFB6D_SIFT_MAX_FRAMES, views cap < 2^31.
+ * Arguments are checked before any launch (FFB6D_ERR_INVALID; FFB6D_ERR_WORKSPACE below
+ * ffb6d_sift_workspace_bytes, which like ffb6d_sift_capacity returns 0 for sizes the entry point refuses).  Launch
+ * shapes depend on the arguments only and neither entry point synchronises: both can be captured in a CUDA graph.
+ * Deterministic: no atomic decides an output position.
+ */
+#define FFB6D_SIFT_MAX_FRAMES 65535
+#define FFB6D_SIFT_MIN_SIDE 4
+#define FFB6D_SIFT_MAX_SIDE 2048
+#define FFB6D_SIFT_MAX_CAP (1 << 26)
+#define FFB6D_SIFT_CHUNK 16
+#define FFB6D_SIFT_MAX_COPIES 18
+int64_t ffb6d_sift_capacity(int64_t H, int64_t W);
+size_t ffb6d_sift_workspace_bytes(int64_t B, int64_t H, int64_t W);
+int ffb6d_sift_detect(const uint8_t *rgb, int64_t B, int64_t H, int64_t W, int32_t *count, float *pt, int32_t *octave,
+                      float *size, float *angle, float *response, int64_t cap, void *workspace,
+                      size_t workspace_bytes, ffb6d_stream_t stream);
+int ffb6d_sift_lift(const int32_t *count, const float *pt, int64_t cap, const float *depth, int64_t B, int64_t H,
+                    int64_t W, const double *intrinsics, int intrinsics_per_frame, const double *RTs, int64_t views,
+                    float *cloud, int32_t *n_points, ffb6d_stream_t stream);
+
 /* ---- keypoint voting and pose fitting (the step after the network) -------- */
 /*
  * Gaussian mean shift of G independent vote sets, replacing MeanShiftTorch.fit
