@@ -57,6 +57,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
   z-buffer rasteriser (DESIGN.md §4.31) standing in for LineMOD's pre-rendered ``render`` pickles;
   :func:`build_ffb6d_train_item` and :class:`GraphedFrameTrainStep` take ``meshes=`` a
   :class:`~ffb6d_b200.render.RenderMeshTable` to render flagged frames of a batch.
+* :func:`fuse_rgbd` (:mod:`ffb6d_b200.fuse_frames`) -- LineMOD's ``fuse`` frames on the GPU: object crops of real
+  frames pasted into a frame (DESIGN.md §4.34); :func:`build_ffb6d_train_item` and :class:`GraphedFrameTrainStep`
+  take ``crops=`` a :class:`~ffb6d_b200.fuse_frames.FuseCropTable` to compose flagged frames of a batch.
 * :func:`orb_detect` / :func:`orb_lift` -- ORB keypoints of ``cv2.ORB_create()``'s defaults on the GPU and their
   lift onto the mesh (DESIGN.md §4.32), the stages behind :func:`ffb6d_b200.objinfo.textured_kp3ds`.
 * :func:`sift_detect` / :func:`sift_lift` -- SIFT keypoints of ``cv2.SIFT_create()``'s defaults on the GPU and
@@ -89,11 +92,13 @@ _GRAPHED = ("GraphedTrainStep", "GraphedEvalStep", "GraphedFrameTrainStep")
 _ESTIMATE = ("estimate_poses", "GraphedPoseStep")
 _EVALUATE = ("GraphedTestStep",)
 _RENDER = ("render_rgbd",)
+_FUSE = ("fuse_rgbd",)
 _SUBMODULES = ("ops", "schedule", "tables", "synthetic", "pipeline", "randla", "modules", "fusion", "dist",
                "helper_tool", "model", "pose", "item", "augment", "loss", "cnn", "graphed", "objinfo", "vis", "estimate", "evaluate", "render",
+               "fuse_frames",
                "_lib")
 
-__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED + _ESTIMATE + _EVALUATE + _RENDER) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "estimate", "evaluate", "render", "DataProcessing"]
+__all__ = list(_OPS + _SCHEDULE + _TABLES + _ITEM + _GRAPHED + _ESTIMATE + _EVALUATE + _RENDER + _FUSE) + ["randla", "modules", "fusion", "pose", "loss", "cnn", "objinfo", "vis", "estimate", "evaluate", "render", "fuse_frames", "DataProcessing"]
 
 
 def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op that is touched
@@ -113,6 +118,8 @@ def __getattr__(name):   # PEP 562: the CUDA library is loaded by the first op t
         return getattr(importlib.import_module(".evaluate", __name__), name)
     if name in _RENDER:
         return getattr(importlib.import_module(".render", __name__), name)
+    if name in _FUSE:
+        return getattr(importlib.import_module(".fuse_frames", __name__), name)
     if name == "DataProcessing":
         return importlib.import_module(".helper_tool", __name__).DataProcessing
     if name in _SUBMODULES:

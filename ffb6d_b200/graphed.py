@@ -38,7 +38,7 @@ from torch.autograd.graph import increment_version
 from . import ops
 from .loss import ffb6d_loss
 from .model import FFB6D, FFB6DFusionNet
-from .schedule import TRAIN_RECORD_KEYS, _train_item, check_render_batch, check_train_batch
+from .schedule import TRAIN_RECORD_KEYS, _train_item, check_fuse_batch, check_render_batch, check_train_batch
 
 
 # Adam's (and AdamW's) state, each created as zeros by its first step: what the warm-up's own first step created is
@@ -432,7 +432,9 @@ class GraphedFrameTrainStep(GraphedTrainStep):
     :func:`~ffb6d_b200.build_ffb6d_train_item` takes it; with ``"device"`` batches hold no ``nrm_map``), ``meshes`` (a
     :class:`~ffb6d_b200.render.RenderMeshTable`, LineMOD with ``normals="device"``: batches then hold the render keys,
     host draws or CUDA tensors, and the flagged frames are rendered into the step's input buffers before the colour
-    jitter) and ``K``
+    jitter), ``crops`` (a :class:`~ffb6d_b200.fuse_frames.FuseCropTable`, LineMOD with ``normals="device"``: batches
+    then hold the fuse keys and a per-frame ``K``, and the flagged frames' crops are pasted into the step's input
+    buffers after the renders) and ``K``
     (copied to the device once; with ``batch['K']`` the per-frame matrices are inputs instead).  Everything else that capture bakes in, and every rule
     that captures again, rejects or restores, is :class:`GraphedTrainStep`'s (DESIGN.md §4.20).
 
@@ -451,12 +453,12 @@ class GraphedFrameTrainStep(GraphedTrainStep):
     _STAGING_SLOTS = 2
 
     def __init__(self, model, optimizer, example_batch, *, dataset, cam_scale, K, n_points=12800, warmup=3,
-                 normals="input", meshes=None):
+                 normals="input", meshes=None, crops=None):
         name = type(self).__name__
         self._check_model(model)
-        check_train_batch(example_batch, dataset, name, normals, meshes)
+        check_train_batch(example_batch, dataset, name, normals, meshes, crops)
         self.dataset, self.cam_scale, self.n_points, self.normals = dataset, cam_scale, int(n_points), normals
-        self.meshes = meshes
+        self.meshes, self.crops = meshes, crops
         self._keys = set(example_batch)
         dev = next(model.parameters()).device
         device_part = {k: v for k, v in example_batch.items() if isinstance(v, torch.Tensor) and v.is_cuda}
@@ -532,7 +534,8 @@ class GraphedFrameTrainStep(GraphedTrainStep):
     def _step(self):
         batch = dict(self._static, **self._records)
         item = _train_item(batch, self.dataset, self.cam_scale, self._intr, self.n_points, self._seed,
-                           records=self._mirror, normals=self.normals, meshes=self.meshes, in_place=True)
+                           records=self._mirror, normals=self.normals, meshes=self.meshes, in_place=True,
+                           crops=self.crops)
         return self._train(item)
 
     def __call__(self, batch, seed):
@@ -540,6 +543,7 @@ class GraphedFrameTrainStep(GraphedTrainStep):
         self._check(self._sync)
         self._check_keys(batch)
         check_render_batch(batch, self.dataset, name, self.meshes, self.normals)
+        check_fuse_batch(batch, self.dataset, name, self.crops, self.normals)
         if isinstance(seed, torch.Tensor):
             ops._device_seed(seed, self._seed.device)
         elif isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:

@@ -462,15 +462,16 @@ TRAIN_RECORD_KEYS = ("jitter", "jittered", "plans", "augment", "apply_rgb")
 TRAIN_BATCH_KEYS = TRAIN_IMAGE_KEYS + TRAIN_RECORD_KEYS + _OBJECT_KEYS
 
 
-def check_train_batch(batch, dataset, name, normals="input", meshes=None):
+def check_train_batch(batch, dataset, name, normals="input", meshes=None, crops=None):
     """``ValueError`` unless ``dataset`` is known and ``batch`` is a dict holding every key of ``TRAIN_BATCH_KEYS``
-    (without ``nrm_map``, which it must not hold, under ``normals="device"``), and with ``meshes`` the render keys
-    (:func:`check_render_batch`)."""
+    (without ``nrm_map``, which it must not hold, under ``normals="device"``), with ``meshes`` the render keys
+    (:func:`check_render_batch`) and with ``crops`` the fuse keys (:func:`check_fuse_batch`)."""
     check_dataset(dataset, name)
     keys = _normal_keys(batch, name, TRAIN_BATCH_KEYS, normals)
     if not isinstance(batch, dict):
         raise ValueError("%s: the batch must be a dict, got %s" % (name, type(batch).__name__))
     check_render_batch(batch, dataset, name, meshes, normals)
+    check_fuse_batch(batch, dataset, name, crops, normals)
     missing = [k for k in keys if k not in batch]
     if missing:
         raise ValueError("%s: the batch lacks %s" % (name, missing))
@@ -517,7 +518,61 @@ def check_render_batch(batch, dataset, name, meshes, normals):
     check_mesh_indices(meshes, batch["render_mesh"], name)
 
 
-def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed, normals="input", meshes=None):
+def check_fuse_batch(batch, dataset, name, crops, normals):
+    """The fuse keys of a training batch (``ffb6d_b200.fuse_frames.FUSE_KEYS``), checked on the host before any CUDA
+    work: with ``crops`` (a :class:`~ffb6d_b200.fuse_frames.FuseCropTable`, LineMOD only, with ``normals="device"``)
+    the batch holds all four, ``fused [B]`` bool, ``fuse_crop [B,M]`` int32, ``fuse_offset [B,M,2]`` int32 and
+    ``fuse_label [B,M]`` uint8, host values or CUDA tensors, and a per-frame ``K [B,3,3]`` float64 (a fused frame's
+    camera is its own); host crop indices lie in ``[-1, len(crops))`` and no host frame is both ``rendered`` and
+    ``fused``.  Without ``crops``, none of the fuse keys.
+
+    ``crops`` with ``normals="input"`` is refused for the reason ``meshes`` is (:func:`check_render_batch`): a fused
+    frame's normals come from its own composed ``dpt_mm`` (linemod_dataset.py:251-254), which exists only on the
+    device."""
+    import numpy as np
+    from .fuse_frames import FUSE_KEYS, FuseCropTable, check_crop_indices
+    held = [k for k in FUSE_KEYS if k in batch]
+    if crops is None:
+        if held:
+            raise ValueError("%s: the batch holds the fuse keys %s but no crops were given (pass crops=, a "
+                             "FuseCropTable)" % (name, held))
+        return
+    if dataset == "ycb":
+        raise ValueError("%s: crops= composes LineMOD's fuse frames; YCB ships its synthetic frames" % name)
+    if not isinstance(crops, FuseCropTable):
+        raise ValueError("%s: crops must be a FuseCropTable, got %s" % (name, type(crops).__name__))
+    if normals != "device":
+        raise ValueError("%s: crops= needs normals='device': a fused frame's normals come from its own depth, which "
+                         "exists only on the device, so a normal map from the batch cannot belong to it" % name)
+    missing = [k for k in FUSE_KEYS if k not in batch]
+    if missing:
+        raise ValueError("%s: crops were given but the batch lacks the fuse keys %s" % (name, missing))
+    if "K" not in batch:
+        raise ValueError("%s: crops= needs a per-frame K [B,3,3] float64 in the batch: a fused frame's camera is its "
+                         "own (draw_fuse_frame)" % name)
+    B = batch["dpt"].shape[0] if hasattr(batch.get("dpt"), "shape") else None
+    M = tuple(batch["fuse_crop"].shape)[1:2] if hasattr(batch["fuse_crop"], "shape") else ()
+    want = {"fused": (torch.bool, (B,)), "fuse_crop": (torch.int32, (B,) + M),
+            "fuse_offset": (torch.int32, (B,) + M + (2,)), "fuse_label": (torch.uint8, (B,) + M),
+            "K": (torch.float64, (B, 3, 3))}
+    host = {}
+    for k, (dtype, shape) in want.items():
+        t = batch[k] if isinstance(batch[k], torch.Tensor) else torch.as_tensor(np.asarray(batch[k]))
+        if t.dtype != dtype or tuple(t.shape) != shape or len(M) != 1:
+            raise ValueError("%s: batch[%r] must be %s %s, got %s %s" % (name, k, dtype, shape, t.dtype,
+                                                                       tuple(t.shape)))
+        host[k] = None if t.is_cuda else t
+    check_crop_indices(crops, batch["fuse_crop"], name)
+    rendered = batch.get("rendered")
+    if host["fused"] is not None and rendered is not None and not (isinstance(rendered, torch.Tensor)
+                                                                   and rendered.is_cuda):
+        both = np.flatnonzero(host["fused"].numpy() & np.asarray(rendered, dtype=bool).reshape(-1))
+        if both.size:
+            raise ValueError("%s: frames %s are flagged both rendered and fused" % (name, both.tolist()))
+
+
+def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed, normals="input", meshes=None,
+                           crops=None):
     """The training ``get_item`` of a collated batch on the GPU, in the reference's order: the colour jitter, the first
     ``rgb_add_noise``, ``add_real_back``, the second ``rgb_add_noise``, :func:`build_ffb6d_item` (``fill=True`` for
     YCB, ``False`` for LineMOD) and ``model_fn``'s ``rgb.float()``.  This is INTEGRATION.md's trainer composition in
@@ -541,10 +596,16 @@ def build_ffb6d_train_item(batch, *, dataset, cam_scale, K, n_points, seed, norm
       as the reference loads a render pickle before ``get_item``'s augmentation.  Every frame's normals are then
       computed from its composed depth, the rendered frames' from the render's.  The renders go into copies; the
       batch's tensors are not written
+    :param crops: LineMOD only, with ``normals="device"``: a :class:`~ffb6d_b200.fuse_frames.FuseCropTable`.  The
+      batch then also holds the fuse keys (``fused [B]`` bool, ``fuse_crop [B,M]`` int32, ``fuse_offset [B,M,2]``
+      int32, ``fuse_label [B,M]`` uint8, host draws or CUDA tensors) and a per-frame ``K``, and the flagged frames'
+      crops are pasted by :func:`~ffb6d_b200.fuse_frames.fuse_rgbd` over their ``dpt`` / ``rgb`` / ``labels``,
+      after the renders and before the colour jitter.  A frame is rendered or fused, not both.  The pastes go into
+      copies; the batch's tensors are not written
     :return: the dict of :func:`build_ffb6d_item` with ``rgb`` as float32
     """
-    check_train_batch(batch, dataset, "build_ffb6d_train_item", normals, meshes)
-    return _train_item(batch, dataset, cam_scale, K, n_points, seed, normals=normals, meshes=meshes)
+    check_train_batch(batch, dataset, "build_ffb6d_train_item", normals, meshes, crops)
+    return _train_item(batch, dataset, cam_scale, K, n_points, seed, normals=normals, meshes=meshes, crops=crops)
 
 
 def _render_frames(batch, meshes, K, in_place):
@@ -559,11 +620,24 @@ def _render_frames(batch, meshes, K, in_place):
     return dict(batch, dpt=out[0], rgb=out[1], labels=out[2])
 
 
+def _fuse_frames(batch, crops, in_place):
+    """The batch with its flagged frames' crops pasted over ``dpt`` / ``rgb`` / ``labels``: into the batch's own
+    tensors with ``in_place`` (a graph's input buffers, or copies the renders already made), else into copies."""
+    from .fuse_frames import fuse_rgbd
+    out = tuple(batch[k] if in_place else batch[k].clone(memory_format=torch.contiguous_format)
+                for k in ("dpt", "rgb", "labels"))
+    B, H, W = out[0].shape
+    fuse_rgbd(crops, batch["fuse_crop"], batch["fuse_offset"], batch["fuse_label"], H, W, active=batch["fused"],
+              out=out)
+    return dict(batch, dpt=out[0], rgb=out[1], labels=out[2])
+
+
 def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None, normals="input", meshes=None,
-                in_place=False):
+                in_place=False, crops=None):
     """:func:`build_ffb6d_train_item` on a checked batch.  ``records``: host copies of ``batch['jitter']`` and
     ``batch['plans']`` when the batch holds those on the device (a graph's input buffers); the host copies are what
-    the entry points check, the device ones what the kernels read.  ``in_place``: render into the batch's tensors."""
+    the entry points check, the device ones what the kernels read.  ``in_place``: render and paste into the batch's
+    tensors."""
     import numpy as np
     from .ops import _frame_intrinsics, add_real_back, color_jitter, rgb_add_noise
     if "K" in batch:
@@ -572,6 +646,8 @@ def _train_item(batch, dataset, cam_scale, K, n_points, seed, records=None, norm
             K = _frame_intrinsics(K)
     if meshes is not None:
         batch = _render_frames(batch, meshes, K, in_place)
+    if crops is not None:
+        batch = _fuse_frames(batch, crops, in_place or meshes is not None)
     if records is None:
         jitter, plans = np.asarray(batch["jitter"]), np.asarray(batch["plans"])
         jitter_d = plans_d = None

@@ -617,6 +617,36 @@ int ffb6d_render_rgbd(const float *xyz, const uint8_t *vrgb, const int32_t *face
                       void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
 
 /*
+ * LineMOD's `fuse` frames (DESIGN.md §4.34): object crops of real frames pasted into a frame, the GPU stand-in for
+ * raster_triangle's fuse pickles (datasets/linemod/linemod_dataset.py:202-213).  Specified here; restated by
+ * oracle/fuse_oracle.py.
+ * Crop table (built by the caller): n_crops crops, crop k of size h x w = crop_hw[2k], crop_hw[2k+1] (int32, >= 1)
+ *   owns the pixels [crop_off[k], crop_off[k] + h w) of the planes, row-major: crop_rgb (3 bytes per pixel),
+ *   crop_dpt (uint16 mm) and crop_sil (uint8, 0 = not the object).  Not checked here: the caller keeps every crop
+ *   inside its planes.
+ * Per frame b and slot s < M: c = crop[b,s] int32 (-1 empty; any value outside [0, n_crops) pastes nothing),
+ *   (row, col) = offset[b,s,0..1] int32, any value (the crop's top-left corner in the frame), label[b,s] uint8.
+ * Pixel (r, c) of frame b takes the highest slot s whose crop holds (r - row, c - col) (computed in int64) inside
+ *   [0, h) x [0, w) with its silhouette set: dpt_mm[b,r,c] and rgb[b,r,c] become the crop's, labels[b,r,c] the
+ *   slot's label.  Slot order is paste order (a later slot covers an earlier one).  A pixel no slot covers, and
+ *   every pixel of an inactive frame (active [B] uint8 != 0, or NULL: every frame), is not written.
+ * 0 <= B <= FFB6D_FUSE_MAX_FRAMES (B = 0 is a no-op), 1 <= H, W, H W <= FFB6D_FUSE_MAX_FRAME_PIXELS,
+ * 1 <= M <= FFB6D_FUSE_MAX_SLOTS (the slot records live in shared memory), 1 <= n_crops <= FFB6D_FUSE_MAX_CROPS;
+ * every pointer non-NULL (active excepted) and aligned to its element.  Checked before any launch
+ * (FFB6D_ERR_INVALID).  One launch whose shape depends on the arguments only, no workspace, no allocation, no host
+ * synchronisation (capturable in a CUDA graph); every output byte is written at most once, without atomics, so the
+ * result is deterministic.
+ */
+#define FFB6D_FUSE_MAX_FRAMES 65535
+#define FFB6D_FUSE_MAX_FRAME_PIXELS 2147483647ll
+#define FFB6D_FUSE_MAX_SLOTS 1024
+#define FFB6D_FUSE_MAX_CROPS 2147483647ll
+int ffb6d_fuse_rgbd(const uint8_t *crop_rgb, const uint16_t *crop_dpt, const uint8_t *crop_sil, const int64_t *crop_off,
+                    const int32_t *crop_hw, int64_t n_crops, const int32_t *crop, const int32_t *offset,
+                    const uint8_t *label, int64_t B, int64_t M, int64_t H, int64_t W, const uint8_t *active,
+                    uint16_t *dpt_mm, uint8_t *rgb, uint8_t *labels, ffb6d_stream_t stream);
+
+/*
  * ORB keypoints of cv2.ORB_create()'s defaults (DESIGN.md §4.32; oracle/orb_oracle.py restates every step), the 2D
  * stage of the reference's textured keypoint tool (utils/dataset_tools/rgbd_rnder_sift_kp3ds.py:138-166).
  * ffb6d_orb_detect: rgb [B,H,W,3] uint8 -> per frame b, count[b] keypoints in pt [B,cap,2] float32 (x, y image
