@@ -56,7 +56,9 @@ Public surface (same names and argument meaning as the reference, ethnhe/FFB6D):
 * :func:`render_rgbd` (:mod:`ffb6d_b200.render`) -- synthetic RGB-D frames of vertex-coloured meshes on the GPU, a
   z-buffer rasteriser (DESIGN.md §4.31) standing in for LineMOD's pre-rendered ``render`` pickles;
   :func:`build_ffb6d_train_item` and :class:`GraphedFrameTrainStep` take ``meshes=`` a
-  :class:`~ffb6d_b200.render.RenderMeshTable` to render flagged frames of a batch.
+  :class:`~ffb6d_b200.render.RenderMeshTable` to render flagged frames of a batch.  A
+  :class:`~ffb6d_b200.render.TexturedMeshTable` renders UV-mapped, mipmapped meshes through the same call (DESIGN.md
+  §4.35), the renders of the dataset tool's pyrender path behind ``objinfo.textured_kp3ds``.
 * :func:`fuse_rgbd` (:mod:`ffb6d_b200.fuse_frames`) -- LineMOD's ``fuse`` frames on the GPU: object crops of real
   frames pasted into a frame (DESIGN.md §4.34); :func:`build_ffb6d_train_item` and :class:`GraphedFrameTrainStep`
   take ``crops=`` a :class:`~ffb6d_b200.fuse_frames.FuseCropTable` to compose flagged frames of a batch.

@@ -55,6 +55,9 @@ RND_MAX_FRAME_FACES = 1 << 32
 RND_GUARD_BAND = 1 << 14
 RND_BIG_FACE_PIXELS = 256
 RND_QUEUE_CAP = 1 << 20
+RND_MAX_TEX_SIDE = 16384
+RND_MAX_TEX_LEVELS = 15
+RND_MAX_UV = 1 << 16
 FUSE_MAX_FRAMES = 65535                          # FFB6D_FUSE_* of include/ffb6d_b200.h
 FUSE_MAX_FRAME_PIXELS = (1 << 31) - 1
 FUSE_MAX_SLOTS = 1024
@@ -160,6 +163,9 @@ def _load():
         "ffb6d_render_workspace_bytes": (sz, [i64, i64, i64, i64, i64, i64]),
         "ffb6d_render_rgbd": (ci, [vp, vp, vp, vp, vp, i64, i64, i64, vp, vp, vp, i64, i64, vp, ci, i64, i64,
                                    C.c_double, vp, vp, vp, vp, vp, vp, sz, vp]),
+        "ffb6d_render_texture_mips": (ci, [vp, vp, vp, i64, i64, vp]),
+        "ffb6d_render_rgbd_textured": (ci, [vp, vp, vp, vp, vp, vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, i64, i64,
+                                            vp, ci, i64, i64, C.c_double, vp, vp, vp, vp, vp, vp, sz, vp]),
         "ffb6d_fuse_rgbd": (ci, [vp, vp, vp, vp, vp, i64, vp, vp, vp, i64, i64, i64, i64, vp, vp, vp, vp, vp]),
         "ffb6d_orb_capacity": (i64, [i64, i64]),
         "ffb6d_orb_workspace_bytes": (sz, [i64, i64, i64]),

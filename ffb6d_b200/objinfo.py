@@ -11,7 +11,9 @@ returns, already divided by ``scale2m``).  The tool's textured keypoints -- ORB 
 views, lifted onto the mesh and reduced by farthest point sampling (rgbd_rnder_sift_kp3ds.py:138-166,
 gen_obj_info.py:119-126), the table the datasets read with ``use_orbfps`` -- run on the GPU through
 :func:`textured_kp3ds` (DESIGN.md §4.32); the tool's ``--extractor SIFT`` (the paper's SIFT-FPS keypoints) through
-``textured_kp3ds(..., extractor="SIFT")`` (§4.33).  Plain numpy; only :func:`gen_obj_info` and :func:`textured_kp3ds` load
+``textured_kp3ds(..., extractor="SIFT")`` (§4.33); a textured object (the tool's ``--use_pyrender`` branch,
+pyrender_sift_kp3ds.py:104-132, YCB's meshes) through ``textured_kp3ds`` of a
+:class:`~ffb6d_b200.render.TexturedMeshTable` (§4.35), centred as that branch centres it.  Plain numpy; only :func:`gen_obj_info` and :func:`textured_kp3ds` load
 the CUDA library.
 """
 import math
@@ -80,36 +82,49 @@ def camera_pose(T):
     return camera
 
 
-def o2c_pose(cam_pose):
-    """``PoseUtils.get_o2c_pose_cv(cam_pose, np.eye(4))``: object to OpenCV camera, ``[4,4]`` float64."""
+def o2c_pose(cam_pose, obj_pose=np.eye(4)):
+    """``PoseUtils.get_o2c_pose_cv(cam_pose, obj_pose)``: object to OpenCV camera, ``[4,4]`` float64; ``obj_pose`` the
+    object's pose in the world (the raster_triangle branch's identity, or the pyrender branch's ``T(-mean)``)."""
     R_bcam2cv = np.array([(1, 0, 0), (0, -1, 0), (0, 0, -1)])
     R_world2bcam = cam_pose[:3, :3].T
     T_world2bcam = -1 * R_world2bcam @ cam_pose[:3, 3]
     RT = np.eye(4)
     RT[:3, :3] = R_bcam2cv @ R_world2bcam
     RT[:3, 3] = R_bcam2cv @ T_world2bcam
-    return np.matmul(RT, np.eye(4))
+    return np.matmul(RT, obj_pose)
 
 
-def sphere_poses(radius, n_longitude=3, n_latitude=3):
+def sphere_poses(radius, n_longitude=3, n_latitude=3, centre=None):
     """The tool's views of an object whose box has radius ``radius`` (``get_r``; a float32 scalar for float32
     vertices, as in the tool): ``[n_longitude * n_latitude, 4, 4]`` float64 object-to-camera poses on a sphere of
-    radius ``radius / 0.035 * 0.18`` (rgbd_rnder_sift_kp3ds.py:147-158)."""
+    radius ``radius / 0.035 * 0.18`` (rgbd_rnder_sift_kp3ds.py:147-158).  With ``centre`` (``[3]``) the object is
+    first moved by ``-centre``, as the pyrender branch moves it by its vertices' mean (pyrender_sift_kp3ds.py:105-120)."""
     sph_r = radius / 0.035 * 0.18
-    return np.stack([o2c_pose(camera_pose(p)) for p in camera_positions(n_longitude, n_latitude, sph_r)])
+    if centre is None:
+        return np.stack([o2c_pose(camera_pose(p)) for p in camera_positions(n_longitude, n_latitude, sph_r)])
+    obj_pose = np.eye(4)
+    obj_pose[:3, 3] = -1.0 * np.asarray(centre, np.float64)
+    return np.stack([o2c_pose(camera_pose(p), obj_pose)
+                     for p in camera_positions(n_longitude, n_latitude, sph_r)])
 
 
 def textured_kp3ds(table, mesh, K=TOOL_K, H=TOOL_H, W=TOOL_W, n_longitude=3, n_latitude=3, radius=None,
-                   extractor="ORB"):
+                   extractor="ORB", centre=None):
     """The tool's ``extract_textured_kp3ds`` on the GPU for one or more meshes of a
     :class:`~ffb6d_b200.render.RenderMeshTable`: each object rendered from its sphere of views (``render_rgbd``),
     ORB keypoints of every render (``orb_detect``) and their lift into the object frame (``orb_lift``); with
-    ``extractor="SIFT"`` the tool's SIFT branch, ``sift_detect`` and ``sift_lift``.
+    ``extractor="SIFT"`` the tool's SIFT branch, ``sift_detect`` and ``sift_lift``.  With a
+    :class:`~ffb6d_b200.render.TexturedMeshTable` the tool's pyrender branch: the same stages on textured renders,
+    each object centred first.
 
     :param mesh: an index into ``table``, or a list of them (one object each)
     :param K, H, W: the camera and frame size (the tool's defaults); :param n_longitude, n_latitude: the views
     :param radius: each object's box radius (:func:`get_r`), or None to compute it from the table's vertices
     :param extractor: ``"ORB"`` or ``"SIFT"``, the tool's ``--extractor``
+    :param centre: each object's centre ``[3]`` (a list of them for several objects), moved to the origin before the
+      views are taken (:func:`sphere_poses`); None: no move for a :class:`RenderMeshTable` (the raster_triangle
+      branch), the mean of the table's vertices for a :class:`TexturedMeshTable`.  The lift takes the float64
+      centred poses and the render their float32 rounding.
     :return: ``(cloud [n_obj, V cap, 3] float32, n_points [n_obj] int32, short [n_obj, V] bool)`` on the device, V =
       n_longitude n_latitude: each object's pooled points, views in order.  A view with fewer than 500 drawn pixels
       contributes no points and is flagged in ``short`` (the tool stops with an error there).
@@ -117,11 +132,13 @@ def textured_kp3ds(table, mesh, K=TOOL_K, H=TOOL_H, W=TOOL_W, n_longitude=3, n_l
     import torch
     from . import _lib
     from .ops import orb_detect, orb_lift, sift_detect, sift_lift
-    from .render import RenderMeshTable, render_rgbd
+    from .render import RenderMeshTable, TexturedMeshTable, render_rgbd
     if extractor not in ("ORB", "SIFT"):
         raise ValueError("textured_kp3ds: extractor must be 'ORB' or 'SIFT', got %r" % (extractor,))
-    if not isinstance(table, RenderMeshTable):
-        raise ValueError("textured_kp3ds: table must be a RenderMeshTable, got %s" % type(table).__name__)
+    textured = isinstance(table, TexturedMeshTable)
+    if not (textured or isinstance(table, RenderMeshTable)):
+        raise ValueError("textured_kp3ds: table must be a RenderMeshTable or a TexturedMeshTable, got %s"
+                         % type(table).__name__)
     objs = [int(m) for m in (mesh if isinstance(mesh, (list, tuple, np.ndarray)) else [mesh])]
     if not objs or min(objs) < 0 or max(objs) >= len(table):
         raise ValueError("textured_kp3ds: mesh indices must lie in [0, %d), got %s" % (len(table), objs))
@@ -134,14 +151,27 @@ def textured_kp3ds(table, mesh, K=TOOL_K, H=TOOL_H, W=TOOL_W, n_longitude=3, n_l
     lo, hi = (_lib.ORB_MIN_SIDE, _lib.ORB_MAX_SIDE) if extractor == "ORB" else (_lib.SIFT_MIN_SIDE, _lib.SIFT_MAX_SIDE)
     if not (lo <= H <= hi and lo <= W <= hi):
         raise ValueError("textured_kp3ds: H and W must lie in [%d, %d], got %dx%d" % (lo, hi, H, W))
-    if radius is None:
+    if radius is None or (centre is None and textured):
         off = np.concatenate([[0], np.cumsum(table.n_verts)])
         xyz = table.xyz.cpu().numpy()
-        radius = [get_r(get_3D_bbox(xyz[off[m]:off[m + 1]])) for m in objs]
+        verts = [xyz[off[m]:off[m + 1]] for m in objs]
+        if radius is None:
+            radius = [get_r(get_3D_bbox(v)) for v in verts]
+        if centre is None and textured:
+            centre = [np.mean(v.astype(np.float64), axis=0) for v in verts]
     radius = list(radius) if isinstance(radius, (list, tuple, np.ndarray)) else [radius]
     if len(radius) != len(objs):
         raise ValueError("textured_kp3ds: %d radii for %d objects" % (len(radius), len(objs)))
-    RT = np.concatenate([sphere_poses(r, n_longitude, n_latitude) for r in radius])
+    if centre is None:
+        centre = [None] * len(objs)
+    else:
+        centre = np.asarray(centre, np.float64)
+        if centre.shape not in ((3,), (len(objs), 3)):
+            raise ValueError("textured_kp3ds: centre must be [3] or [%d,3], got %s" % (len(objs), centre.shape))
+        centre = list(centre.reshape(-1, 3)) if centre.ndim == 2 else [centre]
+        if len(centre) != len(objs):
+            raise ValueError("textured_kp3ds: %d centres for %d objects" % (len(centre), len(objs)))
+    RT = np.concatenate([sphere_poses(r, n_longitude, n_latitude, c) for r, c in zip(radius, centre)])
     dev = table.device
     mesh_idx = np.repeat(np.asarray(objs, np.int32), V)[:, None]
     depth, rgb, _ = render_rgbd(table, mesh_idx, RT[:, None, :3, :].astype(np.float32), np.ones((B, 1), np.uint8),
@@ -164,7 +194,9 @@ def gen_obj_info(points, n_keypoint=8, init_center=False, start=None, *, mesh=No
     :param mesh: None, or a :class:`~ffb6d_b200.render.RenderMeshTable` whose mesh 0 is this object (vertices
       ``points``): then the tool's textured keypoints are computed too (:func:`textured_kp3ds` with ``K``, ``H``,
       ``W``, ``n_longitude``, ``n_latitude``), and their farthest point sampling starts at ``textured_start`` (None:
-      random, as the tool's)
+      random, as the tool's).  A :class:`~ffb6d_b200.render.TexturedMeshTable` runs the tool's ``--use_pyrender``
+      branch: the views are centred on ``np.mean(points, axis=0)`` (taken in float64), the tool's mean of the
+      ``.obj``'s vertices -- pass those as ``points``, not the table's seam-split copy
     :param extractor: the textured keypoints' detector, ``"ORB"`` or ``"SIFT"`` (the tool's ``--extractor``)
     :return: dict ``corners [8,3]``, ``radius``, ``center [3]`` and ``fps [n_keypoint,3]`` (float32 vertices).
       ``fps`` is what ``pose_gt_objects(kps=...)`` and ``cal_frame_poses(mesh_kps=...)`` take as an object's keypoints.
@@ -184,8 +216,10 @@ def gen_obj_info(points, n_keypoint=8, init_center=False, start=None, *, mesh=No
                 fps=farthest_point_sampling(points, n_keypoint, init_center=init_center, start=start))
     if mesh is None:
         return info
+    from .render import TexturedMeshTable
+    centre = np.mean(points.astype(np.float64), axis=0) if isinstance(mesh, TexturedMeshTable) else None
     cloud, n_points, short = textured_kp3ds(mesh, 0, K, H, W, n_longitude, n_latitude, radius=info["radius"],
-                                            extractor=extractor)
+                                            extractor=extractor, centre=centre)
     n = int(n_points[0])
     if not 1 <= n <= FPS_MAX_POINTS:
         raise ValueError("gen_obj_info: %d textured keypoints; farthest point sampling takes 1 to %d" % (n, FPS_MAX_POINTS))

@@ -617,6 +617,62 @@ int ffb6d_render_rgbd(const float *xyz, const uint8_t *vrgb, const int32_t *face
                       void *workspace, size_t workspace_bytes, ffb6d_stream_t stream);
 
 /*
+ * Textured meshes (DESIGN.md §4.35): ffb6d_render_rgbd's rasteriser with per-vertex UVs and a mipmapped RGB texture
+ * per mesh in place of vertex colours, the GPU stand-in for the dataset tool's pyrender path
+ * (utils/dataset_tools/pyrender_sift_kp3ds.py).  Restated by oracle/textured_render_oracle.py.
+ * Everything but a drawn pixel's colour is ffb6d_render_rgbd's: the vertex stage, coverage, depth (and depth_mm),
+ * the visibility key, labels, empty pixels and active.  So depth and labels equal, bit for bit, ffb6d_render_rgbd's
+ * of the same xyz / faces with any vertex colours.  Colour of a drawn pixel, float64 without contraction, one
+ * rounding per operation, with the winning face's w_k, p_k = w_k (1/Z_k) and S = (p0 + p1) + p2:
+ *   UV: uv [V_total,2] float32 per vertex (the .obj / trimesh convention: v = 0 is the bottom row of the image as
+ *     decoded, row 0 its top; a seam is split into separate vertices by the caller).
+ *     u = ((p0 u0 + p1 u1) + p2 u2) / S, and v likewise.
+ *   Screen derivatives, per pixel and analytic (no 2x2 quads): for the edge (a, b) = (V[k+1], V[k+2]) of w_k and
+ *     sgn = sign(A), gx_k = -256 sgn (b.y - a.y) and gy_k = 256 sgn (b.x - a.x), the exact integer steps of w_k per
+ *     pixel.  u_x = (((gx_0 (1/Z_0)) (u_0 - u) + (gx_1 (1/Z_1)) (u_1 - u)) + (gx_2 (1/Z_2)) (u_2 - u)) / S, and
+ *     u_y, v_x, v_y likewise.
+ *   Level of detail, with (Th, Tw) level 0's size and L = floor(log2(max(Th, Tw))) + 1 levels:
+ *     rho = max(sqrt((u_x Tw)^2 + (v_x Th)^2), sqrt((u_y Tw)^2 + (v_y Th)^2)) (correctly rounded square roots; the
+ *     sum before each is (a a) + (b b)).  !(rho > 1): level 0 alone.  rho >= 2^(L-1) (inf included): level L-1
+ *     alone.  Otherwise e = floor(log2 rho), exact from the exponent, t = rho 2^-e - 1 (exact), and the colour blends
+ *     levels e and e+1: c = (1 - t) c_e + t c_{e+1}.  Linear in rho, not GL's frac(log2 rho): exact, and no
+ *     transcendental function.
+ *   Bilinear sample at level l of size W_l x H_l: x = u W_l - 0.5, y = (1 - v) H_l - 0.5, x0 = floor(x),
+ *     fx = x - x0, y0 = floor(y), fy = y - y0; texel columns x0, x0 + 1 and rows y0, y0 + 1 wrap (REPEAT, glTF's
+ *     default): ((n mod W_l) + W_l) mod W_l.  With weights w00 = (1 - fx)(1 - fy), w10 = fx (1 - fy),
+ *     w01 = (1 - fx) fy, w11 = fx fy, each channel c_l = ((w00 t00 + w10 t10) + w01 t01) + w11 t11 (t10: column
+ *     x0 + 1, row y0).  The levels blend before any rounding; the channel written is clamp(floor(c + 0.5), 0, 255).
+ *   Unlit: the colour is the filtered texel.
+ * Texture table (built by the caller, ffb6d_render_texture_mips): tex uint8 RGB texels, row-major, level l of mesh m
+ *   (size max(1, Th >> l) x max(1, Tw >> l)) at texel offset tex_off[m FFB6D_RND_MAX_TEX_LEVELS + l] (int64; byte
+ *   3 tex_off); tex_hw [n_meshes,2] int32 (Th, Tw) of level 0, each in [1, max_tex_side].  Not read here: the caller
+ *   keeps them consistent, with every |uv| <= FFB6D_RND_MAX_UV and finite (checked on the host, as face indices).
+ * 1 <= max_tex_side <= FFB6D_RND_MAX_TEX_SIDE, so a chain has at most FFB6D_RND_MAX_TEX_LEVELS levels; every other
+ * size, pointer and workspace rule is ffb6d_render_rgbd's (same ffb6d_render_workspace_bytes), with uv, tex, tex_hw
+ * and tex_off non-NULL and aligned to their elements.  Checked before any launch (FFB6D_ERR_INVALID /
+ * FFB6D_ERR_WORKSPACE).  One memset and four launches whose shapes depend on the arguments only, no host
+ * synchronisation (capturable in a CUDA graph); texels are software loads, not the hardware filter.
+ *
+ * ffb6d_render_texture_mips: levels 1 .. L-1 of every mesh's chain in place from level 0, one launch per level
+ *   across all meshes, floor(log2 max_tex_side) launches (none for 1).  Texel (i, j) (column,
+ *   row) of level l + 1 is (a + b + c + d + 2) >> 2 of level l's texels (2i, 2j), (2i+1, 2j), (2i, 2j+1),
+ *   (2i+1, 2j+1), each index clamped to level l's last column / row; integer-exact.  Same argument rules.
+ */
+#define FFB6D_RND_MAX_TEX_SIDE 16384
+#define FFB6D_RND_MAX_TEX_LEVELS 15
+#define FFB6D_RND_MAX_UV 65536
+int ffb6d_render_texture_mips(uint8_t *tex, const int32_t *tex_hw, const int64_t *tex_off, int64_t n_meshes,
+                              int64_t max_tex_side, ffb6d_stream_t stream);
+int ffb6d_render_rgbd_textured(const float *xyz, const float *uv, const int32_t *faces, const int64_t *vert_off,
+                               const int64_t *face_off, const uint8_t *tex, const int32_t *tex_hw,
+                               const int64_t *tex_off, int64_t max_tex_side, int64_t n_meshes, int64_t max_verts,
+                               int64_t max_faces, const int32_t *mesh_idx, const float *RTs, const uint8_t *label,
+                               int64_t B, int64_t M, const double *intrinsics, int intrinsics_per_frame, int64_t H,
+                               int64_t W, double z_near, const uint8_t *active, float *depth, uint16_t *depth_mm,
+                               uint8_t *rgb, uint8_t *labels, void *workspace, size_t workspace_bytes,
+                               ffb6d_stream_t stream);
+
+/*
  * LineMOD's `fuse` frames (DESIGN.md §4.34): object crops of real frames pasted into a frame, the GPU stand-in for
  * raster_triangle's fuse pickles (datasets/linemod/linemod_dataset.py:202-213).  Specified here; restated by
  * oracle/fuse_oracle.py.
